@@ -41,7 +41,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops_burst=d["bf16_tflops"],
                     tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tflops_burst=1590.0, tflops_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA's H100 SXM data sheet (dense BF16, HBM3), for a card allowed 700 W: not reached on a power-limited card
+    return dict(hbm_gbs=3350.0, tflops_burst=989.0, tflops_sustained=989.0, source="H100 SXM data sheet (700 W), not measured")
 
 
 class ClockSampler:
@@ -160,7 +161,7 @@ def oracle_cpu_run(steps: int, warmup: int, n_envs: int = N_ENVS, calibrate: boo
 
 
 def _ref_driver_call(n_envs: int, steps: int, warmup: int, threads: int, timeout: int = 1500):
-    """One run of the UNMODIFIED reference (baseline/_ref, driven by oracle/ref_driver.py) in a subprocess (its logger is
+    """One run of the UNMODIFIED reference (oracle/_ref, driven by oracle/ref_driver.py) in a subprocess (its logger is
     chatty and its thread settings are process-wide).  Returns the result dict or None."""
     cmd = [sys.executable, "-m", "oracle.ref_driver", "--n_envs", str(n_envs), "--rollout", str(ROLLOUT), "--obs_dim",
            str(OBS_DIM), "--num_actions", str(N_ACTIONS), "--batch_size", str(n_envs * ROLLOUT // N_MINIBATCH),
@@ -178,9 +179,9 @@ def _ref_driver_call(n_envs: int, steps: int, warmup: int, threads: int, timeout
 
 
 def reference_cpu_run(steps: int, warmup: int, n_envs: int = N_ENVS):
-    """The reference's own CPU implementation of the path (sample-factory 2.1.3 installed in baseline/_ref): serial mode,
+    """The reference's own CPU implementation of the path (sample-factory 2.1.3 installed in oracle/_ref): serial mode,
     batched sampling, torch CPU.  torch CPU throughput on this workload is not monotone in the thread count, so the count
-    is calibrated on a reduced run (1024 envs) and reported as `cores`.  None when baseline/_ref is absent."""
+    is calibrated on a reduced run (1024 envs) and reported as `cores`.  None when oracle/_ref is absent."""
     from oracle import ref_driver
 
     if not ref_driver.available():
@@ -206,13 +207,13 @@ def run_reference(args):
     r = reference_cpu_run(args.steps, args.warmup, n_envs)
     if r is not None:
         kind = "reference"
-        sample = (f"{what}; the unmodified reference (sample-factory 2.1.3 pip-installed into baseline/_ref) driven through "
+        sample = (f"{what}; the unmodified reference (sample-factory 2.1.3 pip-installed into oracle/_ref) driven through "
                   f"BatchedVectorEnvRunner + ActorCritic forward + Learner.train, serial mode, torch CPU, "
                   f"{r['cores']} of {os.cpu_count()} host threads (best of a calibration sweep)")
     else:
         kind = "port"
         r = oracle_cpu_run(args.steps, args.warmup, n_envs)
-        sample = (f"{what}; oracle port (baseline/_ref absent), torch CPU with the best-performing intra-op thread count "
+        sample = (f"{what}; oracle port (oracle/_ref absent), torch CPU with the best-performing intra-op thread count "
                   f"({r['cores']} of {os.cpu_count()} host threads)")
     workload = WORKLOAD if args.gpus == 1 else WORKLOAD.replace("4096 envs per GPU", f"{n_envs} envs (= 4096 per GPU of our arm)")
     out = dict(impl="reference", metric=METRIC, value=r["value"], unit=UNIT, n_gpus=args.gpus, steps=args.steps,
@@ -334,6 +335,43 @@ def dp_check(rank: int, world: int, dev, engine_flag: str, bench_model) -> dict:
     return out
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, runner):
+    """What the timed path computed in its last step, as a caller of Runner.iteration() receives it: the trajectories of
+    the last rollout (policy outputs, env outputs), the learner's returns / advantages and minibatch log, and the updated
+    parameters -- one DIR/<name>.npy each, float32 or float64.  Observations are inputs (a fixed, seeded tape) and are
+    not written.  Arrays beyond the 64 MB budget are cut to a fixed, seeded sample of rows."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    arrays = {}
+    for k, v in runner.traj.items():
+        if k in ("obs", "rnn_states"):
+            continue
+        arrays[f"traj_{k}"] = v
+    learner = runner.learner
+    for k in ("returns", "advantages"):
+        if isinstance(getattr(learner, k, None), torch.Tensor):
+            arrays[f"learner_{k}"] = getattr(learner, k)
+    arrays["learner_minibatch_log"] = learner.minibatch_log()
+    arrays["model_params"] = runner.model.flat
+    budget = DUMP_MAX_BYTES
+    gen = torch.Generator().manual_seed(0)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        t = t.double() if t.dtype == torch.float64 else t.float()
+        if t.numel() * t.element_size() > budget // 4 and t.dim() > 0:
+            keep = max(1, (budget // 4) // max(1, t[0].numel() * t.element_size()))
+            t = t[torch.randperm(t.shape[0], generator=gen)[:keep].sort().values]
+        budget -= t.numel() * t.element_size()
+        if budget < 0:
+            raise RuntimeError("--dump-outputs: the outputs exceed 64 MB")
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.numpy())
+
+
 def run_ours(args):
     from sample_factory_b200 import ops
     from sample_factory_b200.dist_utils import init_from_env
@@ -377,8 +415,8 @@ def run_ours(args):
         torch.cuda.synchronize()
 
     def _ncu_traffic(key):
-        """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture
-        (profiles/traffic.json records the capture it came from); None when no capture is committed."""
+        """DRAM bytes per launch of the dominant kernel from a committed profiler capture (profiles/traffic.json);
+        None when no capture is committed."""
         try:
             with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "traffic.json")) as f:
                 return json.load(f)[key]["traffic_bytes"]
@@ -396,7 +434,7 @@ def run_ours(args):
     runner = Runner(make_cfg("synthetic_tape", args.engine, not args.no_graph, splits=args.splits,
                              learner_graph=not (args.no_learner_graph or args.no_graph)))
     runner.init()
-    engine_name = {0: "simt-fp32", 1: "tcgen05-3xTF32", 2: "tcgen05-TF32"}[runner.engine]
+    engine_name = {0: "simt-fp32", 1: "wgmma-3xTF32", 2: "wgmma-TF32"}[runner.engine]
 
     # live per-kernel timing of the dominant kernel (the learner's layer-2 forward GEMM, M=32768 N=K=512) and of the
     # main HBM-bound kernels, with CUDA events on the launching stream, inside the timed region
@@ -453,6 +491,8 @@ def run_ours(args):
     e1.record()
     barrier()
     timing_on[0] = False
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, runner)
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     gpu_launches = (ops.launch_count() - launches0) + replay_launches
     learner_graphed = bool(runner.learner.use_graph)
@@ -484,7 +524,7 @@ def run_ours(args):
                         traffic=_ncu_traffic("gemm_fwd_l2"), avg_kernel_ms=k["avg_ms"], launches_timed=k["launches"],
                         peak_source=peaks["source"] + ", bf16 sustained (kernel timed inside a long step)",
                         note="fp32-parity GEMM = 3 tensor-core passes per product (hi*hi, hi*lo, lo*hi): the forward layers and dX run "
-                             "them as kind::f16 MMAs on scaled fp16 operand pairs (ceiling = peak/3), dW as kind::tf32 MMAs "
+                             "them as fp16 wgmmas on scaled fp16 operand pairs (ceiling = peak/3), dW as tf32 wgmmas "
                              "(ceiling = peak/6); the simt engine runs on CUDA cores (no tensor pipe)")
     roof2 = []
     for name in ("heads_backward", "normalize_obs", "gae_returns"):
@@ -533,9 +573,9 @@ def run_ours(args):
                         tensor=dict(achieved=samp_tf, unit="TFLOP/s", peak=peaks["tflops_burst"], frac=samp_tf / peaks["tflops_burst"],
                                     algorithmic_flops=samp_flops,
                                     note="policy forward only (0.599 MFLOP per env step, SURVEY 8d) over the whole rollout time; "
-                                         "3-pass fp16-split ceiling = peak / 3; 128 of 148 SMs hold a CTA"),
+                                         "3-pass fp16-split ceiling = peak / 3; 128 CTAs on the 132 SMs"),
                         note="a 4096-env policy step moves 2.35 MB and 2.45 GFLOP: the rollout is bound by the per-step dependency "
-                             "chain (tensor-pipe time of the two layers + epilogues + cluster barriers, profiles/r02_r_rollout_trace.md), "
+                             "chain (tensor-pipe time of the two layers + epilogues + cluster barriers), "
                              "not by HBM bandwidth")
     dp_info = None
     if world > 1 and not args.no_dp_check:
@@ -641,7 +681,7 @@ def run_ours(args):
         if r is not None:
             cpu_baseline = dict(value=r["value"], unit=UNIT, cores=r["cores"], kind="reference", ms_per_step=r["ms_per_step"],
                                 sample="6 full iterations (4096 envs x 32 steps + learner) after 2 warm-up; the unmodified reference "
-                                       "(sample-factory 2.1.3 in baseline/_ref: BatchedVectorEnvRunner + ActorCritic + Learner.train, "
+                                       "(sample-factory 2.1.3 in oracle/_ref: BatchedVectorEnvRunner + ActorCritic + Learner.train, "
                                        f"serial mode, torch CPU), {r['cores']} of {os.cpu_count()} host threads")
         rp = oracle_cpu_run(steps=6, warmup=2)
         port = dict(value=rp["value"], unit=UNIT, cores=rp["cores"], kind="port", ms_per_step=rp["ms_per_step"],
@@ -655,7 +695,7 @@ def run_ours(args):
     if rank == 0:
         out = dict(metric=METRIC, value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=args.warmup,
                    ms_per_step=ms_per_step, higher_is_better=True, scaling="weak", vs_baseline=None,
-                   dtype="f32" + (" (3-pass operand split on tcgen05 -- scaled fp16 hi/lo pairs where the operand ranges are known, tf32 hi/lo pairs elsewhere -- fp32 accumulate in TMEM)" if engine_name == "tcgen05-3xTF32" else ""),
+                   dtype="f32" + (" (3-pass tf32 hi/lo operand split on wgmma, fp32 accumulate)" if engine_name == "wgmma-3xTF32" else ""),
                    data="synthetic",
                    config=dict(workload=WORKLOAD, envs_per_gpu=N_ENVS, rollout=ROLLOUT, global_batch=BATCH * N_MINIBATCH * world,
                                parallelism=f"dp{world} (env shards; per SGD step ONE kernel = NVLink peer all-reduce + grad-norm + clip + Adam)", gemm_engine=engine_name,
@@ -695,7 +735,7 @@ def main():
     ap.add_argument("--no-graph", dest="no_graph", action="store_true")
     ap.add_argument("--no-learner-graph", dest="no_learner_graph", action="store_true",
                     help="launch the learner's kernels one by one instead of replaying Learner.train() as one CUDA graph "
-                         "(--learner_cuda_graph=True; measured 40.4M vs 38.0M env-steps/s, profiles/r01_m_*).  With the graph "
+                         "(--learner_cuda_graph=True).  With the graph "
                          "the per-kernel roofline timings come from three extra eager iterations after the timed region")
     ap.add_argument("--no-e2e", dest="no_e2e", action="store_true")
     ap.add_argument("--no-async", dest="no_async", action="store_true")
@@ -704,6 +744,9 @@ def main():
                     help="N > 1: skip the (untimed) replica / single-GPU equivalence check printed as `dp_check`")
     ap.add_argument("--no-strong", dest="no_strong", action="store_true",
                     help="N > 1: skip the strong-scaling point (4096 envs in total, split over the ranks)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32/64, "
+                         "at most 64 MB; same arguments -> same inputs, so two builds can be compared output for output)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.config != 2:

@@ -4,11 +4,11 @@ headline (config 2) line.  Synthetic tape envs of the named shapes, random-init 
   3  mujoco Ant-like   Box(27) obs -> Box(8) actions, tanh MLP 64-64, learned stddev, fixed-KL, value bootstrap, 2 epochs x 4
                        minibatches (sf_examples/mujoco/mujoco_params.py:1-38), 2048 envs per GPU, rollout 64, async_rl=True
   4  atari-like        uint8 [4,84,84] frames, convnet_atari + FC 512, ReLU, obs_scale 255, 4 epochs x 4 minibatches
-                       (sf_examples/atari/atari_params.py:1-45), 1024 envs in total (BASELINE: "1024 envs, 2 x B200"), rollout 32
+                       (sf_examples/atari/atari_params.py:1-45), 1024 envs in total (1024 envs), rollout 32
                        (the reference's 128 would make one minibatch 32 768 frames; 8 192 keeps the im2col buffers at 3.4 GB)
   5  isaacgym-like     Box(256) obs, MLP 512-256-128 -> LSTM-512, rollout = recurrence = 16, batch 32768, value bootstrap,
                        KL-adaptive lr (sf_examples/isaacgym_examples/train_isaacgym.py:169-208, 310-350), 4096 envs per GPU
-                       (BASELINE: "32768 envs sharded 8 x B200")
+                       (32768 envs sharded over 8 GPUs in BASELINE.json)
 
 `value`: env-steps/s with the env resident in HBM.  `e2e`: the same Runner with a HOST env (numpy tape, pinned staging): the
 observation batch H2D and the actions D2H every env step.  `roofline`: the contraction op with the largest accumulated
@@ -278,7 +278,7 @@ def run_config(args, load_peaks, ClockSampler):
         d = timed[key]
         avg_ms = tot[key] / len(d["ev"])
         ach = d["work"] / (avg_ms * 1e-3) / 1e12
-        roofline = dict(kernel=key + " (tcgen05 3xTF32 engine: ceiling = peak / 6)", bound="tensor", achieved=ach,
+        roofline = dict(kernel=key + " (wgmma 3xTF32 engine: ceiling = peak / 6)", bound="tensor", achieved=ach,
                         peak=peaks["tflops_burst"], unit="TFLOP/s", frac=ach / peaks["tflops_burst"], traffic=None,
                         avg_kernel_ms=avg_ms, launches_timed=len(d["ev"]), share_of_gemm_time=tot[key] / sum(tot.values()),
                         peak_source=peaks["source"] + ", bf16 burst")
@@ -317,7 +317,7 @@ def run_config(args, load_peaks, ClockSampler):
     if rank == 0:
         out = dict(metric=METRIC + f" -- {c['name']}", value=value, unit=UNIT, n_gpus=world, steps=args.steps, warmup=args.warmup,
                    ms_per_step=ms_total / args.steps, higher_is_better=True, scaling="strong" if c["envs_total"] else "weak",
-                   vs_baseline=None, dtype="f32 (3-pass operand split on tcgen05 -- scaled fp16 hi/lo pairs where the operand ranges are known, tf32 hi/lo pairs elsewhere -- fp32 accumulate in TMEM)", data="synthetic",
+                   vs_baseline=None, dtype="f32 (3-pass operand split on wgmma -- scaled fp16 hi/lo pairs where the operand ranges are known, tf32 hi/lo pairs elsewhere -- fp32 accumulate)", data="synthetic",
                    config=dict(workload=c["name"], envs_per_gpu=n_envs, rollout=T, global_batch=world * n_envs * T,
                                parallelism=f"dp{world}", async_rl=c["async_rl"], cuda_graph_learner=learner_graph,
                                l2_policy="trajectory set + learner activations exceed the 126 MB L2; no explicit flush"),

@@ -1,5 +1,5 @@
 /*
- * sfb200.h -- C ABI of libsfb200.so: the B200 (sm_100a) implementation of Sample Factory's APPO hot path
+ * sfb200.h -- C ABI of libsfb200.so: the H100 (sm_90a) implementation of Sample Factory's APPO hot path
  *             (rollout sampler -> PPO / V-trace learner).
  *
  * The reference (alex-petrenko/sample-factory) has no FFI for this path: it is Python calling PyTorch ATen.  Each
@@ -37,8 +37,8 @@ extern "C" {
 
 /* GEMM engine selection for sfb200_linear_* */
 #define SFB200_GEMM_SIMT_FP32 0   /* CUDA-core fp32 FFMA tiles */
-#define SFB200_GEMM_TC_3XTF32 1   /* tcgen05 kind::tf32, error-compensated 3-pass split, fp32 accumulate in TMEM */
-#define SFB200_GEMM_TC_TF32 2     /* tcgen05 kind::tf32 single pass (fast, NOT parity grade) */
+#define SFB200_GEMM_TC_3XTF32 1   /* wgmma tf32, error-compensated 3-pass split, fp32 accumulate */
+#define SFB200_GEMM_TC_TF32 2     /* wgmma tf32 single pass (fast, NOT parity grade) */
 
 /* ---------------------------------------------------------------- library ---- */
 int sfb200_abi_version(void);
@@ -47,18 +47,19 @@ const char* sfb200_last_error(void);
 int sfb200_set_device(int device);
 /* number of SMs of the bound device (grid sizing) */
 int sfb200_sm_count(void);
-/* 1 if the tcgen05/TMA GEMM engine is usable in this process (driver entry points resolved), else 0 */
+/* 1 if the wgmma/TMA GEMM engine is usable in this process (sm_90 device, driver entry points resolved), else 0 */
 int sfb200_tc_available(void);
-/* Pre-split weights for the 3xTF32 engine.  register: from now on every tcgen05-3xTF32 GEMM whose WEIGHT operand lies
- * inside [base, base+n) reads the operand's low tf32 half from `lo` (same offsets) instead of deriving it in shared
- * memory for every output tile, and sfb200_clip_adam_step on a registered buffer keeps `lo` current.  Any other write
+/* Low tf32 halves of the weights for the 3xTF32 engine.  register: marks [base, base+n) as model weights with a twin
+ * `lo` (same offsets) of their low tf32 halves, which sfb200_clip_adam_step keeps current; the fused policy step and the
+ * persistent rollout cover a model only when both its weight matrices are registered (the kernels split the fp32 weights
+ * themselves).  Any other write
  * to the weights (checkpoint load, weight copy) must be followed by sfb200_refresh_tf32_lo(base).  With the
  * environment variable SFB200_CHECK_LO=1 every use verifies the pair on the device and traps on a stale `lo`. */
 int sfb200_register_tf32_lo(const float* base, float* lo, int64_t n);
 int sfb200_unregister_tf32_lo(const float* base);
 int sfb200_refresh_tf32_lo(const float* base, void* stream);
 /* The fp16-split form of the same 3-pass engine (fp32 accuracy class of 3xTF32 -- 22 significand bits per operand --
- * on the kind::f16 tensor-core path: twice the MMA rate, 2/3 of the operand bytes).  A 3xTF32 GEMM takes it when
+ * on the fp16 wgmma path: twice the k per instruction).  A 3xTF32 GEMM takes it when
  *   (1) its WEIGHT operand lies inside a buffer with registered fp16 twins: twins = [hi16[n] | lo16[n]],
  *       hi = fp16(w * 2^8), lo = fp16((w * 2^8 - hi) * 2^11) (|w| < 255); for dX = dz . W, where the weight matrix is read
  *       transposed, a per-matrix transposed copy [hiT[K][N] | loT[K][N]] registered with ..._f16_transposed; and
@@ -197,7 +198,7 @@ int sfb200_heads_from_partials_continuous(const float* head_partials, int P, int
                                           int64_t pv_stride, void* stream);
 
 /* The last hidden layer and the heads in ONE pass (same reference sites as sfb200_linear_act_forward +
- * sfb200_heads_forward): the tcgen05 epilogue forms y = act(x W^T + b) in registers and contracts it at once with
+ * sfb200_heads_forward): the wgmma epilogue forms y = act(x W^T + b) in registers and contracts it at once with
  * [Wv ; Wa], so y is not re-read by a heads kernel -- and not written at all when y == NULL (the sampler never needs
  * it).  Two calls:
  *   P = sfb200_linear_heads_partials(N, A, engine)          0 -> shape/engine not covered: use the two separate calls
@@ -259,8 +260,8 @@ int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, con
                              const double* mean, const double* var, float sub_mean, float inv_scale, float eps, float clip,
                              void* stream);
 /* The whole policy forward of a two-layer MLP (model/encoder.py:72-91 MlpEncoder + actor_critic.py:171-186) up to the head
- * partials in ONE tcgen05 kernel: h1 = act(x W1^T + b1) is produced chunk by chunk in tensor memory and consumed by the
- * layer-2 MMAs without ever reaching shared or global memory; h2 = act(h1 W2^T + b2) is contracted with [Wv ; Wa] in the
+ * partials in ONE wgmma kernel: h1 = act(x W1^T + b1) is produced chunk by chunk in shared memory and consumed by the
+ * layer-2 MMAs without ever reaching global memory; h2 = act(h1 W2^T + b2) is contracted with [Wv ; Wa] in the
  * epilogue (not stored).  Same partial format as sfb200_linear_act_heads_forward -> finish with sfb200_heads_from_partials.
  *   P = sfb200_policy_mlp2_partials(W1, W2, K1, H1, H2, A, engine)   0 -> not covered (needs the 3xTF32 engine, K1 in
  *       {32, 64}, H1 % 32 == 0, H2 % 128 == 0 and <= 512, A <= 8, both weight matrices inside a registered tf32-lo buffer) */

@@ -3,14 +3,14 @@
 A plain PyTorch-fp32 (CPU) restatement of the reference's APPO hot path
 (rollout sampler -> PPO/V-trace learner), written from the reference's
 behaviour and citing the reference file:line each function follows
-(paths relative to /root/reference/sample_factory/).
+(paths relative to the reference's sample_factory/ package).
 
 Who may import this: tests/, __graft_entry__.smoke() and bench.py's
 cpu_baseline / --impl reference leg -- only as the checker / the timed CPU
 baseline.  The product (sample_factory_b200/) must never import it.
 
 Parity pinning: this oracle is PINNED against outputs of the reference itself,
-executed in the build container from /root/reference under oracle/ref_shims.py
+executed in the build container from a reference checkout (oracle/install_ref.py: reference_dir()) under oracle/ref_shims.py
 by tests/golden/make_golden.py; the resulting vectors are committed under
 tests/golden/*.npz and checked by tests/test_oracle_golden.py (no GPU needed).
 The reference's only known-answer vector for this path (logits [0,1,2] ->

@@ -1,19 +1,20 @@
 """TEST INFRASTRUCTURE ONLY -- never imported by the product (sample_factory_b200/).
 
 In-memory stand-ins for the third-party packages the reference imports at module
-load but which are absent from this offline container (signal_slot, faster_fifo,
+load but which an offline install does not have (signal_slot, faster_fifo,
 colorlog, tensorboardX, gymnasium).  They let `tests/golden/make_golden.py`
-import and EXECUTE the unmodified reference classes from /root/reference
+import and EXECUTE the unmodified reference classes from a reference checkout (oracle/install_ref.py: reference_dir())
 (Learner, ActorCritic, BatchedVectorEnvRunner, gae_advantages, ...) so that the
 golden vectors under tests/golden/ are produced by the reference's own code.
 
-Only used in the build container; /root/reference does not exist on the GPU box,
-so nothing here runs there.  None of this is reference code: it is the minimum
+Only used to generate the goldens; no test needs the reference checkout itself, only the
+stored vectors.  None of this is reference code: it is the minimum
 surface (names + trivial behaviour) those imports need.
 """
 from __future__ import annotations
 
 import logging
+import os
 import queue
 import sys
 import types
@@ -27,7 +28,7 @@ def _mod(name: str) -> types.ModuleType:
     return m
 
 
-def install(reference_root: str = "/root/reference") -> None:
+def install(reference_root: str | None = None) -> None:
     if "signal_slot" in sys.modules and getattr(sys.modules["signal_slot"], "_sfb200_shim", False):
         return
 
@@ -301,5 +302,12 @@ def install(reference_root: str = "/root/reference") -> None:
     core.ObservationWrapper, core.RewardWrapper, core.ActionWrapper = ObservationWrapper, RewardWrapper, ActionWrapper
     wrappers.RecordEpisodeStatistics = Wrapper
 
+    if reference_root is None:
+        from oracle.install_ref import reference_dir
+
+        reference_root = reference_dir()
+    if not reference_root or not os.path.isfile(os.path.join(reference_root, "sample_factory", "__init__.py")):
+        raise RuntimeError("no reference checkout: set SF_REFERENCE_DIR to a sample-factory source tree "
+                           "(never this repository's own sample_factory/ re-export package)")
     if reference_root not in sys.path:
         sys.path.insert(0, reference_root)

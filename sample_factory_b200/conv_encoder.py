@@ -1,6 +1,6 @@
 """Conv head of the reference's ConvEncoder (model/encoder.py:88-145) on the device.
 
-Every Conv2d (no padding) runs as  im2col -> GEMM engine  with bias + activation in the GEMM epilogue, so the tcgen05
+Every Conv2d (no padding) runs as  im2col -> GEMM engine  with bias + activation in the GEMM epilogue, so the wgmma
 3xTF32 path and its backward GEMMs are shared with the MLP layers (csrc/conv.cu explains the layouts).  Activations are
 kept NHWC ([B*OH*OW, C] rows = GEMM output); the last layer is permuted to the (C, H, W) flatten order the reference's
 fully connected layers expect (encoder.py:115), so the weights keep the reference layout and checkpoints round-trip.

@@ -1,5 +1,5 @@
 // Convolutional encoder support (reference: model/encoder.py:88-145, ConvEncoderImpl = Conv2d stacks without padding).
-// A Conv2d is run as  im2col -> GEMM engine (tcgen05 / SIMT, bias + activation in the GEMM epilogue)  so the tensor-core
+// A Conv2d is run as  im2col -> GEMM engine (wgmma / SIMT, bias + activation in the GEMM epilogue)  so the tensor-core
 // path, its fp32-parity split and the backward GEMMs are shared with the MLP layers:
 //   forward :  col[m, k] = x[b, ci, oh*s+kh, ow*s+kw]        m = (b, oh, ow), k = (ci, kh, kw)  == Conv2d weight flatten
 //              y[m, co]  = act(col[m, :] . W[co, :] + b[co])  -> activations are kept NHWC ([B*OH*OW, C] row-major)

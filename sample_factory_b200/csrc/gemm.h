@@ -5,9 +5,9 @@
 
 namespace sfb {
 
-constexpr int SFB_TC_UNSUPPORTED = -1000;   // shape/alignment not handled by the tcgen05 engine -> caller uses SIMT
+constexpr int SFB_TC_UNSUPPORTED = -1000;   // shape/alignment not handled by the wgmma engine -> caller uses SIMT
 
-// tcgen05 engine (gemm_tc.cu). Return 0, an error code, or SFB_TC_UNSUPPORTED.
+// wgmma engine (gemm_tc.cu). Return 0, an error code, or SFB_TC_UNSUPPORTED.
 int tc_linear_act_forward(const float* x, int64_t ldx, const float* W, const float* b, float* y, int64_t ldy, int64_t M,
                           int N, int K, int act, int engine, cudaStream_t st);
 int tc_linear_heads_partials(int N, int A, int engine);

@@ -1,5 +1,5 @@
 // CUDA-core fp32 GEMM engine (SFB200_GEMM_SIMT_FP32): exact-fp32 FFMA tiles, the parity-grade baseline engine and
-// the fallback for shapes the tcgen05 engine does not take.  C[m,n] = sum_k A(m,k) * B(n,k) with either operand stored
+// the fallback for shapes the wgmma engine does not take.  C[m,n] = sum_k A(m,k) * B(n,k) with either operand stored
 // K-contiguous ([rows, K]) or row-contiguous ([K, rows]); 128x128x16 CTA tile, 256 threads, 8x8 register micro-tile,
 // double-buffered shared memory, optional split-K (deterministic two-pass reduce).
 #include "common.cuh"

@@ -9,7 +9,7 @@ namespace sfb {
 constexpr int kHeadsMaxGroups = 1024;
 
 
-// Heads from the partial dot products left by the fused GEMM epilogue (gemm_tc.cu, tc_epilogue_tile_heads):
+// Heads from the partial dot products left by the fused GEMM epilogue (wgmma_tile.cuh, heads_tile):
 // part[p][row][kPad], summed over p in fixed order (deterministic).  One warp per row, lane a = output a.
 __global__ void __launch_bounds__(256) heads_from_partials_kernel(const float* __restrict__ part, int P, int64_t rows,
                                                                   const HeadsFinish f) {
@@ -299,7 +299,7 @@ __global__ void __launch_bounds__(256, MINB) heads_backward_vec_kernel(
 }
 
 // Software-pipelined variant for the learner-sized case (two columns per thread).  Two things bound the kernel above
-// (ncu, profiles/r01_m_ncu_heads_backward.md): the compiler keeps ONE row load in flight per thread (load -> 36 FMAs ->
+// (profiled on the previous architecture): the compiler keeps ONE row load in flight per thread (load -> 36 FMAs ->
 // store, serially: ~2 TB/s), and once that is fixed, instruction issue (123 instructions per row and warp, 2/3 of them
 // address arithmetic, guards and scalar shared-memory loads).  Here the row loads run U rows ahead of the arithmetic
 // through a register queue with static slots, all pointers advance by increments, full batches run unguarded, the
@@ -308,7 +308,7 @@ __global__ void __launch_bounds__(256, MINB) heads_backward_vec_kernel(
 // multiple of U.
 constexpr int kHbGP = 20;   // floats per staged coefficient row: 9 duplicated pairs (g, g) + padding to 5 x 16 bytes
 
-// packed fp32 pairs (sm_100 FFMA2: two IEEE fma.rn per instruction -- same results as the scalar form, half the issue slots)
+// packed fp32 pairs: two IEEE fma.rn on the pair's lanes (sm_90 has no packed fp32 FMA; same results as the scalar form)
 __device__ __forceinline__ uint64_t pack2(float lo, float hi) {
     uint64_t r;
     asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -319,10 +319,10 @@ __device__ __forceinline__ float2 unpack2(uint64_t v) {
     asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
     return r;
 }
+// lane-wise fma.rn of two packed floats (two scalar FMAs: sm_90 has no packed fp32 FMA)
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
+    const float2 x = unpack2(a), y = unpack2(b), z = unpack2(c);
+    return pack2(fmaf(x.x, y.x, z.x), fmaf(x.y, y.y, z.y));
 }
 
 // one row of the pipelined kernel: hq = the thread's two h values, gp = the row's duplicated coefficient pairs in smem.
@@ -387,7 +387,7 @@ __global__ void __launch_bounds__(256, MINB) heads_backward_pipe_kernel(
     }
 
     // (staging one 32-row coefficient tile at a time keeps the resident blocks out of phase; staging a whole row group up
-    //  front, with or without L2 prefetches further ahead, measured slower: 54-60 vs 50 us, profiles/r01_m_ncu_heads_backward.md)
+    //  front, with or without L2 prefetches further ahead, measured slower on the previous architecture)
     int k = 0;
     for (int64_t b0 = r_begin; b0 < r_end; b0 += kHbTile) {
         const int nb = (int)((r_end - b0 < kHbTile) ? (r_end - b0) : kHbTile);

@@ -1,356 +1,203 @@
-// The sampler's policy step for MLP policies as ONE tcgen05 kernel (model/actor_critic.py:160-195, model/encoder.py:72-91):
+// The sampler's policy step for MLP policies as ONE wgmma kernel (model/actor_critic.py:160-195, model/encoder.py:72-91):
 //
 //     h1 = act(x W1^T + b1)          [M, H1]   x = normalised observations [M, K1], K1 = 32 or 64
 //     h2 = act(h1 W2^T + b2)         [M, H2]
-//     partial head dot products      h2 . [Wv ; Wa]^T over 64-column segments  (finished by heads_from_partials)
+//     partial head dot products      h2 . [Wv ; Wa]^T over 32-column segments  (finished by heads_from_partials)
 //
-// The stand-alone engine ran this as two GEMM launches with h1 round-tripping through HBM/L2 and a one-wave grid each
-// (profiles/r01_m_launches.md: 15.6 + 22.7 us cold for 2.45 GFLOP).  Here a CTA owns a 128-row x 128-column tile of h2 and
-// walks the K dimension of layer 2 in chunks of 32: for every chunk it first computes the matching 32 columns of h1 ITSELF
-// (layer 1 is short-K, so recomputing it in each of the H2/128 column CTAs costs less than exchanging it: DSMEM moves
-// ~21 B/clk, a 128x512 fp32 tile would take ~5 us), the epilogue warps turn the fp32 accumulator into the next A operand
-// -- bias + activation + tf32 hi/lo split, TMEM -> registers -> TMEM -- and the layer-2 MMAs consume it straight from
-// tensor memory.  h1 never exists in shared or global memory.  All flops are 3xTF32 (two accumulators, see gemm_tc.cu).
+// A CTA owns a 128-row x 128-column tile of h2 and walks the K dimension of layer 2 in chunks of 32: for every chunk it
+// first computes the matching 32 columns of h1 ITSELF (layer 1 is short-K, so recomputing it in each of the H2/128 column
+// CTAs costs less than exchanging it), turns that accumulator into the next A operand in shared memory (bias +
+// activation + tf32 hi/lo split into the swizzled K-major layout) and the layer-2 wgmmas consume it from there.  h1 never
+// exists in global memory.  All flops are 3xTF32 (two accumulators, see gemm_tc.cu).
 //
-//   warp 0      TMA producer: x tile once, then per chunk W1[c*32.., :] and W2[n0.., c*32..] (raw weights + tf32-lo twins)
-//   warp 1      TMEM allocator + single-thread MMA issuer (layer-1 chunk c is issued before layer-2 chunk c-1: the
-//               tensor pipe works on chunk c while the epilogue warps convert chunk c-1)
-//   warps 2-9   h1 chunks 0, 2, 4, ...  (TMEM lane quadrant = warp % 4; warps 2-5 convert columns 0-15 of the chunk,
-//               warps 6-9 columns 16-31)
-//   warps 10-17 h1 chunks 1, 3, 5, ...
-//   warps 2-17  final epilogue: h2 = act(acc + b2), head partials (four 32-column groups per 128-column tile)
-// The chunk conversion is the critical path (accumulator -> bias/activation/split -> A operand: ~4.8 k cycles with four
-// warps per chunk against 2.3 k cycles of MMA work per chunk, ncu r02_d); two sets of eight warps keep it off it.
-//
-// TMEM (512 columns): [0,256) layer-2 accumulator (main | cross), [256,384) two layer-1 accumulators (32 main | 32 cross),
-// [384,512) two A-operand stages (32 hi | 32 lo).
+// 256 threads = two warpgroups of 64 rows each (wgmma M = 64); thread 0 issues the TMA loads: the x tile once, then per
+// chunk W1[c*32.., :] and W2[n0.., c*32..] into a double-buffered raw stage (chunk c+1 is in flight while c is computed).
+// Registers: layer-2 accumulators 2 x 64, layer-1 accumulators 2 x 16 per thread.
 #include <cuda.h>
 
 #include "common.cuh"
 #include "gemm.h"
 #include "heads_tail.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma_tile.cuh"
 
 namespace sfb {
 
-constexpr int PS_THREADS = 576;           // TMA warp, MMA warp, 16 epilogue warps
-constexpr int PS_STAGES = 3;
-constexpr int PS_HEAD_AP = 9;            // value + up to 8 action outputs (same partial format as the fused GEMM epilogue)
-constexpr int PS_W2_BYTES = 2 * 128 * 128;   // [hi 128 rows x 128 B | lo]
-constexpr uint32_t PS_D1_COL = 256, PS_A2_COL = 384;
+constexpr int PS_THREADS = 256;
 constexpr int PS_MAX_H1 = 1024;
 
-template <int KA>
 struct PsSmem {
-    static constexpr int X_BYTES = KA * 16384;            // one half (hi or lo): KA atoms of [128 rows][128 B]
-    static constexpr int W1_BYTES = KA * 8192;            // per atom [hi 32 rows x 128 B | lo 32 rows x 128 B]
-    static constexpr int STAGE_BYTES = W1_BYTES + PS_W2_BYTES;
-    static constexpr int OFF_STAGES = 2 * X_BYTES;
-    static constexpr int OFF_BARS = OFF_STAGES + PS_STAGES * STAGE_BYTES;
-    static constexpr int OFF_B1 = OFF_BARS + 256;
-    static constexpr int OFF_B2 = OFF_B1 + PS_MAX_H1 * 4;
-    static constexpr int OFF_HEADW = OFF_B2 + 128 * 4;
-    static constexpr int TOTAL = OFF_HEADW + PS_HEAD_AP * 128 * 4 + 1024 /*align slack*/;
+    static constexpr int XC = 0;                        // x hi/lo: per 32-k block [hi 16 KB | lo 16 KB], two blocks
+    static constexpr int W1C = XC + 2 * 32768;          // W1 chunk hi/lo: per k block [hi 4 KB | lo 4 KB], two blocks
+    static constexpr int H1C = W1C + 2 * 8192;          // h1 chunk [128 rows][32] hi | lo
+    static constexpr int W2C = H1C + 32768;             // W2 tile [128 n][32 k] hi | lo
+    static constexpr int XRAW = H1C;                    // x raw (two [128][32] boxes) before the chunk loop uses H1C / W2C
+    static constexpr int RAW = W2C + 32768;             // 2 stages x [W1 raw 2 x 4 KB | W2 raw 16 KB]
+    static constexpr int RAW_STAGE = 2 * 4096 + 16384;
+    static constexpr int BARS = RAW + 2 * RAW_STAGE;
+    static constexpr int TOTAL = 1024 + BARS + 64;
 };
-
-// bounded spin: a protocol bug traps instead of hanging the GPU
-__device__ __forceinline__ void ps_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0;
-    uint64_t t0 = 0;
-    for (uint32_t spins = 0; !done; ++spins) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if ((spins & 1023u) == 1023u) {       // ~2 s of wall clock without progress: protocol bug, not load
-            uint64_t now;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(now));
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 2000000000ull) __trap();
-        }
-    }
-}
 
 struct PsArgs {
     int64_t M;
-    int H1, H2, act;
+    int K1, H1, H2, act;
     const float* b1;
     const float* b2;
-    const float* head_wv;
-    const float* head_wa;
-    int head_A;
-    float* head_part;   // [H2/32][M][kHeadPartPad]
+    TcEpilogue epi;     // head weights / head_part; bias = b2
 };
 
-template <int KA, int ACT>
-__global__ void __launch_bounds__(PS_THREADS, 1)
-policy_mlp2_heads_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w1,
-                         const __grid_constant__ CUtensorMap tmap_w1lo, const __grid_constant__ CUtensorMap tmap_w2,
-                         const __grid_constant__ CUtensorMap tmap_w2lo, const PsArgs a) {
-    using S = PsSmem<KA>;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_align_1024(smem_raw);
-    uint8_t* x_hi = smem;
-    uint8_t* x_lo = smem + S::X_BYTES;
-    uint8_t* stages = smem + S::OFF_STAGES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);
-    uint64_t* x_full = bars + 0;        // TMA: x tile landed
-    uint64_t* x_ready = bars + 1;       // x_lo written (256 epilogue threads)
-    uint64_t* w_full = bars + 2;        // [3] TMA: weight chunk landed
-    uint64_t* w_empty = bars + 5;       // [3] MMAs reading the stage retired (tcgen05.commit)
-    uint64_t* d1_full = bars + 8;       // [2] layer-1 accumulator complete (commit)
-    uint64_t* d1_empty = bars + 10;     // [2] drained by its 128 epilogue threads
-    uint64_t* a2_full = bars + 12;      // [2] A stage written (128 threads)
-    uint64_t* a2_empty = bars + 14;     // [2] layer-2 MMAs reading the A stage retired (commit)
-    uint64_t* d2_full = bars + 16;      // layer-2 accumulator complete
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
-    float* b1_s = reinterpret_cast<float*>(smem + S::OFF_B1);
-    float* b2_s = reinterpret_cast<float*>(smem + S::OFF_B2);
-    float* headw_s = reinterpret_cast<float*>(smem + S::OFF_HEADW);   // [PS_HEAD_AP][128]
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n0 = blockIdx.x * 128;                 // this CTA's h2 columns
-    const int64_t m0 = (int64_t)blockIdx.y * 128;    // this CTA's rows
-    const int NC = a.H1 / 32;                        // K chunks of layer 2 == 32-column chunks of h1
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w1) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w1lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w2) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w2lo) : "memory");
-        mbar_init(x_full, 1);
-        mbar_init(x_ready, 512);
-        for (int s = 0; s < PS_STAGES; ++s) {
-            mbar_init(&w_full[s], 1);
-            mbar_init(&w_empty[s], 1);
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&d1_full[b], 1);
-            mbar_init(&d1_empty[b], 256);
-            mbar_init(&a2_full[b], 256);
-            mbar_init(&a2_empty[b], 1);
-        }
-        mbar_init(d2_full, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();      // (everything above is CTA-local; global memory is only touched after the wait)
-    pdl_trigger();
-
-    if (warp == 0) {
-        // ===================================================== TMA producer
-        if (lane == 0) {
-            mbar_expect_tx(x_full, S::X_BYTES);
-            for (int k = 0; k < KA; ++k) tma_load_2d(x_hi + k * 16384, &tmap_x, x_full, k * 32, (int)m0);
-            for (int c = 0; c < NC; ++c) {
-                const int s = c % PS_STAGES;
-                ps_wait(&w_empty[s], ((c / PS_STAGES) & 1) ^ 1);
-                uint8_t* st = stages + s * S::STAGE_BYTES;
-                mbar_expect_tx(&w_full[s], S::STAGE_BYTES);
-                for (int k = 0; k < KA; ++k) {
-                    tma_load_2d(st + k * 8192, &tmap_w1, &w_full[s], k * 32, c * 32);
-                    tma_load_2d(st + k * 8192 + 4096, &tmap_w1lo, &w_full[s], k * 32, c * 32);
-                }
-                tma_load_2d(st + S::W1_BYTES, &tmap_w2, &w_full[s], c * 32, n0);
-                tma_load_2d(st + S::W1_BYTES + 16384, &tmap_w2lo, &w_full[s], c * 32, n0);
-            }
-        }
-    } else if (warp == 1) {
-        // ===================================================== MMA issuer
-        constexpr uint32_t idesc_l1_wide = make_idesc(false, false, 128, 64);     // [main | cross] (+)= x_hi x [W1hi ; W1lo]
-        constexpr uint32_t idesc_l1_cross = make_idesc(false, false, 128, 32);    // cross (+)= x_lo x W1hi
-        constexpr uint32_t idesc_l2_wide = make_idesc(false, false, 128, 256);
-        constexpr uint32_t idesc_l2_cross = make_idesc(false, false, 128, 128);
-        ps_wait(x_full, 0);
-        ps_wait(x_ready, 0);
-        tc_fence_after();
-        for (int c = 0; c <= NC; ++c) {
-            if (c < NC) {
-                const int s = c % PS_STAGES, b = c & 1;
-                ps_wait(&w_full[s], (c / PS_STAGES) & 1);
-                ps_wait(&d1_empty[b], ((c >> 1) & 1) ^ 1);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t st = smem_u32(stages + s * S::STAGE_BYTES);
-                    const uint32_t d1 = tmem_base + PS_D1_COL + 64u * b;
-#pragma unroll
-                    for (int k = 0; k < KA; ++k) {
-                        const uint64_t da_hi = make_smem_desc(smem_u32(x_hi) + k * 16384, false);
-                        const uint64_t da_lo = make_smem_desc(smem_u32(x_lo) + k * 16384, false);
-                        const uint64_t db = make_smem_desc(st + k * 8192, false);
-#pragma unroll
-                        for (int j = 0; j < TBK / UMMA_K; ++j) {
-                            const uint64_t o = (uint64_t)(j * (UMMA_K * 4 >> 4));
-                            umma_tf32(d1, da_hi + o, db + o, idesc_l1_wide, (k | j) != 0);
-                            umma_tf32(d1 + 32, da_lo + o, db + o, idesc_l1_cross, 1);
-                        }
-                    }
-                    umma_commit(&d1_full[b]);
-                }
-                __syncwarp();
-            }
-            if (c >= 1) {
-                const int cp = c - 1, sp = cp % PS_STAGES, bp = cp & 1;
-                ps_wait(&a2_full[bp], (cp >> 1) & 1);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint64_t db = make_smem_desc(smem_u32(stages + sp * S::STAGE_BYTES + S::W1_BYTES), false);
-                    const uint32_t a2 = tmem_base + PS_A2_COL + 64u * bp;
-#pragma unroll
-                    for (int j = 0; j < TBK / UMMA_K; ++j) {
-                        const uint64_t o = (uint64_t)(j * (UMMA_K * 4 >> 4));
-                        umma_tf32_ts(tmem_base, a2 + j * UMMA_K, db + o, idesc_l2_wide, (cp | j) != 0);
-                        umma_tf32_ts(tmem_base + 128, a2 + 32 + j * UMMA_K, db + o, idesc_l2_cross, 1);
-                    }
-                    umma_commit(&w_empty[sp]);
-                    umma_commit(&a2_empty[bp]);
-                    if (cp == NC - 1) umma_commit(d2_full);
-                }
-                __syncwarp();
-            }
-        }
-    } else {
-        // ===================================================== epilogue warps (2..17)
-        const int et = threadIdx.x - 64;                 // 0..511
-        const int set = (warp - 2) >> 3;                 // 0: even h1 chunks, 1: odd chunks
-        const int half = ((warp - 2) >> 2) & 1;          // which 16 of the chunk's 32 columns this warp converts
-        const int quad = warp & 3;                       // TMEM lane quadrant this warp may access
-        const uint32_t lane_sel = (uint32_t)(quad * 32) << 16;
-        // biases + head weights of this CTA's column slice -> shared memory
-        for (int i = et; i < a.H1; i += 512) b1_s[i] = a.b1[i];
-        if (et < 128) b2_s[et] = a.b2[n0 + et];
-        for (int i = et; i < PS_HEAD_AP * 128; i += 512) {
-            const int r = i >> 7, n = i & 127;
-            headw_s[i] = (r == 0) ? a.head_wv[n0 + n] : (r <= a.head_A ? a.head_wa[(int64_t)(r - 1) * a.H2 + n0 + n] : 0.f);
-        }
-        // x_lo = tf32 low half of x (x itself serves as the hi operand: the tensor core truncates the 13 low bits)
-        ps_wait(x_full, 0);
-        {
-            const uint4* h4 = reinterpret_cast<const uint4*>(x_hi);
-            uint4* l4 = reinterpret_cast<uint4*>(x_lo);
-#pragma unroll 4
-            for (int i = et; i < S::X_BYTES / 16; i += 512) {
-                const uint4 v = h4[i];
-                uint4 l;
-                l.x = tf32_lo_bits(v.x); l.y = tf32_lo_bits(v.y); l.z = tf32_lo_bits(v.z); l.w = tf32_lo_bits(v.w);
-                l4[i] = l;
-            }
-        }
-        fence_proxy_async_smem();
-        mbar_arrive(x_ready);
-        asm volatile("bar.sync 1, 512;" ::: "memory");   // b1_s / b2_s / headw_s visible to all epilogue threads
-
-        // ---- layer-1 chunks of this set: accumulator -> act(. + b1) -> (hi, lo) -> A stage
-        for (int c = set; c < NC; c += 2) {
-            const uint32_t u = (uint32_t)(c >> 1);
-            ps_wait(&d1_full[set], u & 1);
-            tc_fence_after();
-            const uint32_t d1 = tmem_base + lane_sel + PS_D1_COL + 64u * set + 16u * half;
-            uint32_t mainv[16], crossv[16];
-            tmem_ld_32x32b_x16(d1, mainv);
-            tmem_ld_32x32b_x16(d1 + 32, crossv);
-            tmem_ld_wait();
-            tc_fence_before();
-            mbar_arrive(&d1_empty[set]);
-            const float* bias = b1_s + c * 32 + 16 * half;
-            uint32_t lo[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                const float z = (__uint_as_float(mainv[j]) + __uint_as_float(crossv[j])) + bias[j];
-                const uint32_t hbits = __float_as_uint(act_fwd_ct<ACT>(z));
-                mainv[j] = hbits;                      // raw fp32 word = hi operand
-                lo[j] = tf32_lo_bits(hbits);
-            }
-            ps_wait(&a2_empty[set], (u & 1) ^ 1);
-            tc_fence_after();
-            const uint32_t a2 = tmem_base + lane_sel + PS_A2_COL + 64u * set + 16u * half;
-            tmem_st_32x32b_x16(a2, mainv);
-            tmem_st_32x32b_x16(a2 + 32, lo);
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&a2_full[set]);
-        }
-
-        // ---- final epilogue: h2 = act(acc + b2) for 32 columns of this thread's row, contracted with the head rows
-        ps_wait(d2_full, 0);
-        tc_fence_after();
-        const int grp = (warp - 2) >> 2;                 // 0..3: columns [32*grp, 32*grp + 32) of the tile
-        const int col0 = grp * 32;
-        float o[32];
-#pragma unroll
-        for (int c0 = 0; c0 < 32; c0 += 16) {
-            uint32_t r[16], r2[16];
-            tmem_ld_32x32b_x16(tmem_base + lane_sel + (uint32_t)(col0 + c0), r);
-            tmem_ld_32x32b_x16(tmem_base + lane_sel + (uint32_t)(128 + col0 + c0), r2);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-                o[c0 + j] = act_fwd_ct<ACT>((__uint_as_float(r[j]) + __uint_as_float(r2[j])) + b2_s[col0 + c0 + j]);
-        }
-        const int64_t m = m0 + quad * 32 + lane;
-        if (m < a.M) {
-            float hp[PS_HEAD_AP];
-#pragma unroll
-            for (int r = 0; r < PS_HEAD_AP; ++r) {
-                const float* w = headw_s + r * 128 + col0;   // warp-uniform address: shared-memory broadcast
-                float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const float4 wv = *reinterpret_cast<const float4*>(w + j);
-                    s0 = fmaf(o[j], wv.x, s0);
-                    s1 = fmaf(o[j + 1], wv.y, s1);
-                    s0 = fmaf(o[j + 2], wv.z, s0);
-                    s1 = fmaf(o[j + 3], wv.w, s1);
-                }
-                hp[r] = s0 + s1;
-            }
-            const int p = blockIdx.x * 4 + grp;
-            float4* dst = reinterpret_cast<float4*>(a.head_part + ((int64_t)p * a.M + m) * kHeadPartPad);
-            dst[0] = make_float4(hp[0], hp[1], hp[2], hp[3]);
-            dst[1] = make_float4(hp[4], hp[5], hp[6], hp[7]);
-            dst[2] = make_float4(hp[8], 0.f, 0.f, 0.f);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
+template <int ACT>
+__device__ __forceinline__ void split_rows32(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) {
+    // [32 rows][32 k] K-major raw -> tf32 hi / lo, swizzled: 256 float4, one per thread
+    const int r = t >> 3, c = t & 7;
+    const uint4 v = reinterpret_cast<const uint4*>(raw)[t];
+    const uint32_t off = (uint32_t)(r * 128 + (((c ^ r) & 7) << 4));
+    *reinterpret_cast<uint4*>(hi + off) = make_uint4(v.x & 0xffffe000u, v.y & 0xffffe000u, v.z & 0xffffe000u, v.w & 0xffffe000u);
+    *reinterpret_cast<uint4*>(lo + off) = make_uint4(tf32_lo_bits(v.x), tf32_lo_bits(v.y), tf32_lo_bits(v.z), tf32_lo_bits(v.w));
 }
 
 template <int KA, int ACT>
-static int launch_ps(const CUtensorMap& tx, const CUtensorMap& tw1, const CUtensorMap& tw1lo, const CUtensorMap& tw2,
-                     const CUtensorMap& tw2lo, const PsArgs& a, cudaStream_t st) {
-    using S = PsSmem<KA>;
+__global__ void __launch_bounds__(PS_THREADS, 1)
+policy_mlp2_heads_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CUtensorMap tw1,
+                         const __grid_constant__ CUtensorMap tw2, const PsArgs a) {
+    using S = PsSmem;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_align_1024(smem_raw);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::BARS);
+    uint64_t* x_bar = bars;
+    uint64_t* full = bars + 1;              // [2] chunk stages
+    const int t = threadIdx.x, wg = t >> 7, lane = t & 31;
+    const int n0 = blockIdx.x * TBN;
+    const int64_t m0 = (int64_t)blockIdx.y * TBM;
+    const int NC = a.H1 / 32;
+
+    if (t == 0) {
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tx) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tw1) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&tw2) : "memory");
+        mbar_init(x_bar, 1);
+        mbar_init(&full[0], 1);
+        mbar_init(&full[1], 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    pdl_wait();
+    pdl_trigger();
+
+    auto issue_chunk = [&](int c) {
+        uint8_t* st = smem + S::RAW + (c & 1) * S::RAW_STAGE;
+        mbar_expect_tx(&full[c & 1], KA * 4096 + 16384);
+        for (int kb = 0; kb < KA; ++kb) tma_load_2d(st + kb * 4096, &tw1, &full[c & 1], 32 * kb, 32 * c);
+        tma_load_2d(st + 2 * 4096, &tw2, &full[c & 1], 32 * c, n0);
+    };
+    if (t == 0) {
+        mbar_expect_tx(x_bar, KA * 16384);
+        for (int kb = 0; kb < KA; ++kb) tma_load_2d(smem + S::XRAW + kb * 16384, &tx, x_bar, 32 * kb, (int)m0);
+        issue_chunk(0);
+    }
+    mbar_wait(x_bar, 0);
+    for (int kb = 0; kb < KA; ++kb)
+        split_tile<false, true>(smem + S::XRAW + kb * 16384, smem + S::XC + kb * 32768, smem + S::XC + kb * 32768 + 16384, t);
+    __syncthreads();
+
+    float acc[64], cross[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+    const int r_in = wg * 64 + ((t >> 5) & 3) * 16 + (lane >> 2);   // first of the thread's two rows in the tile
+    uint8_t* h1_hi = smem + S::H1C;
+    uint8_t* h1_lo = h1_hi + 16384;
+    uint8_t* w2_hi = smem + S::W2C;
+    uint8_t* w2_lo = w2_hi + 16384;
+    for (int c = 0; c < NC; ++c) {
+        if (t == 0 && c + 1 < NC) issue_chunk(c + 1);   // its stage was read by everyone before the last barrier
+        mbar_wait(&full[c & 1], (c >> 1) & 1);
+        const uint8_t* st = smem + S::RAW + (c & 1) * S::RAW_STAGE;
+        for (int kb = 0; kb < KA; ++kb)
+            split_rows32<ACT>(st + kb * 4096, smem + S::W1C + kb * 8192, smem + S::W1C + kb * 8192 + 4096, t);
+        split_tile<false, true>(st + 2 * 4096, w2_hi, w2_lo, t);
+        fence_proxy_async_smem();
+        __syncthreads();
+        // ---- layer 1, columns [32c, 32c+32) of h1 for this warpgroup's 64 rows
+        float d1[16], x1[16];
+        wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < KA; ++kb) {
+            const uint64_t dxh = make_smem_desc(smem_u32(smem + S::XC + kb * 32768 + wg * 8192));
+            const uint64_t dxl = make_smem_desc(smem_u32(smem + S::XC + kb * 32768 + 16384 + wg * 8192));
+            const uint64_t dwh = make_smem_desc(smem_u32(smem + S::W1C + kb * 8192));
+            const uint64_t dwl = make_smem_desc(smem_u32(smem + S::W1C + kb * 8192 + 4096));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t o = (uint64_t)(2 * k);
+                wgmma_m64n32k8_tf32(d1, dxh + o, dwh + o, (kb | k) != 0);
+                wgmma_m64n32k8_tf32(x1, dxh + o, dwl + o, (kb | k) != 0);
+                wgmma_m64n32k8_tf32(x1, dxl + o, dwh + o, 1);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        // bias + activation + tf32 split -> the layer-2 A operand
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+            const int row = r_in + 8 * ((i >> 1) & 1);
+            const float h = act_fwd_ct<ACT>(d1[i] + x1[i] + a.b1[32 * c + col]);
+            const uint32_t w = __float_as_uint(h);
+            const uint32_t off = sw128_offset(row, col);
+            *reinterpret_cast<uint32_t*>(h1_hi + off) = w & 0xffffe000u;
+            *reinterpret_cast<uint32_t*>(h1_lo + off) = tf32_lo_bits(w);
+        }
+        fence_proxy_async_smem();
+        __syncthreads();
+        // ---- layer 2: acc (+)= h1[:, 32c..] . W2[n0.., 32c..]^T
+        const uint64_t dah = make_smem_desc(smem_u32(h1_hi + wg * 8192));
+        const uint64_t dal = make_smem_desc(smem_u32(h1_lo + wg * 8192));
+        const uint64_t dbh = make_smem_desc(smem_u32(w2_hi));
+        const uint64_t dbl = make_smem_desc(smem_u32(w2_lo));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t o = (uint64_t)(2 * k);
+            wgmma_m64n128k8_tf32(acc, dah + o, dbh + o, 1);
+            wgmma_m64n128k8_tf32(cross, dah + o, dbl + o, 1);
+            wgmma_m64n128k8_tf32(cross, dal + o, dbh + o, 1);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncthreads();   // every operand buffer of this chunk is free again
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] += cross[i];
+    TileCoord tc;
+    tc.m0 = m0;
+    tc.n0 = n0;
+    tc.k_begin = 0;
+    tc.num_kb = 0;
+    tc.z = 0;
+    heads_tile<ACT, 4>(acc, tc, m0 + r_in, lane, nullptr, 0, a.M, a.H2, a.epi);
+}
+
+template <int KA, int ACT>
+static int launch_ps(const CUtensorMap& tx, const CUtensorMap& tw1, const CUtensorMap& tw2, const PsArgs& a, cudaStream_t st) {
     auto kern = policy_mlp2_heads_kernel<KA, ACT>;
     static bool attr_set = false;
     if (!attr_set) {
-        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PsSmem::TOTAL));
         attr_set = true;
     }
     const dim3 grid((unsigned)(a.H2 / 128), (unsigned)ceil_div(a.M, 128));
-    SFB_CUDA_OK(launch_pdl(kern, grid, dim3(PS_THREADS), (size_t)S::TOTAL, st, tx, tw1, tw1lo, tw2, tw2lo, a));
+    SFB_CUDA_OK(launch_pdl(kern, grid, dim3(PS_THREADS), (size_t)PsSmem::TOTAL, st, tx, tw1, tw2, a));
     SFB_LAUNCH_OK();
     return 0;
 }
 
 // Does the fused two-layer policy step cover this model?  (3xTF32 engine, registered tf32-lo twins for both weight
-// matrices, K1 in {32, 64}, H1 a multiple of 32, H2 a multiple of 128 up to 512, <= 8 head rows.)
+// matrices -- i.e. the model's own weights --, K1 in {32, 64}, H1 a multiple of 32, H2 a multiple of 128 up to 512,
+// <= 8 head rows.)
 int tc_policy_mlp2_supported(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine) {
     if (engine != SFB200_GEMM_TC_3XTF32 || !tc_init()) return 0;
     if (!(K1 == 32 || K1 == 64) || H1 % 32 != 0 || H1 < 32 || H1 > PS_MAX_H1 || H2 % 128 != 0 || H2 < 128 || H2 > 512) return 0;
-    if (A < 1 || A + 1 > PS_HEAD_AP) return 0;
+    if (A < 1 || A + 1 > kHeadAP) return 0;
     if (!tf32_lo_lookup(W1, (int64_t)H1 * K1) || !tf32_lo_lookup(W2, (int64_t)H2 * H1)) return 0;
     return 4 * (H2 / 128);
 }
@@ -360,29 +207,25 @@ int tc_policy_mlp2_heads_forward(const float* x, int64_t ldx, int64_t M, int K1,
                                  const float* Wa, int A, float* head_part, cudaStream_t st) {
     if (!tc_policy_mlp2_supported(W1, W2, K1, H1, H2, A, engine)) return SFB_TC_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(x) & 15u) || ldx % 4 != 0 || (reinterpret_cast<uintptr_t>(head_part) & 15u) || !b1 || !b2 ||
-        M < 1 || M > 0x7fffffff)
+        (reinterpret_cast<uintptr_t>(Wv) & 7u) || (reinterpret_cast<uintptr_t>(Wa) & 7u) || M < 1 || M > 0x7fffffff)
         return SFB_TC_UNSUPPORTED;
-    const float* W1lo = tf32_lo_lookup(W1, (int64_t)H1 * K1);
-    const float* W2lo = tf32_lo_lookup(W2, (int64_t)H2 * H1);
     if (tf32_lo_check_enabled()) {
-        int rc = tf32_lo_check(W1, W1lo, (int64_t)H1 * K1, st);
-        if (!rc) rc = tf32_lo_check(W2, W2lo, (int64_t)H2 * H1, st);
+        int rc = tf32_lo_check(W1, tf32_lo_lookup(W1, (int64_t)H1 * K1), (int64_t)H1 * K1, st);
+        if (!rc) rc = tf32_lo_check(W2, tf32_lo_lookup(W2, (int64_t)H2 * H1), (int64_t)H2 * H1, st);
         if (rc) return rc;
     }
-    CUtensorMap tx, tw1, tw1lo, tw2, tw2lo;
-    bool ok = make_tmap(&tx, x, (uint64_t)K1, (uint64_t)M, (uint64_t)ldx, 32, 128, false);
-    ok = ok && make_tmap(&tw1, W1, (uint64_t)K1, (uint64_t)H1, (uint64_t)K1, 32, 32, false);
-    ok = ok && make_tmap(&tw1lo, W1lo, (uint64_t)K1, (uint64_t)H1, (uint64_t)K1, 32, 32, false);
-    ok = ok && make_tmap(&tw2, W2, (uint64_t)H1, (uint64_t)H2, (uint64_t)H1, 32, 128, false);
-    ok = ok && make_tmap(&tw2lo, W2lo, (uint64_t)H1, (uint64_t)H2, (uint64_t)H1, 32, 128, false);
+    CUtensorMap tx, tw1, tw2;
+    bool ok = make_tmap(&tx, x, (uint64_t)K1, (uint64_t)M, (uint64_t)ldx, 32, 128);
+    ok = ok && make_tmap(&tw1, W1, (uint64_t)K1, (uint64_t)H1, (uint64_t)K1, 32, 32);
+    ok = ok && make_tmap(&tw2, W2, (uint64_t)H1, (uint64_t)H2, (uint64_t)H1, 32, 128);
     if (!ok) return SFB_TC_UNSUPPORTED;
-    const PsArgs a{M, H1, H2, act, b1, b2, Wv, Wa, A, head_part};
-#define SFB_PS(KAv)                                                                                     \
-    switch (act) {                                                                                      \
-        case SFB200_ACT_ELU: return launch_ps<KAv, SFB200_ACT_ELU>(tx, tw1, tw1lo, tw2, tw2lo, a, st);   \
-        case SFB200_ACT_RELU: return launch_ps<KAv, SFB200_ACT_RELU>(tx, tw1, tw1lo, tw2, tw2lo, a, st); \
-        case SFB200_ACT_TANH: return launch_ps<KAv, SFB200_ACT_TANH>(tx, tw1, tw1lo, tw2, tw2lo, a, st); \
-        default: return launch_ps<KAv, SFB200_ACT_NONE>(tx, tw1, tw1lo, tw2, tw2lo, a, st);              \
+    PsArgs a{M, K1, H1, H2, act, b1, b2, TcEpilogue{1, act, b2, nullptr, 0, Wv, Wa, A, head_part}};
+#define SFB_PS(KAv)                                                                            \
+    switch (act) {                                                                             \
+        case SFB200_ACT_ELU: return launch_ps<KAv, SFB200_ACT_ELU>(tx, tw1, tw2, a, st);        \
+        case SFB200_ACT_RELU: return launch_ps<KAv, SFB200_ACT_RELU>(tx, tw1, tw2, a, st);      \
+        case SFB200_ACT_TANH: return launch_ps<KAv, SFB200_ACT_TANH>(tx, tw1, tw2, a, st);      \
+        default: return launch_ps<KAv, SFB200_ACT_NONE>(tx, tw1, tw2, a, st);                   \
     }
     if (K1 == 64) { SFB_PS(2) }
     SFB_PS(1)

@@ -8,47 +8,39 @@
 // thread-block CLUSTER of CX = H2/128 CTAs owns a row block for the whole rollout and the only synchronisation is the
 // cluster barrier (three per step); there is no grid-wide barrier and no kernel boundary.  CTA c of the cluster computes
 // columns [128c, 128c+128) of h1, then of h2 (partial head products), then finishes rows [32c.., ) of the block.
-// h1 and the head partials cross between the CTAs of a cluster through global memory (L2-resident: 256 KB per block);
-// DSMEM would move ~21 B/clk (B300_MICROARCH), the L2 path is a TMA load like any other A operand.
+// h1 and the head partials cross between the CTAs of a cluster through global memory (L2-resident), read back by TMA.
 //
-// Each GEMM tile is the TMEM-A pipeline of gemm_tc.cu (A raw via TMA -> operand warps split it into tensor memory; B =
-// registered weights, hi and lo tiles straight from TMA; 3xTF32 with main | cross accumulators), the step tail is the code of
-// sampler_tail_tape_kernel (heads.cu).  What the persistent form removes per step: two kernel launches + their prologues
-// (TMEM allocation, barrier init, descriptor prefetch, bias / head-weight staging) and the launch-to-launch dependency gaps.
+// Each GEMM tile is the wgmma tile of gemm_tc.cu (raw fp32 tiles by TMA, split into tf32 hi / lo halves in shared memory,
+// 3xTF32 with main | cross accumulators in registers); the step tail is the code of sampler_tail_tape_kernel (heads.cu).
 //
-//   warp 0      TMA producer            warp 1      MMA issuer (+ TMEM allocation)
-//   warps 2-5   operand warps           warps 6-13  epilogues (h1 tile store; h2 -> head partials)
-//   warps 6-13  the step tail (an 8-lane group per row: four rows per warp, the CTA's 32 rows in one pass)
+//   warps 0-3   idle (the kernel keeps the 384-thread warpgroup layout of gemm_tc.cu; not yet given work)
+//   warps 4-11  two wgmma warpgroups (64 rows each): consumer thread 0 (threadIdx 128) issues the TMA loads of the tiles;
+//               all of them split, multiply, run the epilogues and the step tail (an 8-lane group per row: four rows
+//               per warp).  A first correct port: not tuned on the H100 yet (ptxas reports register spills here).
 #include <cuda.h>
+
+#include <cstdlib>
 
 #include "common.cuh"
 #include "gemm.h"
 #include "heads_tail.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma_tile.cuh"
 
 namespace sfb {
 
-constexpr int RF_THREADS = 448;
-constexpr int RF_TILE_BYTES = 128 * TBK * 4;          // 16 KB: one [128 rows][32 fp32] (or [128][64 fp16]) K-major swizzled tile
-// tf32 split: 4 stages of 32 k, [B hi | B lo | A raw].  fp16 split (F16): 3 stages of 64 k, [B hi16 | B lo16 | A raw x 2]
-template <bool F16> struct RfPipe {
-    static constexpr int STAGES = F16 ? 3 : 4;
-    static constexpr int KB_K = F16 ? 64 : 32;
-    static constexpr int STAGE_BYTES = (F16 ? 4 : 3) * RF_TILE_BYTES;
-};
-constexpr int RF_MAX_STAGES = 4;
-constexpr uint32_t RF_ACOL0 = 256;                    // TMEM: accumulator [0,256) (main | cross), A stages [256, 512)
+constexpr int RF_THREADS = 384;
 constexpr int RF_HEAD_AP = 9;
 constexpr int RF_MAX_DIM = 128;
 
 struct RfSmem {
-    static constexpr int OFF_BARS = 4 * 3 * RF_TILE_BYTES;      // == 3 * 4 * RF_TILE_BYTES: both pipelines fill 192 KB
-    static constexpr int OFF_B1 = OFF_BARS + 256;
-    static constexpr int OFF_B2 = OFF_B1 + 128 * 4;
-    static constexpr int OFF_HEADW = OFF_B2 + 128 * 4;
-    static constexpr int OFF_CSTAT = OFF_HEADW + RF_HEAD_AP * 128 * 4;
+    static constexpr int RAW_STAGE = 2 * 128 * 64 * 4;            // A and B raw tiles of one k-block (64 k: fp16 form)
+    static constexpr int OFF_CONV = 2 * RAW_STAGE;                // two raw stages, then [A hi | A lo | B hi | B lo]
+    static constexpr int OFF_BARS = OFF_CONV + 4 * 128 * TBK * 4;
+    static constexpr int OFF_CSTAT = OFF_BARS + 64;
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
 };
+
 
 struct RolloutArgs {
     int64_t N; int T, K1, H1, H2;
@@ -90,54 +82,86 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     return r;
 }
 
-// bounded spin (same as policy_step.cu): a protocol bug traps instead of hanging the GPU
-__device__ __forceinline__ void rf_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0;
-    uint64_t t0 = 0;
-    for (uint32_t spins = 0; !done; ++spins) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if ((spins & 1023u) == 1023u) {
-            uint64_t now;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(now));
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 2000000000ull) __trap();
+// One 128 x 128 tile acc = A[m0.., :K] . B[n0.., :K]^T by the 256 consumer threads (ct = 0..255); both operands K-major
+// by TMA through two raw stages (k-block kb+1 is in flight while kb is split and multiplied).  `it` counts the raw stages
+// used so far (the mbarrier phases) and advances identically in every consumer thread.  3xTF32, or with F16 the
+// fp16-split form of gemm_tc.cu (A * 2^a_shift, weights * 2^kF16WShift, 64 k per stage).
+template <bool F16>
+__device__ __forceinline__ void rf_tile(const CUtensorMap* ta, const CUtensorMap* tb, int m0, int n0, int K, uint8_t* smem,
+                                        uint64_t* full, uint32_t& it, float (&acc)[64], float (&cross)[64], int ct,
+                                        int a_shift) {
+    using S = RfSmem;
+    constexpr int KBK = F16 ? 64 : TBK;
+    constexpr int B_OFF = 128 * KBK * 4;
+    const int wg = ct >> 7, nkb = K / KBK;
+    uint8_t* conv = smem + S::OFF_CONV;
+    auto issue = [&](uint32_t use, int kb) {
+        uint8_t* st = smem + (use & 1) * S::RAW_STAGE;
+        fence_proxy_async_all();   // generic-proxy global stores of the cluster (h1 / x_norm) -> this TMA read
+        mbar_expect_tx(&full[use & 1], 2 * B_OFF);
+        tma_load_2d(st, ta, &full[use & 1], KBK * kb, m0);
+        tma_load_2d(st + B_OFF, tb, &full[use & 1], KBK * kb, n0);
+    };
+    if (ct == 0) issue(it, 0);
+    const uint64_t da_hi = make_smem_desc(smem_u32(conv + wg * 8192));
+    const uint64_t da_lo = make_smem_desc(smem_u32(conv + 16384 + wg * 8192));
+    const uint64_t db_hi = make_smem_desc(smem_u32(conv + 32768));
+    const uint64_t db_lo = make_smem_desc(smem_u32(conv + 49152));
+    for (int kb = 0; kb < nkb; ++kb, ++it) {
+        if (ct == 0 && kb + 1 < nkb) issue(it + 1, kb + 1);   // that stage was read by everyone before the last barrier
+        mbar_wait(&full[it & 1], (it >> 1) & 1);
+        const uint8_t* st = smem + (it & 1) * S::RAW_STAGE;
+        if constexpr (F16) {
+            split_tile_f16<false>(st, conv, conv + 16384, ct, pow2f_int(a_shift));
+            split_tile_f16<false>(st + B_OFF, conv + 32768, conv + 49152, ct, pow2f_int(kF16WShift));
+        } else {
+            split_tile<false, true>(st, conv, conv + 16384, ct);
+            split_tile<false, true>(st + B_OFF, conv + 32768, conv + 49152, ct);
         }
+        fence_proxy_async_smem();
+        consumer_sync();
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TBK / WG_K; ++k) {
+            const uint64_t o = (uint64_t)(2 * k);
+            if constexpr (F16) {
+                wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, (kb | k) != 0);
+                wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, (kb | k) != 0);
+                wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
+            } else {
+                wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, (kb | k) != 0);
+                wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, (kb | k) != 0);
+                wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        consumer_sync();
+    }
+    if (F16) {
+        const float out_scale = pow2f_int(-(a_shift + kF16WShift));
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = fmaf(cross[i], 1.f / 2048.f, acc[i]) * out_scale;
+    } else {
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] += cross[i];
     }
 }
 
 template <int ACT, bool F16>
 __global__ void __launch_bounds__(RF_THREADS, 1)
 rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w1,
-                         const __grid_constant__ CUtensorMap tmap_w1lo, const __grid_constant__ CUtensorMap tmap_h1,
-                         const __grid_constant__ CUtensorMap tmap_w2, const __grid_constant__ CUtensorMap tmap_w2lo,
+                         const __grid_constant__ CUtensorMap tmap_h1, const __grid_constant__ CUtensorMap tmap_w2,
                          const RolloutArgs a) {
     using S = RfSmem;
-    constexpr int RF_STAGES = RfPipe<F16>::STAGES, RF_STAGE_BYTES = RfPipe<F16>::STAGE_BYTES, KB_K = RfPipe<F16>::KB_K;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);
-    uint64_t* full = bars;                       // [stages] A and B tiles landed (TMA)
-    uint64_t* conv = bars + RF_MAX_STAGES;       // [stages] A in TMEM (128 operand threads)
-    uint64_t* empty = bars + 2 * RF_MAX_STAGES;  // [stages] MMAs of the stage retired
-    uint64_t* acc_full = bars + 3 * RF_MAX_STAGES;
-    uint64_t* acc_empty = bars + 3 * RF_MAX_STAGES + 1;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * RF_MAX_STAGES + 2);
-    float* b1_s = reinterpret_cast<float*>(smem + S::OFF_B1);         // this CTA's 128 columns of b1
-    float* b2_s = reinterpret_cast<float*>(smem + S::OFF_B2);
-    float* headw_s = reinterpret_cast<float*>(smem + S::OFF_HEADW);   // [9][128]
-    float* cstat = reinterpret_cast<float*>(smem + S::OFF_CSTAT);     // [2][K1]: mu, 1 / sigma of the observation normaliser
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);   // [2] raw stages landed (TMA)
+    float* cstat = reinterpret_cast<float*>(smem + S::OFF_CSTAT);       // [2][K1]: mu, 1 / sigma of the observation normaliser
 
     // episode statistics of finished episodes: accumulated per CTA over the WHOLE rollout in shared memory, five global
-    // atomics per CTA at the end (the per-step launches issue them per finished episode: ~370 per step on five addresses --
-    // inside this kernel every cluster barrier's release would have to wait for those same-address atomics to drain)
+    // atomics per CTA at the end (inside this kernel every cluster barrier's release would otherwise have to wait for
+    // hundreds of same-address atomics per step to drain)
     __shared__ double s_stats[5];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x < 5) s_stats[threadIdx.x] = 0.0;
@@ -145,240 +169,56 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     const int CX = gridDim.x;
     const int n0 = cx * 128;
     const int64_t m0 = (int64_t)blockIdx.y * 128;
-    const int KB1 = a.K1 / KB_K, KB2 = a.H1 / KB_K;
     const int P = 2 * CX;
     const bool do_rms = a.mean != nullptr;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w1) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w1lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_h1) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w2) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w2lo) : "memory");
-        for (int s = 0; s < RF_STAGES; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&conv[s], 128);
-            mbar_init(&empty[s], 1);
-        }
-        mbar_init(acc_full, 1);
-        mbar_init(acc_empty, 256);
+        mbar_init(&full[0], 1);
+        mbar_init(&full[1], 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();
     pdl_trigger();
-    // constants of the whole rollout -> shared memory (epilogue warps)
-    if (warp >= 6) {
-        const int et = threadIdx.x - 192;   // 0..255
-        if (et < 128) { b1_s[et] = a.b1[n0 + et]; b2_s[et] = a.b2[n0 + et]; }
-        for (int i = et; i < RF_HEAD_AP * 128; i += 256) {
-            const int r = i >> 7, n = i & 127;
-            headw_s[i] = (r == 0) ? a.wv[n0 + n] : (r <= a.A ? a.wa[(int64_t)(r - 1) * a.H2 + n0 + n] : 0.f);
-        }
-        if (do_rms)
-            for (int c = et; c < a.K1; c += 256) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.K1 + c]);
-    }
+    if (do_rms)
+        for (int c = threadIdx.x; c < a.K1; c += RF_THREADS) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.K1 + c]);
     __syncthreads();
+    const int64_t env_step0 = a.env_step[0];
+    const uint64_t philox0 = a.sampler_step ? (uint64_t)*a.sampler_step : 0ull;
+    const float pv = a.pv_scalar ? *a.pv_scalar : 0.f;
     // fp16-split form: binary shifts of the two activation operands from their bounds (constant over the rollout: the
     // weights, hence the bounds, do not change inside a rollout)
     const int shift_x = F16 ? f16_shift_for_bound(a.bound_x[0]) : 0;
     const int shift_h = F16 ? f16_shift_for_bound(a.bound_h1[0]) : 0;
-    const int64_t env_step0 = a.env_step[0];
-    const uint64_t philox0 = a.sampler_step ? (uint64_t)*a.sampler_step : 0ull;
-    const float pv = a.pv_scalar ? *a.pv_scalar : 0.f;
-
-    int pref = 0;             // producer: stages of the current tile already armed + weight tiles requested
-    const bool tracer = a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 192;
+    const bool tracer = a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 128;
 #define RF_TRACE(slot) do { if (tracer) a.trace[(int64_t)t * 16 + (slot)] = rf_now(); } while (0)
-    uint32_t it = 0;          // stage use counter (every role advances it identically)
-    uint32_t tile_iter = 0;   // accumulator use counter
+    uint32_t it = 0;
+    const TcEpilogue epi_heads{1, ACT, a.b2, nullptr, 0, a.wv, a.wa, a.A, a.part};
+    const TcEpilogue epi_h1{1, ACT, a.b1, nullptr, 0};
 
     for (int t = 0; t < a.T; ++t) {
         RF_TRACE(0);
-#pragma unroll 1
         for (int layer = 0; layer < 2; ++layer) {
-            const int num_kb = layer == 0 ? KB1 : KB2;
-            if (warp == 0) {
-                // ===================================================== TMA producer
-                if (lane == 0) {
-                    if (layer == 1 || t > 0) fence_proxy_async_all();   // peers' generic-proxy writes (h1 / x_norm) -> TMA reads
-                    const CUtensorMap* ta = layer == 0 ? &tmap_x : &tmap_h1;
-                    const CUtensorMap* tb = layer == 0 ? &tmap_w1 : &tmap_w2;
-                    const CUtensorMap* tbl = layer == 0 ? &tmap_w1lo : &tmap_w2lo;
-                    for (int kb = 0; kb < num_kb; ++kb) {
-                        const uint32_t i = it + kb;
-                        const int s = i % RF_STAGES;
-                        uint8_t* sb = smem + s * RF_STAGE_BYTES;
-                        if (kb >= pref) {      // (the first `pref` stages were armed and their weight tiles requested before the barrier)
-                            rf_wait(&empty[s], ((i / RF_STAGES) & 1) ^ 1);
-                            mbar_expect_tx(&full[s], RF_STAGE_BYTES);
-                            tma_load_2d(sb, tb, &full[s], kb * KB_K, n0);
-                            tma_load_2d(sb + RF_TILE_BYTES, tbl, &full[s], kb * KB_K, n0);
-                        }
-                        tma_load_2d(sb + 2 * RF_TILE_BYTES, ta, &full[s], kb * KB_K, (int)m0);
-                        if (F16) tma_load_2d(sb + 3 * RF_TILE_BYTES, ta, &full[s], kb * KB_K + 32, (int)m0);
-                    }
-                    // weight tiles of the NEXT tile do not depend on the cluster barrier: request them now, so that only the
-                    // activation tiles' latency is exposed after it
-                    pref = 0;
-                    const bool has_next = (layer == 0) || (t + 1 < a.T);
-                    if (has_next) {
-                        const int nkb = layer == 0 ? KB2 : KB1;
-                        const CUtensorMap* nb = layer == 0 ? &tmap_w2 : &tmap_w1;
-                        const CUtensorMap* nbl = layer == 0 ? &tmap_w2lo : &tmap_w1lo;
-                        pref = nkb < RF_STAGES ? nkb : RF_STAGES;
-                        for (int kb = 0; kb < pref; ++kb) {
-                            const uint32_t i = it + num_kb + kb;
-                            const int s = i % RF_STAGES;
-                            uint8_t* sb = smem + s * RF_STAGE_BYTES;
-                            rf_wait(&empty[s], ((i / RF_STAGES) & 1) ^ 1);
-                            mbar_expect_tx(&full[s], RF_STAGE_BYTES);
-                            tma_load_2d(sb, nb, &full[s], kb * KB_K, n0);
-                            tma_load_2d(sb + RF_TILE_BYTES, nbl, &full[s], kb * KB_K, n0);
-                        }
-                    }
+            if (warp >= 4) {
+                const int ct = threadIdx.x - 128;
+                float acc[64], cross[64];
+                if (layer == 0) rf_tile<F16>(&tmap_x, &tmap_w1, (int)m0, n0, a.K1, smem, full, it, acc, cross, ct, shift_x);
+                else rf_tile<F16>(&tmap_h1, &tmap_w2, (int)m0, n0, a.H1, smem, full, it, acc, cross, ct, shift_h);
+                TileCoord tc;
+                tc.m0 = m0; tc.n0 = n0; tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
+                const int64_t row_base = m0 + (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
+                if (layer == 0) {
+                    store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
+                    fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
+                } else {
+                    heads_tile<ACT, 2>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
                 }
-                __syncwarp();
-            } else if (warp == 1) {
-                // ===================================================== MMA issuer
-                constexpr uint32_t idesc_wide = F16 ? make_idesc_f16(TBM, 256) : make_idesc(false, false, TBM, 256);
-                constexpr uint32_t idesc_cross = F16 ? make_idesc_f16(TBM, 128) : make_idesc(false, false, TBM, 128);
-                rf_wait(acc_empty, (tile_iter & 1) ^ 1);
-                tc_fence_after();
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    const uint32_t i = it + kb;
-                    const int s = i % RF_STAGES;
-                    rf_wait(&full[s], (i / RF_STAGES) & 1);    // B tiles come straight from TMA
-                    rf_wait(&conv[s], (i / RF_STAGES) & 1);    // A halves are in tensor memory
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint64_t db = make_smem_desc(smem_u32(smem + s * RF_STAGE_BYTES), false);
-                        const uint32_t a_hi = tmem_base + RF_ACOL0 + (uint32_t)s * 64u;
-#pragma unroll
-                        for (int k = 0; k < TBK / UMMA_K; ++k) {
-                            const uint64_t bo = (uint64_t)(k * (UMMA_K * 4 >> 4));     // 32 B per k-step: 8 tf32 or 16 fp16
-                            if (F16) {
-                                umma_f16_ts(tmem_base, a_hi + k * 8, db + bo, idesc_wide, (kb | k) != 0);
-                                umma_f16_ts(tmem_base + 128, a_hi + 32 + k * 8, db + bo, idesc_cross, 1);
-                                continue;
-                            }
-                            umma_tf32_ts(tmem_base, a_hi + k * UMMA_K, db + bo, idesc_wide, (kb | k) != 0);
-                            umma_tf32_ts(tmem_base + 128, a_hi + 32 + k * UMMA_K, db + bo, idesc_cross, 1);
-                        }
-                        umma_commit(&empty[s]);
-                        if (kb == num_kb - 1) umma_commit(acc_full);
-                    }
-                    __syncwarp();
-                }
-            } else if (warp < 6) {
-                // ===================================================== operand warps: A smem -> (hi, lo) -> TMEM
-                const int row = (warp & 3) * 32 + lane;
-                const uint32_t lane_addr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + RF_ACOL0;
-                const int sw = row & 7;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    const uint32_t i = it + kb;
-                    const int s = i % RF_STAGES;
-                    rf_wait(&full[s], (i / RF_STAGES) & 1);
-                    tc_fence_after();
-                    const uint4* arow = reinterpret_cast<const uint4*>(smem + s * RF_STAGE_BYTES + 2 * RF_TILE_BYTES + row * 128);
-                    uint32_t hi[32], lo[32];
-                    if constexpr (F16) {
-                        // 64 k of this thread's row (two 32-k boxes) -> scaled fp16 (hi, lo) pairs, two k per TMEM column
-                        const float a_scale = pow2f_int(layer == 0 ? shift_x : shift_h);
-#pragma unroll
-                        for (int bx = 0; bx < 2; ++bx) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const uint4 q = arow[bx * (RF_TILE_BYTES / 16) + (j ^ sw)];
-                                f16_split2(__uint_as_float(q.x) * a_scale, __uint_as_float(q.y) * a_scale, hi[bx * 16 + 2 * j],
-                                           lo[bx * 16 + 2 * j]);
-                                f16_split2(__uint_as_float(q.z) * a_scale, __uint_as_float(q.w) * a_scale, hi[bx * 16 + 2 * j + 1],
-                                           lo[bx * 16 + 2 * j + 1]);
-                            }
-                        }
-                    } else {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const uint4 q = arow[j ^ sw];
-                        hi[4 * j] = q.x; hi[4 * j + 1] = q.y; hi[4 * j + 2] = q.z; hi[4 * j + 3] = q.w;   // raw word = hi operand
-                        lo[4 * j] = tf32_lo_bits(q.x); lo[4 * j + 1] = tf32_lo_bits(q.y);
-                        lo[4 * j + 2] = tf32_lo_bits(q.z); lo[4 * j + 3] = tf32_lo_bits(q.w);
-                    }
-                    }
-                    tmem_st_32x32b_x32(lane_addr + (uint32_t)s * 64u, hi);
-                    tmem_st_32x32b_x32(lane_addr + (uint32_t)s * 64u + 32u, lo);
-                    tmem_st_wait();
-                    tc_fence_before();
-                    mbar_arrive(&conv[s]);
-                }
-            } else {
-                // ===================================================== epilogue: accumulator -> act(. + bias) -> h1 tile | head partials
-                const int quad = warp & 3;
-                const int half = (warp - 6) >> 2;                  // columns [64*half, 64*half + 64) of the 128-column tile
-                const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(half * 64);
-                const float out_scale = F16 ? pow2f_int(-((layer == 0 ? shift_x : shift_h) + kF16WShift)) : 1.f;
-                rf_wait(acc_full, tile_iter & 1);
-                RF_TRACE(1 + 4 * layer);          // accumulator complete
-                tc_fence_after();
-                float o[64];
-#pragma unroll
-                for (int c0 = 0; c0 < 64; c0 += 16) {
-                    uint32_t r[16], r2[16];
-                    tmem_ld_32x32b_x16(taddr + (uint32_t)c0, r);
-                    tmem_ld_32x32b_x16(taddr + 128u + (uint32_t)c0, r2);
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        if (F16) o[c0 + j] = fmaf(__uint_as_float(r2[j]), 1.f / 2048.f, __uint_as_float(r[j])) * out_scale;
-                        else o[c0 + j] = __uint_as_float(r[j]) + __uint_as_float(r2[j]);
-                    }
-                }
-                tc_fence_before();
-                mbar_arrive(acc_empty);
-                RF_TRACE(2 + 4 * layer);          // drained
-                const float* bias = (layer == 0 ? b1_s : b2_s) + half * 64;
-#pragma unroll
-                for (int j = 0; j < 64; ++j) o[j] = act_fwd_ct<ACT>(o[j] + bias[j]);
-                RF_TRACE(11 + layer);             // bias + activation done
-                const int64_t m = m0 + quad * 32 + lane;
-                if (m < a.N) {
-                    if (layer == 0) {
-                        float4* dst = reinterpret_cast<float4*>(a.h1 + m * a.H1 + n0 + half * 64);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) dst[j] = make_float4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-                    } else {
-                        float hp[RF_HEAD_AP];
-#pragma unroll
-                        for (int r = 0; r < RF_HEAD_AP; ++r) {
-                            const float* w = headw_s + r * 128 + half * 64;   // warp-uniform: shared-memory broadcast
-                            float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-                            for (int j = 0; j < 64; j += 4) {
-                                const float4 wv4 = *reinterpret_cast<const float4*>(w + j);
-                                s0 = fmaf(o[j], wv4.x, s0);
-                                s1 = fmaf(o[j + 1], wv4.y, s1);
-                                s0 = fmaf(o[j + 2], wv4.z, s0);
-                                s1 = fmaf(o[j + 3], wv4.w, s1);
-                            }
-                            hp[r] = s0 + s1;
-                        }
-                        RF_TRACE(13);             // head partial dot products done
-                        float4* dst = reinterpret_cast<float4*>(a.part + ((int64_t)(cx * 2 + half) * a.N + m) * kHeadPartPad);
-                        dst[0] = make_float4(hp[0], hp[1], hp[2], hp[3]);
-                        dst[1] = make_float4(hp[4], hp[5], hp[6], hp[7]);
-                        dst[2] = make_float4(hp[8], 0.f, 0.f, 0.f);
-                    }
-                }
-                if (layer == 0) fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
-                RF_TRACE(3 + 4 * layer);          // epilogue stores issued
+                RF_TRACE(3 + 4 * layer);
             }
-            it += (uint32_t)num_kb;
-            ++tile_iter;
             cluster_sync_all();   // h1 of the row block complete (layer 0) / all head partials of the row block written (layer 1)
             RF_TRACE(4 + 4 * layer);              // past the cluster barrier
         }
@@ -389,7 +229,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         // sums from L2 -> softmax -> Philox -> argmax -> env rule -> stores, ~4.7 us measured) is paid once per step, not once
         // per row a warp owns.  Bit-identical to heads_row_tail: logit a sits at group position (a + 1) % 8, which reproduces
         // the association order of the 32-lane butterfly sums there (lanes 1..8 after the xor-16 / xor-8 steps).
-        if (warp >= 6) {
+        if (warp >= 4) {
             const int g = lane & 7;                       // position inside the 8-lane group
             const int grp = lane >> 3;                    // which of the warp's four rows
             const int act_idx = (g + 7) & 7;              // action index held by this lane (position (a + 1) % 8)
@@ -403,7 +243,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
             const int rpc = 128 / CX;                     // rows of the block this CTA finishes
             const unsigned gmask = 0xffu << (grp * 8);
             for (int base = 0; base < rpc; base += 32) {
-                const int rr = base + (warp - 6) * 4 + grp;
+                const int rr = base + (warp - 4) * 4 + grp;
                 const int64_t row = m0 + cx * rpc + rr;
                 const bool ok = rr < rpc && row < a.N;
                 // ---- loads first: head partials, next observation (K1 / 8 floats per lane), episode accumulators
@@ -541,12 +381,6 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
             if (a.sampler_step) *a.sampler_step = (int64_t)philox0 + a.T;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
 }
 
 template <int ACT, bool F16>
@@ -571,11 +405,13 @@ static int launch_rollout(const CUtensorMap* tm, const RolloutArgs& a, int CX, c
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    SFB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], a));
+    SFB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], a));
     SFB_LAUNCH_OK();
     return 0;
 }
 
+// Covered: 3xTF32 engine, registered tf32-lo twins for both weight matrices (the model's own weights), K1 a multiple of 32
+// up to 128, H1 == H2 in {128, 256, 512}, <= 8 action outputs.
 int tc_rollout_mlp2_supported(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine) {
     if (engine != SFB200_GEMM_TC_3XTF32 || !tc_init()) return 0;
     if (!(K1 == 32 || K1 == 64 || K1 == 96 || K1 == 128) || H1 != H2 || !(H2 == 128 || H2 == 256 || H2 == 512)) return 0;
@@ -585,7 +421,7 @@ int tc_rollout_mlp2_supported(const float* W1, const float* W2, int K1, int H1, 
 }
 
 // fp16-split form (common.cuh): taken when the weights have registered fp16 twins and both activation buffers (x_norm, the
-// h1 scratch) have registered bounds; SFB200_TC_F16=0 keeps the tf32 split
+// h1 scratch) have registered bounds -- the same rule as the per-layer GEMMs; SFB200_TC_F16=0 keeps the tf32 split
 static bool rollout_f16_enabled() {
     static int v = -1;
     if (v < 0) {
@@ -595,9 +431,19 @@ static bool rollout_f16_enabled() {
     return v == 1;
 }
 
+#define SFB_RF_LAUNCH(F16v)                                                                  \
+    switch (act) {                                                                           \
+        case SFB200_ACT_ELU: return launch_rollout<SFB200_ACT_ELU, F16v>(tm, a, CX, st);     \
+        case SFB200_ACT_RELU: return launch_rollout<SFB200_ACT_RELU, F16v>(tm, a, CX, st);   \
+        case SFB200_ACT_TANH: return launch_rollout<SFB200_ACT_TANH, F16v>(tm, a, CX, st);   \
+        default: return launch_rollout<SFB200_ACT_NONE, F16v>(tm, a, CX, st);                \
+    }
+
 int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, const RolloutArgs& a_in, cudaStream_t st) {
     if (!tc_rollout_mlp2_supported(W1, W2, a_in.K1, a_in.H1, a_in.H2, a_in.A, engine)) return SFB_TC_UNSUPPORTED;
+    if ((reinterpret_cast<uintptr_t>(a_in.wv) & 7u) || (reinterpret_cast<uintptr_t>(a_in.wa) & 7u)) return SFB_TC_UNSUPPORTED;
     RolloutArgs a = a_in;
+    const int CX = a.H2 / 128;
     if (rollout_f16_enabled() && a.K1 % 64 == 0 && a.H1 % 64 == 0) {
         const F16Twin t1 = f16_twin_lookup(W1, (int64_t)a.H1 * a.K1), t2 = f16_twin_lookup(W2, (int64_t)a.H2 * a.H1);
         const float* bx = operand_bound_lookup(a.x_norm, a.N * a.K1 * (int64_t)sizeof(float));
@@ -610,46 +456,29 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
             }
             a.bound_x = bx;
             a.bound_h1 = bh;
-            CUtensorMap tm[6];
-            bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 32, 128, false);
-            ok = ok && make_tmap_f16(&tm[1], t1.hi, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 64, 128);
-            ok = ok && make_tmap_f16(&tm[2], t1.lo, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 64, 128);
-            ok = ok && make_tmap(&tm[3], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, 32, 128, false);
-            ok = ok && make_tmap_f16(&tm[4], t2.hi, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 64, 128);
-            ok = ok && make_tmap_f16(&tm[5], t2.lo, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 64, 128);
+            CUtensorMap tm[4];
+            bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 64, 128);
+            ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 64, 128);
+            ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, 64, 128);
+            ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 64, 128);
             if (!ok) return SFB_TC_UNSUPPORTED;
-            const int CX = a.H2 / 128;
-            switch (act) {
-                case SFB200_ACT_ELU: return launch_rollout<SFB200_ACT_ELU, true>(tm, a, CX, st);
-                case SFB200_ACT_RELU: return launch_rollout<SFB200_ACT_RELU, true>(tm, a, CX, st);
-                case SFB200_ACT_TANH: return launch_rollout<SFB200_ACT_TANH, true>(tm, a, CX, st);
-                default: return launch_rollout<SFB200_ACT_NONE, true>(tm, a, CX, st);
-            }
+            SFB_RF_LAUNCH(true)
         }
     }
-    const float* W1lo = tf32_lo_lookup(W1, (int64_t)a.H1 * a.K1);
-    const float* W2lo = tf32_lo_lookup(W2, (int64_t)a.H2 * a.H1);
     if (tf32_lo_check_enabled()) {
-        int rc = tf32_lo_check(W1, W1lo, (int64_t)a.H1 * a.K1, st);
-        if (!rc) rc = tf32_lo_check(W2, W2lo, (int64_t)a.H2 * a.H1, st);
+        int rc = tf32_lo_check(W1, tf32_lo_lookup(W1, (int64_t)a.H1 * a.K1), (int64_t)a.H1 * a.K1, st);
+        if (!rc) rc = tf32_lo_check(W2, tf32_lo_lookup(W2, (int64_t)a.H2 * a.H1), (int64_t)a.H2 * a.H1, st);
         if (rc) return rc;
     }
-    CUtensorMap tm[6];
-    bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 32, 128, false);
-    ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 32, 128, false);
-    ok = ok && make_tmap(&tm[2], W1lo, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 32, 128, false);
-    ok = ok && make_tmap(&tm[3], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, 32, 128, false);
-    ok = ok && make_tmap(&tm[4], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 32, 128, false);
-    ok = ok && make_tmap(&tm[5], W2lo, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 32, 128, false);
+    CUtensorMap tm[4];
+    bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, TBK, 128);
+    ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, TBK, 128);
+    ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, TBK, 128);
+    ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, TBK, 128);
     if (!ok) return SFB_TC_UNSUPPORTED;
-    const int CX = a.H2 / 128;
-    switch (act) {
-        case SFB200_ACT_ELU: return launch_rollout<SFB200_ACT_ELU, false>(tm, a, CX, st);
-        case SFB200_ACT_RELU: return launch_rollout<SFB200_ACT_RELU, false>(tm, a, CX, st);
-        case SFB200_ACT_TANH: return launch_rollout<SFB200_ACT_TANH, false>(tm, a, CX, st);
-        default: return launch_rollout<SFB200_ACT_NONE, false>(tm, a, CX, st);
-    }
+    SFB_RF_LAUNCH(false)
 }
+#undef SFB_RF_LAUNCH
 
 }  // namespace sfb
 

@@ -1,5 +1,5 @@
-// tcgen05 / TMA / mbarrier PTX wrappers, UMMA descriptors and compile-time activations shared by the GEMM engine
-// (gemm_tc.cu) and the fused policy-step kernel (policy_step.cu).  sm_100a only.
+// TMA / mbarrier / wgmma PTX wrappers, wgmma shared-memory descriptors and compile-time activations of the GEMM engine
+// (gemm_tc.cu).  sm_90a only (wgmma.mma_async is an sm_90a instruction).
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -8,16 +8,16 @@
 
 namespace sfb {
 
-constexpr int TBM = 128;        // tile rows  (UMMA M, cta_group::1)
+constexpr int TBM = 128;        // tile rows: two consumer warpgroups of 64 rows (wgmma M = 64)
+constexpr int TBN = 128;        // tile columns (wgmma N)
 constexpr int TBK = 32;         // k per stage: 32 fp32 = 128 B = one swizzle row
-constexpr int UMMA_K = 8;       // tf32
-constexpr int TC_THREADS = 448;   // TMA, MMA, 4 split warps, 8 epilogue warps
+constexpr int WG_K = 8;         // k per tf32 wgmma
 
 // ------------------------------------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 // 1024-byte aligned start inside the dynamic shared-memory window (the 128B swizzle atoms need it).  Plain pointer
 // arithmetic on the __shared__ array -- NOT a round trip through uintptr_t, which makes the compiler forget the address
-// space and emit generic LD.E / ST.E for every shared-memory access derived from it.
+// space and emit generic loads / stores for every shared-memory access derived from it.
 __device__ __forceinline__ uint8_t* smem_align_1024(uint8_t* raw) {
     return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
 }
@@ -46,8 +46,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1) {
     asm volatile(
@@ -57,139 +55,86 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
         : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands from shared memory (K-major, 128B swizzle), fp32
+// accumulators in the registers of the issuing warpgroup (PTX wgmma.mma_async m64n128k8 .tf32).  scale_d = 0 overwrites D.
+// Accumulator fragment: thread t of the warpgroup holds d[i] at row 16*(t/32) + (t%32)/4 + 8*((i/2)%2),
+// column 8*(i/4) + 2*(t%4) + i%2.
+__device__ __forceinline__ void wgmma_m64n128k8_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+        "%64, %65, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+          "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+          "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+          "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// D[64 x 32] (+)= A[64 x 8] * B[32 x 8]^T, tf32 (same operand layouts; d[i] at column 8*(i/4) + 2*(t%4) + i%2)
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand is read from tensor memory (rows = TMEM lanes, k = 32-bit columns)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// The same shape with fp16 operands (k16 per instruction), both K-major (imm-trans 0), fp32 accumulate.
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+          "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+          "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+          "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]),
+          "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+          "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+          "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
-// kind::f16 (fp16 operands, fp32 accumulate), A from tensor memory: two K elements per 32-bit TMEM column
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// kind::f16, both operands from shared memory
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-        "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-        "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tmem_st_cols(uint32_t taddr, const uint32_t (&r)[N]) {
-    static_assert(N == 16 || N == 32, "16 or 32 consecutive TMEM columns per thread");
-    if constexpr (N == 32) tmem_st_32x32b_x32(taddr, r);
-    else tmem_st_32x32b_x16(taddr, r);
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) |
-// version=1 [46,48) | layout type [61,64).
-//   K-major  tile [rows][32 fp32], SWIZZLE_128B (type 2, 16 B chunks XOR row%8): 128 B rows, 8-row atoms 1024 B apart
-//            -> SBO = 1024, LBO unused (1)
-//   MN-major tile = boxes of [32 k][32 rows] (4096 B each, k rows 128 B apart).  For 32-bit MN-major operands the only
-//            legal layout is SWIZZLE_128B_BASE32B (type 1: 32 B chunks XOR k%4, atom = 4 k-rows = 512 B; CUTLASS
-//            sm100_common.inl:92 "for mn-major tf32 operands, SW128_32B is the only available smem layout"), written by
-//            TMA with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B  -> LBO = 4096 (next 32 rows), SBO = 512 (next 4 k)
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, bool mn_major) {
+// wgmma shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64) (1 = 128B swizzle).
+// K-major tile [rows][32 fp32] with the 128B swizzle (16 B chunk index XOR row % 8, 8-row atoms of 1024 B): SBO = 1024
+// (next 8 rows), LBO unused (1).  A k-step of 8 tf32 = 32 B advances the start address inside the swizzle row.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)(mn_major ? (4096u >> 4) : 1u) << 16;
-    d |= (uint64_t)((mn_major ? 512u : 1024u) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)(mn_major ? 1 : 2) << 61;
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024u >> 4) << 32;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32=1 [4,6) | a/b_format TF32=2 [7,10)/[10,13) |
-// a_major [15] | b_major [16] | N>>3 [17,23) | M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(bool a_mn, bool b_mn, int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// byte offset of element (row, k) of a K-major [rows][32 fp32] tile in the 128B-swizzled layout
+__device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
+    return (uint32_t)(row * 128 + ((((k >> 2) ^ row) & 7) << 4) + (k & 3) * 4);
 }
-
-// kind::f16 instruction descriptor: a/b format F16 = 0, c format F32 = 1, both operands K-major
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// the same for a K-major [rows][64 fp16] tile (128 B rows as well, 8 halfs per 16 B chunk)
+__device__ __forceinline__ uint32_t sw128_offset_h(int row, int k) {
+    return (uint32_t)(row * 128 + ((((k >> 3) ^ row) & 7) << 4) + (k & 7) * 2);
 }
 
 template <int ACT>
@@ -213,13 +158,10 @@ __device__ __forceinline__ float act_bwd_ct(float h) {
     return 1.f;
 }
 
-// host side (gemm_tc.cu): driver entry point for cuTensorMapEncodeTiled resolved at run time; 2-D fp32 tensor maps with
-// the 128B swizzle (16 B chunks for K-major tiles, 32 B chunks for MN-major). dim0 = contiguous dimension.
+// host side (gemm_tc.cu): driver entry point for cuTensorMapEncodeTiled resolved at run time; 2-D fp32 tensor maps
+// without swizzle (the engine re-lays the tiles out itself). dim0 = contiguous dimension.
 bool tc_init();
 bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
-               uint32_t box1, bool mn_major);
-// 2-D fp16 tensor map, K-major rows of 64 halfs = 128 B, 128B swizzle
-bool make_tmap_f16(CUtensorMap* out, const uint16_t* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
-                   uint32_t box1);
+               uint32_t box1);
 
 }  // namespace sfb

@@ -1,0 +1,220 @@
+// Device-side building blocks of the wgmma GEMM tiles shared by the GEMM engine (gemm_tc.cu), the fused two-layer
+// policy step (policy_step.cu) and the persistent rollout (rollout_fused.cu): operand split passes into the swizzled
+// K-major layout, tile coordinates and the register epilogues (bias + activation, activation derivative, head partials).
+// sm_90a only.
+#pragma once
+#include "common.cuh"
+#include "heads_tail.cuh"
+#include "tc_ptx.cuh"
+
+namespace sfb {
+
+struct TcEpilogue {
+    int mode;            // 0 plain, 1 act(acc + bias[n]), 2 acc * act'(aux[m,n])
+    int act;
+    const float* bias;
+    const float* aux;
+    int64_t ld_aux;
+    // fused policy/value heads (mode 1 only): partial dot products of the activated output row with [Wv ; Wa] over each
+    // 64-column half of the tile -> head_part[(n_tile*2 + half)][m][kHeadPad]; C may be NULL (output row not stored)
+    const float* head_wv;
+    const float* head_wa;
+    int head_A;
+    float* head_part;
+    // finish the heads inside this kernel: the n-tile CTAs of a 128-row block count themselves in fin_counters[m_block];
+    // the one that arrives last sums the partials of its rows and runs the distribution tail (sampling, log-prob, ...) --
+    // the separate finishing launch disappears.  fin_counters: M/128 zero-initialised ints, left at zero again.
+    int* fin_counters;
+    HeadsFinish fin;
+};
+
+constexpr int kHeadAP = 9;     // value + up to 8 action outputs
+constexpr int kHeadPad = 12;   // floats per (partial, row): three 16 B stores
+constexpr int TC_STAGES = 4;
+constexpr int TC_THREADS = 384;
+
+struct TcSmem {
+    static constexpr int A_BYTES = TBM * TBK * 4;                 // 16 KB
+    static constexpr int B_BYTES = TBN * TBK * 4;                 // 16 KB
+    static constexpr int RAW_STAGE = A_BYTES + B_BYTES;
+    static constexpr int CONV = 2 * A_BYTES + 2 * B_BYTES;        // [A hi | A lo | B hi | B lo], swizzled K-major
+    static constexpr int BARS = 2 * TC_STAGES * 8 + 16;
+    static constexpr int TOTAL = 1024 /*align slack*/ + TC_STAGES * RAW_STAGE + CONV + BARS;
+};
+
+// ELU via the fast exponential: |error| <= ~2.4e-7 absolute (2 ulp of exp on [0,1]) -- inside the 1e-5 parity budget
+__device__ __forceinline__ float act_fwd_fast(float z, int act) {
+    if (act == SFB200_ACT_ELU) return z > 0.f ? z : (__expf(z) - 1.f);
+    return act_fwd(z, act);
+}
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// raw tile (TMA, no swizzle) -> tf32 hi / lo halves in the swizzled K-major layout.  K-major raw: [rows][32 k];
+// MN-major raw: [32 k][rows].  ct = consumer thread 0..255.
+template <bool MN, bool SPLIT3>
+__device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct) {
+#pragma unroll
+    for (int q = 0; q < (TBM * TBK / 4) / 256; ++q) {
+        const int i = ct + 256 * q;
+        const float4 v = reinterpret_cast<const float4*>(raw)[i];
+        const float e[4] = {v.x, v.y, v.z, v.w};
+        if (!MN) {
+            const int r = i >> 3, c = i & 7;                           // row r, k = 4c .. 4c+3
+            const uint32_t off = (uint32_t)(r * 128 + (((c ^ r) & 7) << 4));
+            uint4 h, l;
+            uint32_t* hp = &h.x;
+            uint32_t* lp = &l.x;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t w = __float_as_uint(e[j]);
+                hp[j] = SPLIT3 ? (w & 0xffffe000u) : w;
+                lp[j] = tf32_lo_bits(w);
+            }
+            *reinterpret_cast<uint4*>(hi + off) = h;
+            if (SPLIT3) *reinterpret_cast<uint4*>(lo + off) = l;
+        } else {
+            const int k = i >> 5, r0 = (i & 31) * 4;                   // rows r0 .. r0+3 at k
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t w = __float_as_uint(e[j]);
+                const uint32_t off = sw128_offset(r0 + j, k);
+                *reinterpret_cast<uint32_t*>(hi + off) = SPLIT3 ? (w & 0xffffe000u) : w;
+                if (SPLIT3) *reinterpret_cast<uint32_t*>(lo + off) = tf32_lo_bits(w);
+            }
+        }
+    }
+}
+
+// fp16-split engine: raw fp32 tile of 64 k -> scaled fp16 hi / lo halves (lo carries a 2^11 factor, common.cuh) in the
+// swizzled K-major [rows][64 fp16] layout.  K-major raw: [rows][64 k]; MN-major raw: [64 k][rows].
+template <bool MN>
+__device__ __forceinline__ void split_tile_f16(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct, float scale) {
+#pragma unroll 4
+    for (int q = 0; q < (TBM * 64 / 4) / 256; ++q) {
+        const int i = ct + 256 * q;
+        const float4 v = reinterpret_cast<const float4*>(raw)[i];
+        if (!MN) {
+            const int r = i >> 4, c4 = i & 15;                         // row r, k = 4*c4 .. 4*c4+3
+            const uint32_t off = (uint32_t)(r * 128 + ((((c4 >> 1) ^ r) & 7) << 4) + (c4 & 1) * 8);
+            uint2 h, l;
+            f16_split2(v.x * scale, v.y * scale, h.x, l.x);
+            f16_split2(v.z * scale, v.w * scale, h.y, l.y);
+            *reinterpret_cast<uint2*>(hi + off) = h;
+            *reinterpret_cast<uint2*>(lo + off) = l;
+        } else {
+            const int k = i >> 5, r0 = (i & 31) * 4;                   // rows r0 .. r0+3 at k
+            const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                uint16_t h, l;
+                f16_split1(e[j] * scale, h, l);
+                const uint32_t off = sw128_offset_h(r0 + j, k);
+                *reinterpret_cast<uint16_t*>(hi + off) = h;
+                *reinterpret_cast<uint16_t*>(lo + off) = l;
+            }
+        }
+    }
+}
+
+struct TileCoord {
+    int64_t m0;
+    int n0, k_begin, num_kb, z;
+};
+
+__device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_n, int tiles_per_z, int K, int k_chunk, int kbk = TBK) {
+    TileCoord t;
+    t.z = tile / tiles_per_z;
+    const int r = tile - t.z * tiles_per_z;
+    const int mb = r / tiles_n;
+    t.m0 = (int64_t)mb * TBM;
+    t.n0 = (r - mb * tiles_n) * TBN;
+    t.k_begin = t.z * k_chunk;
+    const int k_end = (t.k_begin + k_chunk < K) ? t.k_begin + k_chunk : K;
+    t.num_kb = (k_end - t.k_begin + kbk - 1) / kbk;
+    return t;
+}
+
+// Epilogue of one warpgroup's 64 x 128 accumulator: pair j (j = 0..31) of a thread is d[2j], d[2j+1] = columns
+// n0 + 8*(j/2) + 2*(lane%4) + {0, 1} of row  row_base + 8*(j%2).
+__device__ __forceinline__ void store_tile(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
+                                           int64_t ldc, int64_t M, int N, int mode, const TcEpilogue& epi) {
+    const bool v2 = (ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(C) & 7u) == 0);
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        const int64_t m = row_base + 8 * (j & 1);
+        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
+        if (m >= M || n >= N) continue;
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        const bool two = n + 1 < N;
+        if (mode == 1) {
+            v0 = act_fwd_fast(v0 + (epi.bias ? epi.bias[n] : 0.f), epi.act);
+            if (two) v1 = act_fwd_fast(v1 + (epi.bias ? epi.bias[n + 1] : 0.f), epi.act);
+        } else if (mode == 2) {
+            const float* h = epi.aux + m * epi.ld_aux + n;
+            v0 *= act_bwd_from_out(h[0], epi.act);
+            if (two) v1 *= act_bwd_from_out(h[1], epi.act);
+        }
+        float* dst = C + m * ldc + n;
+        if (two && v2) {
+            *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+        } else {
+            dst[0] = v0;
+            if (two) dst[1] = v1;
+        }
+    }
+}
+
+// Epilogue with the policy/value heads folded in (forward layers feeding critic_linear / distribution_linear,
+// actor_critic.py:171-186): y = act(acc + bias) is formed in registers, optionally stored, and contracted with the (A+1)
+// head weight rows -- the separate heads kernel's re-read of y disappears.  Per 64-column half of the tile the four
+// threads of a quad hold a row's 64 values; a fixed-order quad reduction gives the partial.  NPART partials per tile
+// (2: per 64-column half, 4: per 32-column quarter).
+template <int ACT, int NPART = 2>
+__device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
+                                           int64_t ldc, int64_t M, int N, const TcEpilogue& epi) {
+    constexpr int JP = 32 / NPART;   // accumulator pairs of a thread per partial (per 128 / NPART columns)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
+        acc[2 * j] = act_fwd_ct<ACT>(acc[2 * j] + epi.bias[n]);
+        acc[2 * j + 1] = act_fwd_ct<ACT>(acc[2 * j + 1] + epi.bias[n + 1]);
+        const int64_t m = row_base + 8 * (j & 1);
+        if (C && m < M) *reinterpret_cast<float2*>(C + m * ldc + n) = make_float2(acc[2 * j], acc[2 * j + 1]);
+    }
+    const int p0 = (tc.n0 / TBN) * NPART;
+#pragma unroll
+    for (int half = 0; half < NPART; ++half) {
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+            float hp[kHeadAP];
+#pragma unroll
+            for (int a = 0; a < kHeadAP; ++a) {
+                float s = 0.f;
+                if (a <= epi.head_A) {
+                    const float* w = a == 0 ? epi.head_wv : epi.head_wa + (int64_t)(a - 1) * N;
+#pragma unroll
+                    for (int jj = 0; jj < JP / 2; ++jj) {
+                        const int j = JP * half + 2 * jj + rs;
+                        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
+                        const float2 wv = __ldg(reinterpret_cast<const float2*>(w + n));
+                        s = fmaf(acc[2 * j], wv.x, s);
+                        s = fmaf(acc[2 * j + 1], wv.y, s);
+                    }
+                }
+                s += __shfl_xor_sync(0xffffffffu, s, 1);
+                s += __shfl_xor_sync(0xffffffffu, s, 2);
+                hp[a] = s;
+            }
+            const int64_t m = row_base + 8 * rs;
+            if ((lane & 3) == 0 && m < M) {
+                float4* dst = reinterpret_cast<float4*>(epi.head_part + ((int64_t)(p0 + half) * M + m) * kHeadPad);
+                dst[0] = make_float4(hp[0], hp[1], hp[2], hp[3]);
+                dst[1] = make_float4(hp[4], hp[5], hp[6], hp[7]);
+                dst[2] = make_float4(hp[8], 0.f, 0.f, 0.f);
+            }
+        }
+    }
+}
+
+}  // namespace sfb

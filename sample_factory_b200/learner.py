@@ -1,7 +1,7 @@
 """Device PPO / V-trace learner mirroring algo/learning/learner.py (Learner.train :1036, _prepare_batch :943-1034,
 _calculate_losses :537-669, _train :671-841) with every tensor op replaced by a libsfb200 kernel.
 
-Differences from the reference that are deliberate (B200-first) and do not change results:
+Differences from the reference that are deliberate (GPU-first) and do not change results:
   * no autograd: the backward pass is explicit (sfb200_ppo_loss_fwd_bwd -> heads_backward -> linear_backward)
   * no per-minibatch host syncs: loss scalars stay in a device stats block and are read once per epoch
   * V-trace runs on the device (the reference moves the minibatch to the CPU, :602-640)
@@ -250,8 +250,7 @@ class Learner:
         # CUDA-graph replay of the whole train() (cfg.learner_cuda_graph): possible when nothing in it depends on host
         # state -- constant lr schedule, one epoch (no early-stopping read-back), Adam.  The step counters and the
         # learning rate then live in device memory (read by the *_dev entry points).  Data parallel: opt-in with
-        # SFB200_DP_GRAPH=1 -- the NCCL all-reduces are then captured with the kernels (measured on 2 x B200: 76.0 M vs
-        # 70.6 M env-steps/s, profiles/r01_m_bench_n2_*.json); off by default until the multi-rank capture is covered
+        # SFB200_DP_GRAPH=1 -- the NCCL all-reduces are then captured with the kernels; off by default until the multi-rank capture is covered
         # by the equivalence test (tests/dp_worker.py, see DESIGN section 7).
         # Data parallel: every exchange is a libsfb200 kernel over NVLink peer memory (csrc/comm.cu) -- the gradient lives in
         # the comm buffer the peers read, so train() is kernels only and is captured like the single-GPU learner.

@@ -1,6 +1,6 @@
 """The registry for custom model parts (the reference's model/model_factory.py:16-60, algo/utils/context.py).
 
-The device engine runs the reference's BUILT-IN model families as hand-written sm_100a kernels (ModelSpec.from_cfg);
+The device engine runs the reference's BUILT-IN model families as hand-written sm_90a kernels (ModelSpec.from_cfg);
 an arbitrary torch module cannot be lowered onto them and there is no eager-PyTorch fallback on this path.  The registry
 therefore keeps the reference's API -- registration succeeds, so import-time `register_*` calls in user scripts work --
 and the runner refuses to start with an explicit message if a custom factory is installed (`check_supported`)."""

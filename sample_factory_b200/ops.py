@@ -429,7 +429,7 @@ def policy_mlp2_partials(W1: Tensor, W2: Tensor, A: int, engine: int) -> int:
 
 def policy_mlp2_heads_forward(x: Tensor, W1: Tensor, b1: Tensor, W2: Tensor, b2: Tensor, act: int, engine: int, Wv: Tensor,
                               Wa: Tensor, head_partials: Tensor) -> None:
-    """x [M, K1] -> partial head dot products of act(act(x W1^T + b1) W2^T + b2) (one tcgen05 kernel, csrc/policy_step.cu)"""
+    """x [M, K1] -> partial head dot products of act(act(x W1^T + b1) W2^T + b2) (one wgmma kernel, csrc/policy_step.cu)"""
     M, K1 = x.shape
     H1, H2, A = W1.shape[0], W2.shape[0], Wa.shape[0]
     assert Wv.is_contiguous() and Wa.is_contiguous() and Wv.numel() == H2 and Wa.shape[1] == H2

@@ -3,7 +3,7 @@
 
 One function serves the three call sites of the hot path (sampler policy step, learner bootstrap value, learner
 minibatch forward).  When the tensor feeding critic_linear / distribution_linear is the output of an MLP layer and the
-tcgen05 engine covers the shape, that layer and the heads run as ONE GEMM whose epilogue leaves partial head dot
+wgmma engine covers the shape, that layer and the heads run as ONE GEMM whose epilogue leaves partial head dot
 products (sfb200_linear_act_heads_forward) followed by a tiny finishing kernel (sfb200_heads_from_partials); the
 activated layer output is stored only if the caller needs it (the learner's backward does, the sampler does not).
 """
@@ -55,17 +55,14 @@ class HeadsPlan:
         if self.P > 0:
             self.part = torch.empty(self.P * max_rows * ops.HEAD_PART_PAD, dtype=torch.float32, device=model.device)
             # optional: the GEMM finishes the heads itself (last-arriving CTA per 128-row block; these are its arrival
-            # counters).  Measured on B200 (profiles/r01_l_heads_finish_in_gemm.md): one launch less per policy step but
-            # the finishing CTA walks its 128 rows 16 deep per warp -> +25 us per step (28.0M vs 37.3M env-steps/s), so
-            # the separate, fully parallel heads_from_partials launch stays the default.
+            # counters).  One launch less per policy step, but the finishing CTA walks its 128 rows 16 deep per warp while
+            # heads_from_partials is fully parallel, so the separate launch stays the default.
             self.counters = torch.zeros((max_rows + 127) // 128, dtype=torch.int32, device=model.device)
             self.finish_in_gemm = os.environ.get("SFB200_HEADS_FINISH_IN_GEMM", "0") == "1"
-        # two-layer MLP policies (BASELINE cfg-2): both layers + the head partials in ONE tcgen05 kernel whenever the last
-        # hidden activation is not needed afterwards (sampler policy step, learner bootstrap value) -- csrc/policy_step.cu.
-        # Opt-in (SFB200_POLICY_FUSED=1): measured on B200 (profiles/r02_e_*) the fused kernel is faster cold (33.5 vs
-        # 25.2 + 15.6 us under ncu) but slower inside the replayed rollout (29.2 vs 26.5 us warm: it re-computes layer 1 in each
-        # of the four column CTAs, +50 % MMA work, and the tf32 MMA rate is what bounds both), so the per-layer launches stay
-        # the default.
+        # two-layer MLP policies (BASELINE cfg-2): both layers + the head partials in ONE kernel whenever the last hidden
+        # activation is not needed afterwards -- csrc/policy_step.cu (wgmma, h1 chunk by chunk in shared memory).  Opt-in
+        # (SFB200_POLICY_FUSED=1): it recomputes layer 1 in each of the H2/128 column CTAs and has not been measured on the
+        # H100, so the per-layer launches stay the default.
         self.mlp2 = False
         self.P_mlp2 = 0
         if (self.P > 0 and self.conv is None and not spec.use_rnn and not spec.decoder_mlp_layers and

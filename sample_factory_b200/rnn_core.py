@@ -5,7 +5,7 @@ The reference packs every run of steps between done-or-invalid boundaries into a
 state across an episode boundary.  On the device the same computation is a masked time loop over the `recurrence`
 steps of all chunks at once: a row whose previous step was done-or-invalid starts from a ZERO state (rnn_utils.py:143-149)
 and the backward pass cuts the gradient at the same places; a chunk's first step starts from the stored rnn_state
-(constant).  Every step is: two GEMMs on the tcgen05 engine (x.W_ih^T batched over ALL steps up front, h.W_hh^T per
+(constant).  Every step is: two GEMMs on the wgmma engine (x.W_ih^T batched over ALL steps up front, h.W_hh^T per
 step) + one fused cell kernel (csrc/rnn.cu).  The weight gradients are two large GEMMs over the stacked time-major
 buffers, not R small ones.
 """

@@ -65,7 +65,7 @@ class _DeviceSamplingLoop:
     def __init__(self, cfg, env_info: Optional[EnvInfo], model: Optional[PolicyModel], record_episodes: bool,
                  deterministic: bool = False):
         if not torch.cuda.is_available():
-            raise RuntimeError("sample_factory_b200 needs a CUDA device (B200); there is no CPU execution path")
+            raise RuntimeError("sample_factory_b200 needs a CUDA device (H100, sm_90a); there is no CPU execution path")
         self.cfg = cfg
         self.device = torch.device("cuda", torch.cuda.current_device())
         ops.bind_device(self.device)

@@ -101,7 +101,7 @@ class Runner:
         cfg = self.cfg
         self.rank, self.local_rank, self.world_size = init_from_env()
         if not torch.cuda.is_available():
-            raise RuntimeError("sample_factory_b200 needs a CUDA device (B200); there is no CPU execution path")
+            raise RuntimeError("sample_factory_b200 needs a CUDA device (H100, sm_90a); there is no CPU execution path")
         self.device = torch.device("cuda", self.local_rank)
         torch.cuda.set_device(self.device)
         ops.bind_device(self.device)

@@ -1,4 +1,4 @@
-"""Generate golden vectors by EXECUTING THE REFERENCE (from /root/reference, under oracle/ref_shims.py).
+"""Generate golden vectors by EXECUTING THE REFERENCE (from a reference checkout (oracle/install_ref.py: reference_dir()), under oracle/ref_shims.py).
 
 Run in the build container only:   python tests/golden/make_golden.py
 Writes tests/golden/<case>.npz.  The reference is a Python package and cannot travel to the GPU box, so the

@@ -74,7 +74,7 @@ def _need(engine):
     from sample_factory_b200 import ops
 
     if engine != "simt" and not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
 
 
 GOLDEN_CASES = ["tiny_gae", "tiny_vtrace", "tiny_gru", "tiny_lstm", "cfg2_small", "tiny_gauss", "tiny_gauss_adaptive", "tiny_conv", "tiny_symkl", "tiny_lamb", "tiny_tuple", "tiny_separate", "tiny_mask"]

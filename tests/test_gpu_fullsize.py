@@ -40,7 +40,7 @@ CASES = {
         # four SGD steps with adam_eps = 1e-5 on 1.7 M conv / FC weights: the few whose |g| ~ eps move by up to lr = 1e-4 per
         # step in a direction a 1e-7 gradient difference decides (measured: 104 of 1 605 632 FC weights off by > 6e-5, max 1.5e-4)
         w_atol=6e-5, w_frac=3e-4,
-        # (after ONE step the first moments agree to 1.4e-7 / 7.7e-4 relative, tools/conv_grad_check.py; the amplified weight
+        # (after ONE step the first moments agree to 1.4e-7 / 7.7e-4 relative, the amplified weight
         # differences feed back into the gradients of steps 2-4)
         m_atol=5e-5),
     # configs[4]: Box(256), MLP 512-256-128 -> LSTM-512, rollout = recurrence = 16, value bootstrap (one GPU's shard, 1024 envs)
@@ -55,7 +55,7 @@ def test_full_size_parity_vs_oracle(name):
     from sample_factory_b200 import ops
 
     if not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     case = CASES[name]
     N, T = case["N"], case["T"]
     dev = torch.device("cuda", 0)

@@ -102,7 +102,7 @@ def test_returns_normalizer_roundtrip(dev):
 def test_linear_act_forward(dev, M, N, K, act, engine):
     ops = _ops()
     if engine != "simt" and not ops.tc_available():
-        pytest.skip("tcgen05 engine not built")
+        pytest.skip("wgmma engine not built")
     x = torch.randn(M, K, generator=g(5))
     W = torch.randn(N, K, generator=g(6)) / math.sqrt(K)
     b = torch.randn(N, generator=g(7)) * 0.1
@@ -115,11 +115,11 @@ def test_linear_act_forward(dev, M, N, K, act, engine):
 
 
 def test_tc_engine_precision_classes(dev):
-    """tcgen05 engine: the 3xTF32 split must be fp32-grade (same error class as the exact-fp32 CUDA-core engine),
+    """wgmma engine: the 3xTF32 split must be fp32-grade (same error class as the exact-fp32 CUDA-core engine),
     the single-pass TF32 mode must be visibly coarser (proves the tensor-core path really ran and the split matters)."""
     ops = _ops()
     if not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     M, N, K = 2048, 512, 512
     x = torch.randn(M, K, generator=g(70))
     W = torch.randn(N, K, generator=g(71)) / math.sqrt(K)
@@ -144,7 +144,7 @@ def test_fp16_split_engine_is_fp32_grade(dev, M, N, K, amp):
     activations of very different magnitudes (the bound sets the power-of-two operand shift) and a loose bound."""
     ops = _ops()
     if not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     x = (torch.randn(M, K, generator=g(170)) * amp).to(dev)
     W = (torch.randn(N, K, generator=g(171)) / math.sqrt(K)).to(dev).contiguous()
     b = (torch.randn(N, generator=g(172)) * 0.1 * amp).to(dev)
@@ -246,7 +246,7 @@ def test_linear_forward_strided_input(dev):
 def test_linear_backward(dev, M, N, K, act_prev, engine):
     ops = _ops()
     if engine != "simt" and not ops.tc_available():
-        pytest.skip("tcgen05 engine not built")
+        pytest.skip("wgmma engine not built")
     dz = torch.randn(M, N, generator=g(10)) / M
     # x is the previous layer's OUTPUT: make it a genuine activation output so act'(x) is well defined
     pre = torch.randn(M, K, generator=g(11))
@@ -774,7 +774,7 @@ def test_bptt_matches_loopy_torch_rnn(dev, T, N, D, random_dones, rnn_type, engi
     from sample_factory_b200.rnn_core import RnnCore
 
     if engine_name != "simt" and not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     engine = ops.ENGINES[engine_name]
     gen = g(1000 + T * 131 + N * 7 + D)
     rnn = (torch.nn.GRU if rnn_type == "gru" else torch.nn.LSTM)(D, D, 1)
@@ -847,7 +847,7 @@ def test_linear_heads_fused_matches_separate(dev, engine_name, M, K, N, A, act):
     ops = _ops()
     engine = {"3xtf32": ops.GEMM_TC_3XTF32, "tf32": ops.GEMM_TC_TF32}[engine_name]
     P = ops.linear_heads_partials(N, A, engine)
-    assert P == 2 * (N // 128), "fused path must cover these shapes on a B200"
+    assert P == 2 * (N // 128), "fused path must cover these shapes on an H100"
     x = torch.randn(M, K, generator=g(60))
     W = torch.randn(N, K, generator=g(61)) / math.sqrt(K)
     b = torch.randn(N, generator=g(62)) * 0.1
@@ -1149,7 +1149,7 @@ def test_conv_head_forward_backward(dev, B, shape, arch, engine_name):
     reference's ConvEncoderImpl executes, model/encoder.py:88-118): features, conv weight / bias gradients."""
     ops = _ops()
     if engine_name != "simt" and not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     from sample_factory_b200.conv_encoder import ConvHead
     from sample_factory_b200.model import ModelSpec, PolicyModel
 
@@ -1367,7 +1367,7 @@ def test_policy_mlp2_heads_forward(dev, M, K1, H1, H2, A, act):
     == a float64 torch reference at fp32-parity tolerance; action indices identical."""
     ops = _ops()
     if not ops.tc_available():
-        pytest.skip("tcgen05 engine not available")
+        pytest.skip("wgmma engine not available")
     engine = ops.GEMM_TC_3XTF32
     flat = torch.empty(H1 * K1 + H2 * H1, device=dev)
     lo = torch.empty_like(flat)

@@ -1,5 +1,5 @@
 """Gradient accuracy of the conv encoder's backward at the cfg-4 parity shape: Adam's first moment after ONE SGD step
-(= 0.1 x clipped gradient) for the tcgen05 3xTF32 engine and the exact-fp32 CUDA-core engine against the CPU oracle."""
+(= 0.1 x clipped gradient) for the wgmma 3xTF32 engine and the exact-fp32 CUDA-core engine against the CPU oracle."""
 import os
 import sys
 

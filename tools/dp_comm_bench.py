@@ -6,7 +6,7 @@
   * device time per SGD-step exchange, eager and replayed from a CUDA graph, next to ncclAllReduce + the two-kernel Adam.
 
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/dp_comm_bench.py
-Prints one JSON line on rank 0 (commit it under profiles/)."""
+Prints one JSON line on rank 0."""
 import json
 import os
 import sys
