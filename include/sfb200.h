@@ -119,6 +119,12 @@ int sfb200_rms_apply_scalar(float* x, int64_t n, const double* mean, const doubl
  * engine: SFB200_GEMM_*.  x row stride ldx (lets the learner feed obs[:, T] rows in place), y row stride ldy. */
 int sfb200_linear_act_forward(const float* x, int64_t ldx, const float* W, const float* b, float* y, int64_t ldy,
                               int64_t M, int N, int K, int act, int engine, void* stream);
+/* The second conv of a ResBlock with its identity path (model/encoder.py:166-169, `out + identity`):
+ *   y[M,N] = (x[M,K] . W[N,K]^T + b[N]) + r[M,N]      r read in the GEMM epilogue at the output's (row, col), row stride ldr.
+ * Same engines and shape coverage as sfb200_linear_act_forward (the wgmma engine where TMA describes the operands, the
+ * SIMT engine otherwise).  r must not overlap y. */
+int sfb200_linear_residual_forward(const float* x, int64_t ldx, const float* W, const float* b, const float* r,
+                                   int64_t ldr, float* y, int64_t ldy, int64_t M, int N, int K, int engine, void* stream);
 
 /* Sampling mode of the calling host thread, picked up by every heads entry below that samples actions (the
  * `action_mask=` argument of ActorCritic.forward, model/actor_critic.py:189-195, filled from the observation dict's
@@ -500,6 +506,31 @@ int sfb200_col2im_act_backward(const float* dcol, const float* x_act, int64_t B,
                                int stride, int act, float* dx, void* stream);
 /* [B, P, C] <-> [B, C, P]: NHWC rows of the last conv layer <-> the (C,H,W) flatten order of encoder.py:115 */
 int sfb200_permute_bpc(const float* src, float* dst, int64_t B, int P, int C, int to_channel_major, void* stream);
+
+/* ResnetEncoder (model/encoder.py:153-221, resnet_impala).  Conv2d(act(x), padding=pad): im2col of the ACTIVATED input
+ * with zero padding applied after the activation (ResBlock, encoder.py:157-162); pad = 0, act = none is sfb200_im2col.
+ *   col[(b,oh,ow), (ci,kh,kw)] = act(x[b, ci, oh*stride+kh-pad, ow*stride+kw-pad])   (0 outside the input)
+ * with OH = (H+2*pad-kernel)/stride+1. */
+int sfb200_im2col_pad_act(const float* x, int in_nchw, int64_t B, int C, int H, int W, int kernel, int stride, int pad,
+                          int act, float* col, void* stream);
+/* backward of sfb200_im2col_pad_act (gather, deterministic), NHWC:
+ *   dx = col2im(dcol) * act'(x_act) (+ dres)
+ * from_input = 0: x_act is the activation's OUTPUT (as sfb200_col2im_act_backward; act = none for a stage-entry conv);
+ * from_input = 1: x_act is its INPUT (the act(x) / act(conv_a) a ResBlock feeds its convs, encoder.py:157-162), as
+ * autograd's elu_backward(is_result=false) uses it; dres (optional, may be NULL) is the gradient of the block's identity
+ * path (encoder.py:166-169), added in the same pass. */
+int sfb200_col2im_pad_act_backward(const float* dcol, const float* x_act, int from_input, const float* dres, int64_t B,
+                                   int C, int H, int W, int kernel, int stride, int pad, int act, float* dx, void* stream);
+/* MaxPool2d(kernel_size=3, stride=2, padding=1) (encoder.py:191) on NHWC rows [B, H, W, C] -> y [B, OH, OW, C],
+ * OH = ceil(H/2), and idx [B, OH, OW, C] = the window position kh*3+kw of the maximum (torch's rule: the first maximum
+ * in row-major window order, NaN propagates; padding never wins). */
+int sfb200_maxpool3s2_forward(const float* x, int64_t B, int C, int H, int W, float* y, uint8_t* idx, void* stream);
+/* its backward from the stored indices (gather, deterministic): dx [B, H, W, C] */
+int sfb200_maxpool3s2_backward(const float* dy, const uint8_t* idx, int64_t B, int C, int H, int W, float* dx,
+                               void* stream);
+/* dst [B, C, P] = act(src [B, P, C]): the ResnetEncoder's final activation (encoder.py:202) fused into the (C,H,W)
+ * flatten of encoder.py:217 */
+int sfb200_act_permute_bpc(const float* src, float* dst, int64_t B, int P, int C, int act, void* stream);
 
 /* ------------------------------------------------------------- learner: backward ---- */
 int64_t sfb200_heads_backward_workspace_bytes(int H, int A);

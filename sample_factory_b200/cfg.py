@@ -201,9 +201,6 @@ def verify_cfg(cfg, num_agents_total: Optional[int] = None) -> bool:
             cfg_error(f"sync mode: samples per training iteration ({cfg.num_batches_per_epoch=} * {cfg.batch_size=} = "
                       f"{per_iteration}) and samples per rollout ({samples}) must divide one another")
     # values the argument parser accepts (reference surface) that the kernel path does not implement: refuse with a reason
-    if getattr(cfg, "encoder_conv_architecture", "convnet_simple") not in ("convnet_simple", "convnet_impala", "convnet_atari"):
-        cfg_error(f"{cfg.encoder_conv_architecture=}: only the plain conv stacks (convnet_simple / convnet_impala / "
-                  "convnet_atari, model/encoder.py:127-134) run on the device path; resnet_impala (encoder.py:153-221) does not")
     if getattr(cfg, "rnn_num_layers", 1) != 1:
         cfg_error(f"{cfg.rnn_num_layers=}: the device path implements the one-layer recurrent core (model/core.py:27-64)")
     if getattr(cfg, "num_policies", 1) < 1:

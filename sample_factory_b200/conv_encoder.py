@@ -91,3 +91,141 @@ class ConvHead:
             else:
                 ops.linear_backward(dz, col, W.view(co, ci * k * k), none, gW.view(co, ci * k * k), None, None,
                                     self.engine, self.lin_ws)
+
+
+class ResnetHead:
+    """Buffers + launch sequence for the reference's ResnetEncoder conv head (model/encoder.py:153-221, resnet_impala) at
+    up to `max_rows` observations per call; the interface of ConvHead (forward -> feat, backward(dfeat), .feat).
+
+    Per stage:  z = conv(x, pad 1)  ->  x0 = maxpool3s2(z) (+ uint8 argmax indices)  ->  per block
+    a = conv_a(act(x_j))  and  x_{j+1} = conv_b(act(a)) + x_j  (residual GEMM epilogue).  Both activations are applied
+    by the im2col that feeds the conv (expm1f for ELU, as torch computes it, rather than the wgmma epilogue's fast-exp
+    ELU), and the backward takes act' from the stored activation inputs x_j and a, as autograd's elu_backward does.
+    After the last stage  feat = act(x)  in (C,H,W) order.
+    Memory: ONE im2col scratch sized by the largest conv (the backward recomputes each conv's im2col instead of keeping
+    one per layer), the block inputs / inner activations (NHWC) and pool indices, one pre-pool scratch shared with the
+    pool's input gradient, and three gradient buffers (ping-pong + the inner d(pre-activation))."""
+
+    def __init__(self, model: PolicyModel, engine: int, max_rows: int, need_backward: bool):
+        self.model, self.engine, self.max_rows = model, engine, max_rows
+        spec = model.spec
+        assert spec.is_resnet
+        self.stages = spec.resnet_stages
+        self.act = ops.ACT[spec.nonlinearity]
+        f32 = dict(dtype=torch.float32, device=model.device)
+        col_k = max(max(h * w * ci * 9, hp * wp * co * 9) for (ci, h, w, co, hp, wp, _b) in self.stages)
+        self.col = torch.empty(max_rows * col_k, **f32)
+        self.z = torch.empty(max_rows * max(h * w * co for (_ci, h, w, co, _hp, _wp, _b) in self.stages), **f32)
+        # x[s] = [x_0, x_1, ..., x_blocks] (block inputs; x_blocks is the stage output), a[s] = conv_a outputs
+        self.x: List[List[Tensor]] = []
+        self.a: List[List[Tensor]] = []
+        self.idx: List[Tensor] = []
+        for (_ci, _h, _w, co, hp, wp, blocks) in self.stages:
+            rows = max_rows * hp * wp
+            self.x.append([torch.empty((rows, co), **f32) for _ in range(blocks + 1)])
+            self.a.append([torch.empty((rows, co), **f32) for _ in range(blocks)])
+            self.idx.append(torch.empty((rows, co), dtype=torch.uint8, device=model.device))
+        self.feat = torch.empty((max_rows, spec.conv_out_size), **f32)
+        self.x_in: Optional[Tensor] = None
+        if need_backward:
+            g = max(hp * wp * co for (_ci, _h, _w, co, hp, wp, _b) in self.stages)
+            self.g = [torch.empty(max_rows * g, **f32) for _ in range(3)]
+            lin_ws, max_c = 4, 1
+            for (ci, h, w, co, hp, wp, _b) in self.stages:
+                lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(max_rows * h * w, co, ci * 9) // 4 + 4,
+                             ops.linear_backward_workspace_bytes(max_rows * hp * wp, co, co * 9) // 4 + 4)
+                max_c = max(max_c, co)
+            self.lin_ws = torch.empty(lin_ws, **f32)
+            self.colsum_ws = torch.empty(ops.colsum_workspace_bytes(max_c) // 4 + 4, **f32)
+
+    @staticmethod
+    def _view(buf: Tensor, rows: int, cols: int) -> Tensor:
+        return buf[: rows * cols].view(rows, cols)
+
+    # ------------------------------------------------------------------------------------------------------------
+    def forward(self, x: Tensor) -> Tensor:
+        """x: [M, C*H*W] normalised observations, rows in (C,H,W) order -> [M, conv_out] = act(conv head output)"""
+        M = x.shape[0]
+        assert M <= self.max_rows
+        if not x.is_contiguous():
+            x = x.contiguous()
+        self.x_in = x                     # the first conv's im2col is recomputed from it in the backward
+        params = iter(self.model.conv_params())
+        none = ops.ACT["none"]
+        src, nchw = x, True
+        for s, (ci, h, w, co, hp, wp, blocks) in enumerate(self.stages):
+            W, b = next(params)
+            col = self._view(self.col, M * h * w, ci * 9)
+            z = self._view(self.z, M * h * w, co)
+            ops.im2col_pad_act(src, nchw, M, ci, h, w, 3, 1, 1, none, col)
+            ops.linear_act_forward(col, W.view(co, ci * 9), b, z, none, self.engine)       # Conv2d(3, padding 1)
+            ops.maxpool3s2_forward(z, M, co, h, w, self.x[s][0][: M * hp * wp], self.idx[s][: M * hp * wp])
+            col = self._view(self.col, M * hp * wp, co * 9)
+            for j in range(blocks):
+                (Wa, ba), (Wb, bb) = next(params), next(params)
+                xj, aj, xn = (t[: M * hp * wp] for t in (self.x[s][j], self.a[s][j], self.x[s][j + 1]))
+                ops.im2col_pad_act(xj, False, M, co, hp, wp, 3, 1, 1, self.act, col)                # act(x), padded
+                ops.linear_act_forward(col, Wa.view(co, co * 9), ba, aj, none, self.engine)       # conv_a(.)
+                ops.im2col_pad_act(aj, False, M, co, hp, wp, 3, 1, 1, self.act, col)                # act(a), padded
+                ops.linear_residual_forward(col, Wb.view(co, co * 9), bb, xj, xn, self.engine)   # conv_b(.) + x
+            src, nchw = self.x[s][blocks][: M * hp * wp], False
+        _ci, _h, _w, co, hp, wp, _b = self.stages[-1]
+        ops.act_permute_bpc(src, self.feat[:M], M, hp * wp, co, self.act)    # act, (C,H,W) flatten (encoder.py:202, 217)
+        return self.feat[:M]
+
+    def backward(self, dfeat: Tensor) -> None:
+        """dfeat: [M, conv_out] gradient w.r.t. the conv head's output BEFORE its final activation, (C,H,W) order (the
+        first fully connected layer's backward applies act' of `feat`).  Writes the conv weight / bias gradients of this
+        minibatch into model.grads.  Needs the activations of the last forward() on the same rows."""
+        M = dfeat.shape[0]
+        none = ops.ACT["none"]
+        params, grads = self.model.conv_params(), self.model.conv_params(grads=True)
+        li = len(params)
+        _ci, _h, _w, co, hp, wp, _b = self.stages[-1]
+        gi = 0                                                        # ping-pong index of the current gradient
+        g = self._view(self.g[gi], M * hp * wp, co)
+        ops.permute_bpc(dfeat, g, M, hp * wp, co, False)
+        for s in range(len(self.stages) - 1, -1, -1):
+            ci, h, w, co, hp, wp, blocks = self.stages[s]
+            rows = M * hp * wp
+            col = self._view(self.col, rows, co * 9)
+            for j in range(blocks - 1, -1, -1):
+                li -= 2
+                (Wa, _), (Wb, _) = params[li], params[li + 1]
+                (gWa, gba), (gWb, gbb) = grads[li], grads[li + 1]
+                xj, aj = self.x[s][j][:rows], self.a[s][j][:rows]
+                dza = self._view(self.g[2], rows, co)
+                # conv_b: dW = g^T im2col(act(a)), db = colsum(g), d(col) = g W (in place of col), then act'(a)
+                ops.colsum(g, gbb, self.colsum_ws)
+                ops.im2col_pad_act(aj, False, M, co, hp, wp, 3, 1, 1, self.act, col)
+                ops.linear_backward(g, col, Wb.view(co, co * 9), none, gWb.view(co, co * 9), col, None, self.engine,
+                                    self.lin_ws)
+                ops.col2im_pad_act_backward(col, aj, True, None, M, co, hp, wp, 3, 1, 1, self.act, dza)
+                # conv_a on act(x_j): dx_j = col2im(dcol) * act'(x_j) + g (identity path)
+                ops.colsum(dza, gba, self.colsum_ws)
+                ops.im2col_pad_act(xj, False, M, co, hp, wp, 3, 1, 1, self.act, col)
+                ops.linear_backward(dza, col, Wa.view(co, co * 9), none, gWa.view(co, co * 9), col, None, self.engine,
+                                    self.lin_ws)
+                gn = self._view(self.g[1 - gi], rows, co)
+                ops.col2im_pad_act_backward(col, xj, True, g, M, co, hp, wp, 3, 1, 1, self.act, gn)
+                g, gi = gn, 1 - gi
+            # max-pool, then the stage-entry conv
+            li -= 1
+            W, _ = params[li]
+            gW, gb = grads[li]
+            dz = self._view(self.z, M * h * w, co)
+            ops.maxpool3s2_backward(g, self.idx[s][:rows], M, co, h, w, dz)
+            ops.colsum(dz, gb, self.colsum_ws)
+            col = self._view(self.col, M * h * w, ci * 9)
+            if s > 0:
+                prev = self.x[s - 1][-1][: M * h * w]
+                ops.im2col_pad_act(prev, False, M, ci, h, w, 3, 1, 1, none, col)
+                ops.linear_backward(dz, col, W.view(co, ci * 9), none, gW.view(co, ci * 9), col, None, self.engine,
+                                    self.lin_ws)
+                gn = self._view(self.g[1 - gi], M * h * w, ci)
+                ops.col2im_pad_act_backward(col, prev, False, None, M, ci, h, w, 3, 1, 1, none, gn)
+                g, gi = gn, 1 - gi
+            else:
+                ops.im2col_pad_act(self.x_in, True, M, ci, h, w, 3, 1, 1, none, col)
+                ops.linear_backward(dz, col, W.view(co, ci * 9), none, gW.view(co, ci * 9), None, None, self.engine,
+                                    self.lin_ws)

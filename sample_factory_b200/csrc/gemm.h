@@ -10,6 +10,9 @@ constexpr int SFB_TC_UNSUPPORTED = -1000;   // shape/alignment not handled by th
 // wgmma engine (gemm_tc.cu). Return 0, an error code, or SFB_TC_UNSUPPORTED.
 int tc_linear_act_forward(const float* x, int64_t ldx, const float* W, const float* b, float* y, int64_t ldy, int64_t M,
                           int N, int K, int act, int engine, cudaStream_t st);
+// y = (x W^T + b) + r (residual epilogue, TcEpilogue mode 3)
+int tc_linear_residual_forward(const float* x, int64_t ldx, const float* W, const float* b, const float* r, int64_t ldr,
+                               float* y, int64_t ldy, int64_t M, int N, int K, int engine, cudaStream_t st);
 int tc_linear_heads_partials(int N, int A, int engine);
 struct HeadsFinish;   // heads_tail.cuh
 // fin + fin_counters (both optional): the kernel also finishes the heads (see TcEpilogue::fin_counters in gemm_tc.cu)

@@ -10,7 +10,7 @@ namespace sfb {
 constexpr int BM = 128, BN = 128, BK = 16, LDS = BM + 4;
 
 struct Epilogue {
-    int mode;            // 0: plain store, 1: act(acc + bias[n]), 2: acc * act'(aux[m,n])
+    int mode;            // 0: plain store, 1: act(acc + bias[n]), 2: acc * act'(aux[m,n]), 3: acc + bias[n] + aux[m,n]
     int act;
     const float* bias;   // [N]
     const float* aux;    // [M, ld_aux]
@@ -20,6 +20,7 @@ struct Epilogue {
 __device__ __forceinline__ float apply_epilogue(float acc, int64_t m, int n, const Epilogue& e) {
     if (e.mode == 1) return act_fwd(acc + (e.bias ? e.bias[n] : 0.f), e.act);
     if (e.mode == 2) return acc * act_bwd_from_out(e.aux[m * e.ld_aux + n], e.act);
+    if (e.mode == 3) return (acc + e.bias[n]) + e.aux[m * e.ld_aux + n];
     return acc;
 }
 
@@ -215,6 +216,19 @@ int choose_splits(int64_t M, int N, int K) {
 int gemm_simt(bool a_kcont, const float* A, int64_t lda, bool b_kcont, const float* B, int64_t ldb, float* C, int64_t ldc,
               int64_t M, int N, int K, int splits, const Epilogue& epi, float* ws, cudaStream_t st) {
     if (M == 0 || N == 0) return 0;
+    // grid.y holds the 128-row blocks (<= 65535): taller outputs (im2col rows of a conv over many frames) run in row slabs
+    constexpr int64_t kMaxRows = 65535LL * BM;
+    if (M > kMaxRows && splits == 1) {
+        for (int64_t m0 = 0; m0 < M; m0 += kMaxRows) {
+            Epilogue e = epi;
+            if (e.aux) e.aux += m0 * e.ld_aux;
+            const float* Am = a_kcont ? A + m0 * lda : A + m0;
+            const int rc = gemm_simt(a_kcont, Am, lda, b_kcont, B, ldb, C + m0 * ldc, ldc,
+                                     (M - m0 < kMaxRows) ? M - m0 : kMaxRows, N, K, 1, e, ws, st);
+            if (rc) return rc;
+        }
+        return 0;
+    }
     SFB_CHECK_ARG(ceil_div(M, BM) <= 65535, "gemm_simt: M too large (%lld)", (long long)M);
     const bool a_vec = (lda % 4 == 0) && aligned16(A) && (a_kcont || true);
     const bool b_vec = (ldb % 4 == 0) && aligned16(B);
@@ -295,6 +309,18 @@ int sfb200_linear_act_forward(const float* x, int64_t ldx, const float* W, const
         // shape not covered by the tensor-core engine: exact-fp32 CUDA-core tiles (still on device)
     }
     Epilogue epi{1, act, b, nullptr, 0};
+    return gemm_simt(true, x, ldx, true, W, K, y, ldy, M, N, K, 1, epi, nullptr, st);
+}
+
+int sfb200_linear_residual_forward(const float* x, int64_t ldx, const float* W, const float* b, const float* r,
+                                   int64_t ldr, float* y, int64_t ldy, int64_t M, int N, int K, int engine, void* stream) {
+    SFB_CHECK_ARG(x && W && b && r && y && M >= 0 && N > 0 && K > 0, "linear_residual_forward: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (engine != SFB200_GEMM_SIMT_FP32) {
+        int rc = tc_linear_residual_forward(x, ldx, W, b, r, ldr, y, ldy, M, N, K, engine, st);
+        if (rc != SFB_TC_UNSUPPORTED) return rc;
+    }
+    Epilogue epi{3, SFB200_ACT_NONE, b, r, ldr};
     return gemm_simt(true, x, ldx, true, W, K, y, ldy, M, N, K, 1, epi, nullptr, st);
 }
 

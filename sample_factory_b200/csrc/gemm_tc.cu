@@ -35,7 +35,8 @@ namespace sfb {
 // F16: the fp16-split engine (A K-major with a registered bound |A| <= a_bound[0], B a weight matrix with |w| < 255):
 // A * 2^a_shift and B * 2^kF16WShift are split into fp16 hi + lo * 2^-11 pairs (22 significand bits like the tf32
 // pair, on the fp16 MMA path at twice the tf32 rate); a stage then covers 64 k.
-template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false>
+// RES: the residual epilogue (store_tile_residual), forward layout only.
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false, bool RES = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
@@ -180,6 +181,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 if (ct == 0) epi.fin_counters[mb] = 0;
             }
         }
+    } else if constexpr (RES) {
+        store_tile_residual(acc, tc, row_base, lane, C, ldc, M, N, epi);
     } else {
         float* Cz = C + (splits > 1 ? (int64_t)tc.z * M * ldc : 0);
         store_tile(acc, tc, row_base, lane, Cz, ldc, M, N, splits == 1 ? epi.mode : 0, epi);
@@ -249,10 +252,10 @@ static bool operand_ok(const float* p, int64_t ld) {
     return ((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && (ld % 4 == 0) && ld > 0;
 }
 
-template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS = false, bool F16 = false>
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS = false, bool F16 = false, bool RES = false>
 static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, int64_t M, int N, int K,
                      int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr) {
-    auto kern = gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16>;
+    auto kern = gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES>;
     static bool attr_set = false;
     if (!attr_set) {
         SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem::TOTAL));
@@ -274,7 +277,7 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
     // fp16-split engine: A is a K-major activation buffer with a registered bound, B a weight matrix with registered fp16
     // twins (the transposed twins when B is read MN-major, i.e. dX = dz . W: both registrations say that |w| < 255),
     // K a multiple of the 64-k stage
-    if (!a_mn && split3 && splits == 1 && K % 64 == 0 && f16_enabled()) {
+    if (!a_mn && split3 && splits == 1 && K % 64 == 0 && f16_enabled() && epi.mode != 3) {
         const float* a_bound = operand_bound_lookup(A, ((int64_t)(M - 1) * lda + K) * (int64_t)sizeof(float));
         F16Twin tw{nullptr, nullptr};
         if (a_bound) {
@@ -318,6 +321,11 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
     const int64_t ld_out = splits > 1 ? N : ldc;
 
     int rc;
+    if (epi.mode == 3) {
+        if (a_mn || b_mn || splits != 1) return SFB_TC_UNSUPPORTED;
+        return split3 ? launch_tc<false, false, true, false, false, true>(ta, tb, C, ldc, M, N, K, K, 1, epi, st)
+                      : launch_tc<false, false, false, false, false, true>(ta, tb, C, ldc, M, N, K, K, 1, epi, st);
+    }
     if (epi.head_part) {
         if (a_mn || b_mn || splits != 1) return SFB_TC_UNSUPPORTED;
         rc = split3 ? launch_tc<false, false, true, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st)
@@ -340,6 +348,12 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
 int tc_linear_act_forward(const float* x, int64_t ldx, const float* W, const float* b, float* y, int64_t ldy, int64_t M,
                           int N, int K, int act, int engine, cudaStream_t st) {
     TcEpilogue epi{1, act, b, nullptr, 0};
+    return gemm_tc(false, x, ldx, false, W, K, y, ldy, M, N, K, 1, epi, nullptr, engine == SFB200_GEMM_TC_3XTF32, st);
+}
+
+int tc_linear_residual_forward(const float* x, int64_t ldx, const float* W, const float* b, const float* r, int64_t ldr,
+                               float* y, int64_t ldy, int64_t M, int N, int K, int engine, cudaStream_t st) {
+    TcEpilogue epi{3, SFB200_ACT_NONE, b, r, ldr};
     return gemm_tc(false, x, ldx, false, W, K, y, ldy, M, N, K, 1, epi, nullptr, engine == SFB200_GEMM_TC_3XTF32, st);
 }
 

@@ -10,7 +10,7 @@
 namespace sfb {
 
 struct TcEpilogue {
-    int mode;            // 0 plain, 1 act(acc + bias[n]), 2 acc * act'(aux[m,n])
+    int mode;            // 0 plain, 1 act(acc + bias[n]), 2 acc * act'(aux[m,n]), 3 residual (store_tile_residual)
     int act;
     const float* bias;
     const float* aux;
@@ -162,6 +162,22 @@ __device__ __forceinline__ void store_tile(const float (&acc)[64], const TileCoo
             dst[0] = v0;
             if (two) dst[1] = v1;
         }
+    }
+}
+
+// Residual epilogue (a ResBlock's second conv plus its identity path, model/encoder.py:166-169): C = (acc + bias[n]) +
+// aux[m, n].  A separate instantiation (gemm_wgmma_kernel<..., RES = true>), so the other epilogues keep their code.
+__device__ __forceinline__ void store_tile_residual(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane,
+                                                    float* C, int64_t ldc, int64_t M, int N, const TcEpilogue& epi) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        const int64_t m = row_base + 8 * (j & 1);
+        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
+        if (m >= M || n >= N) continue;
+        const float* r = epi.aux + m * epi.ld_aux + n;
+        float* dst = C + m * ldc + n;
+        dst[0] = (acc[2 * j] + epi.bias[n]) + r[0];
+        if (n + 1 < N) dst[1] = (acc[2 * j + 1] + epi.bias[n + 1]) + r[1];
     }
 }
 

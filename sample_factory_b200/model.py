@@ -64,16 +64,56 @@ class ModelSpec:
             return []
         c, h, w = self.obs_shape
         out = []
+        if self.is_resnet:
+            return out      # described by resnet_stages
         for (co, k, s) in self.CONV_ARCH[self.encoder_conv_architecture]:
             ho, wo = (h - k) // s + 1, (w - k) // s + 1
             out.append((c, h, w, co, k, s, ho, wo))
             c, h, w = co, ho, wo
         return out
 
+    RESNET_STAGES = [(16, 2), (32, 2), (32, 2)]   # model/encoder.py:182 (resnet_impala): (channels, res blocks)
+
+    @property
+    def is_resnet(self) -> bool:
+        return self.obs_shape is not None and self.encoder_conv_architecture == "resnet_impala"
+
+    @property
+    def resnet_stages(self) -> List[Tuple[int, int, int, int, int, int, int]]:
+        """[(C_in, H, W, C_out, H_pool, W_pool, blocks)] of the ResnetEncoder (encoder.py:173-221): per stage a 3x3 conv
+        with padding 1 (H x W kept), a 3x3 / stride 2 / padding 1 max-pool (-> ceil(H/2) x ceil(W/2)) and `blocks`
+        residual blocks of two 3x3 convs at C_out channels"""
+        c, h, w = self.obs_shape
+        out = []
+        for (co, blocks) in self.RESNET_STAGES:
+            hp, wp = (h + 1) // 2, (w + 1) // 2
+            out.append((c, h, w, co, hp, wp, blocks))
+            c, h, w = co, hp, wp
+        return out
+
     @property
     def conv_out_size(self) -> int:
+        if self.is_resnet:
+            _c, _h, _w, co, hp, wp, _b = self.resnet_stages[-1]
+            return co * hp * wp
         c, _, _, co, _, _, ho, wo = self.conv_layers[-1]
         return co * ho * wo
+
+    def conv_param_layout(self) -> List[Tuple[str, Tuple[int, int, int, int]]]:
+        """[(reference state_dict prefix, weight shape)] of the conv head's Conv2d layers in parameters() order.
+        ResnetEncoder: conv_head.{j} is a stage's entry conv, conv_head.{j}.res_block_core.{1,3} the two convs of a block
+        (Sequential indices of encoder.py:157-162 / 188-202)."""
+        if not self.is_resnet:
+            return [(f"encoder.encoders.obs.enc.conv_head.{2 * i}", (co, ci, k, k))
+                    for i, (ci, _h, _w, co, k, _s, _ho, _wo) in enumerate(self.conv_layers)]
+        out, j = [], 0
+        for (ci, _h, _w, co, _hp, _wp, blocks) in self.resnet_stages:
+            out.append((f"encoder.encoders.obs.conv_head.{j}", (co, ci, 3, 3)))
+            j += 2
+            for _ in range(blocks):
+                out += [(f"encoder.encoders.obs.conv_head.{j}.res_block_core.{r}", (co, co, 3, 3)) for r in (1, 3)]
+                j += 1
+        return out
 
     @property
     def fc_encoder_layers(self) -> List[int]:
@@ -85,6 +125,8 @@ class ModelSpec:
         return self.conv_out_size if self.obs_shape is not None else self.obs_dim
 
     def fc_encoder_name(self, i: int, what: str) -> str:
+        if self.is_resnet:      # ResnetEncoder keeps its mlp_layers directly (no `.enc.` wrapper, encoder.py:208)
+            return f"encoder.encoders.obs.mlp_layers.{2 * i}.{what}"
         if self.obs_shape is not None:
             return f"encoder.encoders.obs.enc.mlp_layers.{2 * i}.{what}"
         return f"encoder.encoders.obs.mlp_head.{2 * i}.{what}"
@@ -178,9 +220,9 @@ class ModelSpec:
             out.append(("action_parameterization.distribution_linear.weight", (self.num_linear_action_outputs, d)))
             out.append(("action_parameterization.distribution_linear.bias", (self.num_linear_action_outputs,)))
             return out
-        for i, (ci, _h, _w, co, k, _s, _ho, _wo) in enumerate(self.conv_layers):
-            out.append((f"encoder.encoders.obs.enc.conv_head.{2 * i}.weight", (co, ci, k, k)))
-            out.append((f"encoder.encoders.obs.enc.conv_head.{2 * i}.bias", (co,)))
+        for prefix, wshape in self.conv_param_layout():
+            out.append((f"{prefix}.weight", wshape))
+            out.append((f"{prefix}.bias", (wshape[0],)))
         d = self.fc_encoder_input
         for i, h in enumerate(self.fc_encoder_layers):
             out.append((self.fc_encoder_name(i, "weight"), (h, d)))
@@ -429,10 +471,9 @@ class PolicyModel:
         self.Wa_cat[:, :H].copy_(self.params["action_parameterization.distribution_linear.weight"])
 
     def conv_params(self, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
-        """[(W [C_out, C_in, k, k], b [C_out])] of the conv head"""
+        """[(W [C_out, C_in, k, k], b [C_out])] of the conv head, in ModelSpec.conv_param_layout() order"""
         src = self.grads if grads else self.params
-        return [(src[f"encoder.encoders.obs.enc.conv_head.{2 * i}.weight"], src[f"encoder.encoders.obs.enc.conv_head.{2 * i}.bias"])
-                for i in range(len(self.spec.conv_layers))]
+        return [(src[f"{p}.weight"], src[f"{p}.bias"]) for p, _ in self.spec.conv_param_layout()]
 
     def decoder_layers(self, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
         src = self.grads if grads else self.params

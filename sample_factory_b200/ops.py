@@ -265,6 +265,51 @@ def permute_bpc(src: Tensor, dst: Tensor, B: int, P: int, C: int, to_channel_maj
     lib().call("sfb200_permute_bpc", _p(src, F32), _p(dst, F32), B, P, C, int(to_channel_major), _stream())
 
 
+def im2col_pad_act(x: Tensor, in_nchw: bool, B: int, C: int, H: int, W: int, kernel: int, stride: int, pad: int, act: int,
+                   col: Tensor) -> None:
+    """col = im2col(act(x)) with `pad` zeros around the activated input (Conv2d(act(x), padding=pad))"""
+    assert x.is_contiguous() and col.is_contiguous()
+    lib().call("sfb200_im2col_pad_act", _p(x, F32), int(in_nchw), B, C, H, W, kernel, stride, pad, act, _p(col, F32),
+               _stream())
+
+
+def col2im_pad_act_backward(dcol: Tensor, x_act: Tensor, from_input: bool, dres: Optional[Tensor], B: int, C: int, H: int,
+                            W: int, kernel: int, stride: int, pad: int, act: int, dx: Tensor) -> None:
+    """dx [B*H*W, C] (NHWC) = col2im(dcol) * act'(x_act) (+ dres); act' from the activation's output or (from_input) input"""
+    assert dcol.is_contiguous() and x_act.is_contiguous() and dx.is_contiguous()
+    assert dres is None or (dres.is_contiguous() and dres.data_ptr() != dx.data_ptr())
+    lib().call("sfb200_col2im_pad_act_backward", _p(dcol, F32), _p(x_act, F32), int(from_input), _p(dres, F32), B, C, H, W,
+               kernel, stride, pad, act, _p(dx, F32), _stream())
+
+
+def maxpool3s2_forward(x: Tensor, B: int, C: int, H: int, W: int, y: Tensor, idx: Tensor) -> None:
+    """MaxPool2d(3, stride 2, padding 1) on NHWC rows: y, idx (uint8 window position of the maximum) [B*ceil(H/2)*ceil(W/2), C]"""
+    assert x.is_contiguous() and y.is_contiguous() and idx.is_contiguous()
+    lib().call("sfb200_maxpool3s2_forward", _p(x, F32), B, C, H, W, _p(y, F32), _p(idx, BYTE), _stream())
+
+
+def maxpool3s2_backward(dy: Tensor, idx: Tensor, B: int, C: int, H: int, W: int, dx: Tensor) -> None:
+    assert dy.is_contiguous() and idx.is_contiguous() and dx.is_contiguous()
+    lib().call("sfb200_maxpool3s2_backward", _p(dy, F32), _p(idx, BYTE), B, C, H, W, _p(dx, F32), _stream())
+
+
+def act_permute_bpc(src: Tensor, dst: Tensor, B: int, P: int, C: int, act: int) -> None:
+    """dst [B, C, P] = act(src [B, P, C])"""
+    assert src.is_contiguous() and dst.is_contiguous()
+    lib().call("sfb200_act_permute_bpc", _p(src, F32), _p(dst, F32), B, P, C, act, _stream())
+
+
+def linear_residual_forward(x: Tensor, W: Tensor, b: Tensor, r: Tensor, out: Tensor, engine: int) -> Tensor:
+    """out = x W^T + b + r  (r read in the GEMM epilogue)"""
+    M, K = x.shape
+    N = W.shape[0]
+    assert W.shape[1] == K and W.is_contiguous() and out.shape == (M, N) and r.shape == (M, N)
+    assert r.data_ptr() != out.data_ptr()
+    lib().call("sfb200_linear_residual_forward", _p(x, F32), x.stride(0), _p(W, F32), _p(b, F32), _p(r, F32), r.stride(0),
+               _p(out, F32), out.stride(0), M, N, K, engine, _stream())
+    return out
+
+
 def register_tf32_lo(base: Tensor, lo: Tensor) -> None:
     """Pair a flat weight buffer with its tf32 low-half twin (see include/sfb200.h) and fill the twin."""
     assert base.is_contiguous() and lo.is_contiguous() and base.numel() == lo.numel()

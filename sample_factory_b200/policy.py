@@ -27,9 +27,9 @@ class HeadsPlan:
         spec = model.spec
         self.conv = None
         if spec.obs_shape is not None:
-            from .conv_encoder import ConvHead
+            from .conv_encoder import ConvHead, ResnetHead
 
-            self.conv = ConvHead(model, engine, max_rows, need_backward)
+            self.conv = (ResnetHead if spec.is_resnet else ConvHead)(model, engine, max_rows, need_backward)
         self.tail_is_mlp = bool(spec.decoder_mlp_layers) or (not spec.use_rnn and bool(spec.fc_encoder_layers))
         # separate actor / critic weights: per-tower activations and ONE concatenated tail [rows, 2H] = [actor | critic]
         self.separate = not spec.share_weights
