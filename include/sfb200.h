@@ -49,15 +49,6 @@ int sfb200_set_device(int device);
 int sfb200_sm_count(void);
 /* 1 if the wgmma/TMA GEMM engine is usable in this process (sm_90 device, driver entry points resolved), else 0 */
 int sfb200_tc_available(void);
-/* Low tf32 halves of the weights for the 3xTF32 engine.  register: marks [base, base+n) as model weights with a twin
- * `lo` (same offsets) of their low tf32 halves, which sfb200_clip_adam_step keeps current; the fused policy step and the
- * persistent rollout cover a model only when both its weight matrices are registered (the kernels split the fp32 weights
- * themselves).  Any other write
- * to the weights (checkpoint load, weight copy) must be followed by sfb200_refresh_tf32_lo(base).  With the
- * environment variable SFB200_CHECK_LO=1 every use verifies the pair on the device and traps on a stale `lo`. */
-int sfb200_register_tf32_lo(const float* base, float* lo, int64_t n);
-int sfb200_unregister_tf32_lo(const float* base);
-int sfb200_refresh_tf32_lo(const float* base, void* stream);
 /* The fp16-split form of the same 3-pass engine (fp32 accuracy class of 3xTF32 -- 22 significand bits per operand --
  * on the fp16 wgmma path: twice the k per instruction).  A 3xTF32 GEMM takes it when
  *   (1) its WEIGHT operand lies inside a buffer with registered fp16 twins: twins = [hi16[n] | lo16[n]],
@@ -243,11 +234,10 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
  * sfb200_sampler_pre_step for step 0 first (x_norm holds the normalised step-0 observations).  Pointers with suffix _0 are
  * the trajectory slots of step 0 ([:, 0]); step t is at + t elements (x A for logits, x dim for traj_obs / rnn rows).
  *   P = sfb200_rollout_mlp2_partials(...)   0 -> not covered (3xTF32 engine, K1 in {32,64,96,128}, H1 == H2 in {128,256,512},
- *       A <= 8, both weight matrices inside a registered tf32-lo buffer); head_partials: P * n_envs * 12 floats,
- *       h1_scratch: n_envs * H1 floats. */
+ *       A <= 8, W1 and W2 16-byte aligned); head_partials: P * n_envs * 12 floats, h1_scratch: n_envs * H1 floats. */
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine);
-/* debug aid: device buffer of T x 16 uint64 that the following rollouts fill with %globaltimer stamps of one CTA's phases
- * (tools/rollout_trace.py); NULL switches it off */
+/* debug aid: device buffer of T x 16 uint64 that the following rollouts fill with %globaltimer stamps of one CTA's phases;
+ * NULL switches it off */
 int sfb200_rollout_set_trace(void* trace_dev);
 int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, const float* b1, int H1, const float* W2,
                              const float* b2, int H2, int act, int engine, const float* Wv, const float* bv, const float* Wa,
@@ -265,16 +255,6 @@ int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, con
                              int64_t traj_obs_stride, const float* rnn, int rnn_dim, float* traj_rnn_0, int64_t traj_rnn_stride,
                              const double* mean, const double* var, float sub_mean, float inv_scale, float eps, float clip,
                              void* stream);
-/* The whole policy forward of a two-layer MLP (model/encoder.py:72-91 MlpEncoder + actor_critic.py:171-186) up to the head
- * partials in ONE wgmma kernel: h1 = act(x W1^T + b1) is produced chunk by chunk in shared memory and consumed by the
- * layer-2 MMAs without ever reaching global memory; h2 = act(h1 W2^T + b2) is contracted with [Wv ; Wa] in the
- * epilogue (not stored).  Same partial format as sfb200_linear_act_heads_forward -> finish with sfb200_heads_from_partials.
- *   P = sfb200_policy_mlp2_partials(W1, W2, K1, H1, H2, A, engine)   0 -> not covered (needs the 3xTF32 engine, K1 in
- *       {32, 64}, H1 % 32 == 0, H2 % 128 == 0 and <= 512, A <= 8, both weight matrices inside a registered tf32-lo buffer) */
-int sfb200_policy_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine);
-int sfb200_policy_mlp2_heads_forward(const float* x, int64_t ldx, int64_t M, int K1, const float* W1, const float* b1, int H1,
-                                     const float* W2, const float* b2, int H2, int act, int engine, const float* Wv,
-                                     const float* Wa, int A, float* head_partials, void* stream);
 int sfb200_heads_from_partials(const float* head_partials, int P, int64_t rows, int A, const float* bv, const float* ba,
                                float* values, int64_t values_stride, float* logits, int64_t logits_stride,
                                const float* noise, uint64_t philox_seed, uint64_t philox_offset,

@@ -12,7 +12,7 @@ struct AdamArgs {
     double lr; const double* lr_dev; double beta1, beta2; int64_t step_host; const int64_t* step_dev;
     float omb1, beta2f, omb2, eps, max_norm;
     const double* lr_num; const double* lr_den;
-    float* grad_norm_out; float* p_lo;
+    float* grad_norm_out;
     uint16_t* p_hi16; int64_t lo16_offset;      // registered fp16 twins of the parameters (api.cu), or NULL
 };
 
@@ -22,7 +22,7 @@ static inline AdamArgs make_adam_args(float* p, const float* g, float* m, float*
                                       float* grad_norm_out) {
     AdamArgs a{p, g, m, v, n, lr, lr_dev, beta1, beta2, step, step_dev,
                (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, (float)max_grad_norm,
-               lr_scale_num, lr_scale_den, grad_norm_out, tf32_lo_lookup_mut(p, n), nullptr, 0};
+               lr_scale_num, lr_scale_den, grad_norm_out, nullptr, 0};
     a.p_hi16 = f16_twin_lookup_mut(p, n, &a.lo16_offset);
     return a;
 }
@@ -62,8 +62,7 @@ __device__ __forceinline__ void clip_adam_body(const AdamArgs& a, const double* 
         const float denom = __fdiv_rn(__fsqrt_rn(vi), bc2_sqrt) + a.eps;
         const float pn = a.p[i] - step_size * __fdiv_rn(mi, denom);   // param.addcdiv_(exp_avg, denom, value=-step_size)
         a.p[i] = pn;
-        if (a.p_lo) a.p_lo[i] = __uint_as_float(tf32_lo_bits(__float_as_uint(pn)));   // registered tf32 low half stays current
-        if (a.p_hi16) f16_split1(pn * (float)(1 << kF16WShift), a.p_hi16[i], a.p_hi16[i + a.lo16_offset]);   // and the fp16 twins
+        if (a.p_hi16) f16_split1(pn * (float)(1 << kF16WShift), a.p_hi16[i], a.p_hi16[i + a.lo16_offset]);   // fp16 twins stay current
         a.m[i] = mi;
         a.v[i] = vi;
     }

@@ -19,23 +19,6 @@ void set_error(const char* fmt, ...) {
     va_end(ap);
 }
 
-struct LoRange {
-    const float* base;
-    float* lo;
-    int64_t n;
-};
-static LoRange g_lo[32];
-static int g_lo_n = 0;
-
-float* tf32_lo_lookup_mut(float* p, int64_t count) {
-    for (int i = 0; i < g_lo_n; ++i) {
-        const LoRange& r = g_lo[i];
-        if (p >= r.base && p + count <= r.base + r.n) return r.lo + (p - r.base);
-    }
-    return nullptr;
-}
-const float* tf32_lo_lookup(const float* p, int64_t count) { return tf32_lo_lookup_mut(const_cast<float*>(p), count); }
-
 // ---- fp16 twins of weight buffers, their transposed per-matrix copies, activation bounds (the fp16-split GEMM engine)
 struct F16Range { const float* base; uint16_t* twins; int64_t n; };            // twins = [hi16[n] | lo16[n]]
 struct F16TRange { const float* W; int N, K; uint16_t* twins; };               // twins = [hiT[K][N] | loT[K][N]]
@@ -168,29 +151,6 @@ __global__ void __launch_bounds__(256) heads_dz_bound_kernel(const float* __rest
     }
 }
 
-bool tf32_lo_check_enabled() {
-    static int v = -1;
-    if (v < 0) {
-        const char* e = getenv("SFB200_CHECK_LO");
-        v = (e && e[0] == '1') ? 1 : 0;
-    }
-    return v == 1;
-}
-
-__global__ void tf32_split_lo_kernel(const float* __restrict__ w, float* __restrict__ lo, int64_t n) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        lo[i] = __uint_as_float(tf32_lo_bits(__float_as_uint(w[i])));
-}
-
-__global__ void tf32_check_lo_kernel(const float* __restrict__ w, const float* __restrict__ lo, int64_t n) {
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        if (__float_as_uint(lo[i]) != tf32_lo_bits(__float_as_uint(w[i]))) {
-            printf("libsfb200: STALE tf32 lo buffer at element %lld (call sfb200_refresh_tf32_lo after writing weights)\n",
-                   (long long)i);
-            __trap();
-        }
-}
-
 // SFB200_CHECK_F16=1 verifies fp16 twins (row-major: ld = K; transposed: element (n, k) at k * N + n) before every use
 __global__ void f16_check_twins_kernel(const float* __restrict__ W, const uint16_t* __restrict__ hi, const uint16_t* __restrict__ lo,
                                        int N, int K, int transposed) {
@@ -211,14 +171,6 @@ int f16_twins_check(const float* W, F16Twin tw, int N, int K, bool transposed, c
     int64_t blocks = ceil_div((int64_t)N * K, 256);
     if (blocks > 1024) blocks = 1024;
     f16_check_twins_kernel<<<(unsigned)blocks, 256, 0, st>>>(W, tw.hi, tw.lo, N, K, transposed ? 1 : 0);
-    SFB_LAUNCH_OK();
-    return 0;
-}
-
-int tf32_lo_check(const float* w, const float* lo, int64_t count, cudaStream_t st) {
-    int64_t blocks = ceil_div(count, 256);
-    if (blocks > 1024) blocks = 1024;
-    tf32_check_lo_kernel<<<(unsigned)blocks, 256, 0, st>>>(w, lo, count);
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -258,41 +210,6 @@ int sfb200_set_device(int device) {
 }
 
 int sfb200_sm_count(void) { return sfb::sm_count(); }
-
-int sfb200_register_tf32_lo(const float* base, float* lo, int64_t n) {
-    SFB_CHECK_ARG(base && lo && n > 0, "register_tf32_lo: bad arguments");
-    for (int i = 0; i < sfb::g_lo_n; ++i)
-        if (sfb::g_lo[i].base == base) {
-            sfb::g_lo[i] = sfb::LoRange{base, lo, n};
-            return 0;
-        }
-    SFB_CHECK_ARG(sfb::g_lo_n < 32, "register_tf32_lo: table full");
-    sfb::g_lo[sfb::g_lo_n++] = sfb::LoRange{base, lo, n};
-    return 0;
-}
-
-int sfb200_unregister_tf32_lo(const float* base) {
-    for (int i = 0; i < sfb::g_lo_n; ++i)
-        if (sfb::g_lo[i].base == base) {
-            sfb::g_lo[i] = sfb::g_lo[--sfb::g_lo_n];
-            return 0;
-        }
-    return 0;
-}
-
-int sfb200_refresh_tf32_lo(const float* base, void* stream) {
-    for (int i = 0; i < sfb::g_lo_n; ++i)
-        if (sfb::g_lo[i].base == base) {
-            const sfb::LoRange& r = sfb::g_lo[i];
-            int64_t blocks = sfb::ceil_div(r.n, 256);
-            if (blocks > 1184) blocks = 1184;
-            sfb::tf32_split_lo_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(r.base, r.lo, r.n);
-            SFB_LAUNCH_OK();
-            return 0;
-        }
-    sfb::set_error("refresh_tf32_lo: buffer is not registered");
-    return 1;
-}
 
 int sfb200_register_f16_twins(const float* base, void* twins, int64_t n) {
     SFB_CHECK_ARG(base && twins && n > 0, "register_f16_twins: bad arguments");

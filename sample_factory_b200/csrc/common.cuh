@@ -40,13 +40,6 @@ void count_launch();   // every kernel launch of this library is counted (sfb200
     } while (0)
 
 int sm_count();
-// Registered "tf32 low halves" of weight buffers (api.cu): for a pointer range [p, p+count) inside a registered buffer,
-// the matching range of lo = ((w - (w & ~0x1fff)) & ~0x1fff) words, else NULL.  The 3xTF32 GEMM then takes the weight
-// operand's lo tile straight from HBM/L2 by TMA instead of splitting it in shared memory for every tile.
-const float* tf32_lo_lookup(const float* p, int64_t count);
-float* tf32_lo_lookup_mut(float* p, int64_t count);
-int tf32_lo_check(const float* w, const float* lo, int64_t count, cudaStream_t st);   // SFB200_CHECK_LO=1: trap if stale
-bool tf32_lo_check_enabled();
 // Registered fp16 twins of weight buffers (api.cu): [hi16[n] | lo16[n]] with hi = fp16(w * 2^kF16WShift),
 // lo = fp16((w * 2^kF16WShift - hi) * 2^kF16LoShift) -- the weight operand of the fp16-split GEMM (gemm_tc.cu, "F16" kernel).
 struct F16Twin { const uint16_t* hi; const uint16_t* lo; };

@@ -237,8 +237,8 @@ static bool f16_enabled() {
     return v == 1;
 }
 
-// SFB200_CHECK_F16=1: verify registered fp16 twins against the weights on the device before every use (debugging aid, like
-// SFB200_CHECK_LO for the tf32 twins): the twins are what selects the fp16-split form, so a stale registration shows here
+// SFB200_CHECK_F16=1: verify registered fp16 twins against the weights on the device before every use (debugging aid):
+// the twins are what selects the fp16-split form, so a stale registration shows here
 bool f16_check_enabled() {
     static int v = -1;
     if (v < 0) {

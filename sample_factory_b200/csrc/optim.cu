@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(256) clip_adam_kernel(const AdamArgs a, const 
 //   stage 1: m, v <- moments(g * clip_coef);  u = m_hat / (sqrt(v_hat) + eps) + wd * p  (written over g);
 //            per-(tensor, chunk) partial sums of p^2 and u^2
 //   stage 2: one warp per tensor: trust = clamp(min(|p|, 10) / |u|, min_trust, 1/min_trust)  (1 if either norm is 0)
-//   stage 3: p -= lr * trust * u   (+ the registered tf32-lo twin)
+//   stage 3: p -= lr * trust * u
 constexpr int kLambChunk = 4096;   // elements per block
 
 __global__ void __launch_bounds__(256) lamb_stage1_kernel(const float* __restrict__ p, float* __restrict__ g,
@@ -119,7 +119,7 @@ __global__ void __launch_bounds__(256) lamb_stage3_kernel(float* __restrict__ p,
                                                           const int64_t* __restrict__ seg_n,
                                                           const float* __restrict__ trust, double lr,
                                                           const double* __restrict__ lr_num,
-                                                          const double* __restrict__ lr_den, float* __restrict__ p_lo) {
+                                                          const double* __restrict__ lr_den) {
     const int t_idx = blockIdx.y;
     const int64_t off = seg_off[t_idx], n = seg_n[t_idx];
     double lr_eff = lr;
@@ -128,9 +128,7 @@ __global__ void __launch_bounds__(256) lamb_stage3_kernel(float* __restrict__ p,
     const int64_t c0 = (int64_t)blockIdx.x * kLambChunk;
     for (int64_t i = c0 + threadIdx.x; i < n && i < c0 + kLambChunk; i += 256) {
         const int64_t j = off + i;
-        const float pn = p[j] - step * u[j];                            // p.add_(adam_step, alpha=-lr * trust_ratio)
-        p[j] = pn;
-        if (p_lo) p_lo[j] = __uint_as_float(tf32_lo_bits(__float_as_uint(pn)));
+        p[j] = p[j] - step * u[j];                                      // p.add_(adam_step, alpha=-lr * trust_ratio)
     }
 }
 
@@ -224,8 +222,7 @@ int sfb200_clip_lamb_step(float* p, float* g, float* m, float* v, int64_t n, con
     SFB_LAUNCH_OK();
     lamb_stage2_kernel<<<(unsigned)num_tensors, 32, 0, st>>>(part, seg_numel, chunks, (float)min_trust, trust);
     SFB_LAUNCH_OK();
-    lamb_stage3_kernel<<<grid, 256, 0, st>>>(p, g, seg_offsets, seg_numel, trust, lr, lr_scale_num, lr_scale_den,
-                                             tf32_lo_lookup_mut(p, n));
+    lamb_stage3_kernel<<<grid, 256, 0, st>>>(p, g, seg_offsets, seg_numel, trust, lr, lr_scale_num, lr_scale_den);
     SFB_LAUNCH_OK();
     return 0;
 }

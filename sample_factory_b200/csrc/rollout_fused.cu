@@ -215,7 +215,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                     store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
                     fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
                 } else {
-                    heads_tile<ACT, 2>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
+                    heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
                 }
                 RF_TRACE(3 + 4 * layer);
             }
@@ -410,13 +410,13 @@ static int launch_rollout(const CUtensorMap* tm, const RolloutArgs& a, int CX, c
     return 0;
 }
 
-// Covered: 3xTF32 engine, registered tf32-lo twins for both weight matrices (the model's own weights), K1 a multiple of 32
-// up to 128, H1 == H2 in {128, 256, 512}, <= 8 action outputs.
+// Covered: 3xTF32 engine, both weight matrices 16-byte aligned (TMA sources), K1 a multiple of 32 up to 128,
+// H1 == H2 in {128, 256, 512}, <= 8 action outputs.
 int tc_rollout_mlp2_supported(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine) {
     if (engine != SFB200_GEMM_TC_3XTF32 || !tc_init()) return 0;
     if (!(K1 == 32 || K1 == 64 || K1 == 96 || K1 == 128) || H1 != H2 || !(H2 == 128 || H2 == 256 || H2 == 512)) return 0;
     if (A < 1 || A + 1 > RF_HEAD_AP) return 0;
-    if (!tf32_lo_lookup(W1, (int64_t)H1 * K1) || !tf32_lo_lookup(W2, (int64_t)H2 * H1)) return 0;
+    if ((reinterpret_cast<uintptr_t>(W1) & 15u) || (reinterpret_cast<uintptr_t>(W2) & 15u)) return 0;
     return 2 * (H2 / 128);
 }
 
@@ -464,11 +464,6 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
             if (!ok) return SFB_TC_UNSUPPORTED;
             SFB_RF_LAUNCH(true)
         }
-    }
-    if (tf32_lo_check_enabled()) {
-        int rc = tf32_lo_check(W1, tf32_lo_lookup(W1, (int64_t)a.H1 * a.K1), (int64_t)a.H1 * a.K1, st);
-        if (!rc) rc = tf32_lo_check(W2, tf32_lo_lookup(W2, (int64_t)a.H2 * a.H1), (int64_t)a.H2 * a.H1, st);
-        if (rc) return rc;
     }
     CUtensorMap tm[4];
     bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, TBK, 128);

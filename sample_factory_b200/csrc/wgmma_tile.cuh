@@ -1,5 +1,5 @@
-// Device-side building blocks of the wgmma GEMM tiles shared by the GEMM engine (gemm_tc.cu), the fused two-layer
-// policy step (policy_step.cu) and the persistent rollout (rollout_fused.cu): operand split passes into the swizzled
+// Device-side building blocks of the wgmma GEMM tiles shared by the GEMM engine (gemm_tc.cu) and the persistent rollout
+// (rollout_fused.cu): operand split passes into the swizzled
 // K-major layout, tile coordinates and the register epilogues (bias + activation, activation derivative, head partials).
 // sm_90a only.
 #pragma once
@@ -184,12 +184,11 @@ __device__ __forceinline__ void store_tile_residual(const float (&acc)[64], cons
 // Epilogue with the policy/value heads folded in (forward layers feeding critic_linear / distribution_linear,
 // actor_critic.py:171-186): y = act(acc + bias) is formed in registers, optionally stored, and contracted with the (A+1)
 // head weight rows -- the separate heads kernel's re-read of y disappears.  Per 64-column half of the tile the four
-// threads of a quad hold a row's 64 values; a fixed-order quad reduction gives the partial.  NPART partials per tile
-// (2: per 64-column half, 4: per 32-column quarter).
-template <int ACT, int NPART = 2>
+// threads of a quad hold a row's 64 values; a fixed-order quad reduction gives the partial.  Two partials per tile.
+template <int ACT>
 __device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
                                            int64_t ldc, int64_t M, int N, const TcEpilogue& epi) {
-    constexpr int JP = 32 / NPART;   // accumulator pairs of a thread per partial (per 128 / NPART columns)
+    constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
         const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
@@ -198,9 +197,9 @@ __device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc
         const int64_t m = row_base + 8 * (j & 1);
         if (C && m < M) *reinterpret_cast<float2*>(C + m * ldc + n) = make_float2(acc[2 * j], acc[2 * j + 1]);
     }
-    const int p0 = (tc.n0 / TBN) * NPART;
+    const int p0 = (tc.n0 / TBN) * 2;
 #pragma unroll
-    for (int half = 0; half < NPART; ++half) {
+    for (int half = 0; half < 2; ++half) {
 #pragma unroll
         for (int rs = 0; rs < 2; ++rs) {
             float hp[kHeadAP];

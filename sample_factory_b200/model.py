@@ -291,18 +291,8 @@ class PolicyModel:
         self.ret_count = torch.ones(1, dtype=torch.float64, device=device)
 
         self._init_weights(seed, policy_init_gain)
-        self._register_lo()
-        self.refresh_cat_heads()
-
-    # ---- tf32 low halves of the weights (3xTF32 engine: the weight operand's lo tile is loaded, not recomputed) -----
-    def _register_lo(self) -> None:
-        self.flat_lo = None
-        if self.flat.is_cuda:
-            from . import ops
-
-            self.flat_lo = torch.empty_like(self.flat)
-            ops.register_tf32_lo(self.flat, self.flat_lo)
         self._register_f16()
+        self.refresh_cat_heads()
 
     # ---- fp16-split form of the 3-pass GEMM engine (include/sfb200.h): fp16 twins of the weights + activation bounds ----
     def _register_f16(self) -> None:
@@ -350,14 +340,13 @@ class PolicyModel:
         ops.register_f16_transposed(W, self.f16_T[name])
 
     def weights_changed(self) -> None:
-        """Call after writing `flat` / `params[...]` by anything other than the Adam kernel (which keeps lo current)."""
-        if self.flat_lo is not None:
+        """Call after writing `flat` / `params[...]` by anything other than the Adam kernel (which keeps the fp16 twins
+        current)."""
+        if self.f16_twins is not None:
             from . import ops
 
-            ops.refresh_tf32_lo(self.flat)
-            if self.f16_twins is not None:
-                ops.refresh_f16_twins(self.flat)
-                self.refresh_bounds()
+            ops.refresh_f16_twins(self.flat)
+            self.refresh_bounds()
         self.refresh_cat_heads()
 
     def rebind_grad(self, grad: Tensor) -> None:
@@ -369,14 +358,14 @@ class PolicyModel:
 
     def __del__(self):
         try:
-            if getattr(self, "flat_lo", None) is not None:
+            # the twin registries are keyed by device address: a stale entry would pick the fp16 form for whatever
+            # buffer the allocator places there next
+            if getattr(self, "f16_twins", None) is not None:
                 from . import ops
 
-                ops.unregister_tf32_lo(self.flat)
-                if getattr(self, "f16_twins", None) is not None:
-                    for name in self.f16_T:
-                        ops.unregister_f16_transposed(self.params[name])
-                    ops.unregister_f16_twins(self.flat)
+                for name in self.f16_T:
+                    ops.unregister_f16_transposed(self.params[name])
+                ops.unregister_f16_twins(self.flat)
         except Exception:
             pass
 
@@ -418,18 +407,16 @@ class PolicyModel:
         twin.grads = {}
         for k in ("obs_mean", "obs_var", "obs_count", "ret_mean", "ret_var", "ret_count"):
             setattr(twin, k, getattr(self, k).clone())
-        twin._register_lo()
+        twin._register_f16()
         twin.refresh_cat_heads()
         return twin
 
     def copy_weights_from(self, other: "PolicyModel") -> None:
-        """Refresh this snapshot from the learner's model (three D2D copies on the current stream)."""
+        """Refresh this snapshot from the learner's model (D2D copies on the current stream)."""
         self.flat.copy_(other.flat)
-        if self.flat_lo is not None and other.flat_lo is not None:
-            self.flat_lo.copy_(other.flat_lo)
-            if self.f16_twins is not None and other.f16_twins is not None:
-                self.f16_twins.copy_(other.f16_twins)
-                self.bound_h.copy_(other.bound_h)      # (scratch words are zero between launches)
+        if self.f16_twins is not None and other.f16_twins is not None:
+            self.f16_twins.copy_(other.f16_twins)
+            self.bound_h.copy_(other.bound_h)      # (scratch words are zero between launches)
             self.refresh_cat_heads()
         else:
             self.weights_changed()

@@ -310,22 +310,6 @@ def linear_residual_forward(x: Tensor, W: Tensor, b: Tensor, r: Tensor, out: Ten
     return out
 
 
-def register_tf32_lo(base: Tensor, lo: Tensor) -> None:
-    """Pair a flat weight buffer with its tf32 low-half twin (see include/sfb200.h) and fill the twin."""
-    assert base.is_contiguous() and lo.is_contiguous() and base.numel() == lo.numel()
-    lib().call("sfb200_register_tf32_lo", _p(base, F32), _p(lo, F32), base.numel())
-    refresh_tf32_lo(base)
-
-
-def unregister_tf32_lo(base: Tensor) -> None:
-    lib().call("sfb200_unregister_tf32_lo", _p(base, F32))
-
-
-def refresh_tf32_lo(base: Tensor) -> None:
-    """Recompute the registered low halves after the weights were written by anything but clip_adam_step."""
-    lib().call("sfb200_refresh_tf32_lo", _p(base, F32), _stream())
-
-
 def register_f16_twins(base: Tensor, twins: Tensor) -> None:
     """Pair a flat weight buffer with its fp16 (hi, lo) twins [hi16[n] | lo16[n]] (include/sfb200.h) and fill them."""
     assert base.is_contiguous() and twins.is_contiguous() and twins.dtype == torch.float16 and twins.numel() == 2 * base.numel()
@@ -461,27 +445,6 @@ def linear_act_heads_forward_fused(x: Tensor, W: Tensor, b: Tensor, out: Optiona
                _p(philox_offset_dev, I64), None if actions_f32 is None else actions_f32.data_ptr(), actions_stride, env_ptr,
                None if log_prob is None else log_prob.data_ptr(), log_prob_stride, _p(policy_version_scalar, F32),
                None if policy_version_out is None else policy_version_out.data_ptr(), pv_stride, _stream())
-
-
-def policy_mlp2_partials(W1: Tensor, W2: Tensor, A: int, engine: int) -> int:
-    """head partials per row the fused two-layer policy step produces, 0 when the model is not covered"""
-    H1, K1 = W1.shape
-    H2 = W2.shape[0]
-    if W2.shape[1] != H1 or not (W1.is_contiguous() and W2.is_contiguous()):
-        return 0
-    return lib().query("sfb200_policy_mlp2_partials", _p(W1, F32), _p(W2, F32), K1, H1, H2, A, engine)
-
-
-def policy_mlp2_heads_forward(x: Tensor, W1: Tensor, b1: Tensor, W2: Tensor, b2: Tensor, act: int, engine: int, Wv: Tensor,
-                              Wa: Tensor, head_partials: Tensor) -> None:
-    """x [M, K1] -> partial head dot products of act(act(x W1^T + b1) W2^T + b2) (one wgmma kernel, csrc/policy_step.cu)"""
-    M, K1 = x.shape
-    H1, H2, A = W1.shape[0], W2.shape[0], Wa.shape[0]
-    assert Wv.is_contiguous() and Wa.is_contiguous() and Wv.numel() == H2 and Wa.shape[1] == H2
-    P = 4 * (H2 // 128)
-    assert head_partials.numel() >= P * M * HEAD_PART_PAD
-    lib().call("sfb200_policy_mlp2_heads_forward", _p(x, F32), x.stride(0), M, K1, _p(W1, F32), _p(b1, F32), H1, _p(W2, F32),
-               _p(b2, F32), H2, act, engine, _p(Wv, F32), _p(Wa, F32), A, _p(head_partials, F32), _stream())
 
 
 def heads_from_partials(head_partials: Tensor, P: int, rows: int, bv: Tensor, ba: Tensor, values: Tensor,

@@ -59,19 +59,6 @@ class HeadsPlan:
             # heads_from_partials is fully parallel, so the separate launch stays the default.
             self.counters = torch.zeros((max_rows + 127) // 128, dtype=torch.int32, device=model.device)
             self.finish_in_gemm = os.environ.get("SFB200_HEADS_FINISH_IN_GEMM", "0") == "1"
-        # two-layer MLP policies (BASELINE cfg-2): both layers + the head partials in ONE kernel whenever the last hidden
-        # activation is not needed afterwards -- csrc/policy_step.cu (wgmma, h1 chunk by chunk in shared memory).  Opt-in
-        # (SFB200_POLICY_FUSED=1): it recomputes layer 1 in each of the H2/128 column CTAs and has not been measured on the
-        # H100, so the per-layer launches stay the default.
-        self.mlp2 = False
-        self.P_mlp2 = 0
-        if (self.P > 0 and self.conv is None and not spec.use_rnn and not spec.decoder_mlp_layers and
-                len(spec.fc_encoder_layers) == 2 and os.environ.get("SFB200_POLICY_FUSED", "0") == "1"):
-            (W1, _), (W2, _) = model.encoder_layers()
-            self.P_mlp2 = ops.policy_mlp2_partials(W1, W2, spec.num_linear_action_outputs, engine)
-            self.mlp2 = self.P_mlp2 > 0
-            if self.P_mlp2 > self.P:     # (32-column partial groups: twice as many partials as the per-layer epilogue leaves)
-                self.part = torch.empty(self.P_mlp2 * max_rows * ops.HEAD_PART_PAD, dtype=torch.float32, device=model.device)
 
 
 def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, engine: int, plan: HeadsPlan,
@@ -90,14 +77,6 @@ def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, 
     Wa, ba = model.actor
     n_mlp = len(enc) + len(dec)
     fused = plan.P > 0
-    if plan.mlp2 and not store_tail and not plan.finish_in_gemm:
-        (W1, b1), (W2, b2) = enc
-        ops.policy_mlp2_heads_forward(x, W1, b1, W2, b2, act, engine, Wv, Wa, plan.part)
-        if finish_fn is not None:
-            finish_fn(plan.part, plan.P_mlp2, M, bv, ba)
-        else:
-            _heads(model, None, Wv, bv, Wa, ba, True, plan, M, heads_kwargs, P=plan.P_mlp2)
-        return None
     k = 0
     tail: Optional[Tensor] = x
     for group, layers in (("enc", enc), ("dec", dec)):
@@ -149,8 +128,8 @@ def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan
 
 
 def _heads(model: PolicyModel, tail: Tensor, Wv: Tensor, bv: Tensor, Wa: Tensor, ba: Tensor, fused: bool, plan: HeadsPlan,
-           M: int, heads_kwargs: Dict, P: Optional[int] = None) -> None:
-    P = plan.P if P is None else P
+           M: int, heads_kwargs: Dict) -> None:
+    P = plan.P
     if model.spec.continuous:   # Box action space: Gaussian heads (action_distributions.py:290-323)
         dk = model.dist_kwargs()
         if fused:

@@ -100,8 +100,8 @@ class DeviceSampler:
         self._eager_rollouts = 0
         self.kernel_launches_per_rollout = 0
         # Fused step tail (csrc/heads.cu sampler_tail_tape_kernel): for the synthetic tape env the heads' finishing step,
-        # the env step, post-step(t) and pre-step(t+1) are ONE launch -- with the fused two-layer policy kernel a policy
-        # step is two launches.  Needs the fused-partials heads path, a plain Discrete action space, float32 observations,
+        # the env step, post-step(t) and pre-step(t+1) are ONE launch.  Needs the fused-partials heads path, a plain
+        # Discrete action space, float32 observations,
         # no recurrent core and an env whose step is the tape rule.  SFB200_TAIL_FUSED=0 restores the separate launches.
         import os
 

@@ -28,9 +28,6 @@ def timeit(fn, reps=12):
 
 for (M, N, K) in [(32768, 512, 512), (32768, 512, 64)]:
     flat = torch.randn(N * K, device=dev) / math.sqrt(K)
-    lo = torch.empty_like(flat)
-    ops.register_tf32_lo(flat, lo)
-    ops.refresh_tf32_lo(flat)
     W = flat.view(N, K)
     x = torch.randn(M, K, device=dev)
     dz = torch.randn(M, N, device=dev)
@@ -56,4 +53,3 @@ for (M, N, K) in [(32768, 512, 512), (32768, 512, 64)]:
         ops.unregister_f16_transposed(W); ops.unregister_f16_twins(flat)
     ref = dz.double().t() @ x.double()
     print("   dW max abs err vs fp64:", float((dW.double() - ref).abs().max()), "of max", float(ref.abs().max()))
-    ops.unregister_tf32_lo(flat)
