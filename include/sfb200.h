@@ -279,6 +279,24 @@ int sfb200_linear_act_heads_forward_fused(
     int64_t log_prob_stride, const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
     void* stream);
 
+/* Heads wider than 31 distribution_linear rows (up to 1024; model/actor_critic.py:171-186 with a large action space).
+ * The caller runs distribution_linear as a GEMM on the regular engine first, writing its outputs (bias included) to
+ * their final place: sfb200_linear_act_forward(h, Wa, ba, logits rows, act NONE) -- for adaptive_stddev=0 into the
+ * means half of each params row.  This entry then computes values[i] = h[i] . Wv + bv and runs the distribution tail
+ * of sfb200_heads_forward / _tuple / _continuous (dist_kind 0 / 1 / 2 as in sfb200_linear_act_heads_forward_fused) on
+ * the stored rows, with the same noise layout, Philox counters, mask and deterministic mode (action_distributions.py:
+ * 84-95, 110-148, 197-286, 290-323).  Box spaces with adaptive_stddev=0: the params rows are completed in place
+ * (tanh-scaled means, the learned log-std vector, action_parameterization.py:64-78).  logits == NULL: values only
+ * (the learner's bootstrap value, learner.py:965-967); then actions_f32 must be NULL too.  One warp per row. */
+int sfb200_heads_tail_wide(const float* h, int64_t ldh, int64_t rows, int H, const float* Wv, const float* bv,
+                           float* logits, int64_t logits_stride, int A, int dist_kind, int act_dim, int adaptive_stddev,
+                           const float* learned_log_std, float tanh_scale, int num_heads, const int32_t* head_sizes_host,
+                           float* values, int64_t values_stride, const float* noise, uint64_t philox_seed,
+                           uint64_t philox_offset, const int64_t* philox_offset_dev, float* actions_f32,
+                           int64_t actions_stride, void* env_actions, float* log_prob, int64_t log_prob_stride,
+                           const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
+                           void* stream);
+
 /* ------------------------------------------------------------- sampler steps ---- */
 /* BatchedVectorEnvRunner.generate_policy_request (algo/sampling/batched_sampling.py:374-388) fused with the
  * inference-side normalisation (inference_worker.py:326):  traj_obs[:, t] = obs ; traj_rnn[:, t] = rnn ;
@@ -415,7 +433,8 @@ int sfb200_adv_stats_finalize(const double* dp_partials, double* stats, void* st
  * exploration_loss: 0 = entropy bonus (learner.py:473-477), 1 = symmetric KL to the uniform prior (:479-486,
  * action_distributions.py:168-177; stats[EXPLORATION_LOSS] = +coeff * min(mean, 30)).
  * All means are over valid entries only (algo/utils/torch_utils.py:50-55).  grad_scale multiplies every gradient
- * (1/world_size under data parallelism). */
+ * (1/world_size under data parallelism).  A <= 1024 (this and the Tuple / continuous variants below: rows wider than 32
+ * run one warp per sample with the same formulas and the same fixed-order reduction). */
 int sfb200_ppo_loss_fwd_bwd(const float* logits, const float* values, int A, const float* actions_f32,
                             const float* log_prob_old, const float* values_old, const float* adv,
                             const float* targets, const uint8_t* valids, const float* logits_old, int64_t batch,
@@ -521,6 +540,23 @@ int64_t sfb200_heads_backward_workspace_bytes(int H, int A);
 int sfb200_heads_backward(const float* h, int64_t ldh, int64_t rows, int H, int A, const float* Wv, const float* Wa,
                           const float* dlogits, const float* dvalues, int act, float* dz, int64_t lddz, float* dWv,
                           float* dbv, float* dWa, float* dba, float* db_prev, void* workspace, void* stream);
+
+/* The same backward for heads wider than 31 rows (the reference's loss.backward() through critic_linear /
+ * distribution_linear, learner.py:779), in two steps:
+ *   sfb200_linear_backward(dlogits, h, Wa, act, dWa, dz, db_prev = NULL)     dWa = dlogits^T.h, dz = (dlogits.Wa)*act'(h)
+ *   sfb200_heads_wide_backward(...)                                           everything else:
+ *     dz[i, value_col + j] (+)= act'(h[i,j]) * dvalues[i] * Wv[j]   (added when accumulate != 0, else written)
+ *     dWv[j] = sum_i dvalues[i] h[i,j] ; dbv = sum_i dvalues[i] ; dba[a] = sum_i dlogits[i,a] ;
+ *     db_prev[c] = sum_i dz[i,c] for the dz columns c < width (skipped when db_prev == NULL)
+ * h [rows, H] is the tensor critic_linear reads (row stride ldh); dz [rows, width] (row stride lddz); dlogits [rows, A]
+ * dense.  Separate actor / critic towers: dz = [actor half | critic half], width = 2H, value_col = H, accumulate = 0.
+ * All sums run in a fixed order (deterministic); workspace >= sfb200_heads_wide_backward_workspace_bytes(rows, width,
+ * H, A). */
+int64_t sfb200_heads_wide_backward_workspace_bytes(int64_t rows, int width, int H, int A);
+int sfb200_heads_wide_backward(const float* h, int64_t ldh, int64_t rows, int H, const float* Wv, const float* dlogits,
+                               int A, const float* dvalues, int act, float* dz, int64_t lddz, int width, int value_col,
+                               int accumulate, float* dWv, float* dbv, float* dba, float* db_prev, void* workspace,
+                               void* stream);
 
 int64_t sfb200_linear_backward_workspace_bytes(int64_t M, int N, int K);
 /* backward of y = act(x.W^T + b) given dz = dL/d(pre-activation) [M,N]:

@@ -493,7 +493,7 @@ static thread_local const uint8_t* g_action_mask = nullptr;
 static thread_local int64_t g_mask_stride = 0;
 static thread_local int g_deterministic = 0;
 
-static int apply_sampling_mode(HeadsOut& out, int A) {
+int apply_sampling_mode(HeadsOut& out, int A) {
     if (out.actions_f32 == nullptr) return 0;     // values / distribution parameters only: nothing is sampled
     out.deterministic = g_deterministic;
     if (g_action_mask) {

@@ -26,6 +26,9 @@ struct HeadsOut {
     const uint8_t* action_mask = nullptr; int64_t mask_stride = 0; int deterministic = 0;
 };
 
+// the calling host thread's sampling mode (sfb200_set_sampling_mode) applied to the outputs of a heads launch (heads.cu)
+int apply_sampling_mode(HeadsOut& out, int A);
+
 constexpr float kStddevMin = 1e-4f, kStddevMax = 1e4f;   // action_distributions.py:291-292
 constexpr float kHalfLog2Pi = 0.91893853320467274178f;   // log(sqrt(2 pi))
 

@@ -600,6 +600,377 @@ __global__ void __launch_bounds__(256) ppo_loss_finalize_kernel(const double* __
     }
 }
 
+// ---- rows wider than 32 (up to kWideMax): one warp per sample -----------------------------------------------------
+// Lane l holds elements l, l+32, ... of a row (LPL per lane).  A block still covers 256 consecutive samples (8 warps x 32
+// rows) and lane r of a warp keeps the statistics of the warp's r-th sample, so ppo_store_partials sees the same thread ->
+// sample map as the thread-per-sample kernels above: same partial slots, same fixed-order reduction, same workspace.
+constexpr int kWideMax = 1024;
+
+template <int LPL>
+__device__ __forceinline__ void wide_load(const float* __restrict__ p, int n, int lane, float (&v)[LPL]) {
+#pragma unroll
+    for (int k = 0; k < LPL; ++k) v[k] = (k * 32 + lane < n) ? p[k * 32 + lane] : 0.f;
+}
+template <int LPL>
+__device__ __forceinline__ void wide_store(float* __restrict__ p, int n, int lane, const float (&v)[LPL]) {
+#pragma unroll
+    for (int k = 0; k < LPL; ++k)
+        if (k * 32 + lane < n) p[k * 32 + lane] = v[k];
+}
+// element a of a row spread over the warp
+template <int LPL>
+__device__ __forceinline__ float wide_get(const float (&v)[LPL], int a, int lane) {
+    float mine = 0.f;
+#pragma unroll
+    for (int k = 0; k < LPL; ++k)
+        if (k == (a >> 5)) mine = v[k];
+    return __shfl_sync(0xffffffffu, mine, a & 31);
+}
+// softmax / log_softmax over the elements [lo, hi) of a row (row_softmax / row_softmax_segs); other slots untouched
+template <int LPL>
+__device__ __forceinline__ void wide_softmax(const float (&l)[LPL], int lo, int hi, int lane, float (&p)[LPL],
+                                             float (&logp)[LPL]) {
+    float m = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < LPL; ++k) {
+        const int a = k * 32 + lane;
+        if (a >= lo && a < hi) m = fmaxf(m, l[k]);
+    }
+    m = warp_max(m);
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < LPL; ++k) {
+        const int a = k * 32 + lane;
+        if (a >= lo && a < hi) { p[k] = expf(l[k] - m); s += p[k]; }
+    }
+    s = warp_sum(s);
+    const float logs = logf(s);
+#pragma unroll
+    for (int k = 0; k < LPL; ++k) {
+        const int a = k * 32 + lane;
+        if (a >= lo && a < hi) { logp[k] = (l[k] - m) - logs; p[k] = __fdiv_rn(p[k], s); }
+    }
+}
+
+#define SFB_WIDE_PROLOGUE                                                                                   \
+    __shared__ double sm[8];                                                                                \
+    const int lane = threadIdx.x & 31;                                                                      \
+    const double n_valid = stats[SFB200_LS_NUM_VALID];                                                      \
+    const float adv_mean = (float)stats[SFB200_LS_ADV_MEAN];                                                \
+    const float adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);                                    \
+    const float w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;                            \
+    PpoAcc acc;   /* statistics of sample blockIdx.x * 256 + threadIdx.x */                                 \
+    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31)
+
+template <int LPL>
+__global__ void __launch_bounds__(256) ppo_loss_wide_kernel(
+    const float* __restrict__ logits, const float* __restrict__ values, int A, const float* __restrict__ actions,
+    const float* __restrict__ lp_old, const float* __restrict__ v_old, const float* __restrict__ adv,
+    const float* __restrict__ targets, const uint8_t* __restrict__ valids, const float* __restrict__ logits_old,
+    int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent, int expl_mode, float c_val, float c_kl,
+    float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues, const double* __restrict__ stats,
+    double* __restrict__ part) {
+    SFB_WIDE_PROLOGUE;
+    for (int r = 0; r < 32; ++r) {
+        const int64_t i = base + r;
+        if (i >= batch) break;   // warp-uniform
+        PpoAcc t;
+        const float v = values[i];
+        t.s_v = v;
+        float dl[LPL];
+#pragma unroll
+        for (int k = 0; k < LPL; ++k) dl[k] = 0.f;
+        float dv = 0.f;
+        if (valids[i]) {
+            t.s_cnt = 1.0;
+            float l[LPL], p[LPL], logp[LPL], lq[LPL];
+            wide_load<LPL>(logits + i * A, A, lane, l);
+            wide_softmax<LPL>(l, 0, A, lane, p, logp);
+            const int act = (int)actions[i];
+            const float lp = wide_get<LPL>(logp, act, lane);
+            const float g_lp = ppo_policy_terms(lp, lp_old[i], adv[i], adv_mean, adv_std, clip_lo, clip_hi, w, t);
+            const float u = 1.f / (float)A, log_u = -logf((float)A);
+            float h = 0.f, s1 = 0.f, s2 = 0.f;
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                if (k * 32 + lane < A) {
+                    h -= logp[k] * p[k];
+                    s1 += p[k] * (logp[k] - log_u);
+                    s2 += u * (log_u - logp[k]);
+                }
+            }
+            const float H = warp_sum(h);
+            t.s_ent = H;
+            float S1 = 0.f;
+            if (expl_mode == 1) {
+                S1 = warp_sum(s1);
+                t.s_skl = 0.5f * (S1 + warp_sum(s2));
+            }
+            float kl = 0.f;
+            if (logits_old) {
+                float lo[LPL], po[LPL];
+                wide_load<LPL>(logits_old + i * A, A, lane, lo);
+                wide_softmax<LPL>(lo, 0, A, lane, po, lq);
+                float klp = 0.f;
+#pragma unroll
+                for (int k = 0; k < LPL; ++k)
+                    if (k * 32 + lane < A) klp += p[k] * (logp[k] - lq[k]);
+                kl = warp_sum(klp);
+                t.s_kl = kl;
+                t.m_kl = kl;
+            }
+            const float we = w * c_ent, wk = (logits_old ? w * c_kl : 0.f);
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                const int a = k * 32 + lane;
+                if (a < A) {
+                    float g = g_lp * ((a == act ? 1.f : 0.f) - p[k]);
+                    if (expl_mode == 1) g += we * 0.5f * (p[k] * ((logp[k] - log_u) - S1) + p[k] - u);
+                    else g += we * p[k] * (logp[k] + H);
+                    if (logits_old) g += wk * p[k] * ((logp[k] - lq[k]) - kl);
+                    dl[k] = g;
+                }
+            }
+            dv = ppo_value_terms(v, v_old[i], targets[i], clip_value, w, c_val, t);
+        }
+        wide_store<LPL>(dlogits + i * A, A, lane, dl);
+        if (lane == 0) dvalues[i] = dv;
+        if (lane == r) acc = t;
+    }
+    ppo_store_partials(acc, part, sm);
+}
+
+template <int LPL>
+__global__ void __launch_bounds__(256) ppo_loss_tuple_wide_kernel(
+    const float* __restrict__ logits, const float* __restrict__ values, int A, Segs sg, const float* __restrict__ actions,
+    const float* __restrict__ lp_old, const float* __restrict__ v_old, const float* __restrict__ adv,
+    const float* __restrict__ targets, const uint8_t* __restrict__ valids, const float* __restrict__ logits_old,
+    int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent, int expl_mode, float c_val, float c_kl,
+    float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues, const double* __restrict__ stats,
+    double* __restrict__ part) {
+    SFB_WIDE_PROLOGUE;
+    for (int r = 0; r < 32; ++r) {
+        const int64_t i = base + r;
+        if (i >= batch) break;
+        PpoAcc t;
+        const float v = values[i];
+        t.s_v = v;
+        float dl[LPL];
+#pragma unroll
+        for (int k = 0; k < LPL; ++k) dl[k] = 0.f;
+        float dv = 0.f;
+        if (valids[i]) {
+            t.s_cnt = 1.0;
+            float l[LPL], p[LPL], logp[LPL], lq[LPL];
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) { p[k] = 0.f; logp[k] = 0.f; lq[k] = 0.f; }
+            wide_load<LPL>(logits + i * A, A, lane, l);
+            float lo[LPL], po[LPL];
+            if (logits_old) wide_load<LPL>(logits_old + i * A, A, lane, lo);
+            float lp = 0.f, Htot = 0.f, kltot = 0.f, skltot = 0.f;
+            float segH[8], segKL[8], segS1[8];
+            int act_idx[8];
+            int start = 0;
+            for (int s = 0; s < sg.n; ++s) {
+                const int end = start + sg.len[s];
+                wide_softmax<LPL>(l, start, end, lane, p, logp);
+                if (logits_old) wide_softmax<LPL>(lo, start, end, lane, po, lq);
+                act_idx[s] = start + (int)actions[i * sg.n + s];
+                lp += wide_get<LPL>(logp, act_idx[s], lane);
+                const float u = 1.f / (float)sg.len[s], log_u = -logf((float)sg.len[s]);
+                float h = 0.f, klp = 0.f, s1 = 0.f, s2 = 0.f;
+#pragma unroll
+                for (int k = 0; k < LPL; ++k) {
+                    const int a = k * 32 + lane;
+                    if (a >= start && a < end) {
+                        h -= logp[k] * p[k];
+                        if (logits_old) klp += p[k] * (logp[k] - lq[k]);
+                        s1 += p[k] * (logp[k] - log_u);
+                        s2 += u * (log_u - logp[k]);
+                    }
+                }
+                segH[s] = warp_sum(h);
+                segKL[s] = warp_sum(klp);
+                segS1[s] = warp_sum(s1);
+                Htot += segH[s];
+                kltot += segKL[s];
+                skltot += 0.5f * (segS1[s] + warp_sum(s2));
+                start = end;
+            }
+            const float g_lp = ppo_policy_terms(lp, lp_old[i], adv[i], adv_mean, adv_std, clip_lo, clip_hi, w, t);
+            t.s_ent = Htot;
+            if (expl_mode == 1) t.s_skl = skltot;
+            if (logits_old) { t.s_kl = kltot; t.m_kl = kltot; }
+            const float we = w * c_ent, wk = (logits_old ? w * c_kl : 0.f);
+            start = 0;
+            for (int s = 0; s < sg.n; ++s) {
+                const int end = start + sg.len[s];
+                const float u = 1.f / (float)sg.len[s], log_u = -logf((float)sg.len[s]);
+#pragma unroll
+                for (int k = 0; k < LPL; ++k) {
+                    const int a = k * 32 + lane;
+                    if (a >= start && a < end) {
+                        float g = g_lp * ((a == act_idx[s] ? 1.f : 0.f) - p[k]);
+                        if (expl_mode == 1) g += we * 0.5f * (p[k] * ((logp[k] - log_u) - segS1[s]) + p[k] - u);
+                        else g += we * p[k] * (logp[k] + segH[s]);
+                        if (logits_old) g += wk * p[k] * ((logp[k] - lq[k]) - segKL[s]);
+                        dl[k] = g;
+                    }
+                }
+                start = end;
+            }
+            dv = ppo_value_terms(v, v_old[i], targets[i], clip_value, w, c_val, t);
+        }
+        wide_store<LPL>(dlogits + i * A, A, lane, dl);
+        if (lane == 0) dvalues[i] = dv;
+        if (lane == r) acc = t;
+    }
+    ppo_store_partials(acc, part, sm);
+}
+
+template <int LPL>
+__global__ void __launch_bounds__(256) ppo_loss_gauss_wide_kernel(
+    const float* __restrict__ params, const float* __restrict__ values, int Ad, int adaptive, float tanh_scale,
+    const float* __restrict__ actions, const float* __restrict__ lp_old, const float* __restrict__ v_old,
+    const float* __restrict__ adv, const float* __restrict__ targets, const uint8_t* __restrict__ valids,
+    const float* __restrict__ params_old, int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent,
+    float c_val, float c_kl, float grad_scale, float* __restrict__ dlogits, float* __restrict__ dlogstd,
+    float* __restrict__ dvalues, const double* __restrict__ stats, double* __restrict__ part) {
+    SFB_WIDE_PROLOGUE;
+    for (int r = 0; r < 32; ++r) {
+        const int64_t i = base + r;
+        if (i >= batch) break;
+        PpoAcc t;
+        const float v = values[i];
+        t.s_v = v;
+        float dm[LPL], ds[LPL];
+#pragma unroll
+        for (int k = 0; k < LPL; ++k) { dm[k] = 0.f; ds[k] = 0.f; }
+        float dv = 0.f;
+        if (valids[i]) {
+            t.s_cnt = 1.0;
+            float m[LPL], s[LPL], a_[LPL], sd[LPL], dlt[LPL];
+            wide_load<LPL>(params + i * 2 * Ad, Ad, lane, m);
+            wide_load<LPL>(params + i * 2 * Ad + Ad, Ad, lane, s);
+            wide_load<LPL>(actions + i * Ad, Ad, lane, a_);
+            float lpp = 0.f, hp = 0.f;
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                sd[k] = clampf(expf(s[k]), kStdMin, kStdMax);
+                dlt[k] = a_[k] - m[k];
+                if (k * 32 + lane < Ad) {
+                    const float lsd = logf(sd[k]);
+                    lpp += -(dlt[k] * dlt[k]) / (2.f * (sd[k] * sd[k])) - lsd - kHalfLog2PiL;
+                    hp += 0.5f + kHalfLog2PiL + lsd;
+                }
+            }
+            const float lp = warp_sum(lpp);
+            const float g_lp = ppo_policy_terms(lp, lp_old[i], adv[i], adv_mean, adv_std, clip_lo, clip_hi, w, t);
+            t.s_ent = warp_sum(hp);
+            const float we = w * c_ent, wk = (params_old ? w * c_kl : 0.f);
+            float mo[LPL], so[LPL];
+            if (params_old) {
+                wide_load<LPL>(params_old + i * 2 * Ad, Ad, lane, mo);
+                wide_load<LPL>(params_old + i * 2 * Ad + Ad, Ad, lane, so);
+            }
+            float klp = 0.f;
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                if (k * 32 + lane < Ad) {
+                    const float ex = expf(s[k]);
+                    const float in_range = (ex >= kStdMin && ex <= kStdMax) ? 1.f : 0.f;
+                    const float inv_var = 1.f / (sd[k] * sd[k]);
+                    float gm = g_lp * dlt[k] * inv_var;
+                    float gs = g_lp * (dlt[k] * dlt[k] * inv_var - 1.f) - we;
+                    if (params_old) {
+                        const float sdo = clampf(expf(so[k]), kStdMin, kStdMax);
+                        const float q = sd[k] / sdo, rr = q * q;
+                        const float dq = (m[k] - mo[k]) / sdo;
+                        klp += 0.5f * (rr + dq * dq - 1.f - logf(rr));
+                        gm += wk * dq / sdo;
+                        gs += wk * (rr - 1.f);
+                    }
+                    gs *= in_range;
+                    if (!adaptive && tanh_scale > 0.f) {
+                        const float tq = m[k] / tanh_scale;
+                        gm *= (1.f - tq * tq);
+                    }
+                    dm[k] = gm;
+                    ds[k] = gs;
+                }
+            }
+            if (params_old) {
+                const float kl = warp_sum(klp);
+                t.s_kl = kl;
+                t.m_kl = kl;
+            }
+            dv = ppo_value_terms(v, v_old[i], targets[i], clip_value, w, c_val, t);
+        }
+        float* drow = dlogits + i * (adaptive ? 2 * Ad : Ad);
+        wide_store<LPL>(drow, Ad, lane, dm);
+        wide_store<LPL>(adaptive ? drow + Ad : dlogstd + i * Ad, Ad, lane, ds);
+        if (lane == 0) dvalues[i] = dv;
+        if (lane == r) acc = t;
+    }
+    ppo_store_partials(acc, part, sm);
+}
+#undef SFB_WIDE_PROLOGUE
+
+// action-ratio pre-pass of V-trace for wide rows: one warp per sample
+template <int LPL>
+__global__ void __launch_bounds__(256) action_ratio_wide_kernel(const float* __restrict__ logits, int A, Segs sg,
+                                                                const float* __restrict__ actions,
+                                                                const float* __restrict__ lp_old, int64_t batch,
+                                                                float* __restrict__ ratio) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    if (i >= batch) return;   // warp-uniform
+    float l[LPL], p[LPL], logp[LPL];
+    wide_load<LPL>(logits + i * A, A, lane, l);
+    float lp = 0.f;
+    int start = 0;
+    for (int s = 0; s < sg.n; ++s) {   // (a plain Discrete space is one segment)
+        const int end = start + sg.len[s];
+        wide_softmax<LPL>(l, start, end, lane, p, logp);
+        lp += wide_get<LPL>(logp, start + (int)actions[i * sg.n + s], lane);
+        start = end;
+    }
+    if (lane == 0) ratio[i] = clampf(expf(lp - lp_old[i]), 0.05f, 20.0f);
+}
+
+template <int LPL>
+__global__ void __launch_bounds__(256) action_ratio_gauss_wide_kernel(const float* __restrict__ params, int Ad,
+                                                                      const float* __restrict__ actions,
+                                                                      const float* __restrict__ lp_old, int64_t batch,
+                                                                      float* __restrict__ ratio) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    if (i >= batch) return;
+    float m[LPL], s[LPL], a_[LPL];
+    wide_load<LPL>(params + i * 2 * Ad, Ad, lane, m);
+    wide_load<LPL>(params + i * 2 * Ad + Ad, Ad, lane, s);
+    wide_load<LPL>(actions + i * Ad, Ad, lane, a_);
+    float lpp = 0.f;
+#pragma unroll
+    for (int k = 0; k < LPL; ++k) {
+        if (k * 32 + lane < Ad) {
+            const float sd = clampf(expf(s[k]), kStdMin, kStdMax);
+            const float d = a_[k] - m[k];
+            lpp += -(d * d) / (2.f * (sd * sd)) - logf(sd) - kHalfLog2PiL;
+        }
+    }
+    const float lp = warp_sum(lpp);
+    if (lane == 0) ratio[i] = clampf(expf(lp - lp_old[i]), 0.05f, 20.0f);
+}
+
+// LPL = elements per lane for a row of n > 32 elements
+#define SFB_WIDE_LPL(n, LAUNCH)          \
+    if ((n) <= 64) LAUNCH(2);            \
+    else if ((n) <= 128) LAUNCH(4);      \
+    else if ((n) <= 256) LAUNCH(8);      \
+    else if ((n) <= 512) LAUNCH(16);     \
+    else LAUNCH(32)
+
 }  // namespace sfb
 
 using namespace sfb;
@@ -614,13 +985,20 @@ int64_t sfb200_loss_workspace_bytes(int64_t batch) {
 int sfb200_action_ratio(const float* logits, int A, const float* actions_f32, const float* log_prob_old, int64_t batch,
                         float* ratio, void* stream) {
     SFB_CHECK_ARG(logits && actions_f32 && log_prob_old && ratio && batch >= 0, "action_ratio: bad arguments");
-    SFB_CHECK_ARG(A >= 1 && A <= 32, "action_ratio: supports 1 <= A <= 32");
+    SFB_CHECK_ARG(A >= 1 && A <= kWideMax, "action_ratio: supports 1 <= A <= %d, got %d", kWideMax, A);
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned g = (unsigned)ceil_div(batch, 256);
     if (A <= 8) action_ratio_kernel<8><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
     else if (A <= 16) action_ratio_kernel<16><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
-    else action_ratio_kernel<32><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
+    else if (A <= 32) action_ratio_kernel<32><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
+    else {
+        const Segs one{1, {A}};
+        const unsigned gw = (unsigned)ceil_div(batch, 8);
+#define SFB_ARW(LPL) action_ratio_wide_kernel<LPL><<<gw, 256, 0, st>>>(logits, A, one, actions_f32, log_prob_old, batch, ratio)
+        SFB_WIDE_LPL(A, SFB_ARW);
+#undef SFB_ARW
+    }
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -656,7 +1034,7 @@ int sfb200_ppo_loss_fwd_bwd(const float* logits, const float* values, int A, con
     SFB_CHECK_ARG(exploration_loss == 0 || exploration_loss == 1, "ppo_loss_fwd_bwd: exploration_loss must be 0 (entropy) or 1 (symmetric_kl)");
     SFB_CHECK_ARG(logits && values && actions_f32 && log_prob_old && values_old && adv && targets && valids && dlogits &&
                       dvalues && stats && workspace && batch > 0, "ppo_loss_fwd_bwd: bad arguments");
-    SFB_CHECK_ARG(A >= 1 && A <= 32, "ppo_loss_fwd_bwd: supports 1 <= A <= 32");
+    SFB_CHECK_ARG(A >= 1 && A <= kWideMax, "ppo_loss_fwd_bwd: supports 1 <= A <= %d, got %d", kWideMax, A);
     cudaStream_t st = (cudaStream_t)stream;
     const float clip_hi = 1.0f + clip_ratio;          // learner.py:544
     const float clip_lo = 1.0f / clip_hi;             // :546
@@ -666,9 +1044,16 @@ int sfb200_ppo_loss_fwd_bwd(const float* logits, const float* values, int A, con
     ppo_loss_kernel<AM><<<g, 256, 0, st>>>(logits, values, A, actions_f32, log_prob_old, values_old, adv, targets,    \
                                            valids, logits_old, batch, clip_lo, clip_hi, clip_value, exploration_coeff, \
                                            exploration_loss, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, stats, part)
+#define SFB_PLW(LPL)                                                                                                  \
+    ppo_loss_wide_kernel<LPL><<<g, 256, 0, st>>>(logits, values, A, actions_f32, log_prob_old, values_old, adv, targets, \
+                                                 valids, logits_old, batch, clip_lo, clip_hi, clip_value,               \
+                                                 exploration_coeff, exploration_loss, value_coeff, kl_coeff, grad_scale, \
+                                                 dlogits, dvalues, stats, part)
     if (A <= 8) SFB_PL(8);
     else if (A <= 16) SFB_PL(16);
-    else SFB_PL(32);
+    else if (A <= 32) SFB_PL(32);
+    else { SFB_WIDE_LPL(A, SFB_PLW); }
+#undef SFB_PLW
 #undef SFB_PL
     SFB_LAUNCH_OK();
     ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff,
@@ -683,7 +1068,8 @@ static int make_segs(Segs& sg, int A, int num_heads, const int32_t* head_sizes) 
     sg.n = num_heads;
     for (int k = 0; k < 8; ++k) sg.len[k] = k < num_heads ? head_sizes[k] : 0;
     for (int k = 0; k < num_heads; ++k) tot += head_sizes[k];
-    SFB_CHECK_ARG(tot == A && A <= 32, "tuple action space: head sizes must sum to A = %d (<= 32), got %d", A, tot);
+    SFB_CHECK_ARG(tot == A && A <= kWideMax, "tuple action space: head sizes must sum to A = %d (<= %d), got %d", A, kWideMax,
+                  tot);
     return 0;
 }
 
@@ -698,7 +1084,13 @@ int sfb200_action_ratio_tuple(const float* logits, int A, int num_heads, const i
     const unsigned g = (unsigned)ceil_div(batch, 256);
     if (A <= 8) action_ratio_tuple_kernel<8><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
     else if (A <= 16) action_ratio_tuple_kernel<16><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
-    else action_ratio_tuple_kernel<32><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
+    else if (A <= 32) action_ratio_tuple_kernel<32><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
+    else {
+        const unsigned gw = (unsigned)ceil_div(batch, 8);
+#define SFB_ARW(LPL) action_ratio_wide_kernel<LPL><<<gw, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio)
+        SFB_WIDE_LPL(A, SFB_ARW);
+#undef SFB_ARW
+    }
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -725,9 +1117,16 @@ int sfb200_ppo_loss_fwd_bwd_tuple(const float* logits, const float* values, int 
                                                  targets, valids, logits_old, batch, clip_lo, clip_hi, clip_value,        \
                                                  exploration_coeff, exploration_loss, value_coeff, kl_coeff, grad_scale,  \
                                                  dlogits, dvalues, stats, part)
+#define SFB_PTW(LPL)                                                                                                     \
+    ppo_loss_tuple_wide_kernel<LPL><<<g, 256, 0, st>>>(logits, values, A, sg, actions_f32, log_prob_old, values_old, adv, \
+                                                       targets, valids, logits_old, batch, clip_lo, clip_hi, clip_value,  \
+                                                       exploration_coeff, exploration_loss, value_coeff, kl_coeff,        \
+                                                       grad_scale, dlogits, dvalues, stats, part)
     if (A <= 8) SFB_PT(8);
     else if (A <= 16) SFB_PT(16);
-    else SFB_PT(32);
+    else if (A <= 32) SFB_PT(32);
+    else { SFB_WIDE_LPL(A, SFB_PTW); }
+#undef SFB_PTW
 #undef SFB_PT
     SFB_LAUNCH_OK();
     ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff,
@@ -739,13 +1138,20 @@ int sfb200_ppo_loss_fwd_bwd_tuple(const float* logits, const float* values, int 
 int sfb200_action_ratio_continuous(const float* params, int act_dim, const float* actions_f32, const float* log_prob_old,
                                    int64_t batch, float* ratio, void* stream) {
     SFB_CHECK_ARG(params && actions_f32 && log_prob_old && ratio && batch >= 0, "action_ratio_continuous: bad arguments");
-    SFB_CHECK_ARG(act_dim >= 1 && act_dim <= 32, "action_ratio_continuous: supports 1 <= act_dim <= 32");
+    SFB_CHECK_ARG(act_dim >= 1 && act_dim <= kWideMax, "action_ratio_continuous: supports 1 <= act_dim <= %d, got %d",
+                  kWideMax, act_dim);
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
     const unsigned g = (unsigned)ceil_div(batch, 256);
     if (act_dim <= 8) action_ratio_gauss_kernel<8><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
     else if (act_dim <= 16) action_ratio_gauss_kernel<16><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
-    else action_ratio_gauss_kernel<32><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
+    else if (act_dim <= 32) action_ratio_gauss_kernel<32><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
+    else {
+        const unsigned gw = (unsigned)ceil_div(batch, 8);
+#define SFB_ARGW(LPL) action_ratio_gauss_wide_kernel<LPL><<<gw, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio)
+        SFB_WIDE_LPL(act_dim, SFB_ARGW);
+#undef SFB_ARGW
+    }
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -759,7 +1165,8 @@ int sfb200_ppo_loss_fwd_bwd_continuous(const float* params, const float* values,
                                        void* workspace, void* stream) {
     SFB_CHECK_ARG(params && values && actions_f32 && log_prob_old && values_old && adv && targets && valids && dlogits &&
                       dvalues && stats && workspace && batch > 0, "ppo_loss_fwd_bwd_continuous: bad arguments");
-    SFB_CHECK_ARG(act_dim >= 1 && act_dim <= 32, "ppo_loss_fwd_bwd_continuous: supports 1 <= act_dim <= 32");
+    SFB_CHECK_ARG(act_dim >= 1 && act_dim <= kWideMax, "ppo_loss_fwd_bwd_continuous: supports 1 <= act_dim <= %d, got %d",
+                  kWideMax, act_dim);
     SFB_CHECK_ARG(adaptive_stddev || dlogstd, "ppo_loss_fwd_bwd_continuous: dlogstd is required when adaptive_stddev=0");
     cudaStream_t st = (cudaStream_t)stream;
     const float clip_hi = 1.0f + clip_ratio;
@@ -771,9 +1178,16 @@ int sfb200_ppo_loss_fwd_bwd_continuous(const float* params, const float* values,
                                                   log_prob_old, values_old, adv, targets, valids, params_old, batch,      \
                                                   clip_lo, clip_hi, clip_value, exploration_coeff, value_coeff, kl_coeff, \
                                                   grad_scale, dlogits, dlogstd, dvalues, stats, part)
+#define SFB_PGW(LPL)                                                                                                    \
+    ppo_loss_gauss_wide_kernel<LPL><<<g, 256, 0, st>>>(params, values, act_dim, adaptive_stddev, tanh_scale, actions_f32, \
+                                                       log_prob_old, values_old, adv, targets, valids, params_old, batch, \
+                                                       clip_lo, clip_hi, clip_value, exploration_coeff, value_coeff,     \
+                                                       kl_coeff, grad_scale, dlogits, dlogstd, dvalues, stats, part)
     if (act_dim <= 8) SFB_PG(8);
     else if (act_dim <= 16) SFB_PG(16);
-    else SFB_PG(32);
+    else if (act_dim <= 32) SFB_PG(32);
+    else { SFB_WIDE_LPL(act_dim, SFB_PGW); }
+#undef SFB_PGW
 #undef SFB_PG
     SFB_LAUNCH_OK();
     ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);

@@ -202,8 +202,14 @@ class Learner:
         self.mb_partials = torch.zeros((cfg.num_batches_per_epoch, 3), dtype=torch.float64, device=dev)
         self.loss_ws = torch.empty(ops.loss_workspace_bytes(max(B, E)) // 8 + 8, dtype=torch.float64, device=dev)
         tail_w = spec.tail_input_size * (1 if spec.share_weights else 2)     # separate weights: [actor tail | critic tail]
-        self.heads_ws = torch.empty(ops.heads_backward_workspace_bytes(tail_w, A_lin) // 4 + 4, **f32)
         lin_ws = 4
+        if spec.wide_heads:
+            # heads wider than 31 rows: linear_backward for dWa / dz, sfb200_heads_wide_backward for the rest
+            self.heads_ws = torch.empty(ops.heads_wide_backward_workspace_bytes(B, tail_w, spec.tail_input_size, A_lin) // 4 + 4,
+                                        **f32)
+            lin_ws = ops.linear_backward_workspace_bytes(B, A_lin, spec.tail_input_size) // 4 + 4
+        else:
+            self.heads_ws = torch.empty(ops.heads_backward_workspace_bytes(tail_w, A_lin) // 4 + 4, **f32)
         d = spec.fc_encoder_input
         for h in spec.fc_encoder_layers:
             lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(B, h, d) // 4 + 4)
@@ -563,10 +569,20 @@ class Learner:
         tail_db = gdec[-1][1] if Ld > 0 else (None if rnn else genc[-1][1])
         if self.dz_bound is not None and tail_is_mlp:
             ops.heads_dz_bound(self.dlogits, self.dvalues, Wv, Wa, self.dz_bound)
-        ops.heads_backward(x, Wv, Wa, self.dlogits, self.dvalues, self.act if tail_is_mlp else none, tail_dz,
-                           g["critic_linear.weight"].view(-1), g["critic_linear.bias"],
-                           g["action_parameterization.distribution_linear.weight"],
-                           g["action_parameterization.distribution_linear.bias"], tail_db, self.heads_ws)
+        tail_act = self.act if tail_is_mlp else none
+        if spec.wide_heads:
+            # dWa = dlogits^T . x and tail_dz = (dlogits . Wa) * act'(x) on the GEMM engine, then the value term, the bias /
+            # value gradients and db_prev (the bound above covers the sum: the formula holds for any number of rows)
+            ops.linear_backward(self.dlogits, x, Wa, tail_act, g["action_parameterization.distribution_linear.weight"],
+                                tail_dz, None, self.engine, self.lin_ws)
+            ops.heads_wide_backward(x, Wv, self.dlogits, self.dvalues, tail_act, tail_dz, 0, True,
+                                    g["critic_linear.weight"].view(-1), g["critic_linear.bias"],
+                                    g["action_parameterization.distribution_linear.bias"], tail_db, self.heads_ws)
+        else:
+            ops.heads_backward(x, Wv, Wa, self.dlogits, self.dvalues, tail_act, tail_dz,
+                               g["critic_linear.weight"].view(-1), g["critic_linear.bias"],
+                               g["action_parameterization.distribution_linear.weight"],
+                               g["action_parameterization.distribution_linear.bias"], tail_db, self.heads_ws)
         for j in range(Ld - 1, -1, -1):
             W, dW = dec[j][0], gdec[j][0]
             if j > 0:
@@ -607,11 +623,22 @@ class Learner:
         H = spec.tail_input_size
         g = m.grads
         none = ops.ACT["none"]
-        ops.heads_backward(plan.tail_cat[:B], m.Wv_cat, m.Wa_cat, self.dlogits, self.dvalues, self.act, plan.dz_cat[:B],
-                           plan.gWv_cat.view(-1), g["critic_linear.bias"], plan.gWa_cat,
-                           g["action_parameterization.distribution_linear.bias"], plan.db_cat, self.heads_ws)
-        g["critic_linear.weight"].copy_(plan.gWv_cat[:, H:])                                   # (the padded halves are not
-        g["action_parameterization.distribution_linear.weight"].copy_(plan.gWa_cat[:, :H])     #  parameters: dropped)
+        if spec.wide_heads:
+            # logits GEMM backward on the actor half (Wa itself, not the zero-padded Wa_cat), then the critic half's value
+            # term and the column sums of both halves
+            Wv, Wa = m.critic[0], m.actor[0]
+            ops.linear_backward(self.dlogits, plan.tail_cat[:B, :H], Wa, self.act,
+                                g["action_parameterization.distribution_linear.weight"], plan.dz_cat[:B, :H], None,
+                                self.engine, self.lin_ws)
+            ops.heads_wide_backward(plan.tail_cat[:B, H:], Wv, self.dlogits, self.dvalues, self.act, plan.dz_cat[:B], H,
+                                    False, g["critic_linear.weight"].view(-1), g["critic_linear.bias"],
+                                    g["action_parameterization.distribution_linear.bias"], plan.db_cat, self.heads_ws)
+        else:
+            ops.heads_backward(plan.tail_cat[:B], m.Wv_cat, m.Wa_cat, self.dlogits, self.dvalues, self.act, plan.dz_cat[:B],
+                               plan.gWv_cat.view(-1), g["critic_linear.bias"], plan.gWa_cat,
+                               g["action_parameterization.distribution_linear.bias"], plan.db_cat, self.heads_ws)
+            g["critic_linear.weight"].copy_(plan.gWv_cat[:, H:])                                   # (the padded halves are
+            g["action_parameterization.distribution_linear.weight"].copy_(plan.gWa_cat[:, :H])     #  not parameters: dropped)
         for tw, col in (("actor_", 0), ("critic_", H)):
             layers, glayers = m.tower_layers(tw), m.tower_layers(tw, grads=True)
             L = len(layers)

@@ -157,6 +157,27 @@ class ModelSpec:
             return self.num_actions
         return 2 * self.num_actions if self.adaptive_stddev else self.num_actions
 
+    NARROW_HEADS_MAX = 31      # rows the warp-per-row heads kernels hold (lane 0 = value, lanes 1..A = logits)
+    MAX_LINEAR_ACTION_OUTPUTS = 1024
+    MAX_TUPLE_HEADS = 8
+
+    @property
+    def wide_heads(self) -> bool:
+        """distribution_linear has more than 31 rows: the heads run as a GEMM on the regular engine plus
+        sfb200_heads_tail_wide instead of the fused warp-per-row heads kernels"""
+        return self.num_linear_action_outputs > self.NARROW_HEADS_MAX
+
+    def __post_init__(self) -> None:
+        if self.action_segments and len(self.action_segments) > self.MAX_TUPLE_HEADS:
+            raise ValueError(f"Tuple action spaces are supported with at most {self.MAX_TUPLE_HEADS} heads, got "
+                             f"{len(self.action_segments)}")
+        n = self.num_linear_action_outputs
+        if n > self.MAX_LINEAR_ACTION_OUTPUTS:
+            what = (f"Box({self.num_actions}) with adaptive_stddev={self.adaptive_stddev}" if self.continuous else
+                    f"{'Tuple' if self.action_segments else 'Discrete'} with {self.num_actions} logits")
+            raise ValueError(f"{what} needs {n} distribution_linear rows; the device path supports at most "
+                             f"{self.MAX_LINEAR_ACTION_OUTPUTS}")
+
     @property
     def num_action_params(self) -> int:
         """calc_num_action_parameters (action_distributions.py:33-44): width of `action_logits`"""
@@ -257,6 +278,7 @@ class PolicyModel:
     def __init__(self, spec: ModelSpec, device: torch.device, seed: int = 0, policy_init_gain: float = 1.0,
                  policy_initialization: str = "orthogonal"):
         assert policy_initialization in ("orthogonal", "xavier_uniform", "torch_default"), policy_initialization
+        spec.__post_init__()      # (the limits of the heads, also for a spec changed after its construction)
         self.policy_initialization = policy_initialization
         self.spec = spec
         self.device = device

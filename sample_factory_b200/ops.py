@@ -244,6 +244,31 @@ def heads_from_partials_continuous(head_partials: Tensor, P: int, rows: int, bv:
                                 policy_version_scalar, policy_version_out, pv_stride))
 
 
+def heads_tail_wide(h: Tensor, Wv: Tensor, bv: Tensor, logits: Optional[Tensor], logits_stride: int, A: int,
+                    values: Tensor, values_stride: int, noise: Optional[Tensor] = None, philox_seed: int = 0,
+                    philox_offset: int = 0, philox_offset_dev: Optional[Tensor] = None,
+                    actions_f32: Optional[Tensor] = None, actions_stride: int = 0, env_actions: Optional[Tensor] = None,
+                    log_prob: Optional[Tensor] = None, log_prob_stride: int = 0,
+                    policy_version_scalar: Optional[Tensor] = None, policy_version_out: Optional[Tensor] = None,
+                    pv_stride: int = 0, *, head_sizes=None, act_dim: int = 0, adaptive_stddev: bool = True,
+                    learned_log_std: Optional[Tensor] = None, tanh_scale: float = 0.0, continuous: bool = False) -> None:
+    """Heads with more than 31 distribution_linear rows: values = h . Wv + bv and the distribution tail over `logits`
+    rows the caller's distribution_linear GEMM already wrote (A = its rows; see sfb200_heads_tail_wide).  logits None:
+    values only."""
+    rows, H = h.shape
+    assert Wv.is_contiguous() and Wv.numel() == H and (noise is None or noise.is_contiguous())
+    kind = 2 if continuous else (1 if head_sizes else 0)
+    env_ptr = None if env_actions is None else _p(env_actions, F32 if continuous else I32)
+    lib().call("sfb200_heads_tail_wide", _p(h, F32), h.stride(0), rows, H, _p(Wv, F32), _p(bv, F32),
+               None if logits is None else logits.data_ptr(), logits_stride, A, kind, act_dim, int(adaptive_stddev),
+               _p(learned_log_std, F32), float(tanh_scale), len(head_sizes) if head_sizes else 0,
+               _seg_array(head_sizes) if head_sizes else None, values.data_ptr(), values_stride, _p(noise, F32),
+               philox_seed, philox_offset, _p(philox_offset_dev, I64),
+               None if actions_f32 is None else actions_f32.data_ptr(), actions_stride, env_ptr,
+               None if log_prob is None else log_prob.data_ptr(), log_prob_stride, _p(policy_version_scalar, F32),
+               None if policy_version_out is None else policy_version_out.data_ptr(), pv_stride, _stream())
+
+
 # ------------------------------------------------------------------------------------------------ conv encoder
 def im2col(x: Tensor, in_nchw: bool, B: int, C: int, H: int, W: int, kernel: int, stride: int, col: Tensor) -> None:
     """x: [B, C*H*W] rows in (C,H,W) order (in_nchw) or [B*H*W, C] NHWC rows; col: [B*OH*OW, C*kernel*kernel]"""
@@ -782,6 +807,25 @@ def heads_backward(h: Tensor, Wv: Tensor, Wa: Tensor, dlogits: Tensor, dvalues: 
     lib().call("sfb200_heads_backward", _p(h, F32), h.stride(0), rows, H, A, _p(Wv, F32), _p(Wa, F32),
                _p(dlogits, F32), _p(dvalues, F32), act, _p(dz, F32), dz.stride(0), _p(dWv, F32), _p(dbv, F32),
                _p(dWa, F32), _p(dba, F32), _p(db_prev, F32), workspace.data_ptr(), _stream())
+
+
+def heads_wide_backward_workspace_bytes(rows: int, width: int, H: int, A: int) -> int:
+    return lib().query("sfb200_heads_wide_backward_workspace_bytes", rows, width, H, A)
+
+
+def heads_wide_backward(h: Tensor, Wv: Tensor, dlogits: Tensor, dvalues: Tensor, act: int, dz: Tensor, value_col: int,
+                        accumulate: bool, dWv: Tensor, dbv: Tensor, dba: Tensor, db_prev: Optional[Tensor],
+                        workspace: Tensor) -> None:
+    """The wide heads' backward besides the two linear_backward GEMMs (sfb200_heads_wide_backward): the value term of dz,
+    dWv, dbv, dba and db_prev = column sums of dz.  h [rows, H] feeds critic_linear; dz [rows, width]."""
+    rows, H = h.shape
+    A = dlogits.shape[1]
+    width = dz.shape[1]
+    assert dlogits.is_contiguous() and dlogits.shape[0] == rows and dz.shape[0] == rows and Wv.numel() == H
+    assert workspace.numel() * workspace.element_size() >= heads_wide_backward_workspace_bytes(rows, width, H, A)
+    lib().call("sfb200_heads_wide_backward", _p(h, F32), h.stride(0), rows, H, _p(Wv, F32), _p(dlogits, F32), A,
+               _p(dvalues, F32), act, _p(dz, F32), dz.stride(0), width, value_col, int(accumulate), _p(dWv, F32),
+               _p(dbv, F32), _p(dba, F32), _p(db_prev, F32), workspace.data_ptr(), _stream())
 
 
 def linear_backward_workspace_bytes(M: int, N: int, K: int) -> int:

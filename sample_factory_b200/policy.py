@@ -6,6 +6,10 @@ minibatch forward).  When the tensor feeding critic_linear / distribution_linear
 wgmma engine covers the shape, that layer and the heads run as ONE GEMM whose epilogue leaves partial head dot
 products (sfb200_linear_act_heads_forward) followed by a tiny finishing kernel (sfb200_heads_from_partials); the
 activated layer output is stored only if the caller needs it (the learner's backward does, the sampler does not).
+
+Models whose distribution_linear has more than 31 rows (ModelSpec.wide_heads) store the last hidden layer, run
+distribution_linear as a GEMM on the same engine straight into the logits' final place, and finish with
+sfb200_heads_tail_wide (value head + distribution tail, one warp per row).
 """
 from __future__ import annotations
 
@@ -31,6 +35,13 @@ class HeadsPlan:
 
             self.conv = (ResnetHead if spec.is_resnet else ConvHead)(model, engine, max_rows, need_backward)
         self.tail_is_mlp = bool(spec.decoder_mlp_layers) or (not spec.use_rnn and bool(spec.fc_encoder_layers))
+        self.engine = engine
+        # heads wider than 31 rows: no fused-partials path (P stays 0); call sites that sample without keeping the logits
+        # get them in this scratch
+        self.wide = spec.wide_heads
+        self.wide_logits: Optional[Tensor] = None
+        if self.wide and not need_backward:
+            self.wide_logits = torch.empty((max_rows, spec.num_action_params), dtype=torch.float32, device=model.device)
         # separate actor / critic weights: per-tower activations and ONE concatenated tail [rows, 2H] = [actor | critic]
         self.separate = not spec.share_weights
         if self.separate:
@@ -43,14 +54,15 @@ class HeadsPlan:
                 A = spec.num_linear_action_outputs
                 self.tower_dz = {tw: [torch.empty((max_rows, w), **f32) for w in widths[:-1]] for tw in ("actor_", "critic_")}
                 self.dz_cat = torch.empty((max_rows, 2 * H), **f32)
-                self.gWv_cat = torch.empty((1, 2 * H), **f32)
-                self.gWa_cat = torch.empty((A, 2 * H), **f32)
                 self.db_cat = torch.empty(2 * H, **f32)
+                if not self.wide:     # (the wide backward writes the heads' gradients directly)
+                    self.gWv_cat = torch.empty((1, 2 * H), **f32)
+                    self.gWa_cat = torch.empty((A, 2 * H), **f32)
         self.P = 0
         if self.separate:
             return
         self.part: Optional[Tensor] = None
-        if self.tail_is_mlp:
+        if self.tail_is_mlp and not self.wide:
             self.P = ops.linear_heads_partials(spec.tail_input_size, spec.num_linear_action_outputs, engine)
         if self.P > 0:
             self.part = torch.empty(self.P * max_rows * ops.HEAD_PART_PAD, dtype=torch.float32, device=model.device)
@@ -100,7 +112,9 @@ def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, 
                 ops.linear_act_forward(tail, W, b, outs[k][:M], act, engine)
                 tail = outs[k][:M]
             k += 1
-    if finish_fn is not None and fused:
+    if plan.wide:
+        _heads_wide(model, tail, tail, Wv, bv, Wa, ba, plan, M, heads_kwargs)
+    elif finish_fn is not None and fused:
         finish_fn(plan.part, plan.P, M, bv, ba)
     else:
         _heads(model, tail, Wv, bv, Wa, ba, fused, plan, M, heads_kwargs)
@@ -120,10 +134,13 @@ def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan
             out = plan.tail_cat[:M, col: col + H] if k == len(layers) - 1 else plan.tower_h[tw][k][:M]
             ops.linear_act_forward(t, W, b, out, act, engine)
             t = out
-    _, bv = model.critic
-    _, ba = model.actor
+    Wv, bv = model.critic
+    Wa, ba = model.actor
     tail = plan.tail_cat[:M]
-    _heads(model, tail, model.Wv_cat, bv, model.Wa_cat, ba, False, plan, M, heads_kwargs)
+    if plan.wide:     # logits from the actor half, the value from the critic half, with the heads' own weights
+        _heads_wide(model, tail[:, :H], tail[:, H:], Wv, bv, Wa, ba, plan, M, heads_kwargs)
+    else:
+        _heads(model, tail, model.Wv_cat, bv, model.Wa_cat, ba, False, plan, M, heads_kwargs)
     return tail
 
 
@@ -145,3 +162,22 @@ def _heads(model: PolicyModel, tail: Tensor, Wv: Tensor, bv: Tensor, Wa: Tensor,
         ops.heads_from_partials(plan.part, P, M, bv, ba, **heads_kwargs)
     else:
         ops.heads_forward(tail, Wv, bv, Wa, ba, **heads_kwargs)
+
+
+def _heads_wide(model: PolicyModel, tail_a: Tensor, tail_v: Tensor, Wv: Tensor, bv: Tensor, Wa: Tensor, ba: Tensor,
+                plan: HeadsPlan, M: int, heads_kwargs: Dict) -> None:
+    """Wide heads: distribution_linear as a GEMM on the regular engine into the logits' final place (the trajectory slot,
+    the learner's minibatch logits, or the plan's scratch; for a learned stddev the means half of each params row), then
+    sfb200_heads_tail_wide.  A values-only call (the bootstrap value) skips the GEMM."""
+    sp = model.spec
+    kw = dict(heads_kwargs)
+    logits, stride = kw.pop("logits", None), kw.pop("logits_stride", 0)
+    if logits is None and kw.get("actions_f32") is not None:
+        logits, stride = plan.wide_logits, plan.wide_logits.stride(0)
+    A = sp.num_linear_action_outputs
+    if logits is not None:
+        dst = logits.as_strided((M, A), (stride, 1))
+        ops.linear_act_forward(tail_a, Wa, ba, dst, ops.ACT["none"], plan.engine)
+    dk = model.dist_kwargs() if sp.continuous else {}
+    ops.heads_tail_wide(tail_v, Wv, bv, logits, stride, A, head_sizes=sp.action_segments, continuous=sp.continuous,
+                        **dk, **kw)
