@@ -10,10 +10,11 @@
 // roundings applied to them.)
 //
 // One CTA per 128 x 128 output tile (x split-K slice), 384 threads = three warpgroups:
-//   warpgroup 0   : TMA producer (one thread): raw fp32 A and B tiles -> a 4-stage shared-memory ring, mbarrier complete_tx
+//   warpgroup 0   : TMA producer (one thread): raw fp32 A and B tiles -> 3-slot shared-memory rings, mbarrier complete_tx
 //   warpgroups 1-2: consumers.  Per k-block of 32 they split the raw tiles into tf32 hi / lo halves written K-major with the
 //                   128B swizzle wgmma reads, release the raw stage to the producer, then each issues the wgmmas of its
-//                   64 output rows (m64n128k8) and finally runs the epilogue from its accumulator registers.
+//                   64 output rows (m64n128k8) -- while those run, the next k-block is split into the other conversion
+//                   buffer -- and finally runs the epilogue from its accumulator registers.
 // Operands may be K-major ([rows, K], K contiguous) or MN-major ([K, rows], rows contiguous): the backward GEMMs
 // (dX = dZ.W, dW = dZ^T.X) read the activations in the layout the forward pass wrote them -- the split pass transposes
 // MN-major tiles on the fly (tf32 wgmma reads K-major operands only).
@@ -33,27 +34,33 @@ namespace sfb {
 
 // ------------------------------------------------------------------------------------------------ the kernel
 // F16: the fp16-split engine (A K-major with a registered bound |A| <= a_bound[0], B a weight matrix with |w| < 255):
-// A * 2^a_shift and B * 2^kF16WShift are split into fp16 hi + lo * 2^-11 pairs (22 significand bits like the tf32
-// pair, on the fp16 MMA path at twice the tf32 rate); a stage then covers 64 k.
+// A * 2^a_shift is split into fp16 hi + lo * 2^-11 pairs (22 significand bits like the tf32 pair, on the fp16 MMA path at
+// twice the tf32 rate); B = W * 2^kF16WShift in the same form is the weight's registered fp16 twins, which tmap_b (a 3-D
+// fp16 map, planes hi / lo) loads with the 128B swizzle straight into the layout wgmma reads.  A stage covers 64 k.
+// B_MN only names the twin the host chose (the transposed one for dX = dz . W), so dX stays its own instantiation.
 // RES: the residual epilogue (store_tile_residual), forward layout only.
+//
+// Mainloop: the split of stage kb+1 runs while the wgmmas of stage kb are in flight (two conversion buffers).  A and B
+// have their own TMA rings: a raw slot goes back to the producer as soon as it is split, an fp16 B slot (the twin tiles
+// the wgmmas read in place) once its wgmmas have completed.  Every accumulator receives the same wgmmas in the same k order as a serial loop would issue.
 template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false, bool RES = false>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
                   const float* __restrict__ a_bound) {
     static_assert(!F16 || (!A_MN && SPLIT3), "fp16-split engine: K-major activations, 3-pass");
-    using S = TcSmem;
-    constexpr int KBK = F16 ? 64 : TBK;                 // k per pipeline stage
-    constexpr int STAGES = F16 ? TC_STAGES / 2 : TC_STAGES;
-    constexpr int RAW_STAGE = (TBM + TBN) * KBK * 4;
-    constexpr int A_RAW = TBM * KBK * 4;
+    using S = TcSmem<F16>;
+    constexpr int KBK = S::KBK;
+    constexpr int SA = S::A_STAGES, SB = S::B_STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
-    uint8_t* conv = smem + TC_STAGES * S::RAW_STAGE;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(conv + S::CONV);
-    uint64_t* full = bars;                  // raw tiles landed (count 1 + tx)
-    uint64_t* empty = bars + TC_STAGES;     // raw stage read by every consumer thread (count 256)
-    int* s_last = reinterpret_cast<int*>(bars + 2 * TC_STAGES);
+    uint8_t* conv = smem + S::CONV_OFF;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::BARS_OFF);
+    uint64_t* full_a = bars;                // A slot landed (count 1 + tx)
+    uint64_t* empty_a = bars + SA;          // A slot split by every consumer thread (count 256)
+    uint64_t* full_b = bars + 2 * SA;
+    uint64_t* empty_b = bars + 2 * SA + SB; // B slot split (tf32) / read by the completed wgmmas (fp16), count 256
+    int* s_last = reinterpret_cast<int*>(bars + 2 * (SA + SB));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_n = (N + TBN - 1) / TBN;
@@ -63,9 +70,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_b) : "memory");
-        for (int s = 0; s < TC_STAGES; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 256);
+        for (int s = 0; s < SA; ++s) {
+            mbar_init(&full_a[s], 1);
+            mbar_init(&empty_a[s], 256);
+        }
+        for (int s = 0; s < SB; ++s) {
+            mbar_init(&full_b[s], 1);
+            mbar_init(&empty_b[s], 256);
         }
         fence_barrier_init();
     }
@@ -79,15 +90,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         // ===================================================== TMA producer
         if (threadIdx.x == 0) {
             for (int kb = 0; kb < tc.num_kb; ++kb) {
-                const int s = kb % STAGES;
-                mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
-                uint8_t* st = smem + s * RAW_STAGE;
-                mbar_expect_tx(&full[s], RAW_STAGE);
                 const int k0 = tc.k_begin + kb * KBK;
-                if (A_MN) tma_load_2d(st, &tmap_a, &full[s], (int)tc.m0, k0);
-                else tma_load_2d(st, &tmap_a, &full[s], k0, (int)tc.m0);
-                if (B_MN) tma_load_2d(st + A_RAW, &tmap_b, &full[s], tc.n0, k0);
-                else tma_load_2d(st + A_RAW, &tmap_b, &full[s], k0, tc.n0);
+                const int sa = kb % SA, sb = kb % SB;
+                mbar_wait(&empty_a[sa], ((kb / SA) & 1) ^ 1);
+                mbar_expect_tx(&full_a[sa], S::A_RAW);
+                uint8_t* pa = smem + sa * S::A_RAW;
+                if (A_MN) tma_load_2d(pa, &tmap_a, &full_a[sa], (int)tc.m0, k0);
+                else tma_load_2d(pa, &tmap_a, &full_a[sa], k0, (int)tc.m0);
+                mbar_wait(&empty_b[sb], ((kb / SB) & 1) ^ 1);
+                mbar_expect_tx(&full_b[sb], S::B_SLOT);
+                uint8_t* pb = smem + S::B_RING + sb * S::B_SLOT;
+                if (F16) tma_load_3d(pb, &tmap_b, &full_b[sb], k0, tc.n0, 0);   // [hi | lo] twin tiles
+                else if (B_MN) tma_load_2d(pb, &tmap_b, &full_b[sb], tc.n0, k0);
+                else tma_load_2d(pb, &tmap_b, &full_b[sb], k0, tc.n0);
             }
         }
         return;
@@ -96,35 +111,41 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // ===================================================== consumers
     const int ct = threadIdx.x - 128;          // 0..255
     const int wg = ct >> 7;                    // 64-row half of the tile
-    uint8_t* a_hi = conv;
-    uint8_t* a_lo = conv + S::A_BYTES;
-    uint8_t* b_hi = conv + 2 * S::A_BYTES;
-    uint8_t* b_lo = b_hi + S::B_BYTES;
-    const uint64_t da_hi = make_smem_desc(smem_u32(a_hi + wg * 64 * 128));
-    const uint64_t da_lo = make_smem_desc(smem_u32(a_lo + wg * 64 * 128));
-    const uint64_t db_hi = make_smem_desc(smem_u32(b_hi));
-    const uint64_t db_lo = make_smem_desc(smem_u32(b_lo));
 
     // fp16-split engine: binary shift of the A operand from its bound (written by an earlier kernel of the stream)
     const int a_shift = F16 ? f16_shift_for_bound(a_bound[0]) : 0;
-    const float a_scale = pow2f_int(a_shift), b_scale = pow2f_int(kF16WShift);
+    const float a_scale = pow2f_int(a_shift);
+    // split stage kb into conversion buffer kb & 1
+    auto split_stage = [&](int kb) {
+        const int sa = kb % SA, sb = kb % SB;
+        const uint8_t* pa = smem + sa * S::A_RAW;
+        uint8_t* cv = conv + (kb & 1) * S::CONV;
+        mbar_wait(&full_a[sa], (kb / SA) & 1);
+        if constexpr (F16) {
+            split_tile_f16<false>(pa, cv, cv + S::A_HALF, ct, a_scale);
+        } else {
+            split_tile<A_MN, SPLIT3>(pa, cv, cv + S::A_HALF, ct);
+            mbar_wait(&full_b[sb], (kb / SB) & 1);
+            split_tile<B_MN, SPLIT3>(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct);
+            mbar_arrive(&empty_b[sb]);
+        }
+        mbar_arrive(&empty_a[sa]);
+        fence_proxy_async_smem();              // generic-proxy writes -> visible to the tensor core (async proxy)
+    };
     float acc[64], cross[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+    split_stage(0);
+    consumer_sync();
     for (int kb = 0; kb < tc.num_kb; ++kb) {
-        const int s = kb % STAGES;
-        mbar_wait(&full[s], (kb / STAGES) & 1);
-        const uint8_t* st = smem + s * RAW_STAGE;
-        if constexpr (F16) {
-            split_tile_f16<A_MN>(st, a_hi, a_lo, ct, a_scale);
-            split_tile_f16<B_MN>(st + A_RAW, b_hi, b_lo, ct, b_scale);
-        } else {
-            split_tile<A_MN, SPLIT3>(st, a_hi, a_lo, ct);
-            split_tile<B_MN, SPLIT3>(st + A_RAW, b_hi, b_lo, ct);
-        }
-        mbar_arrive(&empty[s]);
-        fence_proxy_async_smem();              // generic-proxy writes -> visible to the tensor core (async proxy)
-        consumer_sync();
+        const int sb = kb % SB;
+        const uint8_t* cv = conv + (kb & 1) * S::CONV;
+        const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
+        const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
+        const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
+        const uint64_t db_hi = make_smem_desc(smem_u32(bt));
+        const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
+        if (F16) mbar_wait(&full_b[sb], (kb / SB) & 1);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < TBK / WG_K; ++k) {
@@ -142,8 +163,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
         }
         wgmma_commit();
+        if (kb + 1 < tc.num_kb) split_stage(kb + 1);   // overlaps the wgmmas just issued
         wgmma_wait_all();
-        consumer_sync();                       // both warpgroups done with the split tiles before they are rewritten
+        if (F16) mbar_arrive(&empty_b[sb]);    // the wgmmas are done with the B twin tiles
+        consumer_sync();                       // split kb+1 complete, buffer kb & 1 free for kb+2, in both warpgroups
     }
     if (F16) {
         // (main + cross * 2^-11) * 2^-(operand shifts): exact power-of-two scalings
@@ -227,6 +250,22 @@ bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1
     return r == CUDA_SUCCESS;
 }
 
+// 3-D fp16 map over a weight's [hi | lo] twins, planes lo_offset elements apart, each plane [rows][K] row-major: box
+// 64 k x 128 rows x both planes with the 128B swizzle, i.e. two [128][64 fp16] tiles in the K-major layout wgmma reads
+// (what split_tile_f16 writes).  False when TMA cannot describe the twins (alignment).
+static bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows) {
+    if ((reinterpret_cast<uintptr_t>(hi) & 15u) || (K * 2) % 16 != 0 || (lo_offset * 2) % 16 != 0 || lo_offset <= 0)
+        return false;
+    cuuint64_t gdim[3] = {K, rows, 2};
+    cuuint64_t gstride[2] = {K * 2, (cuuint64_t)lo_offset * 2};
+    cuuint32_t box[3] = {64, TBN, 2};
+    cuuint32_t estride[3] = {1, 1, 1};
+    CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<uint16_t*>(hi), gdim, gstride, box, estride,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
 // SFB200_TC_F16=0 turns the fp16-split engine off (every 3-pass GEMM then runs the tf32 split; A/B comparison)
 static bool f16_enabled() {
     static int v = -1;
@@ -256,13 +295,14 @@ template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS = false, bool F16 = fals
 static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, int64_t M, int N, int K,
                      int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr) {
     auto kern = gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES>;
+    constexpr int smem = TcSmem<F16>::TOTAL;
     static bool attr_set = false;
     if (!attr_set) {
-        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TcSmem::TOTAL));
+        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr_set = true;
     }
     const int64_t tiles = ceil_div(N, TBN) * ceil_div(M, TBM) * splits;
-    SFB_CUDA_OK(launch_pdl(kern, dim3((unsigned)tiles), dim3(TC_THREADS), (size_t)TcSmem::TOTAL, st, ta, tb, C, ldc, M, N, K,
+    SFB_CUDA_OK(launch_pdl(kern, dim3((unsigned)tiles), dim3(TC_THREADS), (size_t)smem, st, ta, tb, C, ldc, M, N, K,
                            k_chunk, splits, epi, a_bound));
     SFB_LAUNCH_OK();
     return 0;
@@ -276,7 +316,7 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
     if (M > 0x7fffffff || ceil_div(M, TBM) * ceil_div(N, TBN) * 64 > 0x7fffffff) return SFB_TC_UNSUPPORTED;
     // fp16-split engine: A is a K-major activation buffer with a registered bound, B a weight matrix with registered fp16
     // twins (the transposed twins when B is read MN-major, i.e. dX = dz . W: both registrations say that |w| < 255),
-    // K a multiple of the 64-k stage
+    // K a multiple of the 64-k stage.  The kernel reads B from the twins, so a twin TMA cannot describe keeps the tf32 form.
     if (!a_mn && split3 && splits == 1 && K % 64 == 0 && f16_enabled() && epi.mode != 3) {
         const float* a_bound = operand_bound_lookup(A, ((int64_t)(M - 1) * lda + K) * (int64_t)sizeof(float));
         F16Twin tw{nullptr, nullptr};
@@ -284,21 +324,17 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
             if (!b_mn && ldb == K) tw = f16_twin_lookup(B, (int64_t)N * K);
             else if (b_mn && ldb == N) tw = f16_twinT_lookup(B, K, N);
         }
-        if (tw.hi) {
+        // (B(n, k) is twin[n][k] in both cases: W[n][k] forward, the transposed twin [K_w][N_w] for dX)
+        CUtensorMap ta16, tb16;
+        if (tw.hi && make_tmap_f16_twins(&tb16, tw.hi, tw.lo - tw.hi, (uint64_t)K, (uint64_t)N) &&
+            (!epi.head_part || !b_mn)) {
             if (f16_check_enabled()) {
                 // B = W[N][K] row-major (forward) or W[K][N] row-major read along its other axis (dX: twins transposed)
                 const int rc_chk = b_mn ? f16_twins_check(B, tw, K, N, true, st) : f16_twins_check(B, tw, N, K, false, st);
                 if (rc_chk) return rc_chk;
             }
-            CUtensorMap ta16, tb16;
-            bool ok16 = make_tmap(&ta16, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, 64, TBM);
-            if (b_mn) ok16 = ok16 && make_tmap(&tb16, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, TBN, 64);
-            else ok16 = ok16 && make_tmap(&tb16, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, 64, TBN);
-            if (!ok16) return SFB_TC_UNSUPPORTED;
-            if (epi.head_part) {
-                if (b_mn) return SFB_TC_UNSUPPORTED;
-                return launch_tc<false, false, true, true, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound);
-            }
+            if (!make_tmap(&ta16, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, 64, TBM)) return SFB_TC_UNSUPPORTED;
+            if (epi.head_part) return launch_tc<false, false, true, true, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound);
             return b_mn ? launch_tc<false, true, true, false, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound)
                         : launch_tc<false, false, true, false, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound);
         }

@@ -55,6 +55,14 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
         : "memory");
 }
 
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1, int c2) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+            smem_u32(smem_dst)),
+        "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -118,10 +126,6 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
 // byte offset of element (row, k) of a K-major [rows][32 fp32] tile in the 128B-swizzled layout
 __device__ __forceinline__ uint32_t sw128_offset(int row, int k) {
     return (uint32_t)(row * 128 + ((((k >> 2) ^ row) & 7) << 4) + (k & 3) * 4);
-}
-// the same for a K-major [rows][64 fp16] tile (128 B rows as well, 8 halfs per 16 B chunk)
-__device__ __forceinline__ uint32_t sw128_offset_h(int row, int k) {
-    return (uint32_t)(row * 128 + ((((k >> 3) ^ row) & 7) << 4) + (k & 7) * 2);
 }
 
 template <int ACT>

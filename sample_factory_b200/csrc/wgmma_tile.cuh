@@ -30,16 +30,32 @@ struct TcEpilogue {
 
 constexpr int kHeadAP = 9;     // value + up to 8 action outputs
 constexpr int kHeadPad = 12;   // floats per (partial, row): three 16 B stores
-constexpr int TC_STAGES = 4;
 constexpr int TC_THREADS = 384;
 
+// Shared memory of gemm_wgmma_kernel: a ring of A_STAGES TMA slots for the raw A tile, a ring of B_STAGES slots for the B
+// tile, two conversion buffers (the split of stage kb+1 is written into one while the wgmmas of stage kb read the other),
+// the mbarriers.
+//   tf32 form: raw A / raw B fp32 tiles of 32 k (16 KB each, both released once split); conversion buffer =
+//              [A hi | A lo | B hi | B lo] (64 KB)
+//   fp16 form: raw A fp32 tile of 64 k (32 KB, released once split); B = the weight tile's fp16 [hi | lo] twins, TMA-loaded
+//              in the swizzled layout wgmma reads (32 KB, released once its wgmmas completed); conversion buffer =
+//              [A hi | A lo] (32 KB)
+template <bool F16>
 struct TcSmem {
-    static constexpr int A_BYTES = TBM * TBK * 4;                 // 16 KB
-    static constexpr int B_BYTES = TBN * TBK * 4;                 // 16 KB
-    static constexpr int RAW_STAGE = A_BYTES + B_BYTES;
-    static constexpr int CONV = 2 * A_BYTES + 2 * B_BYTES;        // [A hi | A lo | B hi | B lo], swizzled K-major
-    static constexpr int BARS = 2 * TC_STAGES * 8 + 16;
-    static constexpr int TOTAL = 1024 /*align slack*/ + TC_STAGES * RAW_STAGE + CONV + BARS;
+    static constexpr int KBK = F16 ? 64 : TBK;                    // k per stage
+    static constexpr int A_STAGES = F16 ? 2 : 3;
+    static constexpr int B_STAGES = 3;
+    static constexpr int A_RAW = TBM * KBK * 4;
+    static constexpr int B_SLOT = F16 ? 2 * TBN * 64 * 2 : TBN * TBK * 4;
+    static constexpr int A_HALF = TBM * 128;                      // one split half of A: [128 rows][128 B], swizzled K-major
+    static constexpr int B_HALF = TBN * 128;
+    static constexpr int CONV = F16 ? 2 * A_HALF : 2 * A_HALF + 2 * B_HALF;
+    static constexpr int B_RING = A_STAGES * A_RAW;               // offsets from the 1024-aligned base
+    static constexpr int CONV_OFF = B_RING + B_STAGES * B_SLOT;
+    static constexpr int BARS_OFF = CONV_OFF + 2 * CONV;
+    static constexpr int BARS = 2 * (A_STAGES + B_STAGES) * 8 + 16;
+    static constexpr int TOTAL = 1024 /*align slack*/ + BARS_OFF + BARS;
+    static_assert(TOTAL <= 227 * 1024, "shared memory");
 };
 
 // ELU via the fast exponential: |error| <= ~2.4e-7 absolute (2 ulp of exp on [0,1]) -- inside the 1e-5 parity budget
@@ -51,7 +67,7 @@ __device__ __forceinline__ float act_fwd_fast(float z, int act) {
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // raw tile (TMA, no swizzle) -> tf32 hi / lo halves in the swizzled K-major layout.  K-major raw: [rows][32 k];
-// MN-major raw: [32 k][rows].  ct = consumer thread 0..255.
+// MN-major raw: [32 k][rows] (transposed on the way).  ct = consumer thread 0..255.
 template <bool MN, bool SPLIT3>
 __device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct) {
 #pragma unroll
@@ -74,46 +90,44 @@ __device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint
             *reinterpret_cast<uint4*>(hi + off) = h;
             if (SPLIT3) *reinterpret_cast<uint4*>(lo + off) = l;
         } else {
-            const int k = i >> 5, r0 = (i & 31) * 4;                   // rows r0 .. r0+3 at k
+            // item i = (row r, 4-k chunk c): four scalar loads down column r of the [32 k][128 rows] raw tile (a warp
+            // reads 32 consecutive rows of one k: 32 banks), one 16 B store per half (the 8 rows of a quarter-warp land
+            // in 8 distinct swizzled chunks: no bank conflict)
+            const int r = i & 127, c = i >> 7;
+            const float* col = reinterpret_cast<const float*>(raw) + c * 4 * TBM + r;
+            const uint32_t off = (uint32_t)(r * 128 + (((c ^ r) & 7) << 4));
+            uint4 h, l;
+            uint32_t* hp = &h.x;
+            uint32_t* lp = &l.x;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const uint32_t w = __float_as_uint(e[j]);
-                const uint32_t off = sw128_offset(r0 + j, k);
-                *reinterpret_cast<uint32_t*>(hi + off) = SPLIT3 ? (w & 0xffffe000u) : w;
-                if (SPLIT3) *reinterpret_cast<uint32_t*>(lo + off) = tf32_lo_bits(w);
+                const uint32_t w = __float_as_uint(col[j * TBM]);
+                hp[j] = SPLIT3 ? (w & 0xffffe000u) : w;
+                lp[j] = tf32_lo_bits(w);
             }
+            *reinterpret_cast<uint4*>(hi + off) = h;
+            if (SPLIT3) *reinterpret_cast<uint4*>(lo + off) = l;
         }
     }
 }
 
-// fp16-split engine: raw fp32 tile of 64 k -> scaled fp16 hi / lo halves (lo carries a 2^11 factor, common.cuh) in the
-// swizzled K-major [rows][64 fp16] layout.  K-major raw: [rows][64 k]; MN-major raw: [64 k][rows].
+// fp16-split engine: raw fp32 K-major tile [rows][64 k] -> scaled fp16 hi / lo halves (lo carries a 2^11 factor,
+// common.cuh) in the swizzled K-major [rows][64 fp16] layout.  (MN-major operands never take the fp16 form: the weight
+// operand of dX comes from its transposed twins instead, gemm_tc.cu.)
 template <bool MN>
 __device__ __forceinline__ void split_tile_f16(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct, float scale) {
+    static_assert(!MN, "fp16 split: K-major tiles only");
 #pragma unroll 4
     for (int q = 0; q < (TBM * 64 / 4) / 256; ++q) {
         const int i = ct + 256 * q;
         const float4 v = reinterpret_cast<const float4*>(raw)[i];
-        if (!MN) {
-            const int r = i >> 4, c4 = i & 15;                         // row r, k = 4*c4 .. 4*c4+3
-            const uint32_t off = (uint32_t)(r * 128 + ((((c4 >> 1) ^ r) & 7) << 4) + (c4 & 1) * 8);
-            uint2 h, l;
-            f16_split2(v.x * scale, v.y * scale, h.x, l.x);
-            f16_split2(v.z * scale, v.w * scale, h.y, l.y);
-            *reinterpret_cast<uint2*>(hi + off) = h;
-            *reinterpret_cast<uint2*>(lo + off) = l;
-        } else {
-            const int k = i >> 5, r0 = (i & 31) * 4;                   // rows r0 .. r0+3 at k
-            const float e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                uint16_t h, l;
-                f16_split1(e[j] * scale, h, l);
-                const uint32_t off = sw128_offset_h(r0 + j, k);
-                *reinterpret_cast<uint16_t*>(hi + off) = h;
-                *reinterpret_cast<uint16_t*>(lo + off) = l;
-            }
-        }
+        const int r = i >> 4, c4 = i & 15;                         // row r, k = 4*c4 .. 4*c4+3
+        const uint32_t off = (uint32_t)(r * 128 + ((((c4 >> 1) ^ r) & 7) << 4) + (c4 & 1) * 8);
+        uint2 h, l;
+        f16_split2(v.x * scale, v.y * scale, h.x, l.x);
+        f16_split2(v.z * scale, v.w * scale, h.y, l.y);
+        *reinterpret_cast<uint2*>(hi + off) = h;
+        *reinterpret_cast<uint2*>(lo + off) = l;
     }
 }
 
