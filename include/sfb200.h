@@ -297,6 +297,44 @@ int sfb200_heads_tail_wide(const float* h, int64_t ldh, int64_t rows, int H, con
                            const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
                            void* stream);
 
+/* Tuple action spaces whose members are Discrete(n) or 1-D Box(d) spaces (TupleActionDistribution,
+ * action_distributions.py:197-286, always with ActionParameterizationDefault, actor_critic.py:43-53): num_heads <= 8
+ * members described by two HOST arrays, head_kinds_host (0 = categorical, 1 = Gaussian with state-dependent log-std) and
+ * head_sizes_host (n or d).  distribution_linear has A = sum(n or 2d) rows, split per member in order; a Box member's
+ * rows are [means | log_std].  params (required) receives the A outputs per row; actions_f32 rows hold W = sum(1 or d)
+ * floats (an index per Discrete member, d values per Box member), log_prob the sum over the members.
+ * env_actions_host: NULL or num_heads pointers (each may be NULL): int32 [rows] per Discrete member, float32 [rows, d]
+ * per Box member (preprocess_actions, batched_sampling.py:46-57).  Explicit noise rows hold W' = sum(n or d) floats in
+ * member order, Exp(1) per logit and N(0,1) per Box dimension; under Philox column c of row r uses subsequence r*W' + c
+ * (curand_uniform -> Exp, or curand_normal).  Deterministic mode: argmax per Discrete member, the means per Box member.
+ * Action masks are rejected.  The tail runs one warp per row over the stored params row.
+ *   _from_partials_mixed: finishes the fused GEMM's partials (A <= 11); _forward_mixed: the unfused heads (A <= 31);
+ *   _tail_wide_mixed: A up to 1024, after the distribution_linear GEMM wrote the params rows in place (as
+ *   sfb200_heads_tail_wide; it also computes the values). */
+int sfb200_heads_from_partials_mixed(const float* head_partials, int P, int64_t rows, int A, int num_heads,
+                                     const int32_t* head_kinds_host, const int32_t* head_sizes_host, const float* bv,
+                                     const float* ba, float* values, int64_t values_stride, float* params,
+                                     int64_t params_stride, const float* noise, uint64_t philox_seed,
+                                     uint64_t philox_offset, const int64_t* philox_offset_dev, float* actions_f32,
+                                     int64_t actions_stride, void** env_actions_host, float* log_prob,
+                                     int64_t log_prob_stride, const float* policy_version_scalar,
+                                     float* policy_version_out, int64_t pv_stride, void* stream);
+int sfb200_heads_forward_mixed(const float* h, int64_t ldh, int64_t rows, int H, int A, int num_heads,
+                               const int32_t* head_kinds_host, const int32_t* head_sizes_host, const float* Wv,
+                               const float* bv, const float* Wa, const float* ba, float* values, int64_t values_stride,
+                               float* params, int64_t params_stride, const float* noise, uint64_t philox_seed,
+                               uint64_t philox_offset, const int64_t* philox_offset_dev, float* actions_f32,
+                               int64_t actions_stride, void** env_actions_host, float* log_prob, int64_t log_prob_stride,
+                               const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
+                               void* stream);
+int sfb200_heads_tail_wide_mixed(const float* h, int64_t ldh, int64_t rows, int H, const float* Wv, const float* bv,
+                                 float* params, int64_t params_stride, int A, int num_heads, const int32_t* head_kinds_host,
+                                 const int32_t* head_sizes_host, float* values, int64_t values_stride, const float* noise,
+                                 uint64_t philox_seed, uint64_t philox_offset, const int64_t* philox_offset_dev,
+                                 float* actions_f32, int64_t actions_stride, void** env_actions_host, float* log_prob,
+                                 int64_t log_prob_stride, const float* policy_version_scalar, float* policy_version_out,
+                                 int64_t pv_stride, void* stream);
+
 /* ------------------------------------------------------------- sampler steps ---- */
 /* BatchedVectorEnvRunner.generate_policy_request (algo/sampling/batched_sampling.py:374-388) fused with the
  * inference-side normalisation (inference_worker.py:326):  traj_obs[:, t] = obs ; traj_rnn[:, t] = rnn ;
@@ -470,6 +508,23 @@ int sfb200_ppo_loss_fwd_bwd_continuous(const float* params, const float* values,
                                        float clip_value, float exploration_coeff, float value_coeff, float kl_coeff,
                                        float grad_scale, float* dlogits, float* dlogstd, float* dvalues, double* stats,
                                        void* workspace, void* stream);
+
+/* The same for a Tuple whose members are Discrete(n) or 1-D Box(d) spaces (the layout of the heads' _mixed entry
+ * points): params / params_old / dlogits [B, A], A = sum(n or 2d); actions_f32 [B, W], W = sum(1 or d).  Log-prob,
+ * entropy and KL are sums over the members; a Box member's stddev is clamp(exp(log_std), 1e-4, 1e4) and passes gradient
+ * inside the clamp only.  The exploration term is always the entropy: the reference's ContinuousActionDistribution has
+ * no symmetric_kl_with_uniform_prior.  One warp per sample at every width (A <= 1024); dlogits goes to the existing
+ * heads backward unchanged. */
+int sfb200_action_ratio_mixed(const float* params, int A, int num_heads, const int32_t* head_kinds_host,
+                              const int32_t* head_sizes_host, const float* actions_f32, const float* log_prob_old,
+                              int64_t batch, float* ratio, void* stream);
+int sfb200_ppo_loss_fwd_bwd_mixed(const float* params, const float* values, int A, int num_heads,
+                                  const int32_t* head_kinds_host, const int32_t* head_sizes_host,
+                                  const float* actions_f32, const float* log_prob_old, const float* values_old,
+                                  const float* adv, const float* targets, const uint8_t* valids, const float* params_old,
+                                  int64_t batch, float clip_ratio, float clip_value, float exploration_coeff,
+                                  float value_coeff, float kl_coeff, float grad_scale, float* dlogits, float* dvalues,
+                                  double* stats, void* workspace, void* stream);
 
 /* uint8 observations (image envs: the reference converts with .float() before sub-mean / scale / running-mean-std,
  * utils/normalize.py:40-67): the same three entry points reading uint8 rows; the raw copy into the trajectory stays

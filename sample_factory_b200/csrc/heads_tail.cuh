@@ -191,6 +191,16 @@ __device__ __forceinline__ void tuple_row_tail(float mine, int lane, int A, int6
 }
 
 
+// warp-wide argmax of (best, idx) pairs, first index on ties
+__device__ __forceinline__ void argmax_first(float& best, int& idx) {   // torch.multinomial(p, 1) == argmax(p / q)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+        if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
+    }
+}
+
 // partial head dot products left by the fused GEMM epilogue: part[p][row][kHeadPartPad]
 constexpr int kHeadPartPad = 12;
 

@@ -29,15 +29,6 @@ __device__ __forceinline__ float wide_pick(const float (&v)[LPL], int a, int lan
     return __shfl_sync(0xffffffffu, mine, q & 31);
 }
 
-__device__ __forceinline__ void argmax_first(float& best, int& idx) {   // torch.multinomial(p, 1) == argmax(p / q)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
-    }
-}
-
 struct WideTail {
     const float* h; int64_t ldh; int H; const float* Wv; const float* bv;   // value head input
     float* lg; int64_t ldl;      // logits / [means | log_std] rows, read (and, for a learned stddev, completed) in place

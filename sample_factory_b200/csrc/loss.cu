@@ -2,6 +2,7 @@
 // statistics (:646-647) and the action-ratio pre-pass V-trace needs (:588-594).  One thread per sample; every input
 // is read exactly once (HBM-bound, ~(2A+9)*4 B read + (A+1)*4 B written per sample).
 #include "common.cuh"
+#include "mixed_layout.cuh"
 
 namespace sfb {
 
@@ -914,7 +915,6 @@ __global__ void __launch_bounds__(256) ppo_loss_gauss_wide_kernel(
     }
     ppo_store_partials(acc, part, sm);
 }
-#undef SFB_WIDE_PROLOGUE
 
 // action-ratio pre-pass of V-trace for wide rows: one warp per sample
 template <int LPL>
@@ -960,6 +960,190 @@ __global__ void __launch_bounds__(256) action_ratio_gauss_wide_kernel(const floa
         }
     }
     const float lp = warp_sum(lpp);
+    if (lane == 0) ratio[i] = clampf(expf(lp - lp_old[i]), 0.05f, 20.0f);
+}
+
+// ---- Tuple of Discrete and Box members (mixed_layout.cuh): one warp per sample at every width --------------------
+// Log-prob, entropy and KL are sums over the members; a categorical member normalises over its own logits, a Gaussian
+// member uses the formulas of ppo_loss_gauss_kernel with its [means | log_std] columns.  Slot k of lane l holds params
+// column k*32 + l; a Gaussian slot reads its partner column (log_std of a mean, mean of a log_std) from memory.
+template <int LPL>
+__device__ __forceinline__ float mixed_log_prob(const float* __restrict__ prow, const float* __restrict__ arow,
+                                                const MixedLayout& ml, int lane, const float (&l)[LPL], float (&p)[LPL],
+                                                float (&logp)[LPL], float (&segH)[kMixedMaxHeads], int (&act_idx)[kMixedMaxHeads],
+                                                float& Htot) {
+    float lp = 0.f, lpg = 0.f, hg = 0.f;
+    Htot = 0.f;
+    for (int s = 0; s < ml.K; ++s) {
+        const int po = ml.pofs[s], n = ml.size[s];
+        if (ml.kind[s] == kMixedCategorical) {
+            wide_softmax<LPL>(l, po, po + n, lane, p, logp);
+            act_idx[s] = po + (int)arow[ml.aofs[s]];
+            lp += wide_get<LPL>(logp, act_idx[s], lane);
+            float h = 0.f;
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                const int a = k * 32 + lane;
+                if (a >= po && a < po + n) h -= logp[k] * p[k];
+            }
+            segH[s] = warp_sum(h);
+            Htot += segH[s];
+        } else {
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) {
+                const int a = k * 32 + lane;
+                if (a >= po && a < po + n) {
+                    const float sd = clampf(expf(prow[a + n]), kStdMin, kStdMax);
+                    const float d = arow[ml.aofs[s] + a - po] - l[k];
+                    const float lsd = logf(sd);
+                    lpg += -(d * d) / (2.f * (sd * sd)) - lsd - kHalfLog2PiL;
+                    hg += 0.5f + kHalfLog2PiL + lsd;
+                }
+            }
+        }
+    }
+    Htot += warp_sum(hg);
+    return lp + warp_sum(lpg);
+}
+
+template <int LPL>
+__global__ void __launch_bounds__(256) ppo_loss_mixed_kernel(
+    const float* __restrict__ params, const float* __restrict__ values, const MixedLayout ml,
+    const float* __restrict__ actions, const float* __restrict__ lp_old, const float* __restrict__ v_old,
+    const float* __restrict__ adv, const float* __restrict__ targets, const uint8_t* __restrict__ valids,
+    const float* __restrict__ params_old, int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent,
+    float c_val, float c_kl, float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues,
+    const double* __restrict__ stats, double* __restrict__ part) {
+    SFB_WIDE_PROLOGUE;
+    const int A = ml.A;
+    for (int r = 0; r < 32; ++r) {
+        const int64_t i = base + r;
+        if (i >= batch) break;   // warp-uniform
+        PpoAcc t;
+        const float v = values[i];
+        t.s_v = v;
+        float dl[LPL];
+#pragma unroll
+        for (int k = 0; k < LPL; ++k) dl[k] = 0.f;
+        float dv = 0.f;
+        if (valids[i]) {
+            t.s_cnt = 1.0;
+            const float* prow = params + i * A;
+            const float* orow = params_old ? params_old + i * A : nullptr;
+            const float* arow = actions + i * ml.W;
+            float l[LPL], p[LPL], logp[LPL], lo[LPL], po_[LPL], lq[LPL];
+#pragma unroll
+            for (int k = 0; k < LPL; ++k) { p[k] = 0.f; logp[k] = 0.f; po_[k] = 0.f; lq[k] = 0.f; }
+            wide_load<LPL>(prow, A, lane, l);
+            float segH[kMixedMaxHeads], segKL[kMixedMaxHeads];
+            int act_idx[kMixedMaxHeads];
+            float Htot;
+            const float lp = mixed_log_prob<LPL>(prow, arow, ml, lane, l, p, logp, segH, act_idx, Htot);
+            float kltot = 0.f;
+            if (orow) {
+                wide_load<LPL>(orow, A, lane, lo);
+                float klg = 0.f;
+                for (int s = 0; s < ml.K; ++s) {
+                    const int po = ml.pofs[s], n = ml.size[s];
+                    if (ml.kind[s] == kMixedCategorical) {
+                        wide_softmax<LPL>(lo, po, po + n, lane, po_, lq);
+                        float klp = 0.f;
+#pragma unroll
+                        for (int k = 0; k < LPL; ++k) {
+                            const int a = k * 32 + lane;
+                            if (a >= po && a < po + n) klp += p[k] * (logp[k] - lq[k]);
+                        }
+                        segKL[s] = warp_sum(klp);
+                        kltot += segKL[s];
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < LPL; ++k) {
+                            const int a = k * 32 + lane;
+                            if (a >= po && a < po + n) {
+                                const float sd = clampf(expf(prow[a + n]), kStdMin, kStdMax);
+                                const float sdo = clampf(expf(orow[a + n]), kStdMin, kStdMax);
+                                const float q = sd / sdo, rr = q * q;
+                                const float dq = (l[k] - lo[k]) / sdo;
+                                klg += 0.5f * (rr + dq * dq - 1.f - logf(rr));
+                            }
+                        }
+                    }
+                }
+                kltot += warp_sum(klg);
+                t.s_kl = kltot;
+                t.m_kl = kltot;
+            }
+            const float g_lp = ppo_policy_terms(lp, lp_old[i], adv[i], adv_mean, adv_std, clip_lo, clip_hi, w, t);
+            t.s_ent = Htot;
+            const float we = w * c_ent, wk = (orow ? w * c_kl : 0.f);
+            for (int s = 0; s < ml.K; ++s) {
+                const int po = ml.pofs[s], n = ml.size[s];
+                if (ml.kind[s] == kMixedCategorical) {
+#pragma unroll
+                    for (int k = 0; k < LPL; ++k) {
+                        const int a = k * 32 + lane;
+                        if (a >= po && a < po + n) {
+                            float g = g_lp * ((a == act_idx[s] ? 1.f : 0.f) - p[k]);
+                            g += we * p[k] * (logp[k] + segH[s]);
+                            if (orow) g += wk * p[k] * ((logp[k] - lq[k]) - segKL[s]);
+                            dl[k] = g;
+                        }
+                    }
+                } else {
+#pragma unroll
+                    for (int k = 0; k < LPL; ++k) {
+                        const int a = k * 32 + lane;
+                        if (a < po || a >= po + 2 * n) continue;
+                        const bool is_mean = a < po + n;
+                        const int j = is_mean ? a - po : a - po - n;
+                        const float m = is_mean ? l[k] : prow[po + j];
+                        const float ls = is_mean ? prow[po + n + j] : l[k];
+                        const float ex = expf(ls);
+                        const float sd = clampf(ex, kStdMin, kStdMax);
+                        const float inv_var = 1.f / (sd * sd);
+                        const float dlt = arow[ml.aofs[s] + j] - m;
+                        float g;
+                        if (is_mean) {
+                            g = g_lp * dlt * inv_var;
+                            if (orow) {
+                                const float sdo = clampf(expf(orow[po + n + j]), kStdMin, kStdMax);
+                                g += wk * ((m - orow[po + j]) / sdo) / sdo;
+                            }
+                        } else {
+                            g = g_lp * (dlt * dlt * inv_var - 1.f) - we;
+                            if (orow) {
+                                const float q = sd / clampf(expf(orow[po + n + j]), kStdMin, kStdMax);
+                                g += wk * (q * q - 1.f);
+                            }
+                            g *= (ex >= kStdMin && ex <= kStdMax) ? 1.f : 0.f;   // the clamp passes gradient inside only
+                        }
+                        dl[k] = g;
+                    }
+                }
+            }
+            dv = ppo_value_terms(v, v_old[i], targets[i], clip_value, w, c_val, t);
+        }
+        wide_store<LPL>(dlogits + i * A, A, lane, dl);
+        if (lane == 0) dvalues[i] = dv;
+        if (lane == r) acc = t;
+    }
+    ppo_store_partials(acc, part, sm);
+}
+
+#undef SFB_WIDE_PROLOGUE
+
+template <int LPL>
+__global__ void __launch_bounds__(256) action_ratio_mixed_kernel(const float* __restrict__ params, const MixedLayout ml,
+                                                                 const float* __restrict__ actions,
+                                                                 const float* __restrict__ lp_old, int64_t batch,
+                                                                 float* __restrict__ ratio) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+    if (i >= batch) return;   // warp-uniform
+    float l[LPL], p[LPL], logp[LPL], segH[kMixedMaxHeads], Htot;
+    int act_idx[kMixedMaxHeads];
+    wide_load<LPL>(params + i * ml.A, ml.A, lane, l);
+    const float lp = mixed_log_prob<LPL>(params + i * ml.A, actions + i * ml.W, ml, lane, l, p, logp, segH, act_idx, Htot);
     if (lane == 0) ratio[i] = clampf(expf(lp - lp_old[i]), 0.05f, 20.0f);
 }
 
@@ -1194,5 +1378,56 @@ int sfb200_ppo_loss_fwd_bwd_continuous(const float* params, const float* values,
     SFB_LAUNCH_OK();
     return 0;
 }
+
+// LPL for a mixed row of A params (one warp per sample at every width)
+#define SFB_MIXED_LPL(A, LAUNCH)         \
+    if ((A) <= 32) LAUNCH(1);            \
+    else { SFB_WIDE_LPL(A, LAUNCH); }
+
+int sfb200_action_ratio_mixed(const float* params, int A, int num_heads, const int32_t* head_kinds_host,
+                              const int32_t* head_sizes_host, const float* actions_f32, const float* log_prob_old,
+                              int64_t batch, float* ratio, void* stream) {
+    SFB_CHECK_ARG(params && actions_f32 && log_prob_old && ratio && batch >= 0, "action_ratio_mixed: bad arguments");
+    MixedLayout ml;
+    if (int rc = make_mixed_layout(ml, A, num_heads, head_kinds_host, head_sizes_host, "action_ratio_mixed")) return rc;
+    if (batch == 0) return 0;
+    cudaStream_t st = (cudaStream_t)stream;
+    const unsigned gw = (unsigned)ceil_div(batch, 8);
+#define SFB_ARM(LPL) action_ratio_mixed_kernel<LPL><<<gw, 256, 0, st>>>(params, ml, actions_f32, log_prob_old, batch, ratio)
+    SFB_MIXED_LPL(A, SFB_ARM);
+#undef SFB_ARM
+    SFB_LAUNCH_OK();
+    return 0;
+}
+
+int sfb200_ppo_loss_fwd_bwd_mixed(const float* params, const float* values, int A, int num_heads,
+                                  const int32_t* head_kinds_host, const int32_t* head_sizes_host,
+                                  const float* actions_f32, const float* log_prob_old, const float* values_old,
+                                  const float* adv, const float* targets, const uint8_t* valids, const float* params_old,
+                                  int64_t batch, float clip_ratio, float clip_value, float exploration_coeff,
+                                  float value_coeff, float kl_coeff, float grad_scale, float* dlogits, float* dvalues,
+                                  double* stats, void* workspace, void* stream) {
+    SFB_CHECK_ARG(params && values && actions_f32 && log_prob_old && values_old && adv && targets && valids && dlogits &&
+                      dvalues && stats && workspace && batch > 0, "ppo_loss_fwd_bwd_mixed: bad arguments");
+    MixedLayout ml;
+    if (int rc = make_mixed_layout(ml, A, num_heads, head_kinds_host, head_sizes_host, "ppo_loss_fwd_bwd_mixed")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const float clip_hi = 1.0f + clip_ratio;
+    const float clip_lo = 1.0f / clip_hi;
+    const unsigned g = (unsigned)ceil_div(batch, 256);
+    double* part = (double*)workspace;
+#define SFB_PM(LPL)                                                                                                     \
+    ppo_loss_mixed_kernel<LPL><<<g, 256, 0, st>>>(params, values, ml, actions_f32, log_prob_old, values_old, adv, targets, \
+                                                  valids, params_old, batch, clip_lo, clip_hi, clip_value,               \
+                                                  exploration_coeff, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, \
+                                                  stats, part)
+    SFB_MIXED_LPL(A, SFB_PM);
+#undef SFB_PM
+    SFB_LAUNCH_OK();
+    ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);
+    SFB_LAUNCH_OK();
+    return 0;
+}
+#undef SFB_MIXED_LPL
 
 }  // extern "C"

@@ -86,7 +86,7 @@ class TapeVecEnv:
 
     def __init__(self, tape: Tensor, num_actions: int, term_period: int = 37, trunc_period: int = 11,
                  env_index_offset: int = 0, continuous: bool = False, obs_shape=None, action_segments=None,
-                 with_action_mask: bool = False):
+                 with_action_mask: bool = False, action_heads=None):
         assert tape.is_cuda and tape.dim() == 3 and tape.is_contiguous()
         assert tape.dtype in (torch.float32, torch.uint8)
         self.tape = tape
@@ -101,6 +101,9 @@ class TapeVecEnv:
         # Tuple(Discrete(n_0), ...) action space: actions arrive as int32 [num_agents, K]; reward = actions[:, 0] / num_actions
         # with num_actions = sum(n_k) (same rule as the oracle's env)
         self.action_segments = None if action_segments is None else list(action_segments)
+        # Tuple with Box members ([("discrete", n) | ("box", d), ...], num_actions = distribution_linear rows): actions
+        # arrive as one tensor per member; the reward comes from member 0 by the rule of its kind
+        self.action_heads = None if action_heads is None else [tuple(h) for h in action_heads]
         self.tape_len, self.num_agents, self.obs_dim = tape.shape
         self.num_actions = num_actions
         self.term_period, self.trunc_period = term_period, trunc_period
@@ -139,7 +142,16 @@ class TapeVecEnv:
         return self._obs_out()
 
     def step(self, actions: Tensor) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
-        if self.continuous:
+        if self.action_heads:
+            a0 = actions[0]
+            if self.action_heads[0][0] == "box":
+                ops.tape_env_step_continuous(a0, self.env_index_offset, self.term_period, self.trunc_period,
+                                             self.step_counter, 0, self._tape_w, self._obs_w, self.rew, self.terminated,
+                                             self.truncated)
+            else:
+                ops.tape_env_step(a0, self.num_actions, self.env_index_offset, self.term_period, self.trunc_period,
+                                  self.step_counter, 0, self._tape_w, self._obs_w, self.rew, self.terminated, self.truncated)
+        elif self.continuous:
             ops.tape_env_step_continuous(actions, self.env_index_offset, self.term_period, self.trunc_period,
                                          self.step_counter, 0, self._tape_w, self._obs_w, self.rew, self.terminated,
                                          self.truncated)

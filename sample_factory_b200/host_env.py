@@ -32,6 +32,18 @@ def _space_info(space) -> Tuple[bool, int]:
     return True, int(shape[0])
 
 
+def _tuple_members(space) -> Optional[List[Tuple[str, int]]]:
+    """[("discrete", n) | ("box", d), ...] of a gymnasium-like Tuple action space, None for any other space"""
+    members = getattr(space, "spaces", None)
+    if not isinstance(members, (tuple, list)):
+        return None
+    out = []
+    for m in members:
+        continuous, n = _space_info(m)
+        out.append(("box" if continuous else "discrete", n))
+    return out
+
+
 def _main_obs_space(obs_space):
     """(space of the policy input, key or None).  Dict observation spaces (make_env.py:147-176 wraps everything into
     Dict(obs=...)): the entry "obs" feeds the policy; an "action_mask" entry is consumed by the sampler.  Dicts with other
@@ -70,7 +82,22 @@ class BatchedHostEnv:
         self.obs_uint8 = np.dtype(getattr(obs_space, "dtype", np.float32)) == np.uint8
         self.obs_shape = shape if len(shape) == 3 else None       # (C, H, W) image observations -> ConvEncoder
         self.obs_dim = int(np.prod(shape))
-        self.continuous, self.num_actions = _space_info(e0.action_space)
+        # Tuple action spaces (preprocess_actions, batched_sampling.py:46-57): all-Discrete -> action_segments (the sampler
+        # hands over int32 [n, K]); with Box members -> action_heads (one device tensor per member) and num_actions = the
+        # rows of distribution_linear.  An env receives a Python tuple per step (Tuple.sample()'s layout), a multi-agent env
+        # the list of per-member batches of its agents.
+        members = _tuple_members(e0.action_space)
+        self.action_segments = self.action_heads = None
+        if members is None:
+            self.continuous, self.num_actions = _space_info(e0.action_space)
+        else:
+            self.continuous = False
+            if all(k == "discrete" for k, _ in members):
+                self.action_segments = [n for _, n in members]
+                self.num_actions = sum(self.action_segments)
+            else:
+                self.action_heads = members
+                self.num_actions = sum(n if k == "discrete" else 2 * n for k, n in members)
         self._seed = seed
         self._seeded = False
         n = self.num_agents
@@ -82,8 +109,15 @@ class BatchedHostEnv:
         odt = torch.uint8 if self.obs_uint8 else torch.float32
         self.obs_host = torch.empty((n, self.obs_dim), dtype=odt).pin_memory()
         self.obs = torch.empty((n, self.obs_dim), dtype=odt, device=device)
-        adt, ashape = (torch.float32, (n, self.num_actions)) if self.continuous else (torch.int32, (n,))
-        self.actions_host = torch.empty(ashape, dtype=adt).pin_memory()
+        if self.action_heads:
+            self.actions_host = [torch.empty(n, dtype=torch.int32).pin_memory() if k == "discrete" else
+                                 torch.empty((n, d), dtype=torch.float32).pin_memory() for k, d in self.action_heads]
+        else:
+            if self.continuous:
+                adt, ashape = torch.float32, (n, self.num_actions)
+            else:
+                adt, ashape = torch.int32, ((n, len(self.action_segments)) if self.action_segments else (n,))
+            self.actions_host = torch.empty(ashape, dtype=adt).pin_memory()
         # reward / terminated / truncated travel in ONE packed staging buffer (one H2D copy instead of three)
         self.pack_host = torch.empty(6 * n, dtype=torch.uint8).pin_memory()
         self.rew_host = self.pack_host[: 4 * n].view(torch.float32)
@@ -134,8 +168,13 @@ class BatchedHostEnv:
         return self.step_wait()
 
     def enqueue_actions_d2h(self, actions: Tensor) -> None:
-        """the D2H copy of the actions into the pinned staging buffer (static pointers: may be captured into a CUDA graph)"""
-        self.actions_host.copy_(actions, non_blocking=True)
+        """the D2H copy of the actions into the pinned staging buffer (static pointers: may be captured into a CUDA graph);
+        a Tuple with Box members copies each member's tensor into its own staging buffer"""
+        if self.action_heads:
+            for h, d in zip(self.actions_host, actions):
+                h.copy_(d, non_blocking=True)
+        else:
+            self.actions_host.copy_(actions, non_blocking=True)
 
     def mark_actions_enqueued(self) -> None:
         if not hasattr(self, "_actions_ready"):
@@ -150,13 +189,14 @@ class BatchedHostEnv:
 
     def step_wait(self) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
         self._actions_ready.synchronize()
-        self.d2h_bytes += self.actions_host.numel() * self.actions_host.element_size()
-        a = self.actions_host.numpy()
+        staged = self.actions_host if self.action_heads else [self.actions_host]
+        self.d2h_bytes += sum(h.numel() * h.element_size() for h in staged)
+        a = [h.numpy() for h in staged] if self.action_heads else self.actions_host.numpy()
         rew, term, trunc = self.rew_host.numpy(), self.term_host.numpy(), self.trunc_host.numpy()
         if self.multi_agent:
             return self._step_multi_agent(a, rew, term, trunc)
         for i, e in enumerate(self.envs):
-            obs, r, tm, tr, info = e.step(a[i] if self.continuous else int(a[i]))
+            obs, r, tm, tr, info = e.step(self._env_action(a, i))
             rew[i], term[i], trunc[i] = r, bool(tm), bool(tr)
             if tm or tr:                             # BatchedMultiAgentWrapper auto-reset (make_env.py:89-94)
                 if info:
@@ -168,12 +208,27 @@ class BatchedHostEnv:
         self.h2d_bytes += self.obs_host.numel() * self.obs_host.element_size() + self.pack_host.numel()
         return self._obs_out(), self.rew, self.terminated, self.truncated
 
+    def _env_action(self, a, row: int):
+        """the action of one single-agent env: an int (Discrete), a float32 row (Box), or a tuple with a numpy integer per
+        Discrete member and a float32 ndarray[d] per Box member (Tuple)"""
+        if self.action_heads:
+            return tuple(m[row] if k == "discrete" else m[row].copy() for m, (k, _) in zip(a, self.action_heads))
+        if self.action_segments:
+            return tuple(a[row])
+        return a[row] if self.continuous else int(a[row])
+
     def _step_multi_agent(self, a, rew, term, trunc):
         A = self.agents_per_env
         self.inactive_host.copy_(self.inactive_next)          # the status the agents had when these actions were computed
         nxt = self.inactive_next.numpy()
         for i, e in enumerate(self.envs):
-            acts = [a[i * A + j] if self.continuous else int(a[i * A + j]) for j in range(A)]
+            rows = slice(i * A, (i + 1) * A)
+            if self.action_heads:           # per member: int32 [A] / float32 [A, d] (preprocess_actions)
+                acts = [m[rows].copy() for m in a]
+            elif self.action_segments:
+                acts = [a[rows, k].copy() for k in range(len(self.action_segments))]
+            else:
+                acts = [a[i * A + j] if self.continuous else int(a[i * A + j]) for j in range(A)]
             obs, r, tm, tr, infos = e.step(acts)               # (multi-agent envs auto-reset themselves)
             for j in range(A):
                 row = i * A + j

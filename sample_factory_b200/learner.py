@@ -129,6 +129,9 @@ class Learner:
         assert cfg.exploration_loss == "entropy" or not spec.continuous, (
             "symmetric_kl is defined for categorical distributions only (ContinuousActionDistribution has no "
             "symmetric_kl_with_uniform_prior in the reference either)")
+        if cfg.exploration_loss == "symmetric_kl" and spec.action_heads:
+            raise ValueError("exploration_loss='symmetric_kl' is not defined for Tuple action spaces with Box members: the "
+                             "reference's ContinuousActionDistribution has no symmetric_kl_with_uniform_prior")
         assert not (spec.continuous and spec.adaptive_stddev and spec.continuous_tanh_scale > 0), (
             "continuous_tanh_scale is only read by the non-adaptive parameterization (action_parameterization.py:33-78)")
         # learner.py:498-526, :707-713: minibatches = a random permutation of recurrence-length chunks of the dataset, drawn
@@ -446,7 +449,7 @@ class Learner:
         mbv = self._mb
         x0 = mbv["obs"][sl]
         actions = mbv["actions"][sl]
-        if not spec.continuous and not spec.action_segments:
+        if not spec.continuous and not spec.action_segments and not spec.action_heads:
             actions = actions.view(-1)
         lp_old = mbv["lp_old"][sl]
         logits_old = mbv["logits_old"][sl]
@@ -462,7 +465,9 @@ class Learner:
         Wv, bv = m.critic
         Wa, ba = m.actor
         if cfg.with_vtrace:                                                                          # :602-640
-            if spec.action_segments:
+            if spec.action_heads:
+                ops.action_ratio_mixed(self.mb_logits, spec.head_kinds, spec.head_sizes, actions, lp_old, self.ratio)
+            elif spec.action_segments:
                 ops.action_ratio_tuple(self.mb_logits, spec.action_segments, actions, lp_old, self.ratio)
             elif spec.continuous:
                 ops.action_ratio_continuous(self.mb_logits, actions, lp_old, self.ratio)
@@ -483,7 +488,12 @@ class Learner:
         else:
             ops.adv_stats(adv, valids, loss_stats, None, self.loss_ws)
         # losses forward + backward (:651-657, :779)
-        if spec.action_segments:
+        if spec.action_heads:
+            ops.ppo_loss_fwd_bwd_mixed(self.mb_logits, self.mb_values, spec.head_kinds, spec.head_sizes, actions, lp_old,
+                                       v_old, adv, targets, valids, logits_old, cfg.ppo_clip_ratio, cfg.ppo_clip_value,
+                                       cfg.exploration_loss_coeff, cfg.value_loss_coeff, cfg.kl_loss_coeff, 1.0,
+                                       self.dlogits, self.dvalues, loss_stats, self.loss_ws)
+        elif spec.action_segments:
             ops.ppo_loss_fwd_bwd_tuple(self.mb_logits, self.mb_values, spec.action_segments, actions, lp_old, v_old, adv,
                                        targets, valids, logits_old, cfg.ppo_clip_ratio, cfg.ppo_clip_value,
                                        cfg.exploration_loss_coeff, cfg.value_loss_coeff, cfg.kl_loss_coeff, 1.0,

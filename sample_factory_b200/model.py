@@ -41,6 +41,11 @@ class ModelSpec:
     # Tuple(Discrete(n_0), ..., Discrete(n_{K-1})) action space (action_distributions.py:197-286): the heads' sizes;
     # num_actions is then sum(n_k) (the number of logits)
     action_segments: Optional[List[int]] = None
+    # Tuple action space with at least one Box member: [("discrete", n) | ("box", d), ...] in member order.  The Tuple
+    # always uses ActionParameterizationDefault (actor_critic.py:43-53): distribution_linear has sum(n or 2d) rows, a Box
+    # member's rows are [means | log_std], and adaptive_stddev / continuous_tanh_scale / initial_stddev are not read.
+    # num_actions is then the number of rows.  An all-Discrete list is stored as action_segments instead.
+    action_heads: Optional[List[Tuple[str, int]]] = None
     # image observations: obs_shape = (C, H, W) selects the ConvEncoder (model/encoder.py:88-145); obs_dim = C*H*W and the
     # fully connected layers after the conv head (encoder_conv_mlp_layers) take the place of encoder_mlp_layers
     obs_shape: Optional[Tuple[int, int, int]] = None
@@ -145,6 +150,7 @@ class ModelSpec:
                    obs_uint8=bool(getattr(env, "obs_uint8", False)),
                    share_weights=bool(getattr(cfg, "actor_critic_share_weights", True)),
                    action_segments=(list(env.action_segments) if getattr(env, "action_segments", None) else None),
+                   action_heads=([tuple(h) for h in env.action_heads] if getattr(env, "action_heads", None) else None),
                    continuous=bool(getattr(env, "continuous", False)),
                    adaptive_stddev=bool(getattr(cfg, "adaptive_stddev", True)),
                    continuous_tanh_scale=float(getattr(cfg, "continuous_tanh_scale", 0.0)),
@@ -168,13 +174,28 @@ class ModelSpec:
         return self.num_linear_action_outputs > self.NARROW_HEADS_MAX
 
     def __post_init__(self) -> None:
-        if self.action_segments and len(self.action_segments) > self.MAX_TUPLE_HEADS:
+        if self.action_heads:
+            heads = [(str(k), int(n)) for k, n in self.action_heads]
+            if any(k not in ("discrete", "box") or n < 1 for k, n in heads):
+                raise ValueError(f"action_heads members are ('discrete', n) or ('box', d) with n, d >= 1, got {heads}")
+            if self.continuous or self.action_segments:
+                raise ValueError("action_heads describes the whole action space: continuous / action_segments must be unset")
+            if all(k == "discrete" for k, _ in heads):        # a Tuple of Discretes keeps its own path
+                self.action_segments, self.action_heads = [n for _, n in heads], None
+            else:
+                self.action_heads = heads
+                rows = sum(n if k == "discrete" else 2 * n for k, n in heads)
+                if self.num_actions != rows:
+                    raise ValueError(f"a Tuple with members {heads} has {rows} distribution_linear rows, num_actions is "
+                                     f"{self.num_actions}")
+        tup = self.action_segments or self.action_heads
+        if tup and len(tup) > self.MAX_TUPLE_HEADS:
             raise ValueError(f"Tuple action spaces are supported with at most {self.MAX_TUPLE_HEADS} heads, got "
-                             f"{len(self.action_segments)}")
+                             f"{len(tup)}")
         n = self.num_linear_action_outputs
         if n > self.MAX_LINEAR_ACTION_OUTPUTS:
             what = (f"Box({self.num_actions}) with adaptive_stddev={self.adaptive_stddev}" if self.continuous else
-                    f"{'Tuple' if self.action_segments else 'Discrete'} with {self.num_actions} logits")
+                    f"{'Tuple' if tup else 'Discrete'} with {self.num_actions} logits")
             raise ValueError(f"{what} needs {n} distribution_linear rows; the device path supports at most "
                              f"{self.MAX_LINEAR_ACTION_OUTPUTS}")
 
@@ -188,7 +209,18 @@ class ModelSpec:
         """calc_num_actions (:16-30): width of `actions`"""
         if self.action_segments:
             return len(self.action_segments)
+        if self.action_heads:
+            return sum(1 if k == "discrete" else n for k, n in self.action_heads)
         return self.num_actions if self.continuous else 1
+
+    @property
+    def head_kinds(self) -> List[int]:
+        """action_heads as the kernels' head_kinds (0 = categorical, 1 = Gaussian with state-dependent log-std)"""
+        return [0 if k == "discrete" else 1 for k, _ in self.action_heads]
+
+    @property
+    def head_sizes(self) -> List[int]:
+        return [n for _, n in self.action_heads]
 
     @property
     def hidden(self) -> List[int]:

@@ -269,6 +269,84 @@ def heads_tail_wide(h: Tensor, Wv: Tensor, bv: Tensor, logits: Optional[Tensor],
                None if policy_version_out is None else policy_version_out.data_ptr(), pv_stride, _stream())
 
 
+def _mixed_env_array(env_actions, kinds):
+    """per-member env action tensors -> the host pointer array of the _mixed entry points"""
+    import ctypes
+
+    if env_actions is None:
+        return None
+    assert len(env_actions) == len(kinds)
+    ptrs = []
+    for t, k in zip(env_actions, kinds):
+        assert t is None or t.is_contiguous()
+        ptrs.append(None if t is None else _p(t, F32 if k else I32))
+    return (ctypes.c_void_p * len(ptrs))(*ptrs)
+
+
+def _mixed_sample_args(kinds, noise, philox_seed, philox_offset, philox_offset_dev, actions_f32, actions_stride,
+                       env_actions, log_prob, log_prob_stride, policy_version_scalar, policy_version_out, pv_stride):
+    """the arguments of the _mixed heads entry points from `noise` on"""
+    assert noise is None or noise.is_contiguous()
+    return (_p(noise, F32), philox_seed, philox_offset, _p(philox_offset_dev, I64),
+            None if actions_f32 is None else actions_f32.data_ptr(), actions_stride, _mixed_env_array(env_actions, kinds),
+            None if log_prob is None else log_prob.data_ptr(), log_prob_stride, _p(policy_version_scalar, F32),
+            None if policy_version_out is None else policy_version_out.data_ptr(), pv_stride, _stream())
+
+
+def heads_forward_mixed(h: Tensor, Wv: Tensor, bv: Tensor, Wa: Tensor, ba: Tensor, head_kinds, head_sizes, values: Tensor,
+                        values_stride: int, logits: Tensor, logits_stride: int, noise: Optional[Tensor] = None,
+                        philox_seed: int = 0, philox_offset: int = 0, philox_offset_dev: Optional[Tensor] = None,
+                        actions_f32: Optional[Tensor] = None, actions_stride: int = 0, env_actions=None,
+                        log_prob: Optional[Tensor] = None, log_prob_stride: int = 0,
+                        policy_version_scalar: Optional[Tensor] = None, policy_version_out: Optional[Tensor] = None,
+                        pv_stride: int = 0) -> None:
+    """Tuple of Discrete / Box members (sfb200_heads_forward_mixed): `logits` receives the params rows, `actions_f32`
+    rows hold one index per Discrete member and d values per Box member; env_actions: one tensor per member"""
+    rows, H = h.shape
+    A = Wa.shape[0]
+    assert Wa.is_contiguous() and Wv.is_contiguous()
+    lib().call("sfb200_heads_forward_mixed", _p(h, F32), h.stride(0), rows, H, A, len(head_kinds), _seg_array(head_kinds),
+               _seg_array(head_sizes), _p(Wv, F32), _p(bv, F32), _p(Wa, F32), _p(ba, F32),
+               values.data_ptr(), values_stride, logits.data_ptr(), logits_stride,
+               *_mixed_sample_args(head_kinds, noise, philox_seed, philox_offset, philox_offset_dev, actions_f32,
+                                   actions_stride, env_actions, log_prob, log_prob_stride, policy_version_scalar,
+                                   policy_version_out, pv_stride))
+
+
+def heads_from_partials_mixed(head_partials: Tensor, P: int, rows: int, bv: Tensor, ba: Tensor, head_kinds, head_sizes,
+                              values: Tensor, values_stride: int, logits: Tensor, logits_stride: int,
+                              noise: Optional[Tensor] = None, philox_seed: int = 0, philox_offset: int = 0,
+                              philox_offset_dev: Optional[Tensor] = None, actions_f32: Optional[Tensor] = None,
+                              actions_stride: int = 0, env_actions=None, log_prob: Optional[Tensor] = None,
+                              log_prob_stride: int = 0, policy_version_scalar: Optional[Tensor] = None,
+                              policy_version_out: Optional[Tensor] = None, pv_stride: int = 0) -> None:
+    A = ba.shape[0]
+    lib().call("sfb200_heads_from_partials_mixed", _p(head_partials, F32), P, rows, A, len(head_kinds),
+               _seg_array(head_kinds), _seg_array(head_sizes), _p(bv, F32), _p(ba, F32),
+               values.data_ptr(), values_stride, logits.data_ptr(), logits_stride,
+               *_mixed_sample_args(head_kinds, noise, philox_seed, philox_offset, philox_offset_dev, actions_f32,
+                                   actions_stride, env_actions, log_prob, log_prob_stride, policy_version_scalar,
+                                   policy_version_out, pv_stride))
+
+
+def heads_tail_wide_mixed(h: Tensor, Wv: Tensor, bv: Tensor, logits: Tensor, logits_stride: int, A: int, head_kinds,
+                          head_sizes, values: Tensor, values_stride: int, noise: Optional[Tensor] = None,
+                          philox_seed: int = 0, philox_offset: int = 0, philox_offset_dev: Optional[Tensor] = None,
+                          actions_f32: Optional[Tensor] = None, actions_stride: int = 0, env_actions=None,
+                          log_prob: Optional[Tensor] = None, log_prob_stride: int = 0,
+                          policy_version_scalar: Optional[Tensor] = None, policy_version_out: Optional[Tensor] = None,
+                          pv_stride: int = 0) -> None:
+    """values = h . Wv + bv and the mixed Tuple tail over `logits` rows the distribution_linear GEMM already wrote"""
+    rows, H = h.shape
+    assert Wv.is_contiguous() and Wv.numel() == H
+    lib().call("sfb200_heads_tail_wide_mixed", _p(h, F32), h.stride(0), rows, H, _p(Wv, F32), _p(bv, F32),
+               logits.data_ptr(), logits_stride, A, len(head_kinds), _seg_array(head_kinds), _seg_array(head_sizes),
+               values.data_ptr(), values_stride,
+               *_mixed_sample_args(head_kinds, noise, philox_seed, philox_offset, philox_offset_dev, actions_f32,
+                                   actions_stride, env_actions, log_prob, log_prob_stride, policy_version_scalar,
+                                   policy_version_out, pv_stride))
+
+
 # ------------------------------------------------------------------------------------------------ conv encoder
 def im2col(x: Tensor, in_nchw: bool, B: int, C: int, H: int, W: int, kernel: int, stride: int, col: Tensor) -> None:
     """x: [B, C*H*W] rows in (C,H,W) order (in_nchw) or [B*H*W, C] NHWC rows; col: [B*OH*OW, C*kernel*kernel]"""
@@ -792,6 +870,32 @@ def ppo_loss_fwd_bwd_continuous(params: Tensor, values: Tensor, adaptive_stddev:
                _p(targets, F32), _p(valids, U8), _p(params_old, F32), B, clip_ratio, clip_value, exploration_coeff,
                value_coeff, kl_coeff, grad_scale, _p(dlogits, F32), _p(dlogstd, F32), _p(dvalues, F32), _p(stats, F64),
                workspace.data_ptr(), _stream())
+
+
+def action_ratio_mixed(params: Tensor, head_kinds, head_sizes, actions_f32: Tensor, log_prob_old: Tensor,
+                       ratio: Tensor) -> None:
+    B, A = params.shape
+    assert params.is_contiguous() and actions_f32.is_contiguous()
+    lib().call("sfb200_action_ratio_mixed", _p(params, F32), A, len(head_kinds), _seg_array(head_kinds),
+               _seg_array(head_sizes), _p(actions_f32, F32), _p(log_prob_old, F32), B, _p(ratio, F32), _stream())
+
+
+def ppo_loss_fwd_bwd_mixed(params: Tensor, values: Tensor, head_kinds, head_sizes, actions_f32: Tensor,
+                           log_prob_old: Tensor, values_old: Tensor, adv: Tensor, targets: Tensor, valids: Tensor,
+                           params_old: Optional[Tensor], clip_ratio: float, clip_value: float, exploration_coeff: float,
+                           value_coeff: float, kl_coeff: float, grad_scale: float, dlogits: Tensor, dvalues: Tensor,
+                           stats: Tensor, workspace: Tensor) -> None:
+    """Tuple of Discrete / Box members: params / params_old / dlogits [B, A], actions_f32 [B, W] (see
+    sfb200_ppo_loss_fwd_bwd_mixed); the exploration term is the entropy"""
+    B, A = params.shape
+    assert params.is_contiguous() and dlogits.is_contiguous() and actions_f32.is_contiguous()
+    assert params_old is None or params_old.is_contiguous()
+    assert workspace.numel() * workspace.element_size() >= loss_workspace_bytes(B)
+    lib().call("sfb200_ppo_loss_fwd_bwd_mixed", _p(params, F32), _p(values, F32), A, len(head_kinds),
+               _seg_array(head_kinds), _seg_array(head_sizes), _p(actions_f32, F32), _p(log_prob_old, F32),
+               _p(values_old, F32), _p(adv, F32), _p(targets, F32), _p(valids, U8), _p(params_old, F32), B, clip_ratio,
+               clip_value, exploration_coeff, value_coeff, kl_coeff, grad_scale, _p(dlogits, F32), _p(dvalues, F32),
+               _p(stats, F64), workspace.data_ptr(), _stream())
 
 
 # ------------------------------------------------------------------------------------------------ learner: backward

@@ -37,10 +37,10 @@ class HeadsPlan:
         self.tail_is_mlp = bool(spec.decoder_mlp_layers) or (not spec.use_rnn and bool(spec.fc_encoder_layers))
         self.engine = engine
         # heads wider than 31 rows: no fused-partials path (P stays 0); call sites that sample without keeping the logits
-        # get them in this scratch
+        # get them in this scratch (so do Tuples with Box members, whose tail reads the stored params rows)
         self.wide = spec.wide_heads
         self.wide_logits: Optional[Tensor] = None
-        if self.wide and not need_backward:
+        if (self.wide or spec.action_heads) and not need_backward:
             self.wide_logits = torch.empty((max_rows, spec.num_action_params), dtype=torch.float32, device=model.device)
         # separate actor / critic weights: per-tower activations and ONE concatenated tail [rows, 2H] = [actor | critic]
         self.separate = not spec.share_weights
@@ -70,7 +70,7 @@ class HeadsPlan:
             # counters).  One launch less per policy step, but the finishing CTA walks its 128 rows 16 deep per warp while
             # heads_from_partials is fully parallel, so the separate launch stays the default.
             self.counters = torch.zeros((max_rows + 127) // 128, dtype=torch.int32, device=model.device)
-            self.finish_in_gemm = os.environ.get("SFB200_HEADS_FINISH_IN_GEMM", "0") == "1"
+            self.finish_in_gemm = os.environ.get("SFB200_HEADS_FINISH_IN_GEMM", "0") == "1" and not spec.action_heads
 
 
 def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, engine: int, plan: HeadsPlan,
@@ -147,6 +147,15 @@ def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan
 def _heads(model: PolicyModel, tail: Tensor, Wv: Tensor, bv: Tensor, Wa: Tensor, ba: Tensor, fused: bool, plan: HeadsPlan,
            M: int, heads_kwargs: Dict) -> None:
     P = plan.P
+    sp = model.spec
+    if sp.action_heads and heads_kwargs.get("actions_f32") is not None:
+        # Tuple with Box members: the params rows are stored (the plan's scratch if the caller keeps none), then the tail
+        kw = _mixed_kwargs(plan, heads_kwargs)
+        if fused:
+            ops.heads_from_partials_mixed(plan.part, P, M, bv, ba, sp.head_kinds, sp.head_sizes, **kw)
+        else:
+            ops.heads_forward_mixed(tail, Wv, bv, Wa, ba, sp.head_kinds, sp.head_sizes, **kw)
+        return
     if model.spec.continuous:   # Box action space: Gaussian heads (action_distributions.py:290-323)
         dk = model.dist_kwargs()
         if fused:
@@ -178,6 +187,17 @@ def _heads_wide(model: PolicyModel, tail_a: Tensor, tail_v: Tensor, Wv: Tensor, 
     if logits is not None:
         dst = logits.as_strided((M, A), (stride, 1))
         ops.linear_act_forward(tail_a, Wa, ba, dst, ops.ACT["none"], plan.engine)
+    if sp.action_heads and kw.get("actions_f32") is not None:
+        ops.heads_tail_wide_mixed(tail_v, Wv, bv, logits, stride, A, sp.head_kinds, sp.head_sizes, **kw)
+        return
     dk = model.dist_kwargs() if sp.continuous else {}
     ops.heads_tail_wide(tail_v, Wv, bv, logits, stride, A, head_sizes=sp.action_segments, continuous=sp.continuous,
                         **dk, **kw)
+
+
+def _mixed_kwargs(plan: HeadsPlan, heads_kwargs: Dict) -> Dict:
+    """heads_kwargs with a params destination: the caller's logits rows, else the plan's scratch"""
+    kw = dict(heads_kwargs)
+    if kw.get("logits") is None:
+        kw["logits"], kw["logits_stride"] = plan.wide_logits, plan.wide_logits.stride(0)
+    return kw

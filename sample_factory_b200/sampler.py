@@ -61,6 +61,9 @@ class DeviceSampler:
         # for a Box action space
         if spec.continuous:
             self.env_actions = torch.empty((self.N, spec.num_actions), dtype=torch.float32, device=dev)
+        elif spec.action_heads:         # Tuple with Box members: one tensor per member (batched_sampling.py:46-57)
+            self.env_actions = [torch.empty(self.N, dtype=torch.int32, device=dev) if k == "discrete" else
+                                torch.empty((self.N, n), dtype=torch.float32, device=dev) for k, n in spec.action_heads]
         elif spec.action_segments:      # Tuple of Discretes: int32 [N, K] (batched_sampling.py:40-41)
             self.env_actions = torch.empty((self.N, len(spec.action_segments)), dtype=torch.int32, device=dev)
         else:
@@ -110,7 +113,7 @@ class DeviceSampler:
                            not env.continuous and not env.action_segments and not env.with_action_mask and
                            not env.obs_uint8 and self.rnn is None and self.heads_plan.P > 0 and
                            not self.heads_plan.finish_in_gemm and not self.heads_plan.separate and
-                           not spec.continuous and not spec.action_segments)
+                           not spec.continuous and not spec.action_segments and not spec.action_heads)
         # Whole rollout as ONE persistent kernel (csrc/rollout_fused.cu): clusters of H2/128 CTAs own a 128-env row block for
         # all T steps.  Same conditions as the fused tail plus a two-layer MLP the kernel covers.  SFB200_ROLLOUT_FUSED=0
         # restores the per-step launches.
@@ -129,7 +132,7 @@ class DeviceSampler:
         mask = obs.get("action_mask")
         if mask is not None:
             spec = self.model.spec
-            if spec.continuous or spec.action_segments:
+            if spec.continuous or spec.action_segments or spec.action_heads:
                 raise NotImplementedError("action masks are supported for plain Discrete action spaces only")
             if self.action_mask is None:
                 self.action_mask = torch.empty((self.N, spec.num_actions), dtype=torch.bool, device=self.device)
