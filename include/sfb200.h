@@ -628,7 +628,8 @@ int64_t sfb200_colsum_workspace_bytes(int N);
 int sfb200_colsum(const float* x, int64_t ldx, int64_t M, int N, float* out, void* workspace, void* stream);
 
 /* ------------------------------------------------------------- recurrent core ---- */
-/* model/core.py:19-64 (ModelCoreRNN: nn.GRU / nn.LSTM, one layer).  The two gate GEMMs gi = x.W_ih^T + b_ih and
+/* model/core.py:19-64 (ModelCoreRNN: nn.GRU / nn.LSTM), one layer per call; a stacked core's layer passes its slice of
+ * the layer-major state rows as a pointer offset with the full row stride.  The two gate GEMMs gi = x.W_ih^T + b_ih and
  * gh = h.W_hh^T + b_hh are sfb200_linear_act_forward calls (act NONE); these kernels do the cell math.
  * GRU (gates r,z,n):  r = s(gi_r+gh_r), z = s(gi_z+gh_z), n = tanh(gi_n + r*gh_n), h' = (1-z)*n + z*h
  *   h_out  [M,H]   the new state / core output

@@ -201,8 +201,8 @@ def verify_cfg(cfg, num_agents_total: Optional[int] = None) -> bool:
             cfg_error(f"sync mode: samples per training iteration ({cfg.num_batches_per_epoch=} * {cfg.batch_size=} = "
                       f"{per_iteration}) and samples per rollout ({samples}) must divide one another")
     # values the argument parser accepts (reference surface) that the kernel path does not implement: refuse with a reason
-    if getattr(cfg, "rnn_num_layers", 1) != 1:
-        cfg_error(f"{cfg.rnn_num_layers=}: the device path implements the one-layer recurrent core (model/core.py:27-64)")
+    if getattr(cfg, "rnn_num_layers", 1) < 1:
+        cfg_error(f"{cfg.rnn_num_layers=} must be >= 1 (the number of stacked GRU / LSTM layers, model/core.py:27-31)")
     if getattr(cfg, "num_policies", 1) < 1:
         cfg_error(f"{cfg.num_policies=} must be >= 1")
     if cfg.use_rnn:                                                                                         # :187-194

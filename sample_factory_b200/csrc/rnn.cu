@@ -1,6 +1,7 @@
-// Recurrent core (reference model/core.py:19-64: nn.GRU / nn.LSTM, one layer) as elementwise cell kernels around the
-// GEMM engine:  gi = x.W_ih^T + b_ih  and  gh = h.W_hh^T + b_hh  are sfb200_linear_act_forward calls, the kernels here
-// do the gate math forward and backward.  All HBM-bound streaming kernels (one pass over the gate tensors).
+// Recurrent core (reference model/core.py:19-64: nn.GRU / nn.LSTM) as elementwise cell kernels around the GEMM engine,
+// one layer per call:  gi = x.W_ih^T + b_ih  and  gh = h.W_hh^T + b_hh  are sfb200_linear_act_forward calls, the kernels
+// here do the gate math forward and backward.  Stacked layers pass their slice of the layer-major state rows as a
+// pointer offset with the full row stride (rnn_core.py).  All HBM-bound streaming kernels (one pass over the gate tensors).
 // Episode-boundary handling (batched_sampling.py:332-335, rnn_utils.py:143-149): a row whose `reset` flag is set starts
 // the NEXT step from a zero state, and no gradient flows back across that boundary.
 #include "common.cuh"

@@ -30,7 +30,7 @@ class ModelSpec:
     normalize_returns: bool = True
     obs_subtract_mean: float = 0.0
     obs_scale: float = 1.0
-    use_rnn: bool = False        # model/core.py: ModelCoreRNN (one layer) between encoder and decoder
+    use_rnn: bool = False        # model/core.py: ModelCoreRNN between encoder and decoder (rnn_num_layers layers)
     rnn_type: str = "gru"
     rnn_size: int = 512
     # Box action space (action_distributions.py:290-323): num_actions is then the action DIMENSION
@@ -55,6 +55,9 @@ class ModelSpec:
     # False -> ActorCriticSeparateWeights (model/actor_critic.py:198-322): an actor tower (encoder + decoder MLP) feeding
     # distribution_linear and a critic tower feeding critic_linear; vector observations, no recurrent core on this path
     share_weights: bool = True
+    # stacked recurrent core: nn.GRU / nn.LSTM(in, rnn_size, rnn_num_layers) (model/core.py:27-31); layer k > 0 reads
+    # layer k-1's new h, the state rows are layer-major [h_0 | h_1 | ...] (GRU) / [h_0 | c_0 | h_1 | c_1 | ...] (LSTM)
+    rnn_num_layers: int = 1
 
     CONV_ARCH = {  # model/encoder.py:127-134: (out_channels, kernel, stride); no padding
         "convnet_simple": [(32, 8, 4), (64, 4, 2), (128, 3, 2)],
@@ -154,7 +157,8 @@ class ModelSpec:
                    continuous=bool(getattr(env, "continuous", False)),
                    adaptive_stddev=bool(getattr(cfg, "adaptive_stddev", True)),
                    continuous_tanh_scale=float(getattr(cfg, "continuous_tanh_scale", 0.0)),
-                   initial_stddev=float(getattr(cfg, "initial_stddev", 1.0)))
+                   initial_stddev=float(getattr(cfg, "initial_stddev", 1.0)),
+                   rnn_num_layers=int(getattr(cfg, "rnn_num_layers", 1)))
 
     @property
     def num_linear_action_outputs(self) -> int:
@@ -174,6 +178,8 @@ class ModelSpec:
         return self.num_linear_action_outputs > self.NARROW_HEADS_MAX
 
     def __post_init__(self) -> None:
+        if self.use_rnn and self.rnn_num_layers < 1:
+            raise ValueError(f"rnn_num_layers must be >= 1, got {self.rnn_num_layers}")
         if self.action_heads:
             heads = [(str(k), int(n)) for k, n in self.action_heads]
             if any(k not in ("discrete", "box") or n < 1 for k, n in heads):
@@ -232,6 +238,11 @@ class ModelSpec:
         """model/model_utils.py:11-24"""
         if not self.use_rnn:
             return 1 if self.share_weights else 2       # "actor and critic need separate states" (model_utils.py:20-22)
+        return self.rnn_layer_state_size * self.rnn_num_layers
+
+    @property
+    def rnn_layer_state_size(self) -> int:
+        """width of one layer's slice of a state row: h (GRU) or [h | c] (LSTM)"""
         return self.rnn_size * (2 if self.rnn_type == "lstm" else 1)
 
     @property
@@ -283,9 +294,10 @@ class ModelSpec:
             d = h
         if self.use_rnn:
             G, H = self.rnn_gates, self.rnn_size
-            out += [("core.core.weight_ih_l0", (G * H, d)), ("core.core.weight_hh_l0", (G * H, H)),
-                    ("core.core.bias_ih_l0", (G * H,)), ("core.core.bias_hh_l0", (G * H,))]
-            d = H
+            for k in range(self.rnn_num_layers):      # nn.GRU / nn.LSTM registration order: per layer ih, hh, biases
+                out += [(f"core.core.weight_ih_l{k}", (G * H, d)), (f"core.core.weight_hh_l{k}", (G * H, H)),
+                        (f"core.core.bias_ih_l{k}", (G * H,)), (f"core.core.bias_hh_l{k}", (G * H,))]
+                d = H
         for i, h in enumerate(self.decoder_mlp_layers):
             out.append((f"decoder.mlp.{2 * i}.weight", (h, d)))
             out.append((f"decoder.mlp.{2 * i}.bias", (h,)))
@@ -521,11 +533,12 @@ class PolicyModel:
         return [(src[f"decoder.mlp.{2 * i}.weight"], src[f"decoder.mlp.{2 * i}.bias"])
                 for i in range(len(self.spec.decoder_mlp_layers))]
 
-    def rnn_params(self, grads: bool = False) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
-        """(W_ih [G*H, in], W_hh [G*H, H], b_ih, b_hh) of the one-layer GRU/LSTM core"""
+    def rnn_params(self, grads: bool = False, layer: int = 0) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """(W_ih [G*H, in], W_hh [G*H, H], b_ih, b_hh) of one layer of the GRU/LSTM core (in = H above layer 0)"""
         src = self.grads if grads else self.params
-        return (src["core.core.weight_ih_l0"], src["core.core.weight_hh_l0"], src["core.core.bias_ih_l0"],
-                src["core.core.bias_hh_l0"])
+        k = layer
+        return (src[f"core.core.weight_ih_l{k}"], src[f"core.core.weight_hh_l{k}"], src[f"core.core.bias_ih_l{k}"],
+                src[f"core.core.bias_hh_l{k}"])
 
     def hidden_layer_grads(self) -> List[Tuple[Tensor, Tensor]]:
         return self.encoder_layers(grads=True) + self.decoder_layers(grads=True)

@@ -133,7 +133,6 @@ class Runner:
 
         global_model_factory().check_supported()      # custom torch modules: explicit error through the registry API
         spec = ModelSpec.from_cfg(cfg, self.env)
-        assert cfg.rnn_num_layers == 1, "the device path implements the one-layer recurrent core"
         # (population members start from different weights: seed + index)
         self.model = PolicyModel(spec, self.device, seed=(cfg.seed or 0) + p_idx, policy_init_gain=cfg.policy_init_gain,
                                  policy_initialization=getattr(cfg, "policy_initialization", "orthogonal"))
