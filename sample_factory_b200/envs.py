@@ -9,6 +9,9 @@ GPU-env contract the device sampler drives (what the reference's BatchedVecEnv g
         obs        float32 [num_agents, obs_dim]
         rew        float32 [num_agents]; terminated / truncated bool [num_agents]
     auto-reset is the env's job (make_env.py:89-94).
+    env.obs_keys (optional): a Dict observation of 1-D keys, [(key, d), ...] in sorted key order.  Each obs row is then the
+        keys laid side by side as float32 (key k in columns [c_k, c_k + d_k), obs_dim = sum(d)), and the model builds one
+        encoder per key (MultiInputEncoder).  An "action_mask" key is not part of the row.
 
 `TapeVecEnv` is the synthetic env of BASELINE.json config 2 (Box(64) obs, Discrete(8)): GPU-resident, one CUDA kernel
 per step, buffers reused across steps so a whole rollout can be captured in a CUDA graph.  `HostTapeVecEnv` is the
@@ -86,8 +89,11 @@ class TapeVecEnv:
 
     def __init__(self, tape: Tensor, num_actions: int, term_period: int = 37, trunc_period: int = 11,
                  env_index_offset: int = 0, continuous: bool = False, obs_shape=None, action_segments=None,
-                 with_action_mask: bool = False, action_heads=None):
+                 with_action_mask: bool = False, action_heads=None, obs_keys=None):
         assert tape.is_cuda and tape.dim() == 3 and tape.is_contiguous()
+        # Dict observation layout over the tape row ([(key, d), ...], see the module docstring); the env rules are unchanged
+        self.obs_keys = None if obs_keys is None else [(str(k), int(d)) for k, d in obs_keys]
+        assert self.obs_keys is None or sum(d for _, d in self.obs_keys) == tape.shape[2]
         assert tape.dtype in (torch.float32, torch.uint8)
         self.tape = tape
         # image observations: uint8 tape rows of C*H*W bytes with obs_shape = (C, H, W) -> the model builds a ConvEncoder

@@ -45,20 +45,29 @@ def _tuple_members(space) -> Optional[List[Tuple[str, int]]]:
 
 
 def _main_obs_space(obs_space):
-    """(space of the policy input, key or None).  Dict observation spaces (make_env.py:147-176 wraps everything into
-    Dict(obs=...)): the entry "obs" feeds the policy; an "action_mask" entry is consumed by the sampler.  Dicts with other
-    entries would need the reference's MultiInputEncoder (one encoder per key, encoder.py:33-70), which the kernel path does
-    not have."""
+    """(space of the policy input, key or None, obs_keys or None).  Dict observation spaces (make_env.py:147-176 wraps
+    everything into Dict(obs=...)): an "action_mask" entry is consumed by the sampler (actor_critic.py:345-351).  The key
+    "obs" alone keeps its space (any shape); other keys must be 1-D and are packed side by side in sorted key order
+    (MultiInputEncoder's order, encoder.py:36), one encoder per key: obs_keys = [(key, d), ...]."""
     spaces = getattr(obs_space, "spaces", None)
     if not isinstance(spaces, dict):
-        return obs_space, None
-    extra = [k for k in spaces if k not in ("obs", "action_mask")]
-    if "obs" not in spaces or extra:
-        raise NotImplementedError(
-            f"Dict observation space with keys {sorted(spaces)}: the device path encodes ONE array observation (key 'obs', "
-            "optionally with 'action_mask'); multi-input observations (MultiInputEncoder) are not supported -- flatten / "
-            "concatenate them in an env wrapper.")
-    return spaces["obs"], "obs"
+        return obs_space, None, None
+    keys = sorted(k for k in spaces if k != "action_mask")
+    if not keys:
+        raise NotImplementedError("Dict observation space without a policy input (only 'action_mask')")
+    if keys == ["obs"]:
+        return spaces["obs"], "obs", None
+    obs_keys = []
+    for k in keys:
+        shape = tuple(getattr(spaces[k], "shape", None) or ())
+        if len(shape) == 0:
+            raise NotImplementedError(f"Dict observation key {k!r} is a scalar space {spaces[k]}: MultiInputEncoder "
+                                      "supports 1-D (vector) keys here (the reference raises for scalar keys too)")
+        if len(shape) > 1:
+            raise NotImplementedError(f"Dict observation key {k!r} has shape {shape}: the device path supports Dict "
+                                      "observations of 1-D keys only (image keys in a Dict are not supported yet)")
+        obs_keys.append((k, int(shape[0])))
+    return None, None, obs_keys
 
 
 class BatchedHostEnv:
@@ -76,12 +85,23 @@ class BatchedHostEnv:
         self.multi_agent = bool(getattr(e0, "is_multiagent", False)) or self.agents_per_env > 1
         self.num_agents = num_envs * self.agents_per_env
         self.device = device
-        obs_space, self._obs_key = _main_obs_space(e0.observation_space)
-        self._mask_key = "action_mask" if (self._obs_key and "action_mask" in e0.observation_space.spaces) else None
-        shape = tuple(obs_space.shape)
-        self.obs_uint8 = np.dtype(getattr(obs_space, "dtype", np.float32)) == np.uint8
-        self.obs_shape = shape if len(shape) == 3 else None       # (C, H, W) image observations -> ConvEncoder
-        self.obs_dim = int(np.prod(shape))
+        obs_space, self._obs_key, self.obs_keys = _main_obs_space(e0.observation_space)
+        is_dict = isinstance(getattr(e0.observation_space, "spaces", None), dict)
+        self._mask_key = "action_mask" if (is_dict and "action_mask" in e0.observation_space.spaces) else None
+        if self.obs_keys is not None:
+            # Dict of 1-D keys: every key's array is cast to float32 (normalize.py:43-45) into its columns of the packed row
+            self.obs_uint8, self.obs_shape = False, None
+            self.obs_dim = sum(d for _, d in self.obs_keys)
+            self._key_cols = []
+            c = 0
+            for _, d in self.obs_keys:
+                self._key_cols.append(slice(c, c + d))
+                c += d
+        else:
+            shape = tuple(obs_space.shape)
+            self.obs_uint8 = np.dtype(getattr(obs_space, "dtype", np.float32)) == np.uint8
+            self.obs_shape = shape if len(shape) == 3 else None       # (C, H, W) image observations -> ConvEncoder
+            self.obs_dim = int(np.prod(shape))
         # Tuple action spaces (preprocess_actions, batched_sampling.py:46-57): all-Discrete -> action_segments (the sampler
         # hands over int32 [n, K]); with Box members -> action_heads (one device tensor per member) and num_actions = the
         # rows of distribution_linear.  An env receives a Python tuple per step (Tuple.sample()'s layout), a multi-agent env
@@ -135,9 +155,14 @@ class BatchedHostEnv:
             self.action_mask = torch.ones((n, self.num_actions), dtype=torch.bool, device=device)
 
     def _put_obs(self, i: int, obs) -> None:
+        if self._mask_key:
+            self.mask_host[i].copy_(torch.as_tensor(np.asarray(obs[self._mask_key])).reshape(-1) != 0)
+        if self.obs_keys is not None:
+            row = self.obs_host[i].numpy()
+            for (k, _), cols in zip(self.obs_keys, self._key_cols):
+                row[cols] = np.asarray(obs[k]).reshape(-1)
+            return
         if self._obs_key is not None:
-            if self._mask_key:
-                self.mask_host[i].copy_(torch.as_tensor(np.asarray(obs[self._mask_key])).reshape(-1) != 0)
             obs = obs[self._obs_key]
         self.obs_host[i].copy_(torch.as_tensor(np.asarray(obs)).reshape(-1))
 

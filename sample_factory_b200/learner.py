@@ -139,7 +139,8 @@ class Learner:
         # device, and ONE gather pass per train() rearranges every per-sample array the minibatch steps read; the steps then
         # run on contiguous slices exactly as in the unshuffled case.
         self.shuffle = bool(cfg.shuffle_minibatches) and cfg.num_batches_per_epoch > 1
-        assert len(spec.hidden) > 0 or spec.use_rnn, "the device path needs at least one hidden layer or an RNN core"
+        assert len(spec.hidden) > 0 or spec.use_rnn or (spec.dict_obs and spec.encoder_mlp_layers), (
+            "the device path needs at least one hidden layer or an RNN core")
         assert spec.obs_shape is None or len(spec.fc_encoder_layers) > 0, (
             "ConvEncoder on the device path needs at least one fully connected layer after the conv head "
             "(encoder_conv_mlp_layers, reference default [512])")
@@ -213,6 +214,11 @@ class Learner:
             lin_ws = ops.linear_backward_workspace_bytes(B, A_lin, spec.tail_input_size) // 4 + 4
         else:
             self.heads_ws = torch.empty(ops.heads_backward_workspace_bytes(tail_w, A_lin) // 4 + 4, **f32)
+        if spec.dict_obs:
+            for _, d in spec.obs_keys:       # the key encoders' chains
+                for h in spec.encoder_mlp_layers:
+                    lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(B, h, d) // 4 + 4)
+                    d = h
         d = spec.fc_encoder_input
         for h in spec.fc_encoder_layers:
             lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(B, h, d) // 4 + 4)
@@ -574,9 +580,19 @@ class Learner:
         genc, gdec = m.encoder_layers(grads=True), m.decoder_layers(grads=True)
         Le, Ld = len(enc), len(dec)
         rnn = self.rnn is not None
+        plan = self.heads_plan
+        B = x0.shape[0]
+        # the encoder's output as the next stage reads it: (activations, activation, their gradient, gradient of the bias that
+        # made them); Dict models: the key encoders' concatenation (identity encoders: the normalised rows, no gradient)
+        if plan.keys:
+            x_enc, act_enc, d_enc, db_enc = plan.enc_cat[:B], self.act, plan.denc_cat[:B], plan.db_enc_cat
+        elif Le > 0:
+            x_enc, act_enc, d_enc, db_enc = self.h[Le - 1], self.act, self.dz[Le - 1], genc[-1][1]
+        else:
+            x_enc, act_enc, d_enc, db_enc = x0, none, None, None
         tail_is_mlp = Ld > 0 or not rnn            # is the tensor feeding the heads an activated MLP output?
-        tail_dz = self.dz[Le + Ld - 1] if tail_is_mlp else self.d_core
-        tail_db = gdec[-1][1] if Ld > 0 else (None if rnn else genc[-1][1])
+        tail_dz = (self.dz[Le + Ld - 1] if Ld > 0 else d_enc) if tail_is_mlp else self.d_core
+        tail_db = gdec[-1][1] if Ld > 0 else (None if rnn else db_enc)
         if self.dz_bound is not None and tail_is_mlp:
             ops.heads_dz_bound(self.dlogits, self.dvalues, Wv, Wa, self.dz_bound)
         tail_act = self.act if tail_is_mlp else none
@@ -600,17 +616,15 @@ class Learner:
             elif rnn:
                 x_in, act_prev, dx, dbp = self.rnn_bufs["core_out"], none, self.d_core, None
             else:
-                x_in, act_prev, dx, dbp = self.h[Le - 1], self.act, self.dz[Le - 1], genc[-1][1]
+                x_in, act_prev, dx, dbp = x_enc, act_enc, d_enc, db_enc
             ops.linear_backward(self.dz[Le + j], x_in, W, act_prev, dW, dx, dbp, self.engine, self.lin_ws)
         if rnn:
             dgi_all = self.rnn.backward_bptt(self.d_core, self.rnn_bufs, self.lin_ws)
             W_ih = m.rnn_params()[0]
             dW_ih = m.rnn_params(grads=True)[0]
-            if Le > 0:
-                ops.linear_backward(dgi_all, self.h[Le - 1], W_ih, self.act, dW_ih, self.dz[Le - 1], genc[-1][1],
-                                    self.engine, self.lin_ws)
-            else:
-                ops.linear_backward(dgi_all, x0, W_ih, none, dW_ih, None, None, self.engine, self.lin_ws)
+            ops.linear_backward(dgi_all, x_enc, W_ih, act_enc, dW_ih, d_enc, db_enc, self.engine, self.lin_ws)
+        if plan.keys:
+            self._backward_keys(x0)
         for li in range(Le - 1, -1, -1):
             W, dW = enc[li][0], genc[li][0]
             if li > 0:
@@ -624,6 +638,30 @@ class Learner:
                 conv.backward(self.dfeat)
             else:
                 ops.linear_backward(self.dz[li], x0, W, none, dW, None, None, self.engine, self.lin_ws)
+
+    def _backward_keys(self, x0: Tensor) -> None:
+        """backward of the key encoders (MultiInputEncoder): key k's chain starts from its column block of d(concatenation),
+        and the bias gradient of its last layer is its block of the concatenation's column sums"""
+        m, spec, plan = self.model, self.model.spec, self.heads_plan
+        B = x0.shape[0]
+        none = ops.ACT["none"]
+        col = 0
+        for k, (layers, glayers, c, (_, d)) in enumerate(zip(m.key_encoder_layers(), m.key_encoder_layers(grads=True),
+                                                            spec.key_offsets, spec.obs_keys)):
+            n = spec.key_out_sizes[k]
+            L = len(layers)
+            glayers[L - 1][1].copy_(plan.db_enc_cat[col: col + n])
+            dz = plan.denc_cat[:B, col: col + n]
+            for i in range(L - 1, -1, -1):
+                W, dW = layers[i][0], glayers[i][0]
+                if i > 0:
+                    dx = plan.key_dz[k][i - 1][:B]
+                    ops.linear_backward(dz, plan.key_h[k][i - 1][:B], W, self.act, dW, dx, glayers[i - 1][1], self.engine,
+                                        self.lin_ws)
+                    dz = dx
+                else:
+                    ops.linear_backward(dz, x0[:, c: c + d], W, none, dW, None, None, self.engine, self.lin_ws)
+            col += n
 
     def _backward_separate(self, x0: Tensor) -> None:
         """backward of ActorCriticSeparateWeights: one heads-backward over the concatenated tail [B, 2H] (zero-padded head

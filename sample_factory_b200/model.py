@@ -15,7 +15,8 @@ from typing import Dict, List, Optional, Tuple
 import torch
 from torch import Tensor
 
-OBS_NORM_PREFIX = "obs_normalizer.running_mean_std.running_mean_std.obs."
+OBS_NORM_PREFIX_BASE = "obs_normalizer.running_mean_std.running_mean_std."
+OBS_NORM_PREFIX = OBS_NORM_PREFIX_BASE + "obs."
 RET_NORM_PREFIX = "returns_normalizer."
 
 
@@ -55,6 +56,11 @@ class ModelSpec:
     # False -> ActorCriticSeparateWeights (model/actor_critic.py:198-322): an actor tower (encoder + decoder MLP) feeding
     # distribution_linear and a critic tower feeding critic_linear; vector observations, no recurrent core on this path
     share_weights: bool = True
+    # Dict observations of 1-D keys (MultiInputEncoder, model/encoder.py:33-70): [(key, d), ...] in sorted key order.  The
+    # keys lie side by side in one packed row, key k in columns [c_k, c_k + d_k); every key has its own MlpEncoder with
+    # encoder_mlp_layers ([] = identity) and the encoders' outputs are concatenated.  One key takes the single-key path,
+    # with the parameter and normaliser names of that key.  Keyword-only: positional construction keeps its meaning.
+    obs_keys: Optional[List[Tuple[str, int]]] = field(default=None, kw_only=True)
     # stacked recurrent core: nn.GRU / nn.LSTM(in, rnn_size, rnn_num_layers) (model/core.py:27-31); layer k > 0 reads
     # layer k-1's new h, the state rows are layer-major [h_0 | h_1 | ...] (GRU) / [h_0 | c_0 | h_1 | c_1 | ...] (LSTM)
     rnn_num_layers: int = 1
@@ -124,12 +130,44 @@ class ModelSpec:
         return out
 
     @property
+    def dict_obs(self) -> bool:
+        """several observation keys: per-key encoders whose outputs are concatenated (the key encoder stage)"""
+        return self.obs_keys is not None and len(self.obs_keys) > 1
+
+    @property
+    def obs_key(self) -> str:
+        """the observation key of a single-key model"""
+        return self.obs_keys[0][0] if self.obs_keys else "obs"
+
+    @property
+    def key_offsets(self) -> List[int]:
+        """first column of each key in the packed observation row"""
+        out, c = [], 0
+        for _, d in self.obs_keys:
+            out.append(c)
+            c += d
+        return out
+
+    @property
+    def key_out_sizes(self) -> List[int]:
+        """width of each key encoder's output: encoder_mlp_layers[-1], or d_k for the identity encoder"""
+        return [self.encoder_mlp_layers[-1] if self.encoder_mlp_layers else d for _, d in self.obs_keys]
+
+    def key_encoder_name(self, key: str, i: int, what: str) -> str:
+        return f"encoder.encoders.{key}.mlp_head.{2 * i}.{what}"
+
+    @property
     def fc_encoder_layers(self) -> List[int]:
-        """widths of the fully connected encoder layers (after the conv head for image observations)"""
+        """widths of the fully connected encoder layers (after the conv head for image observations; none after the
+        key encoders of a Dict model)"""
+        if self.dict_obs:
+            return []
         return list(self.encoder_conv_mlp_layers) if self.obs_shape is not None else list(self.encoder_mlp_layers)
 
     @property
     def fc_encoder_input(self) -> int:
+        if self.dict_obs:       # the concatenated key encoder outputs
+            return sum(self.key_out_sizes)
         return self.conv_out_size if self.obs_shape is not None else self.obs_dim
 
     def fc_encoder_name(self, i: int, what: str) -> str:
@@ -137,13 +175,26 @@ class ModelSpec:
             return f"encoder.encoders.obs.mlp_layers.{2 * i}.{what}"
         if self.obs_shape is not None:
             return f"encoder.encoders.obs.enc.mlp_layers.{2 * i}.{what}"
-        return f"encoder.encoders.obs.mlp_head.{2 * i}.{what}"
+        return self.key_encoder_name(self.obs_key, i, what)
+
+    @property
+    def obs_norm_prefixes(self) -> List[Tuple[str, int, int]]:
+        """[(state_dict prefix, first column, width)] of the per-key RunningMeanStdInPlace (running_mean_std.py:113-136)"""
+        if self.obs_keys is None:
+            return [(OBS_NORM_PREFIX, 0, self.obs_dim)]
+        return [(f"{OBS_NORM_PREFIX_BASE}{k}.", c, d) for (k, d), c in zip(self.obs_keys, self.key_offsets)]
 
     @classmethod
     def from_cfg(cls, cfg, env) -> "ModelSpec":
         """The model the reference would build for this cfg / env (model/actor_critic.py:136-158, create_actor_critic):
         Discrete(n) envs expose `num_actions = n`; Box(A) envs expose `continuous = True` and `num_actions = A`."""
         obs_shape = getattr(env, "obs_shape", None)   # (C, H, W) image observations -> ConvEncoder (encoder.py:218-227)
+        obs_keys = getattr(env, "obs_keys", None)
+        keys_to_normalize = getattr(cfg, "normalize_input_keys", None)
+        if obs_keys and len(obs_keys) > 1 and keys_to_normalize is not None and (
+                set(keys_to_normalize) != {k for k, _ in obs_keys}):
+            raise ValueError(f"normalize_input_keys={list(keys_to_normalize)} selects a subset of the Dict observation keys "
+                             f"{[k for k, _ in obs_keys]}: the device path normalises every key of a multi-key Dict")
         return cls(env.obs_dim, env.num_actions, list(cfg.encoder_mlp_layers), list(cfg.decoder_mlp_layers),
                    cfg.nonlinearity, cfg.normalize_input, cfg.normalize_returns, cfg.obs_subtract_mean, cfg.obs_scale,
                    bool(cfg.use_rnn), cfg.rnn_type, cfg.rnn_size,
@@ -158,7 +209,8 @@ class ModelSpec:
                    adaptive_stddev=bool(getattr(cfg, "adaptive_stddev", True)),
                    continuous_tanh_scale=float(getattr(cfg, "continuous_tanh_scale", 0.0)),
                    initial_stddev=float(getattr(cfg, "initial_stddev", 1.0)),
-                   rnn_num_layers=int(getattr(cfg, "rnn_num_layers", 1)))
+                   rnn_num_layers=int(getattr(cfg, "rnn_num_layers", 1)),
+                   obs_keys=([tuple(k) for k in obs_keys] if obs_keys else None))
 
     @property
     def num_linear_action_outputs(self) -> int:
@@ -194,6 +246,8 @@ class ModelSpec:
                 if self.num_actions != rows:
                     raise ValueError(f"a Tuple with members {heads} has {rows} distribution_linear rows, num_actions is "
                                      f"{self.num_actions}")
+        if self.obs_keys is not None:
+            self._check_obs_keys()
         tup = self.action_segments or self.action_heads
         if tup and len(tup) > self.MAX_TUPLE_HEADS:
             raise ValueError(f"Tuple action spaces are supported with at most {self.MAX_TUPLE_HEADS} heads, got "
@@ -204,6 +258,26 @@ class ModelSpec:
                     f"{'Tuple' if tup else 'Discrete'} with {self.num_actions} logits")
             raise ValueError(f"{what} needs {n} distribution_linear rows; the device path supports at most "
                              f"{self.MAX_LINEAR_ACTION_OUTPUTS}")
+
+    def _check_obs_keys(self) -> None:
+        keys = [(str(k), int(d)) for k, d in self.obs_keys]
+        names = [k for k, _ in keys]
+        if not keys or names != sorted(set(names)):
+            raise ValueError(f"obs_keys must be unique keys in sorted order (MultiInputEncoder's order), got {names}")
+        if any(d < 1 for _, d in keys):
+            raise ValueError(f"obs_keys widths must be >= 1, got {keys}")
+        if sum(d for _, d in keys) != self.obs_dim:
+            raise ValueError(f"obs_keys {keys} span {sum(d for _, d in keys)} columns, obs_dim is {self.obs_dim}")
+        self.obs_keys = keys
+        if len(keys) == 1:
+            return
+        if self.obs_shape is not None:
+            raise ValueError("Dict observations with several keys: 1-D keys only (image keys are not supported)")
+        if not self.share_weights:
+            raise ValueError("Dict observations with several keys are not supported with actor_critic_share_weights=False")
+        if abs(self.obs_subtract_mean) > 1e-8 or abs(self.obs_scale - 1.0) > 1e-8:
+            raise ValueError("Dict observations with several keys: obs_subtract_mean / obs_scale apply to the key 'obs' only "
+                             "(normalize.py:59-65) and are not supported; leave them at 0 / 1")
 
     @property
     def num_action_params(self) -> int:
@@ -256,7 +330,7 @@ class ModelSpec:
             return self.decoder_mlp_layers[-1]     # (separate weights: the width of ONE tower's tail)
         if self.use_rnn:
             return self.rnn_size
-        return self.fc_encoder_layers[-1]
+        return self.fc_encoder_layers[-1] if self.fc_encoder_layers else self.fc_encoder_input
 
     def param_shapes(self) -> List[Tuple[str, Tuple[int, ...]]]:
         """(reference state_dict key, shape) in nn.Module.parameters() order."""
@@ -284,6 +358,12 @@ class ModelSpec:
             out.append(("action_parameterization.distribution_linear.weight", (self.num_linear_action_outputs, d)))
             out.append(("action_parameterization.distribution_linear.bias", (self.num_linear_action_outputs,)))
             return out
+        if self.dict_obs:       # MultiInputEncoder: encoders.{key}, keys in sorted order (encoder.py:36-48)
+            for key, d in self.obs_keys:
+                for i, h in enumerate(self.encoder_mlp_layers):
+                    out.append((self.key_encoder_name(key, i, "weight"), (h, d)))
+                    out.append((self.key_encoder_name(key, i, "bias"), (h,)))
+                    d = h
         for prefix, wshape in self.conv_param_layout():
             out.append((f"{prefix}.weight", wshape))
             out.append((f"{prefix}.bias", (wshape[0],)))
@@ -370,7 +450,7 @@ class PolicyModel:
         self.f16_T: Dict[str, Tensor] = {}
         self.bound_x = self.bound_h = None
         ok = (self.flat.is_cuda and sp.normalize_input and sp.obs_shape is None and not sp.use_rnn and sp.share_weights
-              and not sp.decoder_mlp_layers and len(sp.hidden) >= 1)
+              and not sp.decoder_mlp_layers and not sp.dict_obs and len(sp.hidden) >= 1)
         if not ok:
             return
         from . import ops
@@ -501,6 +581,13 @@ class PolicyModel:
         return [(src[sp.fc_encoder_name(i, "weight")], src[sp.fc_encoder_name(i, "bias")])
                 for i in range(len(sp.fc_encoder_layers))]
 
+    def key_encoder_layers(self, grads: bool = False) -> List[List[Tuple[Tensor, Tensor]]]:
+        """Dict models: per key (sorted order) the [(W, b)] of its MlpEncoder ([] for identity encoders)"""
+        src = self.grads if grads else self.params
+        sp = self.spec
+        return [[(src[sp.key_encoder_name(k, i, "weight")], src[sp.key_encoder_name(k, i, "bias")])
+                 for i in range(len(sp.encoder_mlp_layers))] for k, _ in sp.obs_keys]
+
     def tower_layers(self, tower: str, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
         """separate actor / critic weights: [(W, b)] of one tower ("actor_" / "critic_"), encoder then decoder MLP"""
         src = self.grads if grads else self.params
@@ -567,10 +654,13 @@ class PolicyModel:
     def state_dict(self) -> Dict[str, Tensor]:
         sd: Dict[str, Tensor] = {}
         if self.spec.normalize_input:
-            shp = self.spec.obs_shape if self.spec.obs_shape is not None else (self.spec.obs_dim,)
-            sd[OBS_NORM_PREFIX + "running_mean"] = self.obs_mean.clone().view(shp)   # reference shape = obs space shape
-            sd[OBS_NORM_PREFIX + "running_var"] = self.obs_var.clone().view(shp)
-            sd[OBS_NORM_PREFIX + "count"] = self.obs_count.clone()
+            # one RunningMeanStdInPlace per key (running_mean_std.py:113-136), statistics of the key's own shape; the keys of
+            # a packed row share one count
+            for prefix, c, d in self.spec.obs_norm_prefixes:
+                shp = self.spec.obs_shape if self.spec.obs_shape is not None else (d,)
+                sd[prefix + "running_mean"] = self.obs_mean[c: c + d].clone().view(shp)
+                sd[prefix + "running_var"] = self.obs_var[c: c + d].clone().view(shp)
+                sd[prefix + "count"] = self.obs_count.clone()
         if self.spec.normalize_returns:
             sd[RET_NORM_PREFIX + "running_mean"] = self.ret_mean.clone()
             sd[RET_NORM_PREFIX + "running_var"] = self.ret_var.clone()
@@ -581,16 +671,18 @@ class PolicyModel:
 
     def load_state_dict(self, sd: Dict[str, Tensor], strict: bool = True) -> None:
         known = set(self.names)
+        obs_norm = {}       # state_dict key -> (buffer, first column, width) of the per-key normaliser statistics
+        for prefix, c, d in self.spec.obs_norm_prefixes:
+            obs_norm[prefix + "running_mean"] = (self.obs_mean, c, d)
+            obs_norm[prefix + "running_var"] = (self.obs_var, c, d)
+            obs_norm[prefix + "count"] = (self.obs_count, 0, 1)
         for k, v in sd.items():
             v = torch.as_tensor(v)
             if k in known:
                 self.params[k].copy_(v.to(self.device, torch.float32).view(self.params[k].shape))
-            elif k == OBS_NORM_PREFIX + "running_mean":
-                self.obs_mean.copy_(v.to(self.device).reshape(-1))     # image observations: [C,H,W] statistics, flat here
-            elif k == OBS_NORM_PREFIX + "running_var":
-                self.obs_var.copy_(v.to(self.device).reshape(-1))
-            elif k == OBS_NORM_PREFIX + "count":
-                self.obs_count.copy_(v.to(self.device).view(1))
+            elif k in obs_norm:
+                buf, c, d = obs_norm[k]
+                buf[c: c + d].copy_(v.to(self.device).reshape(-1))     # image observations: [C,H,W] statistics, flat here
             elif k == RET_NORM_PREFIX + "running_mean":
                 self.ret_mean.copy_(v.to(self.device).view(1))
             elif k == RET_NORM_PREFIX + "running_var":

@@ -7,6 +7,10 @@ wgmma engine covers the shape, that layer and the heads run as ONE GEMM whose ep
 products (sfb200_linear_act_heads_forward) followed by a tiny finishing kernel (sfb200_heads_from_partials); the
 activated layer output is stored only if the caller needs it (the learner's backward does, the sampler does not).
 
+Dict observations with several keys (MultiInputEncoder) start with a key encoder stage: each key's MLP runs on its column
+slice of the normalised rows and its last layer writes its block of one concatenated buffer, which then feeds the
+recurrent core, the decoder MLP or (unfused) the heads like the output of a single encoder would.
+
 Models whose distribution_linear has more than 31 rows (ModelSpec.wide_heads) store the last hidden layer, run
 distribution_linear as a GEMM on the same engine straight into the logits' final place, and finish with
 sfb200_heads_tail_wide (value head + distribution tail, one warp per row).
@@ -36,6 +40,18 @@ class HeadsPlan:
             self.conv = (ResnetHead if spec.is_resnet else ConvHead)(model, engine, max_rows, need_backward)
         self.tail_is_mlp = bool(spec.decoder_mlp_layers) or (not spec.use_rnn and bool(spec.fc_encoder_layers))
         self.engine = engine
+        # Dict observations: per key the hidden activations of its MLP but the last, and the [rows, sum of the key output
+        # widths] concatenation the last layers write (identity encoders: the normalised row itself is the concatenation)
+        self.keys = spec.dict_obs and bool(spec.encoder_mlp_layers)
+        if self.keys:
+            f32 = dict(dtype=torch.float32, device=model.device)
+            widths = spec.encoder_mlp_layers
+            self.key_h = [[torch.empty((max_rows, w), **f32) for w in widths[:-1]] for _ in spec.obs_keys]
+            self.enc_cat = torch.empty((max_rows, spec.fc_encoder_input), **f32)
+            if need_backward:
+                self.key_dz = [[torch.empty((max_rows, w), **f32) for w in widths[:-1]] for _ in spec.obs_keys]
+                self.denc_cat = torch.empty((max_rows, spec.fc_encoder_input), **f32)
+                self.db_enc_cat = torch.empty(spec.fc_encoder_input, **f32)
         # heads wider than 31 rows: no fused-partials path (P stays 0); call sites that sample without keeping the logits
         # get them in this scratch (so do Tuples with Box members, whose tail reads the stored params rows)
         self.wide = spec.wide_heads
@@ -84,6 +100,8 @@ def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, 
         return _forward_separate(model, x, act, engine, plan, heads_kwargs)
     if plan.conv is not None:        # ConvEncoder: conv head first, its fully connected layers are `enc` below
         x = plan.conv.forward(x)
+    if plan.keys:                    # MultiInputEncoder: the key encoders write the concatenation, `enc` below is empty
+        x = _forward_keys(model, x, act, engine, plan)
     enc, dec = model.encoder_layers(), model.decoder_layers()
     Wv, bv = model.critic
     Wa, ba = model.actor
@@ -119,6 +137,23 @@ def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, 
     else:
         _heads(model, tail, Wv, bv, Wa, ba, fused, plan, M, heads_kwargs)
     return tail
+
+
+def _forward_keys(model: PolicyModel, x: Tensor, act: int, engine: int, plan: HeadsPlan) -> Tensor:
+    """MultiInputEncoder.forward (encoder.py:50-60): key k's MlpEncoder on the column slice x[:, c_k : c_k + d_k] (a
+    pointer offset at the full row stride); its last layer writes columns [k*N, (k+1)*N) of the concatenation"""
+    M = x.shape[0]
+    sp = model.spec
+    col = 0
+    for k, (layers, c, (_, d)) in enumerate(zip(model.key_encoder_layers(), sp.key_offsets, sp.obs_keys)):
+        t = x[:, c: c + d]
+        n = sp.key_out_sizes[k]
+        for i, (W, b) in enumerate(layers):
+            out = plan.enc_cat[:M, col: col + n] if i == len(layers) - 1 else plan.key_h[k][i][:M]
+            ops.linear_act_forward(t, W, b, out, act, engine)
+            t = out
+        col += n
+    return plan.enc_cat[:M]
 
 
 def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan: HeadsPlan, heads_kwargs: Dict) -> Tensor:

@@ -115,11 +115,11 @@ class DeviceSampler:
                            not self.heads_plan.finish_in_gemm and not self.heads_plan.separate and
                            not spec.continuous and not spec.action_segments and not spec.action_heads)
         # Whole rollout as ONE persistent kernel (csrc/rollout_fused.cu): clusters of H2/128 CTAs own a 128-env row block for
-        # all T steps.  Same conditions as the fused tail plus a two-layer MLP the kernel covers.  SFB200_ROLLOUT_FUSED=0
-        # restores the per-step launches.
+        # all T steps.  Same conditions as the fused tail plus a two-layer MLP the kernel covers (one encoder: not the key
+        # encoders of a Dict model).  SFB200_ROLLOUT_FUSED=0 restores the per-step launches.
         self.fused_rollout = False
         if (self.fused_tail and os.environ.get("SFB200_ROLLOUT_FUSED", "1") != "0" and not deterministic and
-                len(spec.fc_encoder_layers) == 2 and not spec.decoder_mlp_layers and self.heads_plan.conv is None):
+                not spec.dict_obs and len(spec.fc_encoder_layers) == 2 and not spec.decoder_mlp_layers and self.heads_plan.conv is None):
             (W1, _), (W2, _) = model.encoder_layers()
             self.fused_rollout = ops.rollout_mlp2_partials(W1, W2, spec.num_linear_action_outputs, engine) == self.heads_plan.P
 
