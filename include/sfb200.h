@@ -234,11 +234,16 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
  * sfb200_sampler_pre_step for step 0 first (x_norm holds the normalised step-0 observations).  Pointers with suffix _0 are
  * the trajectory slots of step 0 ([:, 0]); step t is at + t elements (x A for logits, x dim for traj_obs / rnn rows).
  *   P = sfb200_rollout_mlp2_partials(...)   0 -> not covered (3xTF32 engine, K1 in {32,64,96,128}, H1 == H2 in {128,256,512},
- *       A <= 8, W1 and W2 16-byte aligned); head_partials: P * n_envs * 12 floats, h1_scratch: n_envs * H1 floats. */
+ *       A <= 8, W1 and W2 16-byte aligned); head_partials: P * n_envs * 12 floats, h1_scratch: n_envs * H1 floats.
+ *   The kernel takes the fp16-split form when W1 and W2 have registered fp16 twins and x_norm and h1_scratch registered
+ *   bounds (K1, H1 multiples of 64); the h1 scratch then holds h1 * 2^shift split into fp16 planes: hi [n_envs][H1] halves,
+ *   then lo n_envs * H1 halves later (the same bytes).  Otherwise (tf32 form) it holds h1 as fp32 [n_envs][H1]. */
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine);
 /* debug aid: device buffer of T x 16 uint64 that the following rollouts fill with %globaltimer stamps of one CTA's phases;
  * NULL switches it off */
 int sfb200_rollout_set_trace(void* trace_dev);
+/* form the last sfb200_rollout_mlp2_tape call launched: 1 fp16 split, 0 tf32 split, -1 none yet */
+int sfb200_rollout_last_form(void);
 int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, const float* b1, int H1, const float* W2,
                              const float* b2, int H2, int act, int engine, const float* Wv, const float* bv, const float* Wa,
                              const float* ba, int A, float* h1_scratch, float* head_partials, float* x_norm,

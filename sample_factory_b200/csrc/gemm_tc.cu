@@ -253,7 +253,7 @@ bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1
 // 3-D fp16 map over a weight's [hi | lo] twins, planes lo_offset elements apart, each plane [rows][K] row-major: box
 // 64 k x 128 rows x both planes with the 128B swizzle, i.e. two [128][64 fp16] tiles in the K-major layout wgmma reads
 // (what split_tile_f16 writes).  False when TMA cannot describe the twins (alignment).
-static bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows) {
+bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows) {
     if ((reinterpret_cast<uintptr_t>(hi) & 15u) || (K * 2) % 16 != 0 || (lo_offset * 2) % 16 != 0 || lo_offset <= 0)
         return false;
     cuuint64_t gdim[3] = {K, rows, 2};

@@ -10,13 +10,25 @@
 // columns [128c, 128c+128) of h1, then of h2 (partial head products), then finishes rows [32c.., ) of the block.
 // h1 and the head partials cross between the CTAs of a cluster through global memory (L2-resident), read back by TMA.
 //
-// Each GEMM tile is the wgmma tile of gemm_tc.cu (raw fp32 tiles by TMA, split into tf32 hi / lo halves in shared memory,
-// 3xTF32 with main | cross accumulators in registers); the step tail is the code of sampler_tail_tape_kernel (heads.cu).
+// Each GEMM tile is the wgmma tile of gemm_tc.cu (3-pass split operands, main | cross accumulators in registers); the step
+// tail is the code of sampler_tail_tape_kernel (heads.cu).
 //
-//   warps 0-3   idle (the kernel keeps the 384-thread warpgroup layout of gemm_tc.cu; not yet given work)
-//   warps 4-11  two wgmma warpgroups (64 rows each): consumer thread 0 (threadIdx 128) issues the TMA loads of the tiles;
-//               all of them split, multiply, run the epilogues and the step tail (an 8-lane group per row: four rows
-//               per warp).  A first correct port: not tuned on the H100 yet (ptxas reports register spills here).
+//   warps 0-3   TMA producer (one elected thread; the warpgroup gives its registers to the consumers).  It walks the
+//               same sequence of ring uses as the consumers and puts the weight tiles, which do not depend on the step,
+//               in flight across the cluster barriers: the first W2 tiles between its arrive at and its wait on barrier 1,
+//               the next step's W1 tiles between its arrive at and its wait on barrier 2.  h1 and x_norm tiles are issued
+//               only after the barrier that publishes them.
+//   warps 4-11  two wgmma warpgroups (64 rows each): multiply, run the epilogues and the step tail (an 8-lane group per
+//               row: four rows per warp).  One wgmma group stays in flight; a ring slot goes back to the producer when
+//               its wgmmas have completed.
+//
+// fp16-split form (weights with registered fp16 twins, bounded activations): a stage covers 64 k.  The weight tiles are
+// the twins, TMA-loaded in the swizzled layout wgmma reads.  The layer-1 epilogue writes h1 * 2^shift_h already split into
+// fp16 [hi | lo] planes (the h1 scratch holds the hi plane, then the lo plane N*H1 halves later), so layer 2 -- 8 of the 9
+// stages of a step at H1 = 512 -- is pure TMA -> wgmma.  Only x_norm (layer 1's A, written as fp32 by the step tail) is
+// split in shared memory.  Every wgmma receives the operands the fp32 buffers would give after split_tile_f16.
+// tf32 form: raw fp32 tiles of 32 k; the consumers split both operands (A into the conversion buffer, B into the upper
+// half of its ring slot), as gemm_tc.cu's tf32 form does.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -32,13 +44,23 @@ namespace sfb {
 constexpr int RF_THREADS = 384;
 constexpr int RF_HEAD_AP = 9;
 constexpr int RF_MAX_DIM = 128;
+// register budgets after the hand-over: 128 x 40 + 256 x 232 = the 384 x 168 the launch gets
+constexpr int RF_PRODUCER_REGS = 40;
+constexpr int RF_CONSUMER_REGS = 232;
 
+// Ring slot (64 KB): [A 32 KB | B 32 KB].
+//   fp16 form: A = raw fp32 x_norm tile (layer 1) or the [hi | lo] h1 tiles (layer 2); B = the weight's [hi | lo] twin tiles.
+//   tf32 form: [A raw 16 KB | B raw 16 KB | B hi | B lo].
+// Conversion buffer (32 KB): [A hi | A lo] of the operands split in shared memory.
 struct RfSmem {
-    static constexpr int RAW_STAGE = 2 * 128 * 64 * 4;            // A and B raw tiles of one k-block (64 k: fp16 form)
-    static constexpr int OFF_CONV = 2 * RAW_STAGE;                // two raw stages, then [A hi | A lo | B hi | B lo]
-    static constexpr int OFF_BARS = OFF_CONV + 4 * 128 * TBK * 4;
+    static constexpr int STAGES = 3;
+    static constexpr int SLOT = 65536;
+    static constexpr int B_OFF = 32768;
+    static constexpr int OFF_CONV = STAGES * SLOT;
+    static constexpr int OFF_BARS = OFF_CONV + 32768;                // full[STAGES], empty[STAGES]
     static constexpr int OFF_CSTAT = OFF_BARS + 64;
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
+    static_assert(2 * STAGES * 8 <= 64 && TOTAL + 64 <= 227 * 1024, "shared memory");
 };
 
 
@@ -64,9 +86,11 @@ struct RolloutArgs {
     const float* bound_x; const float* bound_h1;   // fp16-split form: bounds of |x_norm| and |h1| (device floats), else NULL
 };
 
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+    cluster_arrive();
+    cluster_wait();
 }
 // generic-proxy global stores -> async-proxy (TMA) loads: the .global form is a single FENCE.VIEW.ASYNC.G; the unqualified
 // form adds a MEMBAR.ALL.GPU (the cluster barrier's release already carries one)
@@ -82,44 +106,115 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     return r;
 }
 
-// One 128 x 128 tile acc = A[m0.., :K] . B[n0.., :K]^T by the 256 consumer threads (ct = 0..255); both operands K-major
-// by TMA through two raw stages (k-block kb+1 is in flight while kb is split and multiplied).  `it` counts the raw stages
-// used so far (the mbarrier phases) and advances identically in every consumer thread.  3xTF32, or with F16 the
-// fp16-split form of gemm_tc.cu (A * 2^a_shift, weights * 2^kF16WShift, 64 k per stage).
+// The ring: use u (counted from 0 over the whole rollout, identically by the producer and the consumers) lives in slot
+// u % STAGES; its full / empty mbarriers are in phase (u / STAGES) & 1.  A step uses the ring K1/KBK + H1/KBK times
+// (layer 1, then layer 2).
+// TMA producer, run by all of warpgroup 0 (every warp takes part in the cluster barriers); `leader` issues the loads.
 template <bool F16>
-__device__ __forceinline__ void rf_tile(const CUtensorMap* ta, const CUtensorMap* tb, int m0, int n0, int K, uint8_t* smem,
-                                        uint64_t* full, uint32_t& it, float (&acc)[64], float (&cross)[64], int ct,
-                                        int a_shift) {
+__device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUtensorMap* tmap_w1, const CUtensorMap* tmap_h1,
+                                           const CUtensorMap* tmap_w2, int T, int K1, int H1, int m0, int n0, uint8_t* smem,
+                                           uint64_t* full, uint64_t* empty, bool leader) {
     using S = RfSmem;
     constexpr int KBK = F16 ? 64 : TBK;
-    constexpr int B_OFF = 128 * KBK * 4;
-    const int wg = ct >> 7, nkb = K / KBK;
-    uint8_t* conv = smem + S::OFF_CONV;
-    auto issue = [&](uint32_t use, int kb) {
-        uint8_t* st = smem + (use & 1) * S::RAW_STAGE;
-        fence_proxy_async_all();   // generic-proxy global stores of the cluster (h1 / x_norm) -> this TMA read
-        mbar_expect_tx(&full[use & 1], 2 * B_OFF);
-        tma_load_2d(st, ta, &full[use & 1], KBK * kb, m0);
-        tma_load_2d(st + B_OFF, tb, &full[use & 1], KBK * kb, n0);
+    constexpr uint32_t STAGE_TX = F16 ? 2 * 32768 : 2 * 16384;
+    const int n1 = K1 / KBK, n2 = H1 / KBK;
+    uint32_t pu = 0;   // next use to claim
+    // claim the next use: wait until its slot is free, expect the whole stage, load the weight tile (B)
+    auto weight = [&](const CUtensorMap* tb, int kb) {
+        const uint32_t s = pu % S::STAGES;
+        mbar_wait(&empty[s], ((pu / S::STAGES) & 1) ^ 1);
+        mbar_expect_tx(&full[s], STAGE_TX);
+        uint8_t* dst = smem + s * S::SLOT + (F16 ? S::B_OFF : 16384);
+        if (F16) tma_load_3d(dst, tb, &full[s], 64 * kb, n0, 0);   // [hi | lo] twin tiles
+        else tma_load_2d(dst, tb, &full[s], TBK * kb, n0);
+        ++pu;
     };
-    if (ct == 0) issue(it, 0);
-    const uint64_t da_hi = make_smem_desc(smem_u32(conv + wg * 8192));
-    const uint64_t da_lo = make_smem_desc(smem_u32(conv + 16384 + wg * 8192));
-    const uint64_t db_hi = make_smem_desc(smem_u32(conv + 32768));
-    const uint64_t db_lo = make_smem_desc(smem_u32(conv + 49152));
-    for (int kb = 0; kb < nkb; ++kb, ++it) {
-        if (ct == 0 && kb + 1 < nkb) issue(it + 1, kb + 1);   // that stage was read by everyone before the last barrier
-        mbar_wait(&full[it & 1], (it >> 1) & 1);
-        const uint8_t* st = smem + (it & 1) * S::RAW_STAGE;
-        if constexpr (F16) {
-            split_tile_f16<false>(st, conv, conv + 16384, ct, pow2f_int(a_shift));
-            split_tile_f16<false>(st + B_OFF, conv + 32768, conv + 49152, ct, pow2f_int(kF16WShift));
-        } else {
-            split_tile<false, true>(st, conv, conv + 16384, ct);
-            split_tile<false, true>(st + B_OFF, conv + 32768, conv + 49152, ct);
+    // the activation tile (A) of a claimed use
+    auto activation = [&](uint32_t u, const CUtensorMap* ta, bool planes, int kb) {
+        const uint32_t s = u % S::STAGES;
+        if (planes) tma_load_3d(smem + s * S::SLOT, ta, &full[s], 64 * kb, m0, 0);   // [hi | lo] h1 tiles
+        else tma_load_2d(smem + s * S::SLOT, ta, &full[s], KBK * kb, m0);
+    };
+    // Claims made before a cluster barrier only wait for slots the consumers free before they arrive there (uses of the
+    // previous phase), so no claim can wait on the barrier it precedes: at most STAGES uses ahead.
+    const int pre2 = n2 < S::STAGES ? n2 : S::STAGES;
+    int pre1 = 0;   // W1 tiles of this step already in flight
+    for (int t = 0; t < T; ++t) {
+        // x_norm(t) is published (pre-step(0) before the launch, the tail of step t-1 before barrier 3)
+        if (leader) {
+            fence_proxy_async_all();
+            const uint32_t u1 = pu - pre1;
+            for (int j = 0; j < n1; ++j) {
+                if (j >= pre1) weight(tmap_w1, j);
+                activation(u1 + j, tmap_x, false, j);
+            }
         }
-        fence_proxy_async_smem();
-        consumer_sync();
+        __syncwarp();
+        cluster_arrive();                   // barrier 1: h1 of the row block complete
+        const uint32_t u2 = pu;
+        if (leader)
+            for (int j = 0; j < pre2; ++j) weight(tmap_w2, j);
+        __syncwarp();
+        cluster_wait();
+        if (leader) {
+            fence_proxy_async_all();
+            for (int j = 0; j < n2; ++j) {
+                if (j >= pre2) weight(tmap_w2, j);
+                activation(u2 + j, tmap_h1, F16, j);
+            }
+        }
+        __syncwarp();
+        cluster_arrive();                   // barrier 2: all head partials of the row block written
+        pre1 = t + 1 < T ? (n1 < S::STAGES ? n1 : S::STAGES) : 0;
+        if (leader)
+            for (int j = 0; j < pre1; ++j) weight(tmap_w1, j);
+        __syncwarp();
+        cluster_wait();
+        cluster_sync_all();                 // barrier 3: the next policy input complete
+    }
+}
+
+// One 128 x 128 tile acc = A[m0.., :K] . B[n0.., :K]^T (nkb stages) by the 256 consumer threads (ct = 0..255), `cu` the
+// consumers' use counter.  SPLIT_A: the A tile is raw fp32, split here (each warpgroup its own 64 rows) into the
+// conversion buffer; the tf32 form splits both operands.  3xTF32, or with F16 the fp16-split form of gemm_tc.cu (A *
+// 2^a_shift, weights * 2^kF16WShift, 64 k per stage).  Every accumulator receives its wgmmas in k order.
+template <bool F16, bool SPLIT_A>
+__device__ __forceinline__ void rf_tile(int nkb, uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& cu,
+                                        float (&acc)[64], float (&cross)[64], int ct, int a_shift) {
+    using S = RfSmem;
+    const int wg = ct >> 7, lt = ct & 127;
+    uint8_t* conv = smem + S::OFF_CONV;
+    // (the first wgmmas overwrite them; defined values keep the accumulators from being live across the whole rollout)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+    int held = -1;   // slot of the wgmma group still in flight
+    for (int kb = 0; kb < nkb; ++kb, ++cu) {
+        const int s = (int)(cu % S::STAGES);
+        uint8_t* slot = smem + s * S::SLOT;
+        mbar_wait(&full[s], (cu / S::STAGES) & 1);
+        const uint8_t* at = slot;
+        if (SPLIT_A || !F16) {
+            // the conversion buffer is read by this warpgroup's wgmmas in flight
+            if (held >= 0) {
+                wgmma_wait_all();
+                mbar_arrive(&empty[held]);
+                held = -1;
+            }
+            if constexpr (F16) {
+                split_tile_f16<false, 64>(slot + wg * 64 * 256, conv + wg * 8192, conv + 16384 + wg * 8192, lt,
+                                          pow2f_int(a_shift));
+            } else {
+                split_tile<false, true, 64>(slot + wg * 64 * 128, conv + wg * 8192, conv + 16384 + wg * 8192, lt);
+                split_tile<false, true>(slot + 16384, slot + S::B_OFF, slot + S::B_OFF + 16384, ct);
+            }
+            fence_proxy_async_smem();
+            consumer_sync();
+            at = conv;
+        }
+        const uint64_t da_hi = make_smem_desc(smem_u32(at + wg * 8192));
+        const uint64_t da_lo = make_smem_desc(smem_u32(at + 16384 + wg * 8192));
+        const uint64_t db_hi = make_smem_desc(smem_u32(slot + S::B_OFF));
+        const uint64_t db_lo = make_smem_desc(smem_u32(slot + S::B_OFF + 16384));
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < TBK / WG_K; ++k) {
@@ -135,9 +230,14 @@ __device__ __forceinline__ void rf_tile(const CUtensorMap* ta, const CUtensorMap
             }
         }
         wgmma_commit();
-        wgmma_wait_all();
-        consumer_sync();
+        if (held >= 0) {
+            wgmma_wait_1();                  // the previous stage's wgmmas are done with its slot
+            mbar_arrive(&empty[held]);
+        }
+        held = s;
     }
+    wgmma_wait_all();
+    mbar_arrive(&empty[held]);
     if (F16) {
         const float out_scale = pow2f_int(-(a_shift + kF16WShift));
 #pragma unroll
@@ -148,15 +248,37 @@ __device__ __forceinline__ void rf_tile(const CUtensorMap* ta, const CUtensorMap
     }
 }
 
+// Layer-1 epilogue of the fp16 form: h1 = act(acc + b1) exactly as store_tile forms it, times 2^shift_h, split by
+// f16_split2 into the hi plane (`hi`, [N][H1] halves) and the lo plane (lo_off halves later) -- the bits split_tile_f16
+// would make of the fp32 h1 tile.
+__device__ __forceinline__ void store_h1_split(const float (&acc)[64], int n0, int64_t row_base, int lane, uint16_t* hi,
+                                               int64_t lo_off, int64_t M, int H1, const float* bias, int act, float scale) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        const int64_t m = row_base + 8 * (j & 1);
+        const int n = n0 + 8 * (j >> 1) + 2 * (lane & 3);
+        if (m >= M) continue;
+        const float v0 = act_fwd_fast(acc[2 * j] + bias[n], act);
+        const float v1 = act_fwd_fast(acc[2 * j + 1] + bias[n + 1], act);
+        uint32_t h, l;
+        f16_split2(v0 * scale, v1 * scale, h, l);
+        uint16_t* dst = hi + m * H1 + n;
+        *reinterpret_cast<uint32_t*>(dst) = h;
+        *reinterpret_cast<uint32_t*>(dst + lo_off) = l;
+    }
+}
+
 template <int ACT, bool F16>
 __global__ void __launch_bounds__(RF_THREADS, 1)
 rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w1,
                          const __grid_constant__ CUtensorMap tmap_h1, const __grid_constant__ CUtensorMap tmap_w2,
                          const RolloutArgs a) {
     using S = RfSmem;
+    constexpr int KBK = F16 ? 64 : TBK;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);   // [2] raw stages landed (TMA)
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);   // [STAGES] slot landed (TMA)
+    uint64_t* empty = full + S::STAGES;                                  // [STAGES] slot read by every consumer's wgmmas
     float* cstat = reinterpret_cast<float*>(smem + S::OFF_CSTAT);       // [2][K1]: mu, 1 / sigma of the observation normaliser
 
     // episode statistics of finished episodes: accumulated per CTA over the WHOLE rollout in shared memory, five global
@@ -177,8 +299,10 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w1) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_h1) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_w2) : "memory");
-        mbar_init(&full[0], 1);
-        mbar_init(&full[1], 1);
+        for (int s = 0; s < S::STAGES; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], 256);
+        }
         fence_barrier_init();
     }
     __syncthreads();
@@ -189,186 +313,200 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     __syncthreads();
     const int64_t env_step0 = a.env_step[0];
     const uint64_t philox0 = a.sampler_step ? (uint64_t)*a.sampler_step : 0ull;
-    const float pv = a.pv_scalar ? *a.pv_scalar : 0.f;
-    // fp16-split form: binary shifts of the two activation operands from their bounds (constant over the rollout: the
-    // weights, hence the bounds, do not change inside a rollout)
-    const int shift_x = F16 ? f16_shift_for_bound(a.bound_x[0]) : 0;
-    const int shift_h = F16 ? f16_shift_for_bound(a.bound_h1[0]) : 0;
-    const bool tracer = a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 128;
+
+    if (warp < 4) {
+        setmaxnreg_dec<RF_PRODUCER_REGS>();
+        rf_produce<F16>(&tmap_x, &tmap_w1, &tmap_h1, &tmap_w2, a.T, a.K1, a.H1, (int)m0, n0, smem, full, empty,
+                        threadIdx.x == 0);
+    } else {
+        setmaxnreg_inc<RF_CONSUMER_REGS>();
+        const float pv = a.pv_scalar ? *a.pv_scalar : 0.f;
+        // fp16-split form: binary shifts of the two activation operands from their bounds (constant over the rollout: the
+        // weights, hence the bounds, do not change inside a rollout)
+        const int shift_x = F16 ? f16_shift_for_bound(a.bound_x[0]) : 0;
+        const int shift_h = F16 ? f16_shift_for_bound(a.bound_h1[0]) : 0;
+        const bool tracer = a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 128;
 #define RF_TRACE(slot) do { if (tracer) a.trace[(int64_t)t * 16 + (slot)] = rf_now(); } while (0)
-    uint32_t it = 0;
-    const TcEpilogue epi_heads{1, ACT, a.b2, nullptr, 0, a.wv, a.wa, a.A, a.part};
-    const TcEpilogue epi_h1{1, ACT, a.b1, nullptr, 0};
+        uint32_t cu = 0;
+        const TcEpilogue epi_heads{1, ACT, a.b2, nullptr, 0, a.wv, a.wa, a.A, a.part};
+        const TcEpilogue epi_h1{1, ACT, a.b1, nullptr, 0};
+        const int ct = threadIdx.x - 128;
+        const int64_t row_base = m0 + (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
+        TileCoord tc;
+        tc.m0 = m0; tc.n0 = n0; tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
 
-    for (int t = 0; t < a.T; ++t) {
-        RF_TRACE(0);
-        for (int layer = 0; layer < 2; ++layer) {
-            if (warp >= 4) {
-                const int ct = threadIdx.x - 128;
+        for (int t = 0; t < a.T; ++t) {
+            RF_TRACE(0);
+            {
                 float acc[64], cross[64];
-                if (layer == 0) rf_tile<F16>(&tmap_x, &tmap_w1, (int)m0, n0, a.K1, smem, full, it, acc, cross, ct, shift_x);
-                else rf_tile<F16>(&tmap_h1, &tmap_w2, (int)m0, n0, a.H1, smem, full, it, acc, cross, ct, shift_h);
-                TileCoord tc;
-                tc.m0 = m0; tc.n0 = n0; tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
-                const int64_t row_base = m0 + (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
-                if (layer == 0) {
+                rf_tile<F16, true>(a.K1 / KBK, smem, full, empty, cu, acc, cross, ct, shift_x);
+                if (F16)
+                    store_h1_split(acc, n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1, a.b1, ACT,
+                                   pow2f_int(shift_h));
+                else
                     store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
-                    fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
-                } else {
-                    heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
-                }
-                RF_TRACE(3 + 4 * layer);
+                fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
+                RF_TRACE(3);
             }
-            cluster_sync_all();   // h1 of the row block complete (layer 0) / all head partials of the row block written (layer 1)
-            RF_TRACE(4 + 4 * layer);              // past the cluster barrier
-        }
+            cluster_sync_all();   // h1 of the row block complete
+            RF_TRACE(4);
+            {
+                float acc[64], cross[64];
+                rf_tile<F16, !F16>(a.H1 / KBK, smem, full, empty, cu, acc, cross, ct, shift_h);
+                heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
+                RF_TRACE(7);
+            }
+            cluster_sync_all();   // all head partials of the row block written
+            RF_TRACE(8);
 
-        // ===================================================== step tail: this CTA's share of the block's rows.
-        // FOUR rows per warp at a time: an 8-lane group owns a row (one lane per action logit, the group leader also the value
-        // and the env's scalars), so the 32 rows of a CTA are ONE pass of eight warps -- the per-row dependency chain (partial
-        // sums from L2 -> softmax -> Philox -> argmax -> env rule -> stores, ~4.7 us measured) is paid once per step, not once
-        // per row a warp owns.  Bit-identical to heads_row_tail: logit a sits at group position (a + 1) % 8, which reproduces
-        // the association order of the 32-lane butterfly sums there (lanes 1..8 after the xor-16 / xor-8 steps).
-        if (warp >= 4) {
-            const int g = lane & 7;                       // position inside the 8-lane group
-            const int grp = lane >> 3;                    // which of the warp's four rows
-            const int act_idx = (g + 7) & 7;              // action index held by this lane (position (a + 1) % 8)
-            const bool has_logit = act_idx < a.A;
-            const bool leader = g == 0;
-            const bool last = (t + 1 == a.T);
-            const int64_t step = env_step0 + t;
-            const uint64_t offset = philox0 + (uint64_t)t;
-            const float* src_step = a.tape + ((step + 1) % a.tape_len) * a.N * a.K1;
-            const float* noise_t = a.noise ? a.noise + (int64_t)t * a.N * a.A : nullptr;
-            const int rpc = 128 / CX;                     // rows of the block this CTA finishes
-            const unsigned gmask = 0xffu << (grp * 8);
-            for (int base = 0; base < rpc; base += 32) {
-                const int rr = base + (warp - 4) * 4 + grp;
-                const int64_t row = m0 + cx * rpc + rr;
-                const bool ok = rr < rpc && row < a.N;
-                // ---- loads first: head partials, next observation (K1 / 8 floats per lane), episode accumulators
-                float x = 0.f, val = 0.f;
-                float ob[RF_MAX_DIM / 8];
-                float er0 = 0.f, mn0 = 0.f, mx0 = 0.f;
-                int32_t el0 = 0;
-                const int cpl = a.K1 >> 3;                // observation columns per lane (K1 is a multiple of 32)
-                if (ok) {
-                    if (has_logit)
-                        for (int p = 0; p < P; ++p) x += a.part[((int64_t)p * a.N + row) * kHeadPartPad + 1 + act_idx];
-                    if (leader)
-                        for (int p = 0; p < P; ++p) val += a.part[((int64_t)p * a.N + row) * kHeadPartPad];
-                    const float4* src4 = reinterpret_cast<const float4*>(src_step + row * a.K1 + g * cpl);
+            // ===================================================== step tail: this CTA's share of the block's rows.
+            // FOUR rows per warp at a time: an 8-lane group owns a row (one lane per action logit, the group leader also the value
+            // and the env's scalars), so the 32 rows of a CTA are ONE pass of eight warps -- the per-row dependency chain (partial
+            // sums from L2 -> softmax -> Philox -> argmax -> env rule -> stores, ~4.7 us measured) is paid once per step, not once
+            // per row a warp owns.  Bit-identical to heads_row_tail: logit a sits at group position (a + 1) % 8, which reproduces
+            // the association order of the 32-lane butterfly sums there (lanes 1..8 after the xor-16 / xor-8 steps).
+            {
+                const int g = lane & 7;                       // position inside the 8-lane group
+                const int grp = lane >> 3;                    // which of the warp's four rows
+                const int act_idx = (g + 7) & 7;              // action index held by this lane (position (a + 1) % 8)
+                const bool has_logit = act_idx < a.A;
+                const bool leader = g == 0;
+                const bool last = (t + 1 == a.T);
+                const int64_t step = env_step0 + t;
+                const uint64_t offset = philox0 + (uint64_t)t;
+                const float* src_step = a.tape + ((step + 1) % a.tape_len) * a.N * a.K1;
+                const float* noise_t = a.noise ? a.noise + (int64_t)t * a.N * a.A : nullptr;
+                const int rpc = 128 / CX;                     // rows of the block this CTA finishes
+                const unsigned gmask = 0xffu << (grp * 8);
+                for (int base = 0; base < rpc; base += 32) {
+                    const int rr = base + (warp - 4) * 4 + grp;
+                    const int64_t row = m0 + cx * rpc + rr;
+                    const bool ok = rr < rpc && row < a.N;
+                    // ---- loads first: head partials, next observation (K1 / 8 floats per lane), episode accumulators
+                    float x = 0.f, val = 0.f;
+                    float ob[RF_MAX_DIM / 8];
+                    float er0 = 0.f, mn0 = 0.f, mx0 = 0.f;
+                    int32_t el0 = 0;
+                    const int cpl = a.K1 >> 3;                // observation columns per lane (K1 is a multiple of 32)
+                    if (ok) {
+                        if (has_logit)
+                            for (int p = 0; p < P; ++p) x += a.part[((int64_t)p * a.N + row) * kHeadPartPad + 1 + act_idx];
+                        if (leader)
+                            for (int p = 0; p < P; ++p) val += a.part[((int64_t)p * a.N + row) * kHeadPartPad];
+                        const float4* src4 = reinterpret_cast<const float4*>(src_step + row * a.K1 + g * cpl);
 #pragma unroll
-                    for (int q = 0; q < RF_MAX_DIM / 32; ++q)
-                        if (4 * q < cpl) {
-                            const float4 f4 = src4[q];
-                            ob[4 * q] = f4.x; ob[4 * q + 1] = f4.y; ob[4 * q + 2] = f4.z; ob[4 * q + 3] = f4.w;
-                        }
-                    if (leader && a.ep_ret) { er0 = a.ep_ret[row]; el0 = a.ep_len[row]; mn0 = a.ep_min[row]; mx0 = a.ep_max[row]; }
-                }
-                // ---- CategoricalActionDistribution on the group (action_distributions.py:110-148), as heads_row_tail
-                x += has_logit ? a.ba[act_idx] : 0.f;
-                val += a.bv[0];
-                const float xl = has_logit ? x : -INFINITY;
-                float m = xl;
-#pragma unroll
-                for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                const float ex = has_logit ? expf(xl - m) : 0.f;
-                float ssum = ex;
-#pragma unroll
-                for (int o = 4; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
-                const float pr = __fdiv_rn(ex, ssum);                       // softmax :116
-                const float logp = (xl - m) - logf(ssum);                   // log_softmax :125
-                float q = 1.f;
-                if (ok && has_logit) {
-                    if (noise_t) q = noise_t[row * a.A + act_idx];
-                    else {
-                        curandStatePhilox4_32_10_t st;
-                        curand_init(a.seed, (unsigned long long)(row * a.A + act_idx), offset, &st);
-                        q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);    // Exp(1)
-                    }
-                }
-                float best = has_logit ? __fdiv_rn(pr, q) : -INFINITY;      // multinomial == argmax(p / q), first index on ties
-                int idx = has_logit ? act_idx : 0x7fffffff;
-#pragma unroll
-                for (int o = 4; o > 0; o >>= 1) {
-                    const float ob_ = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-                    if (ob_ > best || (ob_ == best && oi < idx)) { best = ob_; idx = oi; }
-                }
-                const float lp = __shfl_sync(0xffffffffu, logp, (grp << 3) | ((idx + 1) & 7));   // log_prob :145-148
-                (void)gmask;
-                if (!ok) continue;
-                // ---- trajectory slot t, env step, post step, pre step of t + 1
-                if (has_logit) a.logits[row * a.logits_rs + (int64_t)t * a.A + act_idx] = x;
-                const int64_t env = a.env_off + row;
-                const float r_raw = (float)idx / (float)a.A;
-                const bool tm = ((step * 7 + env * 13) % a.term_period) == 0;
-                const bool tr = (((step + env) % a.trunc_period) == 0) && !tm;
-                float* obs_next = a.traj_obs + row * a.traj_obs_rs + (int64_t)(t + 1) * a.K1 + g * cpl;
-                float* env_o = a.env_obs + row * a.K1 + g * cpl;
-                float* xn = a.x_norm + row * a.K1 + g * cpl;
-#pragma unroll
-                for (int q4 = 0; q4 < RF_MAX_DIM / 32; ++q4)
-                    if (4 * q4 < cpl) {
-                        const float4 f4 = make_float4(ob[4 * q4], ob[4 * q4 + 1], ob[4 * q4 + 2], ob[4 * q4 + 3]);
-                        reinterpret_cast<float4*>(env_o)[q4] = f4;
-                        reinterpret_cast<float4*>(obs_next)[q4] = f4;
-                        if (!last) {
-                            const int c = g * cpl + 4 * q4;
-                            float4 y;
-                            y.x = norm_one(f4.x, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c] : 0.f, do_rms ? cstat[a.K1 + c] : 1.f, a.clip);
-                            y.y = norm_one(f4.y, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 1] : 0.f, do_rms ? cstat[a.K1 + c + 1] : 1.f, a.clip);
-                            y.z = norm_one(f4.z, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 2] : 0.f, do_rms ? cstat[a.K1 + c + 2] : 1.f, a.clip);
-                            y.w = norm_one(f4.w, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 3] : 0.f, do_rms ? cstat[a.K1 + c + 3] : 1.f, a.clip);
-                            reinterpret_cast<float4*>(xn)[q4] = y;
-                        }
-                    }
-                if (a.rnn)
-                    for (int j = g; j < a.rnn_dim; j += 8)
-                        a.traj_rnn[row * a.traj_rnn_rs + (int64_t)(t + 1) * a.rnn_dim + j] = a.rnn[row * a.rnn_dim + j];
-                if (leader) {
-                    a.values[row * a.values_rs + t] = val;
-                    a.actions[row * a.actions_rs + t] = (float)idx;
-                    a.env_actions[row] = idx;
-                    a.log_prob[row * a.lp_rs + t] = lp;
-                    a.pv_out[row * a.pv_rs + t] = pv;
-                    a.env_rew[row] = r_raw;
-                    a.env_term[row] = tm;
-                    a.env_trunc[row] = tr;
-                    const bool done = tm || tr;                                     // batched_sampling.py:317
-                    float r = __fmul_rn(r_raw, a.reward_scale);                     // :209
-                    r = clampf(r, -a.reward_clip, a.reward_clip);                   // :210
-                    a.t_rew[row * a.stride + t] = r;
-                    a.t_done[row * a.stride + t] = done ? 1 : 0;
-                    a.t_to[row * a.stride + t] = tr ? 1 : 0;                        // :328
-                    a.t_pid[row * a.stride + t] = a.policy_id;
-                    if (a.ep_ret) {                                                 // _process_env_step :215-287 (raw reward)
-                        float er = er0 + r_raw;
-                        int32_t el = el0 + a.len_inc;
-                        float mn = fminf(mn0, r_raw), mx = fmaxf(mx0, r_raw);
-                        if (a.fin_ret) {
-                            a.fin_ret[row * a.stride + t] = done ? er : __int_as_float(0x7fc00000);
-                            a.fin_len[row * a.stride + t] = done ? el : -1;
-                        }
-                        if (done) {
-                            if (a.stats) {
-                                atomicAdd(&s_stats[0], 1.0); atomicAdd(&s_stats[1], (double)er); atomicAdd(&s_stats[2], (double)el);
-                                atomicAdd(&s_stats[3], (double)mn); atomicAdd(&s_stats[4], (double)mx);
+                        for (int q = 0; q < RF_MAX_DIM / 32; ++q)
+                            if (4 * q < cpl) {
+                                const float4 f4 = src4[q];
+                                ob[4 * q] = f4.x; ob[4 * q + 1] = f4.y; ob[4 * q + 2] = f4.z; ob[4 * q + 3] = f4.w;
                             }
-                            er = 0.f; el = 0; mn = INFINITY; mx = -INFINITY;
+                        if (leader && a.ep_ret) { er0 = a.ep_ret[row]; el0 = a.ep_len[row]; mn0 = a.ep_min[row]; mx0 = a.ep_max[row]; }
+                    }
+                    // ---- CategoricalActionDistribution on the group (action_distributions.py:110-148), as heads_row_tail
+                    x += has_logit ? a.ba[act_idx] : 0.f;
+                    val += a.bv[0];
+                    const float xl = has_logit ? x : -INFINITY;
+                    float m = xl;
+#pragma unroll
+                    for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+                    const float ex = has_logit ? expf(xl - m) : 0.f;
+                    float ssum = ex;
+#pragma unroll
+                    for (int o = 4; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
+                    const float pr = __fdiv_rn(ex, ssum);                       // softmax :116
+                    const float logp = (xl - m) - logf(ssum);                   // log_softmax :125
+                    float q = 1.f;
+                    if (ok && has_logit) {
+                        if (noise_t) q = noise_t[row * a.A + act_idx];
+                        else {
+                            curandStatePhilox4_32_10_t st;
+                            curand_init(a.seed, (unsigned long long)(row * a.A + act_idx), offset, &st);
+                            q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);    // Exp(1)
                         }
-                        a.ep_ret[row] = er; a.ep_len[row] = el; a.ep_min[row] = mn; a.ep_max[row] = mx;
+                    }
+                    float best = has_logit ? __fdiv_rn(pr, q) : -INFINITY;      // multinomial == argmax(p / q), first index on ties
+                    int idx = has_logit ? act_idx : 0x7fffffff;
+#pragma unroll
+                    for (int o = 4; o > 0; o >>= 1) {
+                        const float ob_ = __shfl_xor_sync(0xffffffffu, best, o);
+                        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+                        if (ob_ > best || (ob_ == best && oi < idx)) { best = ob_; idx = oi; }
+                    }
+                    const float lp = __shfl_sync(0xffffffffu, logp, (grp << 3) | ((idx + 1) & 7));   // log_prob :145-148
+                    (void)gmask;
+                    if (!ok) continue;
+                    // ---- trajectory slot t, env step, post step, pre step of t + 1
+                    if (has_logit) a.logits[row * a.logits_rs + (int64_t)t * a.A + act_idx] = x;
+                    const int64_t env = a.env_off + row;
+                    const float r_raw = (float)idx / (float)a.A;
+                    const bool tm = ((step * 7 + env * 13) % a.term_period) == 0;
+                    const bool tr = (((step + env) % a.trunc_period) == 0) && !tm;
+                    float* obs_next = a.traj_obs + row * a.traj_obs_rs + (int64_t)(t + 1) * a.K1 + g * cpl;
+                    float* env_o = a.env_obs + row * a.K1 + g * cpl;
+                    float* xn = a.x_norm + row * a.K1 + g * cpl;
+#pragma unroll
+                    for (int q4 = 0; q4 < RF_MAX_DIM / 32; ++q4)
+                        if (4 * q4 < cpl) {
+                            const float4 f4 = make_float4(ob[4 * q4], ob[4 * q4 + 1], ob[4 * q4 + 2], ob[4 * q4 + 3]);
+                            reinterpret_cast<float4*>(env_o)[q4] = f4;
+                            reinterpret_cast<float4*>(obs_next)[q4] = f4;
+                            if (!last) {
+                                const int c = g * cpl + 4 * q4;
+                                float4 y;
+                                y.x = norm_one(f4.x, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c] : 0.f, do_rms ? cstat[a.K1 + c] : 1.f, a.clip);
+                                y.y = norm_one(f4.y, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 1] : 0.f, do_rms ? cstat[a.K1 + c + 1] : 1.f, a.clip);
+                                y.z = norm_one(f4.z, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 2] : 0.f, do_rms ? cstat[a.K1 + c + 2] : 1.f, a.clip);
+                                y.w = norm_one(f4.w, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 3] : 0.f, do_rms ? cstat[a.K1 + c + 3] : 1.f, a.clip);
+                                reinterpret_cast<float4*>(xn)[q4] = y;
+                            }
+                        }
+                    if (a.rnn)
+                        for (int j = g; j < a.rnn_dim; j += 8)
+                            a.traj_rnn[row * a.traj_rnn_rs + (int64_t)(t + 1) * a.rnn_dim + j] = a.rnn[row * a.rnn_dim + j];
+                    if (leader) {
+                        a.values[row * a.values_rs + t] = val;
+                        a.actions[row * a.actions_rs + t] = (float)idx;
+                        a.env_actions[row] = idx;
+                        a.log_prob[row * a.lp_rs + t] = lp;
+                        a.pv_out[row * a.pv_rs + t] = pv;
+                        a.env_rew[row] = r_raw;
+                        a.env_term[row] = tm;
+                        a.env_trunc[row] = tr;
+                        const bool done = tm || tr;                                     // batched_sampling.py:317
+                        float r = __fmul_rn(r_raw, a.reward_scale);                     // :209
+                        r = clampf(r, -a.reward_clip, a.reward_clip);                   // :210
+                        a.t_rew[row * a.stride + t] = r;
+                        a.t_done[row * a.stride + t] = done ? 1 : 0;
+                        a.t_to[row * a.stride + t] = tr ? 1 : 0;                        // :328
+                        a.t_pid[row * a.stride + t] = a.policy_id;
+                        if (a.ep_ret) {                                                 // _process_env_step :215-287 (raw reward)
+                            float er = er0 + r_raw;
+                            int32_t el = el0 + a.len_inc;
+                            float mn = fminf(mn0, r_raw), mx = fmaxf(mx0, r_raw);
+                            if (a.fin_ret) {
+                                a.fin_ret[row * a.stride + t] = done ? er : __int_as_float(0x7fc00000);
+                                a.fin_len[row * a.stride + t] = done ? el : -1;
+                            }
+                            if (done) {
+                                if (a.stats) {
+                                    atomicAdd(&s_stats[0], 1.0); atomicAdd(&s_stats[1], (double)er); atomicAdd(&s_stats[2], (double)el);
+                                    atomicAdd(&s_stats[3], (double)mn); atomicAdd(&s_stats[4], (double)mx);
+                                }
+                                er = 0.f; el = 0; mn = INFINITY; mx = -INFINITY;
+                            }
+                            a.ep_ret[row] = er; a.ep_len[row] = el; a.ep_min[row] = mn; a.ep_max[row] = mx;
+                        }
                     }
                 }
+                fence_proxy_async_all();   // x_norm stores -> the peers' TMA loads of the next step
+                RF_TRACE(9);                          // tail done
             }
-            fence_proxy_async_all();   // x_norm stores -> the peers' TMA loads of the next step
-            RF_TRACE(9);                          // tail done
+
+            cluster_sync_all();   // the row block's next policy input is complete; nobody still reads this step's partials
+            RF_TRACE(10);
         }
-        cluster_sync_all();   // the row block's next policy input is complete; nobody still reads this step's partials
-        RF_TRACE(10);
-    }
 #undef RF_TRACE
+    }
 
     // every block has read the two step counters at its start; the last one to finish advances them by T
     __syncthreads();
@@ -439,6 +577,8 @@ static bool rollout_f16_enabled() {
         default: return launch_rollout<SFB200_ACT_NONE, F16v>(tm, a, CX, st);                \
     }
 
+static int g_rollout_form = -1;   // form of the last launch: 1 fp16 split, 0 tf32 split
+
 int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, const RolloutArgs& a_in, cudaStream_t st) {
     if (!tc_rollout_mlp2_supported(W1, W2, a_in.K1, a_in.H1, a_in.H2, a_in.A, engine)) return SFB_TC_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(a_in.wv) & 7u) || (reinterpret_cast<uintptr_t>(a_in.wa) & 7u)) return SFB_TC_UNSUPPORTED;
@@ -456,21 +596,27 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
             }
             a.bound_x = bx;
             a.bound_h1 = bh;
+            // the h1 scratch (N x H1 floats) holds the split h1: hi plane [N][H1] halves, then the lo plane
             CUtensorMap tm[4];
             bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 64, 128);
-            ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, 64, 128);
-            ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, 64, 128);
-            ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, 64, 128);
-            if (!ok) return SFB_TC_UNSUPPORTED;
-            SFB_RF_LAUNCH(true)
+            ok = ok && make_tmap_f16_twins(&tm[1], t1.hi, t1.lo - t1.hi, (uint64_t)a.K1, (uint64_t)a.H1);
+            ok = ok && make_tmap_f16_twins(&tm[2], reinterpret_cast<const uint16_t*>(a.h1), a.N * a.H1, (uint64_t)a.H1,
+                                           (uint64_t)a.N);
+            ok = ok && make_tmap_f16_twins(&tm[3], t2.hi, t2.lo - t2.hi, (uint64_t)a.H1, (uint64_t)a.H2);
+            if (ok) {   // (twins TMA cannot describe keep the tf32 form, as in gemm_tc)
+                g_rollout_form = 1;
+                SFB_RF_LAUNCH(true)
+            }
         }
     }
+    a.bound_x = a.bound_h1 = nullptr;
     CUtensorMap tm[4];
     bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, TBK, 128);
     ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, TBK, 128);
     ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, TBK, 128);
     ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, TBK, 128);
     if (!ok) return SFB_TC_UNSUPPORTED;
+    g_rollout_form = 0;
     SFB_RF_LAUNCH(false)
 }
 #undef SFB_RF_LAUNCH
@@ -482,11 +628,13 @@ using namespace sfb;
 extern "C" {
 
 static unsigned long long* g_rollout_trace = nullptr;
-/* debug: device buffer of T x 12 uint64 that the next rollouts fill with phase time stamps (NULL switches it off) */
+/* debug: device buffer of T x 16 uint64 that the next rollouts fill with phase time stamps (NULL switches it off) */
 int sfb200_rollout_set_trace(void* trace_dev) {
     g_rollout_trace = (unsigned long long*)trace_dev;
     return 0;
 }
+
+int sfb200_rollout_last_form(void) { return g_rollout_form; }
 
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine) {
     return tc_rollout_mlp2_supported(W1, W2, K1, H1, H2, A, engine);

@@ -66,6 +66,14 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed wgmma group of this warpgroup have completed
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+// warpgroup-wide register budget hand-over (every warp of the warpgroup executes it)
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 // D[64 x 128] (+)= A[64 x 8] * B[128 x 8]^T, tf32 operands from shared memory (K-major, 128B swizzle), fp32
 // accumulators in the registers of the issuing warpgroup (PTX wgmma.mma_async m64n128k8 .tf32).  scale_d = 0 overwrites D.
@@ -154,5 +162,8 @@ __device__ __forceinline__ float act_bwd_ct(float h) {
 bool tc_init();
 bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
                uint32_t box1);
+// 3-D fp16 map over a [hi | lo] pair of row-major [rows][K] planes, lo_offset elements apart: box 64 k x 128 rows x both
+// planes with the 128B swizzle (the weights' registered twins; the rollout's split h1 scratch)
+bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows);
 
 }  // namespace sfb

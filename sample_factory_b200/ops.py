@@ -710,6 +710,12 @@ def rollout_mlp2_tape(T: int, W1: Tensor, b1: Tensor, W2: Tensor, b2: Tensor, ac
                inv_scale, eps, clip, _stream())
 
 
+def rollout_last_form() -> int:
+    """form of the last rollout_mlp2_tape launch: 1 fp16 split (weight twins and activation bounds registered), 0 tf32
+    split, -1 none yet"""
+    return lib().query("sfb200_rollout_last_form")
+
+
 def gather_rows(src: Tensor, idx: Tensor, dst: Tensor) -> None:
     """dst[r] = src[idx[r]] along dim 0 (dense rows of any dtype) -- the shuffled-minibatch gather"""
     assert src.is_contiguous() and dst.is_contiguous() and src.dtype == dst.dtype and src.shape[1:] == dst.shape[1:]
