@@ -1,6 +1,8 @@
 // PPO loss, forward and backward fused (algo/learning/learner.py:586-657, :431-477), plus the per-minibatch advantage
 // statistics (:646-647) and the action-ratio pre-pass V-trace needs (:588-594).  One thread per sample; every input
 // is read exactly once (HBM-bound, ~(2A+9)*4 B read + (A+1)*4 B written per sample).
+#include <type_traits>
+
 #include "common.cuh"
 #include "mixed_layout.cuh"
 
@@ -184,6 +186,19 @@ __device__ __forceinline__ float ppo_value_terms(float v, float vo, float R, flo
     return w * c_val * gv;
 }
 
+// the minibatch constants every loss kernel starts from: advantage mean / std and the gradient weight grad_scale / n_valid
+struct PpoW {
+    float adv_mean, adv_std, w;
+};
+__device__ __forceinline__ PpoW ppo_weights(const double* __restrict__ stats, float grad_scale) {
+    const double n_valid = stats[SFB200_LS_NUM_VALID];
+    PpoW pw;
+    pw.adv_mean = (float)stats[SFB200_LS_ADV_MEAN];
+    pw.adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);   // clamp_min :647
+    pw.w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;
+    return pw;
+}
+
 __device__ __forceinline__ void ppo_store_partials(const PpoAcc& a, double* __restrict__ part, double* sm) {
     double* my = part + (int64_t)blockIdx.x * kNumPart;
     double t;
@@ -211,10 +226,8 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(
     double* __restrict__ part) {
     __shared__ double sm[8];
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    const double n_valid = stats[SFB200_LS_NUM_VALID];
-    const float adv_mean = (float)stats[SFB200_LS_ADV_MEAN];
-    const float adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);   // clamp_min :647
-    const float w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
     PpoAcc acc;
 
     if (i < batch) {
@@ -323,10 +336,8 @@ __global__ void __launch_bounds__(256) ppo_loss_tuple_kernel(
     double* __restrict__ part) {
     __shared__ double sm[8];
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    const double n_valid = stats[SFB200_LS_NUM_VALID];
-    const float adv_mean = (float)stats[SFB200_LS_ADV_MEAN];
-    const float adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);
-    const float w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
     PpoAcc acc;
 
     if (i < batch) {
@@ -454,10 +465,8 @@ __global__ void __launch_bounds__(256) ppo_loss_gauss_kernel(
     float* __restrict__ dvalues, const double* __restrict__ stats, double* __restrict__ part) {
     __shared__ double sm[8];
     const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-    const double n_valid = stats[SFB200_LS_NUM_VALID];
-    const float adv_mean = (float)stats[SFB200_LS_ADV_MEAN];
-    const float adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);
-    const float w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
     PpoAcc acc;
 
     if (i < batch) {
@@ -653,15 +662,6 @@ __device__ __forceinline__ void wide_softmax(const float (&l)[LPL], int lo, int 
     }
 }
 
-#define SFB_WIDE_PROLOGUE                                                                                   \
-    __shared__ double sm[8];                                                                                \
-    const int lane = threadIdx.x & 31;                                                                      \
-    const double n_valid = stats[SFB200_LS_NUM_VALID];                                                      \
-    const float adv_mean = (float)stats[SFB200_LS_ADV_MEAN];                                                \
-    const float adv_std = fmaxf((float)stats[SFB200_LS_ADV_STD], 1e-7f);                                    \
-    const float w = n_valid > 0.0 ? (float)((double)grad_scale / n_valid) : 0.f;                            \
-    PpoAcc acc;   /* statistics of sample blockIdx.x * 256 + threadIdx.x */                                 \
-    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31)
 
 template <int LPL>
 __global__ void __launch_bounds__(256) ppo_loss_wide_kernel(
@@ -671,7 +671,12 @@ __global__ void __launch_bounds__(256) ppo_loss_wide_kernel(
     int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent, int expl_mode, float c_val, float c_kl,
     float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues, const double* __restrict__ stats,
     double* __restrict__ part) {
-    SFB_WIDE_PROLOGUE;
+    __shared__ double sm[8];
+    const int lane = threadIdx.x & 31;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
+    PpoAcc acc;   // statistics of sample blockIdx.x * 256 + threadIdx.x
+    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31);
     for (int r = 0; r < 32; ++r) {
         const int64_t i = base + r;
         if (i >= batch) break;   // warp-uniform
@@ -749,7 +754,12 @@ __global__ void __launch_bounds__(256) ppo_loss_tuple_wide_kernel(
     int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent, int expl_mode, float c_val, float c_kl,
     float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues, const double* __restrict__ stats,
     double* __restrict__ part) {
-    SFB_WIDE_PROLOGUE;
+    __shared__ double sm[8];
+    const int lane = threadIdx.x & 31;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
+    PpoAcc acc;   // statistics of sample blockIdx.x * 256 + threadIdx.x
+    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31);
     for (int r = 0; r < 32; ++r) {
         const int64_t i = base + r;
         if (i >= batch) break;
@@ -837,7 +847,12 @@ __global__ void __launch_bounds__(256) ppo_loss_gauss_wide_kernel(
     const float* __restrict__ params_old, int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent,
     float c_val, float c_kl, float grad_scale, float* __restrict__ dlogits, float* __restrict__ dlogstd,
     float* __restrict__ dvalues, const double* __restrict__ stats, double* __restrict__ part) {
-    SFB_WIDE_PROLOGUE;
+    __shared__ double sm[8];
+    const int lane = threadIdx.x & 31;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
+    PpoAcc acc;   // statistics of sample blockIdx.x * 256 + threadIdx.x
+    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31);
     for (int r = 0; r < 32; ++r) {
         const int64_t i = base + r;
         if (i >= batch) break;
@@ -1014,7 +1029,12 @@ __global__ void __launch_bounds__(256) ppo_loss_mixed_kernel(
     const float* __restrict__ params_old, int64_t batch, float clip_lo, float clip_hi, float clip_value, float c_ent,
     float c_val, float c_kl, float grad_scale, float* __restrict__ dlogits, float* __restrict__ dvalues,
     const double* __restrict__ stats, double* __restrict__ part) {
-    SFB_WIDE_PROLOGUE;
+    __shared__ double sm[8];
+    const int lane = threadIdx.x & 31;
+    const PpoW pw = ppo_weights(stats, grad_scale);
+    const float adv_mean = pw.adv_mean, adv_std = pw.adv_std, w = pw.w;
+    PpoAcc acc;   // statistics of sample blockIdx.x * 256 + threadIdx.x
+    const int64_t base = blockIdx.x * (int64_t)blockDim.x + (threadIdx.x & ~31);
     const int A = ml.A;
     for (int r = 0; r < 32; ++r) {
         const int64_t i = base + r;
@@ -1130,8 +1150,6 @@ __global__ void __launch_bounds__(256) ppo_loss_mixed_kernel(
     ppo_store_partials(acc, part, sm);
 }
 
-#undef SFB_WIDE_PROLOGUE
-
 template <int LPL>
 __global__ void __launch_bounds__(256) action_ratio_mixed_kernel(const float* __restrict__ params, const MixedLayout ml,
                                                                  const float* __restrict__ actions,
@@ -1147,13 +1165,77 @@ __global__ void __launch_bounds__(256) action_ratio_mixed_kernel(const float* __
     if (lane == 0) ratio[i] = clampf(expf(lp - lp_old[i]), 0.05f, 20.0f);
 }
 
-// LPL = elements per lane for a row of n > 32 elements
-#define SFB_WIDE_LPL(n, LAUNCH)          \
-    if ((n) <= 64) LAUNCH(2);            \
-    else if ((n) <= 128) LAUNCH(4);      \
-    else if ((n) <= 256) LAUNCH(8);      \
-    else if ((n) <= 512) LAUNCH(16);     \
-    else LAUNCH(32)
+// ---- host side: width -> kernel instantiation, and the tail every loss entry point shares -----------------------------
+template <int N>
+using Int = std::integral_constant<int, N>;
+
+// f(Int<LPL>) for a one-warp-per-sample row of n > 32 elements (LPL = elements per lane)
+template <class F>
+static void with_lpl(int n, F&& f) {
+    if (n <= 64) f(Int<2>{});
+    else if (n <= 128) f(Int<4>{});
+    else if (n <= 256) f(Int<8>{});
+    else if (n <= 512) f(Int<16>{});
+    else f(Int<32>{});
+}
+
+// narrow(Int<AMAX>) for rows of up to 32 elements (one thread per sample), else wide(Int<LPL>)
+template <class Narrow, class Wide>
+static void with_width(int n, Narrow&& narrow, Wide&& wide) {
+    if (n <= 8) narrow(Int<8>{});
+    else if (n <= 16) narrow(Int<16>{});
+    else if (n <= 32) narrow(Int<32>{});
+    else with_lpl(n, wide);
+}
+
+// a mixed Tuple takes one warp per sample at every width
+template <class F>
+static void with_mixed_lpl(int A, F&& f) {
+    if (A <= 32) f(Int<1>{});
+    else with_lpl(A, f);
+}
+
+// the launch of a loss kernel: clip window, grid, and the workspace split (loss partials first, ppo_loss_finalize_kernel
+// reduces them)
+struct LossLaunch {
+    float clip_lo, clip_hi;
+    unsigned grid;
+    double* part;
+    cudaStream_t st;
+};
+
+static LossLaunch loss_launch(int64_t batch, float clip_ratio, void* workspace, void* stream) {
+    LossLaunch L;
+    L.clip_hi = 1.0f + clip_ratio;      // learner.py:544
+    L.clip_lo = 1.0f / L.clip_hi;       // :546
+    L.grid = (unsigned)ceil_div(batch, 256);
+    L.part = (double*)workspace;
+    L.st = (cudaStream_t)stream;
+    return L;
+}
+
+// checks the loss kernel's launch and runs the finalize
+static int loss_finalize(const LossLaunch& L, int64_t batch, float c_ent, int expl_mode, float c_val, float c_kl,
+                         double* stats) {
+    SFB_LAUNCH_OK();
+    ppo_loss_finalize_kernel<<<1, 256, 0, L.st>>>(L.part, (int)L.grid, batch, c_ent, expl_mode, c_val, c_kl, stats);
+    SFB_LAUNCH_OK();
+    return 0;
+}
+
+// grid of a ratio kernel: 256 samples per block (one per thread) or 8 (one per warp)
+static unsigned ratio_grid(int64_t batch, bool wide) { return (unsigned)ceil_div(batch, wide ? 8 : 256); }
+
+static int make_segs(Segs& sg, int A, int num_heads, const int32_t* head_sizes) {
+    SFB_CHECK_ARG(num_heads >= 1 && num_heads <= 8 && head_sizes, "tuple action space: 1 <= number of heads <= 8");
+    int tot = 0;
+    sg.n = num_heads;
+    for (int k = 0; k < 8; ++k) sg.len[k] = k < num_heads ? head_sizes[k] : 0;
+    for (int k = 0; k < num_heads; ++k) tot += head_sizes[k];
+    SFB_CHECK_ARG(tot == A && A <= kWideMax, "tuple action space: head sizes must sum to A = %d (<= %d), got %d", A, kWideMax,
+                  tot);
+    return 0;
+}
 
 }  // namespace sfb
 
@@ -1172,17 +1254,17 @@ int sfb200_action_ratio(const float* logits, int A, const float* actions_f32, co
     SFB_CHECK_ARG(A >= 1 && A <= kWideMax, "action_ratio: supports 1 <= A <= %d, got %d", kWideMax, A);
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    if (A <= 8) action_ratio_kernel<8><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
-    else if (A <= 16) action_ratio_kernel<16><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
-    else if (A <= 32) action_ratio_kernel<32><<<g, 256, 0, st>>>(logits, A, actions_f32, log_prob_old, batch, ratio);
-    else {
-        const Segs one{1, {A}};
-        const unsigned gw = (unsigned)ceil_div(batch, 8);
-#define SFB_ARW(LPL) action_ratio_wide_kernel<LPL><<<gw, 256, 0, st>>>(logits, A, one, actions_f32, log_prob_old, batch, ratio)
-        SFB_WIDE_LPL(A, SFB_ARW);
-#undef SFB_ARW
-    }
+    const Segs one{1, {A}};
+    with_width(
+        A,
+        [&](auto am) {
+            action_ratio_kernel<decltype(am)::value><<<ratio_grid(batch, false), 256, 0, st>>>(logits, A, actions_f32,
+                                                                                              log_prob_old, batch, ratio);
+        },
+        [&](auto lpl) {
+            action_ratio_wide_kernel<decltype(lpl)::value><<<ratio_grid(batch, true), 256, 0, st>>>(
+                logits, A, one, actions_f32, log_prob_old, batch, ratio);
+        });
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -1219,42 +1301,15 @@ int sfb200_ppo_loss_fwd_bwd(const float* logits, const float* values, int A, con
     SFB_CHECK_ARG(logits && values && actions_f32 && log_prob_old && values_old && adv && targets && valids && dlogits &&
                       dvalues && stats && workspace && batch > 0, "ppo_loss_fwd_bwd: bad arguments");
     SFB_CHECK_ARG(A >= 1 && A <= kWideMax, "ppo_loss_fwd_bwd: supports 1 <= A <= %d, got %d", kWideMax, A);
-    cudaStream_t st = (cudaStream_t)stream;
-    const float clip_hi = 1.0f + clip_ratio;          // learner.py:544
-    const float clip_lo = 1.0f / clip_hi;             // :546
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    double* part = (double*)workspace;
-#define SFB_PL(AM)                                                                                                   \
-    ppo_loss_kernel<AM><<<g, 256, 0, st>>>(logits, values, A, actions_f32, log_prob_old, values_old, adv, targets,    \
-                                           valids, logits_old, batch, clip_lo, clip_hi, clip_value, exploration_coeff, \
-                                           exploration_loss, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, stats, part)
-#define SFB_PLW(LPL)                                                                                                  \
-    ppo_loss_wide_kernel<LPL><<<g, 256, 0, st>>>(logits, values, A, actions_f32, log_prob_old, values_old, adv, targets, \
-                                                 valids, logits_old, batch, clip_lo, clip_hi, clip_value,               \
-                                                 exploration_coeff, exploration_loss, value_coeff, kl_coeff, grad_scale, \
-                                                 dlogits, dvalues, stats, part)
-    if (A <= 8) SFB_PL(8);
-    else if (A <= 16) SFB_PL(16);
-    else if (A <= 32) SFB_PL(32);
-    else { SFB_WIDE_LPL(A, SFB_PLW); }
-#undef SFB_PLW
-#undef SFB_PL
-    SFB_LAUNCH_OK();
-    ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff,
-                                                stats);
-    SFB_LAUNCH_OK();
-    return 0;
-}
-
-static int make_segs(Segs& sg, int A, int num_heads, const int32_t* head_sizes) {
-    SFB_CHECK_ARG(num_heads >= 1 && num_heads <= 8 && head_sizes, "tuple action space: 1 <= number of heads <= 8");
-    int tot = 0;
-    sg.n = num_heads;
-    for (int k = 0; k < 8; ++k) sg.len[k] = k < num_heads ? head_sizes[k] : 0;
-    for (int k = 0; k < num_heads; ++k) tot += head_sizes[k];
-    SFB_CHECK_ARG(tot == A && A <= kWideMax, "tuple action space: head sizes must sum to A = %d (<= %d), got %d", A, kWideMax,
-                  tot);
-    return 0;
+    const LossLaunch L = loss_launch(batch, clip_ratio, workspace, stream);
+    auto launch = [&](auto kernel) {
+        kernel<<<L.grid, 256, 0, L.st>>>(logits, values, A, actions_f32, log_prob_old, values_old, adv, targets, valids,
+                                         logits_old, batch, L.clip_lo, L.clip_hi, clip_value, exploration_coeff,
+                                         exploration_loss, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, stats, L.part);
+    };
+    with_width(A, [&](auto am) { launch(ppo_loss_kernel<decltype(am)::value>); },
+               [&](auto lpl) { launch(ppo_loss_wide_kernel<decltype(lpl)::value>); });
+    return loss_finalize(L, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff, stats);
 }
 
 int sfb200_action_ratio_tuple(const float* logits, int A, int num_heads, const int32_t* head_sizes_host,
@@ -1265,16 +1320,11 @@ int sfb200_action_ratio_tuple(const float* logits, int A, int num_heads, const i
     if (int rc = make_segs(sg, A, num_heads, head_sizes_host)) return rc;
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    if (A <= 8) action_ratio_tuple_kernel<8><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
-    else if (A <= 16) action_ratio_tuple_kernel<16><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
-    else if (A <= 32) action_ratio_tuple_kernel<32><<<g, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
-    else {
-        const unsigned gw = (unsigned)ceil_div(batch, 8);
-#define SFB_ARW(LPL) action_ratio_wide_kernel<LPL><<<gw, 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio)
-        SFB_WIDE_LPL(A, SFB_ARW);
-#undef SFB_ARW
-    }
+    auto launch = [&](auto kernel, bool wide) {
+        kernel<<<ratio_grid(batch, wide), 256, 0, st>>>(logits, A, sg, actions_f32, log_prob_old, batch, ratio);
+    };
+    with_width(A, [&](auto am) { launch(action_ratio_tuple_kernel<decltype(am)::value>, false); },
+               [&](auto lpl) { launch(action_ratio_wide_kernel<decltype(lpl)::value>, true); });
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -1291,32 +1341,15 @@ int sfb200_ppo_loss_fwd_bwd_tuple(const float* logits, const float* values, int 
     SFB_CHECK_ARG(exploration_loss == 0 || exploration_loss == 1, "ppo_loss_fwd_bwd_tuple: exploration_loss must be 0 or 1");
     Segs sg;
     if (int rc = make_segs(sg, A, num_heads, head_sizes_host)) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    const float clip_hi = 1.0f + clip_ratio;
-    const float clip_lo = 1.0f / clip_hi;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    double* part = (double*)workspace;
-#define SFB_PT(AM)                                                                                                       \
-    ppo_loss_tuple_kernel<AM><<<g, 256, 0, st>>>(logits, values, A, sg, actions_f32, log_prob_old, values_old, adv,       \
-                                                 targets, valids, logits_old, batch, clip_lo, clip_hi, clip_value,        \
-                                                 exploration_coeff, exploration_loss, value_coeff, kl_coeff, grad_scale,  \
-                                                 dlogits, dvalues, stats, part)
-#define SFB_PTW(LPL)                                                                                                     \
-    ppo_loss_tuple_wide_kernel<LPL><<<g, 256, 0, st>>>(logits, values, A, sg, actions_f32, log_prob_old, values_old, adv, \
-                                                       targets, valids, logits_old, batch, clip_lo, clip_hi, clip_value,  \
-                                                       exploration_coeff, exploration_loss, value_coeff, kl_coeff,        \
-                                                       grad_scale, dlogits, dvalues, stats, part)
-    if (A <= 8) SFB_PT(8);
-    else if (A <= 16) SFB_PT(16);
-    else if (A <= 32) SFB_PT(32);
-    else { SFB_WIDE_LPL(A, SFB_PTW); }
-#undef SFB_PTW
-#undef SFB_PT
-    SFB_LAUNCH_OK();
-    ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff,
-                                                stats);
-    SFB_LAUNCH_OK();
-    return 0;
+    const LossLaunch L = loss_launch(batch, clip_ratio, workspace, stream);
+    auto launch = [&](auto kernel) {
+        kernel<<<L.grid, 256, 0, L.st>>>(logits, values, A, sg, actions_f32, log_prob_old, values_old, adv, targets, valids,
+                                         logits_old, batch, L.clip_lo, L.clip_hi, clip_value, exploration_coeff,
+                                         exploration_loss, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, stats, L.part);
+    };
+    with_width(A, [&](auto am) { launch(ppo_loss_tuple_kernel<decltype(am)::value>); },
+               [&](auto lpl) { launch(ppo_loss_tuple_wide_kernel<decltype(lpl)::value>); });
+    return loss_finalize(L, batch, exploration_coeff, exploration_loss, value_coeff, kl_coeff, stats);
 }
 
 int sfb200_action_ratio_continuous(const float* params, int act_dim, const float* actions_f32, const float* log_prob_old,
@@ -1326,16 +1359,11 @@ int sfb200_action_ratio_continuous(const float* params, int act_dim, const float
                   kWideMax, act_dim);
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    if (act_dim <= 8) action_ratio_gauss_kernel<8><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
-    else if (act_dim <= 16) action_ratio_gauss_kernel<16><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
-    else if (act_dim <= 32) action_ratio_gauss_kernel<32><<<g, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
-    else {
-        const unsigned gw = (unsigned)ceil_div(batch, 8);
-#define SFB_ARGW(LPL) action_ratio_gauss_wide_kernel<LPL><<<gw, 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio)
-        SFB_WIDE_LPL(act_dim, SFB_ARGW);
-#undef SFB_ARGW
-    }
+    auto launch = [&](auto kernel, bool wide) {
+        kernel<<<ratio_grid(batch, wide), 256, 0, st>>>(params, act_dim, actions_f32, log_prob_old, batch, ratio);
+    };
+    with_width(act_dim, [&](auto ah) { launch(action_ratio_gauss_kernel<decltype(ah)::value>, false); },
+               [&](auto lpl) { launch(action_ratio_gauss_wide_kernel<decltype(lpl)::value>, true); });
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -1352,37 +1380,17 @@ int sfb200_ppo_loss_fwd_bwd_continuous(const float* params, const float* values,
     SFB_CHECK_ARG(act_dim >= 1 && act_dim <= kWideMax, "ppo_loss_fwd_bwd_continuous: supports 1 <= act_dim <= %d, got %d",
                   kWideMax, act_dim);
     SFB_CHECK_ARG(adaptive_stddev || dlogstd, "ppo_loss_fwd_bwd_continuous: dlogstd is required when adaptive_stddev=0");
-    cudaStream_t st = (cudaStream_t)stream;
-    const float clip_hi = 1.0f + clip_ratio;
-    const float clip_lo = 1.0f / clip_hi;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    double* part = (double*)workspace;
-#define SFB_PG(AHV)                                                                                                      \
-    ppo_loss_gauss_kernel<AHV><<<g, 256, 0, st>>>(params, values, act_dim, adaptive_stddev, tanh_scale, actions_f32,      \
-                                                  log_prob_old, values_old, adv, targets, valids, params_old, batch,      \
-                                                  clip_lo, clip_hi, clip_value, exploration_coeff, value_coeff, kl_coeff, \
-                                                  grad_scale, dlogits, dlogstd, dvalues, stats, part)
-#define SFB_PGW(LPL)                                                                                                    \
-    ppo_loss_gauss_wide_kernel<LPL><<<g, 256, 0, st>>>(params, values, act_dim, adaptive_stddev, tanh_scale, actions_f32, \
-                                                       log_prob_old, values_old, adv, targets, valids, params_old, batch, \
-                                                       clip_lo, clip_hi, clip_value, exploration_coeff, value_coeff,     \
-                                                       kl_coeff, grad_scale, dlogits, dlogstd, dvalues, stats, part)
-    if (act_dim <= 8) SFB_PG(8);
-    else if (act_dim <= 16) SFB_PG(16);
-    else if (act_dim <= 32) SFB_PG(32);
-    else { SFB_WIDE_LPL(act_dim, SFB_PGW); }
-#undef SFB_PGW
-#undef SFB_PG
-    SFB_LAUNCH_OK();
-    ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);
-    SFB_LAUNCH_OK();
-    return 0;
+    const LossLaunch L = loss_launch(batch, clip_ratio, workspace, stream);
+    auto launch = [&](auto kernel) {
+        kernel<<<L.grid, 256, 0, L.st>>>(params, values, act_dim, adaptive_stddev, tanh_scale, actions_f32, log_prob_old,
+                                         values_old, adv, targets, valids, params_old, batch, L.clip_lo, L.clip_hi,
+                                         clip_value, exploration_coeff, value_coeff, kl_coeff, grad_scale, dlogits, dlogstd,
+                                         dvalues, stats, L.part);
+    };
+    with_width(act_dim, [&](auto ah) { launch(ppo_loss_gauss_kernel<decltype(ah)::value>); },
+               [&](auto lpl) { launch(ppo_loss_gauss_wide_kernel<decltype(lpl)::value>); });
+    return loss_finalize(L, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);
 }
-
-// LPL for a mixed row of A params (one warp per sample at every width)
-#define SFB_MIXED_LPL(A, LAUNCH)         \
-    if ((A) <= 32) LAUNCH(1);            \
-    else { SFB_WIDE_LPL(A, LAUNCH); }
 
 int sfb200_action_ratio_mixed(const float* params, int A, int num_heads, const int32_t* head_kinds_host,
                               const int32_t* head_sizes_host, const float* actions_f32, const float* log_prob_old,
@@ -1392,10 +1400,10 @@ int sfb200_action_ratio_mixed(const float* params, int A, int num_heads, const i
     if (int rc = make_mixed_layout(ml, A, num_heads, head_kinds_host, head_sizes_host, "action_ratio_mixed")) return rc;
     if (batch == 0) return 0;
     cudaStream_t st = (cudaStream_t)stream;
-    const unsigned gw = (unsigned)ceil_div(batch, 8);
-#define SFB_ARM(LPL) action_ratio_mixed_kernel<LPL><<<gw, 256, 0, st>>>(params, ml, actions_f32, log_prob_old, batch, ratio)
-    SFB_MIXED_LPL(A, SFB_ARM);
-#undef SFB_ARM
+    with_mixed_lpl(A, [&](auto lpl) {
+        action_ratio_mixed_kernel<decltype(lpl)::value><<<ratio_grid(batch, true), 256, 0, st>>>(params, ml, actions_f32,
+                                                                                                 log_prob_old, batch, ratio);
+    });
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -1411,23 +1419,13 @@ int sfb200_ppo_loss_fwd_bwd_mixed(const float* params, const float* values, int 
                       dvalues && stats && workspace && batch > 0, "ppo_loss_fwd_bwd_mixed: bad arguments");
     MixedLayout ml;
     if (int rc = make_mixed_layout(ml, A, num_heads, head_kinds_host, head_sizes_host, "ppo_loss_fwd_bwd_mixed")) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    const float clip_hi = 1.0f + clip_ratio;
-    const float clip_lo = 1.0f / clip_hi;
-    const unsigned g = (unsigned)ceil_div(batch, 256);
-    double* part = (double*)workspace;
-#define SFB_PM(LPL)                                                                                                     \
-    ppo_loss_mixed_kernel<LPL><<<g, 256, 0, st>>>(params, values, ml, actions_f32, log_prob_old, values_old, adv, targets, \
-                                                  valids, params_old, batch, clip_lo, clip_hi, clip_value,               \
-                                                  exploration_coeff, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, \
-                                                  stats, part)
-    SFB_MIXED_LPL(A, SFB_PM);
-#undef SFB_PM
-    SFB_LAUNCH_OK();
-    ppo_loss_finalize_kernel<<<1, 256, 0, st>>>(part, (int)g, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);
-    SFB_LAUNCH_OK();
-    return 0;
+    const LossLaunch L = loss_launch(batch, clip_ratio, workspace, stream);
+    with_mixed_lpl(A, [&](auto lpl) {
+        ppo_loss_mixed_kernel<decltype(lpl)::value><<<L.grid, 256, 0, L.st>>>(
+            params, values, ml, actions_f32, log_prob_old, values_old, adv, targets, valids, params_old, batch, L.clip_lo,
+            L.clip_hi, clip_value, exploration_coeff, value_coeff, kl_coeff, grad_scale, dlogits, dvalues, stats, L.part);
+    });
+    return loss_finalize(L, batch, exploration_coeff, 0, value_coeff, kl_coeff, stats);
 }
-#undef SFB_MIXED_LPL
 
 }  // extern "C"
