@@ -493,16 +493,60 @@ static thread_local const uint8_t* g_action_mask = nullptr;
 static thread_local int64_t g_mask_stride = 0;
 static thread_local int g_deterministic = 0;
 
-int apply_sampling_mode(HeadsOut& out, int A) {
+int make_heads_layout(HeadsOut& out, int space, int A, int num_heads, const int32_t* kinds, const int32_t* sizes,
+                      int act_dim, int adaptive_stddev, const float* learned_log_std, float tanh_scale, void* env_actions,
+                      void* const* env_members, const char* who) {
+    ActionLayout& L = out.lay;
+    L = ActionLayout{};
+    MixedLayout& m = L.m;
+    if (space == 3) {
+        if (int rc = make_mixed_layout(m, A, num_heads, kinds, sizes, who)) return rc;
+        SFB_CHECK_ARG(out.values && out.logits && out.actions_f32, "%s: values, params and actions are required", who);
+        for (int k = 0; k < num_heads; ++k) {
+            L.env[k] = env_members ? env_members[k] : nullptr;
+            L.env_stride[k] = m.kind[k] == kMixedCategorical ? 1 : m.size[k];
+        }
+    } else if (space == 1) {
+        SFB_CHECK_ARG(num_heads >= 1 && num_heads <= kMixedMaxHeads && sizes, "%s (tuple): 1 <= number of heads <= 8", who);
+        int tot = 0;
+        for (int k = 0; k < num_heads; ++k) {
+            SFB_CHECK_ARG(sizes[k] >= 1, "%s (tuple): empty head", who);
+            m.kind[k] = kMixedCategorical;
+            m.size[k] = sizes[k];
+            m.pofs[k] = m.nofs[k] = tot;
+            m.aofs[k] = k;
+            L.env[k] = env_actions ? static_cast<int32_t*>(env_actions) + k : nullptr;
+            L.env_stride[k] = num_heads;
+            tot += sizes[k];
+        }
+        SFB_CHECK_ARG(tot == A, "%s (tuple): the heads' sizes sum to %d but distribution_linear has %d rows", who, tot, A);
+        m.K = num_heads;
+        m.A = m.Wn = A;
+        m.W = num_heads;
+    } else {   // one member covering the row
+        const bool box = space == 2;
+        if (box)
+            SFB_CHECK_ARG(adaptive_stddev || learned_log_std, "%s: learned_log_std is required when adaptive_stddev=0", who);
+        m.K = 1;
+        m.kind[0] = !box ? kMixedCategorical : (adaptive_stddev ? kMixedGaussian : kMixedGaussianLearned);
+        m.size[0] = box ? act_dim : A;
+        m.A = A;
+        m.W = box ? act_dim : 1;
+        m.Wn = m.size[0];
+        L.env[0] = env_actions;
+        L.env_stride[0] = box ? act_dim : 1;
+        L.learned_log_std = learned_log_std;
+        L.tanh_scale = tanh_scale;
+    }
     if (out.actions_f32 == nullptr) return 0;     // values / distribution parameters only: nothing is sampled
-    out.deterministic = g_deterministic;
+    L.deterministic = g_deterministic;
     if (g_action_mask) {
-        SFB_CHECK_ARG(out.dist == 0 && out.num_seg <= 1,
+        SFB_CHECK_ARG(space == 0 || (space == 1 && num_heads == 1),
                       "action masks are supported for a plain Discrete action space only (the reference indexes a Tuple's "
                       "mask by head along the batch axis, action_distributions.py:224)");
         SFB_CHECK_ARG(g_mask_stride >= A, "action mask: row stride %lld < %d actions", (long long)g_mask_stride, A);
-        out.action_mask = g_action_mask;
-        out.mask_stride = g_mask_stride;
+        L.action_mask = g_action_mask;
+        L.mask_stride = g_mask_stride;
     }
     return 0;
 }
@@ -526,10 +570,8 @@ static int launch_heads_forward(const float* h, int64_t ldh, int64_t rows, int H
 
 // A = rows of distribution_linear (n for Discrete(n); 2*act_dim or act_dim for a Box action space)
 static int heads_forward_impl(const float* h, int64_t ldh, int64_t rows, int H, int A, const float* Wv, const float* bv,
-                              const float* Wa, const float* ba, const HeadsOut& out_in, const float* noise, uint64_t seed,
+                              const float* Wa, const float* ba, const HeadsOut& out, const float* noise, uint64_t seed,
                               uint64_t offset, const int64_t* offset_dev, const float* pv_scalar, cudaStream_t st) {
-    HeadsOut out = out_in;
-    if (int rc = apply_sampling_mode(out, A)) return rc;
     SFB_CHECK_ARG(h && Wv && bv && Wa && ba && out.values && rows >= 0 && H > 0, "heads_forward: bad arguments");
     SFB_CHECK_ARG(A >= 1 && A <= 31, "heads_forward: supports 1 <= distribution_linear rows <= 31, got %d", A);
     SFB_CHECK_ARG((size_t)(A + 1) * H * sizeof(float) <= 200 * 1024, "heads_forward: (A+1)*H too large for smem");
@@ -554,17 +596,15 @@ static int heads_forward_impl(const float* h, int64_t ldh, int64_t rows, int H, 
 }
 
 static int heads_from_partials_impl(const float* head_partials, int P, int64_t rows, int A, const float* bv,
-                                    const float* ba, const HeadsOut& out_in, const float* noise, uint64_t seed,
+                                    const float* ba, const HeadsOut& out, const float* noise, uint64_t seed,
                                     uint64_t offset, const int64_t* offset_dev, const float* pv_scalar, cudaStream_t st) {
-    HeadsOut out = out_in;
-    if (int rc = apply_sampling_mode(out, A)) return rc;
     SFB_CHECK_ARG(head_partials && bv && ba && out.values && rows >= 0 && P >= 1, "heads_from_partials: bad arguments");
     SFB_CHECK_ARG(A >= 1 && A + 1 <= kHeadPartPad, "heads_from_partials: supports 1 <= A <= %d, got %d", kHeadPartPad - 1, A);
     if (rows == 0) return 0;
     int64_t blocks = ceil_div(rows, 8);
     const int64_t cap = (int64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
-    const HeadsFinish fin{out, bv, ba, noise, seed, offset, offset_dev, pv_scalar, A};
+    const HeadsFinish fin{out, bv, ba, noise, seed, offset, offset_dev, pv_scalar};
     SFB_CUDA_OK(launch_pdl(heads_from_partials_kernel, dim3((unsigned)blocks), dim3(256), 0, st, head_partials, P, rows, fin));
     SFB_LAUNCH_OK();
     return 0;
@@ -691,17 +731,13 @@ __global__ void __launch_bounds__(256) sampler_tail_tape_kernel(const float* __r
     }
 }
 
-static int make_gaussian_out(HeadsOut& out, int act_dim, int adaptive_stddev, const float* learned_log_std,
-                             float tanh_scale, float* values, int64_t values_stride, float* params,
-                             int64_t params_stride, float* actions_f32, int64_t actions_stride, float* env_actions_f32,
-                             float* log_prob, int64_t log_prob_stride, float* pv_out, int64_t pv_stride) {
-    SFB_CHECK_ARG(act_dim >= 1 && (adaptive_stddev ? 2 * act_dim : act_dim) <= 31,
-                  "heads (continuous): act_dim %d needs more than 31 distribution_linear rows", act_dim);
-    SFB_CHECK_ARG(adaptive_stddev || learned_log_std, "heads (continuous): learned_log_std is required when adaptive_stddev=0");
-    out = HeadsOut{values, values_stride, params, params_stride, actions_f32, actions_stride, nullptr, log_prob,
-                   log_prob_stride, pv_out, pv_stride, adaptive_stddev ? 1 : 2, act_dim, learned_log_std, tanh_scale,
-                   env_actions_f32};
-    return 0;
+// a Box action space on the heads of up to 31 distribution_linear rows
+static int make_narrow_box(HeadsOut& out, int act_dim, int adaptive_stddev, const float* learned_log_std, float tanh_scale,
+                           void* env_actions_f32) {
+    const int A = adaptive_stddev ? 2 * act_dim : act_dim;
+    SFB_CHECK_ARG(act_dim >= 1 && A <= 31, "heads (continuous): act_dim %d needs more than 31 distribution_linear rows", act_dim);
+    return make_heads_layout(out, 2, A, 0, nullptr, nullptr, act_dim, adaptive_stddev, learned_log_std, tanh_scale,
+                             env_actions_f32, nullptr, "heads (continuous)");
 }
 
 }  // namespace sfb
@@ -724,8 +760,10 @@ int sfb200_heads_forward(const float* h, int64_t ldh, int64_t rows, int H, int A
                          const int64_t* philox_offset_dev, float* actions_f32, int64_t actions_stride, int32_t* env_actions_i32, float* log_prob,
                          int64_t log_prob_stride, const float* policy_version_scalar, float* policy_version_out,
                          int64_t pv_stride, void* stream) {
-    const HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, env_actions_i32,
-                       log_prob, log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
+    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_heads_layout(out, 0, A, 0, nullptr, nullptr, 0, 0, nullptr, 0.f, env_actions_i32, nullptr, "heads"))
+        return rc;
     return heads_forward_impl(h, ldh, rows, H, A, Wv, bv, Wa, ba, out, noise, philox_seed, philox_offset,
                               philox_offset_dev, policy_version_scalar, (cudaStream_t)stream);
 }
@@ -737,8 +775,10 @@ int sfb200_heads_from_partials(const float* head_partials, int P, int64_t rows, 
                                int32_t* env_actions_i32, float* log_prob, int64_t log_prob_stride,
                                const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
                                void* stream) {
-    const HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, env_actions_i32,
-                       log_prob, log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
+    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_heads_layout(out, 0, A, 0, nullptr, nullptr, 0, 0, nullptr, 0.f, env_actions_i32, nullptr, "heads"))
+        return rc;
     return heads_from_partials_impl(head_partials, P, rows, A, bv, ba, out, noise, philox_seed, philox_offset,
                                     philox_offset_dev, policy_version_scalar, (cudaStream_t)stream);
 }
@@ -758,9 +798,10 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
                                   const float* rnn, int rnn_dim, float* traj_rnn_next, int64_t traj_rnn_stride, float* x_norm,
                                   const double* mean, const double* var, float sub_mean, float inv_scale, float eps,
                                   float clip, void* stream) {
-    HeadsOut out{values_t, values_stride, logits_t, logits_stride, actions_t, actions_stride, env_actions,
-                 log_prob_t, log_prob_stride, policy_version_t, pv_stride, 0, 0, nullptr, 0.f, nullptr};
-    if (int rc = apply_sampling_mode(out, A)) return rc;
+    HeadsOut out{values_t, values_stride, logits_t, logits_stride, actions_t, actions_stride, log_prob_t, log_prob_stride,
+                 policy_version_t, pv_stride};
+    if (int rc = make_heads_layout(out, 0, A, 0, nullptr, nullptr, 0, 0, nullptr, 0.f, env_actions, nullptr, "heads"))
+        return rc;
     SFB_CHECK_ARG(head_partials && bv && ba && values_t && actions_t && env_actions && n_envs >= 0 && P >= 1 && A >= 1 &&
                       A + 1 <= kHeadPartPad, "sampler_tail_tape_step: bad heads arguments");
     SFB_CHECK_ARG(tape && tape_len > 0 && dim > 0 && term_period > 0 && trunc_period > 0 && env_step_counter && env_obs &&
@@ -778,7 +819,7 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
                          len_increment, stats, sampler_step, fin_return_t, fin_len_t, traj_obs_next, traj_obs_stride, x_norm,
                          mean, var, sub_mean, inv_scale, fabsf(sub_mean) > 1e-8f ? 1 : 0, fabsf(inv_scale - 1.0f) > 1e-8f ? 1 : 0,
                          eps, clip, with_rnn ? rnn : nullptr, rnn_dim, traj_rnn_next, traj_rnn_stride};
-    const HeadsFinish fin{out, bv, ba, noise, philox_seed, 0ull, sampler_step, policy_version_scalar, A};
+    const HeadsFinish fin{out, bv, ba, noise, philox_seed, 0ull, sampler_step, policy_version_scalar};
     int64_t blocks = ceil_div(n_envs, 8);
     const int64_t cap = (int64_t)sm_count() * 8;
     if (blocks > cap) blocks = cap;
@@ -786,19 +827,6 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
     SFB_CUDA_OK(launch_pdl(sampler_tail_tape_kernel, dim3((unsigned)blocks), dim3(256), (size_t)(2 * dim * sizeof(float)),
                            (cudaStream_t)stream, head_partials, P, n_envs, fin, a));
     SFB_LAUNCH_OK();
-    return 0;
-}
-
-static int make_tuple_out(HeadsOut& out, int A, int num_seg, const int32_t* seg_lens) {
-    SFB_CHECK_ARG(num_seg >= 1 && num_seg <= 8 && seg_lens, "heads (tuple): 1 <= number of heads <= 8");
-    int tot = 0;
-    for (int k = 0; k < num_seg; ++k) {
-        SFB_CHECK_ARG(seg_lens[k] >= 1, "heads (tuple): empty head");
-        out.seg_len[k] = seg_lens[k];
-        tot += seg_lens[k];
-    }
-    SFB_CHECK_ARG(tot == A, "heads (tuple): the heads' sizes sum to %d but distribution_linear has %d rows", tot, A);
-    out.num_seg = num_seg;
     return 0;
 }
 
@@ -810,9 +838,11 @@ int sfb200_heads_forward_tuple(const float* h, int64_t ldh, int64_t rows, int H,
                                int32_t* env_actions_i32, float* log_prob, int64_t log_prob_stride,
                                const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
                                void* stream) {
-    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, env_actions_i32,
-                 log_prob, log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
-    if (int rc = make_tuple_out(out, A, num_heads, head_sizes_host)) return rc;
+    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_heads_layout(out, 1, A, num_heads, nullptr, head_sizes_host, 0, 0, nullptr, 0.f, env_actions_i32,
+                                   nullptr, "heads"))
+        return rc;
     return heads_forward_impl(h, ldh, rows, H, A, Wv, bv, Wa, ba, out, noise, philox_seed, philox_offset,
                               philox_offset_dev, policy_version_scalar, (cudaStream_t)stream);
 }
@@ -824,9 +854,11 @@ int sfb200_heads_from_partials_tuple(const float* head_partials, int P, int64_t 
                                      float* actions_f32, int64_t actions_stride, int32_t* env_actions_i32,
                                      float* log_prob, int64_t log_prob_stride, const float* policy_version_scalar,
                                      float* policy_version_out, int64_t pv_stride, void* stream) {
-    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, env_actions_i32,
-                 log_prob, log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
-    if (int rc = make_tuple_out(out, A, num_heads, head_sizes_host)) return rc;
+    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_heads_layout(out, 1, A, num_heads, nullptr, head_sizes_host, 0, 0, nullptr, 0.f, env_actions_i32,
+                                   nullptr, "heads"))
+        return rc;
     return heads_from_partials_impl(head_partials, P, rows, A, bv, ba, out, noise, philox_seed, philox_offset,
                                     philox_offset_dev, policy_version_scalar, (cudaStream_t)stream);
 }
@@ -844,21 +876,16 @@ int sfb200_linear_act_heads_forward_fused(
                   "linear_act_heads_forward_fused: bad arguments");
     SFB_CHECK_ARG(dist_kind >= 0 && dist_kind <= 2, "linear_act_heads_forward_fused: dist_kind 0 categorical, 1 tuple, 2 Gaussian");
     if (M == 0) return 0;
-    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, nullptr, log_prob,
-                 log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
+    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
     if (dist_kind == 2) {
-        if (int rc = make_gaussian_out(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, values, values_stride, logits,
-                                       logits_stride, actions_f32, actions_stride, (float*)env_actions, log_prob,
-                                       log_prob_stride, policy_version_out, pv_stride))
-            return rc;
+        if (int rc = make_narrow_box(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, env_actions)) return rc;
         SFB_CHECK_ARG(A == (adaptive_stddev ? 2 * act_dim : act_dim), "linear_act_heads_forward_fused: A does not match act_dim");
-    } else {
-        out.env_actions = (int32_t*)env_actions;
-        if (dist_kind == 1)
-            if (int rc = make_tuple_out(out, A, num_heads, head_sizes_host)) return rc;
+    } else if (int rc = make_heads_layout(out, dist_kind, A, num_heads, nullptr, head_sizes_host, 0, 0, nullptr, 0.f,
+                                          env_actions, nullptr, "heads")) {
+        return rc;
     }
-    if (int rc = apply_sampling_mode(out, A)) return rc;
-    const HeadsFinish fin{out, bv, ba, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar, A};
+    const HeadsFinish fin{out, bv, ba, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar};
     int rc = tc_linear_act_heads_forward(x, ldx, W, b, y, ldy, M, N, K, act, engine, Wv, Wa, A, head_partials,
                                          (cudaStream_t)stream, &fin, finish_counters);
     SFB_CHECK_ARG(rc != SFB_TC_UNSUPPORTED,
@@ -875,11 +902,9 @@ int sfb200_heads_forward_continuous(const float* h, int64_t ldh, int64_t rows, i
                                     float* actions_f32, int64_t actions_stride, float* env_actions_f32, float* log_prob,
                                     int64_t log_prob_stride, const float* policy_version_scalar,
                                     float* policy_version_out, int64_t pv_stride, void* stream) {
-    HeadsOut out;
-    if (int rc = make_gaussian_out(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, values, values_stride, params,
-                                   params_stride, actions_f32, actions_stride, env_actions_f32, log_prob, log_prob_stride,
-                                   policy_version_out, pv_stride))
-        return rc;
+    HeadsOut out{values, values_stride, params, params_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_narrow_box(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, env_actions_f32)) return rc;
     return heads_forward_impl(h, ldh, rows, H, adaptive_stddev ? 2 * act_dim : act_dim, Wv, bv, Wa, ba, out, noise,
                               philox_seed, philox_offset, philox_offset_dev, policy_version_scalar, (cudaStream_t)stream);
 }
@@ -893,11 +918,9 @@ int sfb200_heads_from_partials_continuous(const float* head_partials, int P, int
                                           float* env_actions_f32, float* log_prob, int64_t log_prob_stride,
                                           const float* policy_version_scalar, float* policy_version_out,
                                           int64_t pv_stride, void* stream) {
-    HeadsOut out;
-    if (int rc = make_gaussian_out(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, values, values_stride, params,
-                                   params_stride, actions_f32, actions_stride, env_actions_f32, log_prob, log_prob_stride,
-                                   policy_version_out, pv_stride))
-        return rc;
+    HeadsOut out{values, values_stride, params, params_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                 policy_version_out, pv_stride};
+    if (int rc = make_narrow_box(out, act_dim, adaptive_stddev, learned_log_std, tanh_scale, env_actions_f32)) return rc;
     return heads_from_partials_impl(head_partials, P, rows, adaptive_stddev ? 2 * act_dim : act_dim, bv, ba, out, noise,
                                     philox_seed, philox_offset, philox_offset_dev, policy_version_scalar,
                                     (cudaStream_t)stream);

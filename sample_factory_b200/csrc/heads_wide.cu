@@ -1,266 +1,81 @@
-// Heads of models whose distribution_linear has more than 31 rows (ModelSpec.wide_heads): the logits are a GEMM on the
-// regular engine (sfb200_linear_act_forward, bias included) written straight into their final place, so what is left
-// here is the value head, the distribution tail over the stored logits, and the parts of the backward the two
-// linear_backward GEMMs do not cover.  Same semantics as heads_row_tail / tuple_row_tail / gaussian_row_tail
-// (heads_tail.cuh), for up to kWideMaxRows logits per row.
+// Heads over stored params rows.  Models whose distribution_linear has more than 31 rows (ModelSpec.wide_heads): the
+// logits are a GEMM on the regular engine (sfb200_linear_act_forward, bias included) written straight into their final
+// place, so what is left here is the value head, the distribution tail over the stored logits, and the parts of the
+// backward the two linear_backward GEMMs do not cover.  A Tuple space with Box members (mixed_layout.cuh): its params
+// rows come from the regular heads kernels run in values / logits-only mode (up to 31 rows: fused partials or
+// heads_forward) or from the distribution_linear GEMM (wider rows), and the tail runs over the stored rows at every width.
+#include <type_traits>
+
 #include "heads_tail.cuh"
 
 namespace sfb {
 
 constexpr int kWideMaxRows = 1024;
 
-// One warp per row, LPL slots per lane.  Slot q = k*32 + lane holds element (q - 1) mod 32*LPL: up to 31 elements sit
-// on the lanes the narrow tail puts them on (lane a+1 = element a), so every warp reduction below adds the same terms
-// in the same order as heads_row_tail (the empty slots contribute exact zeros / -inf); a row of exactly 32*LPL
-// elements puts the last one in slot 0.
-template <int LPL>
-__device__ __forceinline__ int wide_elem(int k, int lane) {
-    const int q = k * 32 + lane;
-    return q == 0 ? 32 * LPL - 1 : q - 1;
-}
-// the lane / slot holding element a
-template <int LPL>
-__device__ __forceinline__ float wide_pick(const float (&v)[LPL], int a, int lane) {
-    const int q = (a + 1) & (32 * LPL - 1);
-    float mine = 0.f;
-#pragma unroll
-    for (int k = 0; k < LPL; ++k)
-        if (k == (q >> 5)) mine = v[k];
-    return __shfl_sync(0xffffffffu, mine, q & 31);
-}
-
-struct WideTail {
-    const float* h; int64_t ldh; int H; const float* Wv; const float* bv;   // value head input
-    float* lg; int64_t ldl;      // logits / [means | log_std] rows, read (and, for a learned stddev, completed) in place
-    int A;                       // rows of distribution_linear
-    const float* noise; uint64_t seed, offset_host; const int64_t* offset_dev; const float* pv_scalar;
-};
-
-// CategoricalActionDistribution with the optional mask (heads_row_tail)
-template <int LPL>
-__device__ __forceinline__ void wide_categorical(int lane, int64_t row, const WideTail& w, const HeadsOut& out,
-                                                 uint64_t offset, float pv) {
-    const int A = w.A;
-    const float* lr = w.lg + row * w.ldl;
-    const bool masked = out.action_mask != nullptr;
-    float x[LPL], e[LPL];
-    bool ok[LPL];
-    float mloc = -INFINITY;
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        const int a = wide_elem<LPL>(k, lane);
-        const bool is_logit = a < A;
-        const bool allowed = is_logit && (!masked || out.action_mask[row * out.mask_stride + a] != 0);
-        float v = is_logit ? lr[a] : -INFINITY;
-        if (masked && is_logit && !allowed) v = __fadd_rn(v, -1.0e9f);   // masked_softmax :84-95
-        x[k] = v;
-        ok[k] = allowed;
-        mloc = fmaxf(mloc, v);
-    }
-    const float m = warp_max(mloc);
-    float sl = 0.f;
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        e[k] = (wide_elem<LPL>(k, lane) < A) ? expf(x[k] - m) : 0.f;
-        sl += e[k];
-    }
-    const float s = warp_sum(sl);
-    const float logs = logf(s);
-    float p[LPL];
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) p[k] = __fdiv_rn(e[k], s);                 // softmax :116
-    if (masked) {
-        float ps = 0.f;
-#pragma unroll
-        for (int k = 0; k < LPL; ++k) {
-            p[k] = __fmul_rn(p[k], ok[k] ? 1.f : 0.f);                         // :88
-            ps += p[k];
-        }
-        const float den = __fadd_rn(warp_sum(ps), 1.0e-13f);                   // :89
-        bool any = false;
-#pragma unroll
-        for (int k = 0; k < LPL; ++k) {
-            p[k] = __fdiv_rn(p[k], den);
-            any |= p[k] > 0.f;
-        }
-        if (__ballot_sync(0xffffffffu, any) == 0u)                             // :137-140 nothing allowed: uniform
-#pragma unroll
-            for (int k = 0; k < LPL; ++k) p[k] = 1.0e-6f;
-    }
-    float best = -INFINITY;
-    int idx = 0x7fffffff;
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        const int a = wide_elem<LPL>(k, lane);
-        if (a >= A) continue;
-        float q = 1.f;
-        if (!out.deterministic) {
-            if (w.noise) q = w.noise[row * A + a];
-            else {
-                curandStatePhilox4_32_10_t st;
-                curand_init(w.seed, (unsigned long long)(row * A + a), offset, &st);
-                q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);              // Exp(1); uniform is in (0, 1]
-            }
-        }
-        const float r = __fdiv_rn(p[k], q);
-        if (r > best || (r == best && a < idx)) { best = r; idx = a; }
-    }
-    argmax_first(best, idx);
-    float logp[LPL];
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) logp[k] = (x[k] - m) - logs;                 // log_softmax :125
-    const float lp = wide_pick<LPL>(logp, idx, lane);                           // log_prob :145-148
-    if (lane == 0) {
-        out.actions_f32[row * out.actions_stride] = (float)idx;
-        if (out.env_actions) out.env_actions[row] = idx;
-        if (out.log_prob) out.log_prob[row * out.log_prob_stride] = lp;
-        if (out.pv_out) out.pv_out[row * out.pv_stride] = pv;
-    }
-}
-
-// TupleActionDistribution (tuple_row_tail): the categorical recipe per head over its own logit segment
-template <int LPL>
-__device__ __forceinline__ void wide_tuple(int lane, int64_t row, const WideTail& w, const HeadsOut& out, uint64_t offset,
-                                           float pv) {
-    const int A = w.A;
-    const float* lr = w.lg + row * w.ldl;
-    float x[LPL], q[LPL];
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        const int a = wide_elem<LPL>(k, lane);
-        x[k] = a < A ? lr[a] : 0.f;
-        q[k] = 1.f;
-        if (a < A && !out.deterministic) {
-            if (w.noise) q[k] = w.noise[row * A + a];
-            else {
-                curandStatePhilox4_32_10_t st;
-                curand_init(w.seed, (unsigned long long)(row * A + a), offset, &st);
-                q[k] = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);
-            }
-        }
-    }
-    float lp_total = 0.f;
-    int start = 0;
-    const int K = out.num_seg;
-    for (int s = 0; s < K; ++s) {
-        const int n = out.seg_len[s];
-        float mloc = -INFINITY;
-#pragma unroll
-        for (int k = 0; k < LPL; ++k) {
-            const int a = wide_elem<LPL>(k, lane);
-            if (a >= start && a < start + n) mloc = fmaxf(mloc, x[k]);
-        }
-        const float m = warp_max(mloc);
-        float e[LPL], sl = 0.f;
-#pragma unroll
-        for (int k = 0; k < LPL; ++k) {
-            const int a = wide_elem<LPL>(k, lane);
-            e[k] = (a >= start && a < start + n) ? expf(x[k] - m) : 0.f;
-            sl += e[k];
-        }
-        const float sum = warp_sum(sl);
-        const float logs = logf(sum);
-        float best = -INFINITY, logp[LPL];
-        int idx = 0x7fffffff;
-#pragma unroll
-        for (int k = 0; k < LPL; ++k) {
-            const int a = wide_elem<LPL>(k, lane);
-            logp[k] = (x[k] - m) - logs;
-            if (a >= start && a < start + n) {
-                const float r = __fdiv_rn(__fdiv_rn(e[k], sum), q[k]);
-                if (r > best || (r == best && a - start < idx)) { best = r; idx = a - start; }
-            }
-        }
-        argmax_first(best, idx);
-        lp_total += wide_pick<LPL>(logp, start + idx, lane);
-        if (lane == 0) {
-            out.actions_f32[row * out.actions_stride + s] = (float)idx;
-            if (out.env_actions) out.env_actions[row * K + s] = idx;
-        }
-        start += n;
-    }
-    if (lane == 0) {
-        if (out.log_prob) out.log_prob[row * out.log_prob_stride] = lp_total;
-        if (out.pv_out) out.pv_out[row * out.pv_stride] = pv;
-    }
-}
-
-// ContinuousActionDistribution (gaussian_row_tail).  The params row is completed in place: tanh-scaled means and the
-// learned log-stddev vector (adaptive_stddev=False, action_parameterization.py:64-78); an adaptive row is left as the
-// GEMM wrote it.
-template <int LPL>
-__device__ __forceinline__ void wide_gaussian(int lane, int64_t row, const WideTail& w, const HeadsOut& out,
-                                              uint64_t offset, float pv) {
-    const int Ad = out.act_dim;
-    float* lr = w.lg + row * w.ldl;
-    float mean[LPL], lstd[LPL];
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        const int d = wide_elem<LPL>(k, lane);
-        mean[k] = 0.f;
-        lstd[k] = 0.f;
-        if (d < Ad) {
-            mean[k] = lr[d];
-            if (out.dist == 1) lstd[k] = lr[Ad + d];
-            else {
-                lstd[k] = out.learned_log_std[d];
-                if (out.tanh_scale > 0.f) mean[k] = tanhf(__fdiv_rn(mean[k], out.tanh_scale)) * out.tanh_scale;
-                lr[d] = mean[k];
-                lr[Ad + d] = lstd[k];
-            }
-        }
-    }
-    if (out.actions_f32 == nullptr) return;   // distribution parameters only (warp-uniform)
-    float lps = 0.f;
-#pragma unroll
-    for (int k = 0; k < LPL; ++k) {
-        const int d = wide_elem<LPL>(k, lane);
-        if (d >= Ad) continue;
-        const float sd = clampf(expf(lstd[k]), kStddevMin, kStddevMax);
-        float eps = 0.f;
-        if (!out.deterministic) {
-            if (w.noise) eps = w.noise[row * Ad + d];
-            else {
-                curandStatePhilox4_32_10_t st;
-                curand_init(w.seed, (unsigned long long)(row * Ad + d), offset, &st);
-                eps = curand_normal(&st);
-            }
-        }
-        const float a = __fadd_rn(__fmul_rn(eps, sd), mean[k]);   // Normal.sample(): product and sum rounded separately
-        const float dd = a - mean[k];
-        lps += -(dd * dd) / (2.f * (sd * sd)) - logf(sd) - kHalfLog2Pi;
-        out.actions_f32[row * out.actions_stride + d] = a;
-        if (out.env_actions_f32) out.env_actions_f32[row * Ad + d] = a;
-    }
-    const float lp = warp_sum(lps);
-    if (lane == 0) {
-        if (out.log_prob) out.log_prob[row * out.log_prob_stride] = lp;
-        if (out.pv_out) out.pv_out[row * out.pv_stride] = pv;
-    }
-}
-
-template <int LPL>
-__global__ void __launch_bounds__(256) heads_tail_wide_kernel(int64_t rows, const WideTail w, const HeadsOut out) {
+// One warp per stored params row (the logits a distribution_linear GEMM wrote in place, the trajectory's action_logits
+// slot, the learner's minibatch logits or a plan's scratch): the value head when h is given, then row_tail over the row
+// held LPL elements per lane under slot map S.  Without actions, only a learned-stddev row has anything left to do.
+template <int LPL, int S>
+__global__ void __launch_bounds__(256) heads_tail_rows_kernel(int64_t rows, const float* __restrict__ h, int64_t ldh, int H,
+                                                              const float* __restrict__ Wv, const HeadsFinish f) {
     pdl_wait();
     pdl_trigger();
     const int lane = threadIdx.x & 31;
     const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const float pv = w.pv_scalar ? *w.pv_scalar : 0.f;
-    const uint64_t offset = w.offset_host + (w.offset_dev ? (uint64_t)*w.offset_dev : 0ull);
+    const HeadsOut& out = f.out;
+    const float pv = f.pv_scalar ? *f.pv_scalar : 0.f;
+    const uint64_t offset = f.offset_host + (f.offset_dev ? (uint64_t)*f.offset_dev : 0ull);
+    const bool tail = out.logits && (out.actions_f32 || out.lay.m.kind[0] == kMixedGaussianLearned);
     for (int64_t row = warp; row < rows; row += nwarps) {
-        // critic_linear: fixed-order lane partials + butterfly (deterministic)
-        const float* hr = w.h + row * w.ldh;
-        float acc = 0.f;
-        for (int j = lane; j < w.H; j += 32) acc = fmaf(hr[j], w.Wv[j], acc);
-        const float v = warp_sum(acc) + w.bv[0];
-        if (lane == 0) out.values[row * out.values_stride] = v;
-        if (w.lg == nullptr) continue;             // values only (the learner's bootstrap value)
-        if (out.dist != 0) wide_gaussian<LPL>(lane, row, w, out, offset, pv);
-        else if (out.actions_f32 == nullptr) continue;
-        else if (out.num_seg > 1) wide_tuple<LPL>(lane, row, w, out, offset, pv);
-        else wide_categorical<LPL>(lane, row, w, out, offset, pv);
+        if (h) {   // critic_linear: fixed-order lane partials + butterfly (deterministic)
+            const float* hr = h + row * ldh;
+            float acc = 0.f;
+            for (int j = lane; j < H; j += 32) acc = fmaf(hr[j], Wv[j], acc);
+            const float v = warp_sum(acc) + f.bv[0];
+            if (lane == 0) out.values[row * out.values_stride] = v;
+        }
+        if (!tail) continue;
+        const float* lr = out.logits + row * out.logits_stride;
+        float x[LPL];
+#pragma unroll
+        for (int k = 0; k < LPL; ++k) {
+            const int a = slot_elem<LPL, S>(k, lane);
+            x[k] = a < out.lay.m.A ? lr[a] : 0.f;
+        }
+        row_tail<LPL, S>(x, lane, row, out, f.noise, f.seed, offset, pv);
     }
+}
+
+template <int N>
+using Int = std::integral_constant<int, N>;
+
+// A wide Discrete / Tuple / Box row (S = 1, LPL >= 2 by the widest member) bit-matches the narrow heads up to 31
+// elements.  A mixed Tuple takes S = 0 at every width (LPL >= 1 by the row width).
+static int launch_tail_rows(int64_t rows, const float* h, int64_t ldh, int H, const float* Wv, const HeadsFinish& f,
+                            bool mixed, cudaStream_t st) {
+    if (rows == 0) return 0;
+    const MixedLayout& m = f.out.lay.m;
+    const int width = (!mixed && m.kind[0] != kMixedCategorical) ? m.size[0] : m.A;
+    int64_t blocks = ceil_div(rows, 8);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    if (blocks > cap) blocks = cap;
+    auto go = [&](auto lpl, auto s) {
+        return launch_pdl(heads_tail_rows_kernel<decltype(lpl)::value, decltype(s)::value>, dim3((unsigned)blocks), dim3(256),
+                          0, st, rows, h, ldh, H, Wv, f);
+    };
+    auto with_s = [&](auto s) {
+        if constexpr (decltype(s)::value == 0)
+            if (width <= 32) return go(Int<1>{}, s);
+        if (width <= 64) return go(Int<2>{}, s);
+        if (width <= 128) return go(Int<4>{}, s);
+        if (width <= 256) return go(Int<8>{}, s);
+        if (width <= 512) return go(Int<16>{}, s);
+        return go(Int<32>{}, s);
+    };
+    SFB_CUDA_OK(mixed ? with_s(Int<0>{}) : with_s(Int<1>{}));
+    SFB_LAUNCH_OK();
+    return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -352,51 +167,76 @@ int sfb200_heads_tail_wide(const float* h, int64_t ldh, int64_t rows, int H, con
                   kWideMaxRows, A);
     SFB_CHECK_ARG(dist_kind >= 0 && dist_kind <= 2, "heads_tail_wide: dist_kind 0 categorical, 1 tuple, 2 Gaussian");
     SFB_CHECK_ARG(logits || !actions_f32, "heads_tail_wide: sampling needs the logits rows");
-    HeadsOut out{values, values_stride, logits, logits_stride, actions_f32, actions_stride, nullptr, log_prob,
-                 log_prob_stride, policy_version_out, pv_stride, 0, 0, nullptr, 0.f, nullptr};
-    int slots = A;
-    if (dist_kind == 2) {
+    if (dist_kind == 2)
         SFB_CHECK_ARG(act_dim >= 1 && A == (adaptive_stddev ? 2 * act_dim : act_dim),
                       "heads_tail_wide: A = %d does not match act_dim %d", A, act_dim);
-        SFB_CHECK_ARG(adaptive_stddev || learned_log_std, "heads_tail_wide: learned_log_std is required when adaptive_stddev=0");
-        out.dist = adaptive_stddev ? 1 : 2;
-        out.act_dim = act_dim;
-        out.learned_log_std = learned_log_std;
-        out.tanh_scale = tanh_scale;
-        out.env_actions_f32 = (float*)env_actions;
-        slots = act_dim;
-    } else {
-        out.env_actions = (int32_t*)env_actions;
-        if (dist_kind == 1) {
-            SFB_CHECK_ARG(num_heads >= 1 && num_heads <= 8 && head_sizes_host, "heads_tail_wide (tuple): 1 <= number of heads <= 8");
-            int tot = 0;
-            for (int k = 0; k < num_heads; ++k) {
-                SFB_CHECK_ARG(head_sizes_host[k] >= 1, "heads_tail_wide (tuple): empty head");
-                out.seg_len[k] = head_sizes_host[k];
-                tot += head_sizes_host[k];
-            }
-            SFB_CHECK_ARG(tot == A, "heads_tail_wide (tuple): the heads' sizes sum to %d but distribution_linear has %d rows",
-                          tot, A);
-            out.num_seg = num_heads;
-        }
-    }
-    if (int rc = apply_sampling_mode(out, A)) return rc;
-    if (rows == 0) return 0;
-    const WideTail w{h, ldh, H, Wv, bv, logits, logits_stride, A, noise, philox_seed, philox_offset, philox_offset_dev,
-                     policy_version_scalar};
-    int64_t blocks = ceil_div(rows, 8);
-    const int64_t cap = (int64_t)sm_count() * 8;
-    if (blocks > cap) blocks = cap;
-    cudaStream_t st = (cudaStream_t)stream;
-#define SFB_HTW(LPL) SFB_CUDA_OK(launch_pdl(heads_tail_wide_kernel<LPL>, dim3((unsigned)blocks), dim3(256), 0, st, rows, w, out))
-    if (slots <= 64) SFB_HTW(2);
-    else if (slots <= 128) SFB_HTW(4);
-    else if (slots <= 256) SFB_HTW(8);
-    else if (slots <= 512) SFB_HTW(16);
-    else SFB_HTW(32);
-#undef SFB_HTW
-    SFB_LAUNCH_OK();
-    return 0;
+    HeadsFinish f{{values, values_stride, logits, logits_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                   policy_version_out, pv_stride},
+                  bv, nullptr, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar};
+    if (int rc = make_heads_layout(f.out, dist_kind, A, num_heads, nullptr, head_sizes_host, act_dim, adaptive_stddev,
+                                   learned_log_std, tanh_scale, env_actions, nullptr, "heads_tail_wide"))
+        return rc;
+    return launch_tail_rows(rows, h, ldh, H, Wv, f, false, (cudaStream_t)stream);
+}
+
+// The three entry points of a Tuple space with Box members: the tail always runs over the stored params rows
+int sfb200_heads_tail_wide_mixed(const float* h, int64_t ldh, int64_t rows, int H, const float* Wv, const float* bv,
+                                 float* params, int64_t params_stride, int A, int num_heads, const int32_t* head_kinds_host,
+                                 const int32_t* head_sizes_host, float* values, int64_t values_stride, const float* noise,
+                                 uint64_t philox_seed, uint64_t philox_offset, const int64_t* philox_offset_dev,
+                                 float* actions_f32, int64_t actions_stride, void** env_actions_host, float* log_prob,
+                                 int64_t log_prob_stride, const float* policy_version_scalar, float* policy_version_out,
+                                 int64_t pv_stride, void* stream) {
+    SFB_CHECK_ARG(h && Wv && bv && rows >= 0 && H > 0, "heads_tail_wide_mixed: bad arguments");
+    HeadsFinish f{{values, values_stride, params, params_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                   policy_version_out, pv_stride},
+                  bv, nullptr, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar};
+    if (int rc = make_heads_layout(f.out, 3, A, num_heads, head_kinds_host, head_sizes_host, 0, 0, nullptr, 0.f, nullptr,
+                                   env_actions_host, "heads_tail_wide_mixed"))
+        return rc;
+    return launch_tail_rows(rows, h, ldh, H, Wv, f, true, (cudaStream_t)stream);
+}
+
+int sfb200_heads_forward_mixed(const float* h, int64_t ldh, int64_t rows, int H, int A, int num_heads,
+                               const int32_t* head_kinds_host, const int32_t* head_sizes_host, const float* Wv,
+                               const float* bv, const float* Wa, const float* ba, float* values, int64_t values_stride,
+                               float* params, int64_t params_stride, const float* noise, uint64_t philox_seed,
+                               uint64_t philox_offset, const int64_t* philox_offset_dev, float* actions_f32,
+                               int64_t actions_stride, void** env_actions_host, float* log_prob, int64_t log_prob_stride,
+                               const float* policy_version_scalar, float* policy_version_out, int64_t pv_stride,
+                               void* stream) {
+    HeadsFinish f{{values, values_stride, params, params_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                   policy_version_out, pv_stride},
+                  bv, ba, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar};
+    if (int rc = make_heads_layout(f.out, 3, A, num_heads, head_kinds_host, head_sizes_host, 0, 0, nullptr, 0.f, nullptr,
+                                   env_actions_host, "heads_forward_mixed"))
+        return rc;
+    // values and the params rows (nothing is sampled without actions), then the tail over the stored rows
+    if (int rc = sfb200_heads_forward(h, ldh, rows, H, A, Wv, bv, Wa, ba, values, values_stride, params, params_stride,
+                                      nullptr, 0, 0, nullptr, nullptr, 0, nullptr, nullptr, 0, nullptr, nullptr, 0, stream))
+        return rc;
+    return launch_tail_rows(rows, nullptr, 0, 0, nullptr, f, true, (cudaStream_t)stream);
+}
+
+int sfb200_heads_from_partials_mixed(const float* head_partials, int P, int64_t rows, int A, int num_heads,
+                                     const int32_t* head_kinds_host, const int32_t* head_sizes_host, const float* bv,
+                                     const float* ba, float* values, int64_t values_stride, float* params,
+                                     int64_t params_stride, const float* noise, uint64_t philox_seed,
+                                     uint64_t philox_offset, const int64_t* philox_offset_dev, float* actions_f32,
+                                     int64_t actions_stride, void** env_actions_host, float* log_prob,
+                                     int64_t log_prob_stride, const float* policy_version_scalar,
+                                     float* policy_version_out, int64_t pv_stride, void* stream) {
+    HeadsFinish f{{values, values_stride, params, params_stride, actions_f32, actions_stride, log_prob, log_prob_stride,
+                   policy_version_out, pv_stride},
+                  bv, ba, noise, philox_seed, philox_offset, philox_offset_dev, policy_version_scalar};
+    if (int rc = make_heads_layout(f.out, 3, A, num_heads, head_kinds_host, head_sizes_host, 0, 0, nullptr, 0.f, nullptr,
+                                   env_actions_host, "heads_from_partials_mixed"))
+        return rc;
+    if (int rc = sfb200_heads_from_partials(head_partials, P, rows, A, bv, ba, values, values_stride, params, params_stride,
+                                            nullptr, 0, 0, nullptr, nullptr, 0, nullptr, nullptr, 0, nullptr, nullptr, 0,
+                                            stream))
+        return rc;
+    return launch_tail_rows(rows, nullptr, 0, 0, nullptr, f, true, (cudaStream_t)stream);
 }
 
 int64_t sfb200_heads_wide_backward_workspace_bytes(int64_t rows, int width, int H, int A) {

@@ -1,5 +1,5 @@
 """Throughput of Tuple action spaces with Box members (ModelSpec.action_heads) on the device path, and the profiled share
-of the mixed kernels (heads_tail_mixed_kernel, ppo_loss_mixed_kernel, action_ratio_mixed_kernel):
+of the mixed kernels (heads_tail_rows_kernel, ppo_loss_mixed_kernel, action_ratio_mixed_kernel):
 
   (i)  4096 tape envs, Tuple(Discrete(5), Box(3), Discrete(3)) (14 distribution_linear rows), MLP 512-512, rollout 32,
        4 x 32768 minibatches
@@ -28,7 +28,7 @@ CASES = {
     "d5_b3_d3_mlp512": [("discrete", 5), ("box", 3), ("discrete", 3)],
     "d24_b8_d5_mlp512_wide": [("discrete", 24), ("box", 8), ("discrete", 5)],
 }
-MIXED_KERNELS = ("mixed",)
+MIXED_KERNELS = ("mixed", "heads_tail_rows")
 
 
 def run(name, heads, iters, warmup, engine):

@@ -28,7 +28,7 @@ CASES = {
                                                                  encoder_mlp_layers=[256, 128, 64], batch_size=32768,
                                                                  num_batches_per_epoch=4)),
 }
-WIDE_KERNELS = ("wide",)      # heads_tail_wide_kernel, ppo_loss_*wide*, action_ratio_*wide*, heads_wide_backward_*
+WIDE_KERNELS = ("wide", "heads_tail_rows")   # ppo_loss_*wide*, action_ratio_*wide*, heads_wide_backward_*, the stored-row tail
 
 
 def run(name, spec, iters, warmup, engine):
