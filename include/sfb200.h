@@ -228,8 +228,9 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
                                   const double* mean, const double* var, float sub_mean, float inv_scale, float eps,
                                   float clip, void* stream);
 /* A WHOLE ROLLOUT of a two-layer MLP policy over the synthetic tape env as one persistent kernel (csrc/rollout_fused.cu):
- * T x { layer 1, layer 2 + head partials, sfb200_sampler_tail_tape_step } with thread-block clusters of H2/128 CTAs owning a
- * 128-env row block for all T steps (cluster barriers only; no kernel boundary inside the rollout).  Replaces, per rollout,
+ * T x { layer 1, layer 2 + head partials, sfb200_sampler_tail_tape_step } with thread-block clusters of H2/256 CTAs owning a
+ * 64-env row block (H2 = 128: one CTA per 128-env block) for all T steps (cluster barriers only; no kernel boundary inside
+ * the rollout).  Replaces, per rollout,
  * T x (sfb200_linear_act_forward + sfb200_linear_act_heads_forward + sfb200_sampler_tail_tape_step); the caller runs
  * sfb200_sampler_pre_step for step 0 first (x_norm holds the normalised step-0 observations).  Pointers with suffix _0 are
  * the trajectory slots of step 0 ([:, 0]); step t is at + t elements (x A for logits, x dim for traj_obs / rnn rows).
@@ -239,11 +240,17 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
  *   bounds (K1, H1 multiples of 64); the h1 scratch then holds h1 * 2^shift split into fp16 planes: hi [n_envs][H1] halves,
  *   then lo n_envs * H1 halves later (the same bytes).  Otherwise (tf32 form) it holds h1 as fp32 [n_envs][H1]. */
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine);
-/* debug aid: device buffer of T x 16 uint64 that the following rollouts fill with %globaltimer stamps of one CTA's phases;
- * NULL switches it off */
+/* debug aid: device buffer of uint64 that the following rollouts fill with %globaltimer stamps: T x 16 phase stamps of one
+ * CTA, then 4 words per CTA (index blockIdx.y * gridDim.x + blockIdx.x): %smid, entry, after the programmatic-dependency
+ * wait, exit.  T x 16 + 4 x (n_envs / 32 + 4) words cover every launch shape; NULL switches it off */
 int sfb200_rollout_set_trace(void* trace_dev);
 /* form the last sfb200_rollout_mlp2_tape call launched: 1 fp16 split, 0 tf32 split, -1 none yet */
 int sfb200_rollout_last_form(void);
+/* debug aid: the clusters a rollout launch over n_envs needs and how many of them the device holds at once
+ * (cudaOccupancyMaxActiveClusters of the same launch configuration; the fp16-split instance when the shape allows it).
+ * More needed than resident means the launch runs in more than one wave. */
+int sfb200_rollout_occupancy(int64_t n_envs, int K1, int H1, int H2, int A, int engine, int act, int* clusters_needed,
+                             int* clusters_resident);
 int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, const float* b1, int H1, const float* W2,
                              const float* b2, int H2, int act, int engine, const float* Wv, const float* bv, const float* Wa,
                              const float* ba, int A, float* h1_scratch, float* head_partials, float* x_norm,

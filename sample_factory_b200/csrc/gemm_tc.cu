@@ -251,14 +251,15 @@ bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1
 }
 
 // 3-D fp16 map over a weight's [hi | lo] twins, planes lo_offset elements apart, each plane [rows][K] row-major: box
-// 64 k x 128 rows x both planes with the 128B swizzle, i.e. two [128][64 fp16] tiles in the K-major layout wgmma reads
-// (what split_tile_f16 writes).  False when TMA cannot describe the twins (alignment).
-bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows) {
+// 64 k x box_rows rows x both planes with the 128B swizzle, i.e. two [box_rows][64 fp16] tiles in the K-major layout
+// wgmma reads (what split_tile_f16 writes).  False when TMA cannot describe the twins (alignment).
+bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows,
+                         uint32_t box_rows) {
     if ((reinterpret_cast<uintptr_t>(hi) & 15u) || (K * 2) % 16 != 0 || (lo_offset * 2) % 16 != 0 || lo_offset <= 0)
         return false;
     cuuint64_t gdim[3] = {K, rows, 2};
     cuuint64_t gstride[2] = {K * 2, (cuuint64_t)lo_offset * 2};
-    cuuint32_t box[3] = {64, TBN, 2};
+    cuuint32_t box[3] = {64, box_rows, 2};
     cuuint32_t estride[3] = {1, 1, 1};
     CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<uint16_t*>(hi), gdim, gstride, box, estride,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -326,7 +327,7 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
         }
         // (B(n, k) is twin[n][k] in both cases: W[n][k] forward, the transposed twin [K_w][N_w] for dX)
         CUtensorMap ta16, tb16;
-        if (tw.hi && make_tmap_f16_twins(&tb16, tw.hi, tw.lo - tw.hi, (uint64_t)K, (uint64_t)N) &&
+        if (tw.hi && make_tmap_f16_twins(&tb16, tw.hi, tw.lo - tw.hi, (uint64_t)K, (uint64_t)N, TBN) &&
             (!epi.head_part || !b_mn)) {
             if (f16_check_enabled()) {
                 // B = W[N][K] row-major (forward) or W[K][N] row-major read along its other axis (dX: twins transposed)

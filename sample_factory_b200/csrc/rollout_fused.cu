@@ -3,12 +3,17 @@
 // pre-step of the next step } without leaving the SMs (batched_sampling.py:298-388 + inference_worker.py:313-341 +
 // actor_critic.py:160-195 for every step of the rollout).
 //
-// Decomposition: all data dependencies of a step stay inside a 128-row block of envs -- layer 2 needs all H1 columns of the
+// Decomposition: all data dependencies of a step stay inside a block of BM env rows -- layer 2 needs all H1 columns of the
 // block's h1, the heads need all H2 columns of its h2, the next step's layer 1 needs the block's new observations -- so a
-// thread-block CLUSTER of CX = H2/128 CTAs owns a row block for the whole rollout and the only synchronisation is the
+// thread-block CLUSTER of CX = H2/BN CTAs owns a row block for the whole rollout and the only synchronisation is the
 // cluster barrier (three per step); there is no grid-wide barrier and no kernel boundary.  CTA c of the cluster computes
-// columns [128c, 128c+128) of h1, then of h2 (partial head products), then finishes rows [32c.., ) of the block.
+// columns [BN c, BN c + BN) of h1, then of h2 (partial head products), then finishes rows [c BM/CX.., ) of the block.
 // h1 and the head partials cross between the CTAs of a cluster through global memory (L2-resident), read back by TMA.
+// The CTA tile (rf_wide): BM x BN = 64 x 256 for H2 >= 256 (the two consumer warpgroups side by side on N over one 64-row
+// A tile), 128 x 128 for H2 = 128 (the warpgroups stacked on M).  At H2 = 512 that makes clusters of two: a TPC is two SMs,
+// so every GPC holds a whole number of them and the whole grid (64 clusters at 4096 envs) is resident at once.  Clusters
+// of four strand two SMs in every GPC of 14 or 18 SMs: on the H100 measured (DESIGN §7) 30 of the 32 clusters of the
+// old 128 x 128 decomposition were resident, and the last two ran as a second wave after the first.
 //
 // Each GEMM tile is the wgmma tile of gemm_tc.cu (3-pass split operands, main | cross accumulators in registers); the step
 // tail is the code of sampler_tail_tape_kernel (heads.cu).
@@ -18,7 +23,7 @@
 //               in flight across the cluster barriers: the first W2 tiles between its arrive at and its wait on barrier 1,
 //               the next step's W1 tiles between its arrive at and its wait on barrier 2.  h1 and x_norm tiles are issued
 //               only after the barrier that publishes them.
-//   warps 4-11  two wgmma warpgroups (64 rows each): multiply, run the epilogues and the step tail (an 8-lane group per
+//   warps 4-11  two wgmma warpgroups (64 x 128 each): multiply, run the epilogues and the step tail (an 8-lane group per
 //               row: four rows per warp).  One wgmma group stays in flight; a ring slot goes back to the producer when
 //               its wgmmas have completed.
 //
@@ -27,8 +32,8 @@
 // fp16 [hi | lo] planes (the h1 scratch holds the hi plane, then the lo plane N*H1 halves later), so layer 2 -- 8 of the 9
 // stages of a step at H1 = 512 -- is pure TMA -> wgmma.  Only x_norm (layer 1's A, written as fp32 by the step tail) is
 // split in shared memory.  Every wgmma receives the operands the fp32 buffers would give after split_tile_f16.
-// tf32 form: raw fp32 tiles of 32 k; the consumers split both operands (A into the conversion buffer, B into the upper
-// half of its ring slot), as gemm_tc.cu's tf32 form does.
+// tf32 form: raw fp32 tiles of 32 k; the consumers split both operands (A into the conversion buffer, B into the back of
+// its ring slot), as gemm_tc.cu's tf32 form does.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -48,19 +53,31 @@ constexpr int RF_MAX_DIM = 128;
 constexpr int RF_PRODUCER_REGS = 40;
 constexpr int RF_CONSUMER_REGS = 232;
 
-// Ring slot (64 KB): [A 32 KB | B 32 KB].
-//   fp16 form: A = raw fp32 x_norm tile (layer 1) or the [hi | lo] h1 tiles (layer 2); B = the weight's [hi | lo] twin tiles.
-//   tf32 form: [A raw 16 KB | B raw 16 KB | B hi | B lo].
-// Conversion buffer (32 KB): [A hi | A lo] of the operands split in shared memory.
+// CTA tile of a layer: BM x BN = 64 x 256 (warpgroup w: columns n0 + 128 w of the same 64 rows) for H2 >= 256, else
+// 128 x 128 (warpgroup w: rows m0 + 64 w).  Same rule on the host (launch shape, TMA boxes) and in the kernel.
+__host__ __device__ __forceinline__ bool rf_wide(int H2) { return H2 >= 256; }
+__host__ __device__ __forceinline__ int rf_bm(int H2) { return rf_wide(H2) ? 64 : 128; }
+__host__ __device__ __forceinline__ int rf_bn(int H2) { return rf_wide(H2) ? 256 : 128; }
+
+// Ring slot of a stage (KBK k) for a BM x BN tile; all offsets multiples of 1024 B (the 128B swizzle atoms):
+//   fp16 form: [A BM x 256 B | B hi BN x 128 B | B lo]: A = raw fp32 x_norm tile (layer 1) or the [hi | lo] h1 planes
+//              (layer 2), B = the weight's [hi | lo] twin planes.  80 KB for 64 x 256, 64 KB for 128 x 128.
+//   tf32 form: [A raw BM x 128 B | B raw BN x 128 B | B hi | B lo].  104 KB for 64 x 256, 64 KB for 128 x 128.
+// Two slots: three 80 KB stages do not fit.  The conversion buffer [A hi | A lo] (BM x 256 B: the operands split in shared
+// memory) follows the slots, the mbarriers and the normaliser statistics follow the largest layout.
+template <bool F16>
 struct RfSmem {
-    static constexpr int STAGES = 3;
-    static constexpr int SLOT = 65536;
-    static constexpr int B_OFF = 32768;
-    static constexpr int OFF_CONV = STAGES * SLOT;
-    static constexpr int OFF_BARS = OFF_CONV + 32768;                // full[STAGES], empty[STAGES]
+    static constexpr int STAGES = 2;
+    static constexpr int KBK = F16 ? 64 : TBK;
+    __host__ __device__ static constexpr int slot(int bm, int bn) { return F16 ? (bm + bn) * 256 : (bm + 3 * bn) * 128; }
+    __host__ __device__ static constexpr int a_bytes(int bm) { return bm * KBK * 4; }   // A of a stage; B starts here
+    __host__ __device__ static constexpr int b_hi(int bm, int bn) { return F16 ? bm * 256 : (bm + bn) * 128; }
+    __host__ __device__ static constexpr int stage_tx(int bm, int bn) { return (bm + bn) * KBK * 4; }
+    static constexpr int OFF_BARS = STAGES * slot(64, 256) + 64 * 256;   // full[STAGES], empty[STAGES]
     static constexpr int OFF_CSTAT = OFF_BARS + 64;
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
     static_assert(2 * STAGES * 8 <= 64 && TOTAL + 64 <= 227 * 1024, "shared memory");
+    static_assert(STAGES * slot(128, 128) + 128 * 256 <= OFF_BARS, "the 128 x 128 layout fits below the barriers");
 };
 
 
@@ -82,7 +99,9 @@ struct RolloutArgs {
     float* traj_obs; int64_t traj_obs_rs; const float* rnn; int rnn_dim; float* traj_rnn; int64_t traj_rnn_rs;
     const double* mean; const double* var; float sub, inv_scale; int do_sub, do_scale; float eps, clip;
     unsigned int* ticket;
-    unsigned long long* trace;   // debug: [T][16] globaltimer stamps of CTA (0,0)'s first epilogue thread, or NULL
+    // debug, or NULL: [T][16] globaltimer stamps of CTA (0,0)'s first epilogue thread, then per CTA (blockIdx.y * gridDim.x
+    // + blockIdx.x) four words: %smid, globaltimer at entry, after the programmatic-dependency wait, at exit
+    unsigned long long* trace;
     const float* bound_x; const float* bound_h1;   // fp16-split form: bounds of |x_norm| and |h1| (device floats), else NULL
 };
 
@@ -100,6 +119,11 @@ __device__ __forceinline__ unsigned long long rf_now() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
+__device__ __forceinline__ uint32_t smid() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+    return r;
+}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -112,19 +136,20 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 // TMA producer, run by all of warpgroup 0 (every warp takes part in the cluster barriers); `leader` issues the loads.
 template <bool F16>
 __device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUtensorMap* tmap_w1, const CUtensorMap* tmap_h1,
-                                           const CUtensorMap* tmap_w2, int T, int K1, int H1, int m0, int n0, uint8_t* smem,
-                                           uint64_t* full, uint64_t* empty, bool leader) {
-    using S = RfSmem;
-    constexpr int KBK = F16 ? 64 : TBK;
-    constexpr uint32_t STAGE_TX = F16 ? 2 * 32768 : 2 * 16384;
+                                           const CUtensorMap* tmap_w2, int T, int K1, int H1, int bm, int bn, int m0, int n0,
+                                           uint8_t* smem, uint64_t* full, uint64_t* empty, bool leader) {
+    using S = RfSmem<F16>;
+    constexpr int KBK = S::KBK;
+    const int slot_bytes = S::slot(bm, bn), b_off = S::a_bytes(bm);
+    const uint32_t stage_tx = (uint32_t)S::stage_tx(bm, bn);
     const int n1 = K1 / KBK, n2 = H1 / KBK;
     uint32_t pu = 0;   // next use to claim
     // claim the next use: wait until its slot is free, expect the whole stage, load the weight tile (B)
     auto weight = [&](const CUtensorMap* tb, int kb) {
         const uint32_t s = pu % S::STAGES;
         mbar_wait(&empty[s], ((pu / S::STAGES) & 1) ^ 1);
-        mbar_expect_tx(&full[s], STAGE_TX);
-        uint8_t* dst = smem + s * S::SLOT + (F16 ? S::B_OFF : 16384);
+        mbar_expect_tx(&full[s], stage_tx);
+        uint8_t* dst = smem + s * slot_bytes + b_off;
         if (F16) tma_load_3d(dst, tb, &full[s], 64 * kb, n0, 0);   // [hi | lo] twin tiles
         else tma_load_2d(dst, tb, &full[s], TBK * kb, n0);
         ++pu;
@@ -132,8 +157,8 @@ __device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUte
     // the activation tile (A) of a claimed use
     auto activation = [&](uint32_t u, const CUtensorMap* ta, bool planes, int kb) {
         const uint32_t s = u % S::STAGES;
-        if (planes) tma_load_3d(smem + s * S::SLOT, ta, &full[s], 64 * kb, m0, 0);   // [hi | lo] h1 tiles
-        else tma_load_2d(smem + s * S::SLOT, ta, &full[s], KBK * kb, m0);
+        if (planes) tma_load_3d(smem + s * slot_bytes, ta, &full[s], 64 * kb, m0, 0);   // [hi | lo] h1 tiles
+        else tma_load_2d(smem + s * slot_bytes, ta, &full[s], KBK * kb, m0);
     };
     // Claims made before a cluster barrier only wait for slots the consumers free before they arrive there (uses of the
     // previous phase), so no claim can wait on the barrier it precedes: at most STAGES uses ahead.
@@ -174,47 +199,56 @@ __device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUte
     }
 }
 
-// One 128 x 128 tile acc = A[m0.., :K] . B[n0.., :K]^T (nkb stages) by the 256 consumer threads (ct = 0..255), `cu` the
-// consumers' use counter.  SPLIT_A: the A tile is raw fp32, split here (each warpgroup its own 64 rows) into the
-// conversion buffer; the tf32 form splits both operands.  3xTF32, or with F16 the fp16-split form of gemm_tc.cu (A *
-// 2^a_shift, weights * 2^kF16WShift, 64 k per stage).  Every accumulator receives its wgmmas in k order.
+// One BM x BN tile acc = A[m0.., :K] . B[n0.., :K]^T (nkb stages) by the 256 consumer threads (ct = 0..255), each
+// warpgroup its 64 x 128 piece; `cu` the consumers' use counter.  SPLIT_A: the A tile is raw fp32, split here into the
+// conversion buffer (each warpgroup its own 64 rows of a 128-row tile; both together the one 64-row tile of the wide
+// layout, which both read); the tf32 form splits both operands.  3xTF32, or with F16 the fp16-split form of gemm_tc.cu
+// (A * 2^a_shift, weights * 2^kF16WShift, 64 k per stage).  Every accumulator receives its wgmmas in k order.
 template <bool F16, bool SPLIT_A>
-__device__ __forceinline__ void rf_tile(int nkb, uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& cu,
+__device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& cu,
                                         float (&acc)[64], float (&cross)[64], int ct, int a_shift) {
-    using S = RfSmem;
+    using S = RfSmem<F16>;
     const int wg = ct >> 7, lt = ct & 127;
-    uint8_t* conv = smem + S::OFF_CONV;
+    const int bm = wide ? 64 : 128, bn = wide ? 256 : 128;
+    const int slot_bytes = S::slot(bm, bn), b_hi = S::b_hi(bm, bn);
+    const int a_row = wide ? 0 : 64 * wg, b_row = wide ? 128 * wg : 0;   // this warpgroup's rows of the A / B tiles
+    uint8_t* conv = smem + S::STAGES * slot_bytes;
     // (the first wgmmas overwrite them; defined values keep the accumulators from being live across the whole rollout)
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
     int held = -1;   // slot of the wgmma group still in flight
     for (int kb = 0; kb < nkb; ++kb, ++cu) {
         const int s = (int)(cu % S::STAGES);
-        uint8_t* slot = smem + s * S::SLOT;
+        uint8_t* slot = smem + s * slot_bytes;
         mbar_wait(&full[s], (cu / S::STAGES) & 1);
         const uint8_t* at = slot;
         if (SPLIT_A || !F16) {
-            // the conversion buffer is read by this warpgroup's wgmmas in flight
+            // the conversion buffer is read by the wgmmas in flight: this warpgroup's, and in the wide layout the other's
             if (held >= 0) {
                 wgmma_wait_all();
                 mbar_arrive(&empty[held]);
                 held = -1;
+                if (wide) consumer_sync();
             }
             if constexpr (F16) {
-                split_tile_f16<false, 64>(slot + wg * 64 * 256, conv + wg * 8192, conv + 16384 + wg * 8192, lt,
-                                          pow2f_int(a_shift));
+                if (wide) split_tile_f16<false, 64, 256>(slot, conv, conv + 8192, ct, pow2f_int(a_shift));
+                else split_tile_f16<false, 64>(slot + wg * 64 * 256, conv + wg * 8192, conv + 16384 + wg * 8192, lt,
+                                               pow2f_int(a_shift));
+            } else if (wide) {
+                split_tile<false, true, 64, 256>(slot, conv, conv + 8192, ct);
+                split_tile<false, true, 256, 256>(slot + 8192, slot + b_hi, slot + b_hi + 32768, ct);
             } else {
                 split_tile<false, true, 64>(slot + wg * 64 * 128, conv + wg * 8192, conv + 16384 + wg * 8192, lt);
-                split_tile<false, true>(slot + 16384, slot + S::B_OFF, slot + S::B_OFF + 16384, ct);
+                split_tile<false, true>(slot + 16384, slot + b_hi, slot + b_hi + 16384, ct);
             }
             fence_proxy_async_smem();
             consumer_sync();
             at = conv;
         }
-        const uint64_t da_hi = make_smem_desc(smem_u32(at + wg * 8192));
-        const uint64_t da_lo = make_smem_desc(smem_u32(at + 16384 + wg * 8192));
-        const uint64_t db_hi = make_smem_desc(smem_u32(slot + S::B_OFF));
-        const uint64_t db_lo = make_smem_desc(smem_u32(slot + S::B_OFF + 16384));
+        const uint64_t da_hi = make_smem_desc(smem_u32(at + a_row * 128));
+        const uint64_t da_lo = make_smem_desc(smem_u32(at + bm * 128 + a_row * 128));
+        const uint64_t db_hi = make_smem_desc(smem_u32(slot + b_hi + b_row * 128));
+        const uint64_t db_lo = make_smem_desc(smem_u32(slot + b_hi + bn * 128 + b_row * 128));
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < TBK / WG_K; ++k) {
@@ -273,8 +307,8 @@ __global__ void __launch_bounds__(RF_THREADS, 1)
 rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w1,
                          const __grid_constant__ CUtensorMap tmap_h1, const __grid_constant__ CUtensorMap tmap_w2,
                          const RolloutArgs a) {
-    using S = RfSmem;
-    constexpr int KBK = F16 ? 64 : TBK;
+    using S = RfSmem<F16>;
+    constexpr int KBK = S::KBK;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_align_1024(smem_raw);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);   // [STAGES] slot landed (TMA)
@@ -289,10 +323,18 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     if (threadIdx.x < 5) s_stats[threadIdx.x] = 0.0;
     const int cx = (int)cluster_ctarank();           // == blockIdx.x (cluster spans the x dimension)
     const int CX = gridDim.x;
-    const int n0 = cx * 128;
-    const int64_t m0 = (int64_t)blockIdx.y * 128;
-    const int P = 2 * CX;
+    const bool wide = rf_wide(a.H2);
+    const int BM = rf_bm(a.H2), BN = rf_bn(a.H2);
+    const int n0 = cx * BN;
+    const int64_t m0 = (int64_t)blockIdx.y * BM;
+    const int P = a.H2 / 64;                         // head partials per row: one per 64 columns
     const bool do_rms = a.mean != nullptr;
+    unsigned long long* cta_trace =
+        a.trace ? a.trace + (int64_t)a.T * 16 + 4 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
+    if (cta_trace && threadIdx.x == 0) {
+        cta_trace[0] = smid();
+        cta_trace[1] = rf_now();
+    }
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_x) : "memory");
@@ -308,6 +350,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     __syncthreads();
     pdl_wait();
     pdl_trigger();
+    if (cta_trace && threadIdx.x == 0) cta_trace[2] = rf_now();
     if (do_rms)
         for (int c = threadIdx.x; c < a.K1; c += RF_THREADS) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.K1 + c]);
     __syncthreads();
@@ -316,7 +359,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
 
     if (warp < 4) {
         setmaxnreg_dec<RF_PRODUCER_REGS>();
-        rf_produce<F16>(&tmap_x, &tmap_w1, &tmap_h1, &tmap_w2, a.T, a.K1, a.H1, (int)m0, n0, smem, full, empty,
+        rf_produce<F16>(&tmap_x, &tmap_w1, &tmap_h1, &tmap_w2, a.T, a.K1, a.H1, BM, BN, (int)m0, n0, smem, full, empty,
                         threadIdx.x == 0);
     } else {
         setmaxnreg_inc<RF_CONSUMER_REGS>();
@@ -331,17 +374,18 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         const TcEpilogue epi_heads{1, ACT, a.b2, nullptr, 0, a.wv, a.wa, a.A, a.part};
         const TcEpilogue epi_h1{1, ACT, a.b1, nullptr, 0};
         const int ct = threadIdx.x - 128;
-        const int64_t row_base = m0 + (ct >> 7) * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
+        // this warpgroup's 64 x 128 piece of the CTA tile: rows m0 + 64 wg (128 x 128) or columns n0 + 128 wg (64 x 256)
+        const int64_t row_base = m0 + (wide ? 0 : (ct >> 7) * 64) + ((ct >> 5) & 3) * 16 + (lane >> 2);
         TileCoord tc;
-        tc.m0 = m0; tc.n0 = n0; tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
+        tc.m0 = m0; tc.n0 = n0 + (wide ? (ct >> 7) * 128 : 0); tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
 
         for (int t = 0; t < a.T; ++t) {
             RF_TRACE(0);
             {
                 float acc[64], cross[64];
-                rf_tile<F16, true>(a.K1 / KBK, smem, full, empty, cu, acc, cross, ct, shift_x);
+                rf_tile<F16, true>(a.K1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_x);
                 if (F16)
-                    store_h1_split(acc, n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1, a.b1, ACT,
+                    store_h1_split(acc, tc.n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1, a.b1, ACT,
                                    pow2f_int(shift_h));
                 else
                     store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
@@ -352,7 +396,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
             RF_TRACE(4);
             {
                 float acc[64], cross[64];
-                rf_tile<F16, !F16>(a.H1 / KBK, smem, full, empty, cu, acc, cross, ct, shift_h);
+                rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h);
                 heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
                 RF_TRACE(7);
             }
@@ -376,7 +420,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                 const uint64_t offset = philox0 + (uint64_t)t;
                 const float* src_step = a.tape + ((step + 1) % a.tape_len) * a.N * a.K1;
                 const float* noise_t = a.noise ? a.noise + (int64_t)t * a.N * a.A : nullptr;
-                const int rpc = 128 / CX;                     // rows of the block this CTA finishes
+                const int rpc = BM / CX;                      // rows of the block this CTA finishes
                 const unsigned gmask = 0xffu << (grp * 8);
                 for (int base = 0; base < rpc; base += 32) {
                     const int rr = base + (warp - 4) * 4 + grp;
@@ -512,6 +556,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     __syncthreads();
     if (threadIdx.x < 5 && a.stats && s_stats[0] > 0.0) atomicAdd(a.stats + threadIdx.x, s_stats[threadIdx.x]);
     if (threadIdx.x == 0) {
+        if (cta_trace) cta_trace[3] = rf_now();
         __threadfence();
         if (atomicAdd(a.ticket, 1u) == gridDim.x * gridDim.y - 1u) {
             *a.ticket = 0u;
@@ -521,20 +566,22 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     }
 }
 
+// The launch configuration of rollout_mlp2_tape_kernel<ACT, F16> for N envs and hidden width H2 -- what the launch and the
+// occupancy query (sfb200_rollout_occupancy) both use.  `attr` must outlive cfg.
 template <int ACT, bool F16>
-static int launch_rollout(const CUtensorMap* tm, const RolloutArgs& a, int CX, cudaStream_t st) {
+static int rollout_launch_config(int64_t N, int H2, cudaStream_t st, cudaLaunchConfig_t& cfg, cudaLaunchAttribute (&attr)[2]) {
     auto kern = rollout_mlp2_tape_kernel<ACT, F16>;
     static bool attr_set = false;
     if (!attr_set) {
-        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RfSmem::TOTAL));
+        SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, RfSmem<F16>::TOTAL));
         attr_set = true;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)CX, (unsigned)ceil_div(a.N, 128));
+    const int CX = H2 / rf_bn(H2);
+    cfg = {};
+    cfg.gridDim = dim3((unsigned)CX, (unsigned)ceil_div(N, rf_bm(H2)));
     cfg.blockDim = dim3(RF_THREADS);
-    cfg.dynamicSmemBytes = RfSmem::TOTAL;
+    cfg.dynamicSmemBytes = RfSmem<F16>::TOTAL;
     cfg.stream = st;
-    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = (unsigned)CX;
     attr[0].val.clusterDim.y = 1;
@@ -543,8 +590,29 @@ static int launch_rollout(const CUtensorMap* tm, const RolloutArgs& a, int CX, c
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    SFB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], a));
+    return 0;
+}
+
+template <int ACT, bool F16>
+static int launch_rollout(const CUtensorMap* tm, const RolloutArgs& a, cudaStream_t st) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[2];
+    const int rc = rollout_launch_config<ACT, F16>(a.N, a.H2, st, cfg, attr);
+    if (rc) return rc;
+    SFB_CUDA_OK(cudaLaunchKernelEx(&cfg, rollout_mlp2_tape_kernel<ACT, F16>, tm[0], tm[1], tm[2], tm[3], a));
     SFB_LAUNCH_OK();
+    return 0;
+}
+
+// clusters the launch for N envs needs, and how many of them the device holds at once (cudaOccupancyMaxActiveClusters)
+template <int ACT, bool F16>
+static int rollout_occupancy(int64_t N, int H2, int* needed, int* resident) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[2];
+    const int rc = rollout_launch_config<ACT, F16>(N, H2, 0, cfg, attr);
+    if (rc) return rc;
+    SFB_CUDA_OK(cudaOccupancyMaxActiveClusters(resident, rollout_mlp2_tape_kernel<ACT, F16>, &cfg));
+    *needed = (int)(cfg.gridDim.x * cfg.gridDim.y / attr[0].val.clusterDim.x);
     return 0;
 }
 
@@ -571,10 +639,10 @@ static bool rollout_f16_enabled() {
 
 #define SFB_RF_LAUNCH(F16v)                                                                  \
     switch (act) {                                                                           \
-        case SFB200_ACT_ELU: return launch_rollout<SFB200_ACT_ELU, F16v>(tm, a, CX, st);     \
-        case SFB200_ACT_RELU: return launch_rollout<SFB200_ACT_RELU, F16v>(tm, a, CX, st);   \
-        case SFB200_ACT_TANH: return launch_rollout<SFB200_ACT_TANH, F16v>(tm, a, CX, st);   \
-        default: return launch_rollout<SFB200_ACT_NONE, F16v>(tm, a, CX, st);                \
+        case SFB200_ACT_ELU: return launch_rollout<SFB200_ACT_ELU, F16v>(tm, a, st);     \
+        case SFB200_ACT_RELU: return launch_rollout<SFB200_ACT_RELU, F16v>(tm, a, st);   \
+        case SFB200_ACT_TANH: return launch_rollout<SFB200_ACT_TANH, F16v>(tm, a, st);   \
+        default: return launch_rollout<SFB200_ACT_NONE, F16v>(tm, a, st);                \
     }
 
 static int g_rollout_form = -1;   // form of the last launch: 1 fp16 split, 0 tf32 split
@@ -583,7 +651,7 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
     if (!tc_rollout_mlp2_supported(W1, W2, a_in.K1, a_in.H1, a_in.H2, a_in.A, engine)) return SFB_TC_UNSUPPORTED;
     if ((reinterpret_cast<uintptr_t>(a_in.wv) & 7u) || (reinterpret_cast<uintptr_t>(a_in.wa) & 7u)) return SFB_TC_UNSUPPORTED;
     RolloutArgs a = a_in;
-    const int CX = a.H2 / 128;
+    const uint32_t BM = (uint32_t)rf_bm(a.H2), BN = (uint32_t)rf_bn(a.H2);   // TMA boxes: A tiles BM rows, weight tiles BN
     if (rollout_f16_enabled() && a.K1 % 64 == 0 && a.H1 % 64 == 0) {
         const F16Twin t1 = f16_twin_lookup(W1, (int64_t)a.H1 * a.K1), t2 = f16_twin_lookup(W2, (int64_t)a.H2 * a.H1);
         const float* bx = operand_bound_lookup(a.x_norm, a.N * a.K1 * (int64_t)sizeof(float));
@@ -598,11 +666,11 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
             a.bound_h1 = bh;
             // the h1 scratch (N x H1 floats) holds the split h1: hi plane [N][H1] halves, then the lo plane
             CUtensorMap tm[4];
-            bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 64, 128);
-            ok = ok && make_tmap_f16_twins(&tm[1], t1.hi, t1.lo - t1.hi, (uint64_t)a.K1, (uint64_t)a.H1);
+            bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, 64, BM);
+            ok = ok && make_tmap_f16_twins(&tm[1], t1.hi, t1.lo - t1.hi, (uint64_t)a.K1, (uint64_t)a.H1, BN);
             ok = ok && make_tmap_f16_twins(&tm[2], reinterpret_cast<const uint16_t*>(a.h1), a.N * a.H1, (uint64_t)a.H1,
-                                           (uint64_t)a.N);
-            ok = ok && make_tmap_f16_twins(&tm[3], t2.hi, t2.lo - t2.hi, (uint64_t)a.H1, (uint64_t)a.H2);
+                                           (uint64_t)a.N, BM);
+            ok = ok && make_tmap_f16_twins(&tm[3], t2.hi, t2.lo - t2.hi, (uint64_t)a.H1, (uint64_t)a.H2, BN);
             if (ok) {   // (twins TMA cannot describe keep the tf32 form, as in gemm_tc)
                 g_rollout_form = 1;
                 SFB_RF_LAUNCH(true)
@@ -611,10 +679,10 @@ int tc_rollout_mlp2_tape(const float* W1, const float* W2, int act, int engine, 
     }
     a.bound_x = a.bound_h1 = nullptr;
     CUtensorMap tm[4];
-    bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, TBK, 128);
-    ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, TBK, 128);
-    ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, TBK, 128);
-    ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, TBK, 128);
+    bool ok = make_tmap(&tm[0], a.x_norm, (uint64_t)a.K1, (uint64_t)a.N, (uint64_t)a.K1, TBK, BM);
+    ok = ok && make_tmap(&tm[1], W1, (uint64_t)a.K1, (uint64_t)a.H1, (uint64_t)a.K1, TBK, BN);
+    ok = ok && make_tmap(&tm[2], a.h1, (uint64_t)a.H1, (uint64_t)a.N, (uint64_t)a.H1, TBK, BM);
+    ok = ok && make_tmap(&tm[3], W2, (uint64_t)a.H1, (uint64_t)a.H2, (uint64_t)a.H1, TBK, BN);
     if (!ok) return SFB_TC_UNSUPPORTED;
     g_rollout_form = 0;
     SFB_RF_LAUNCH(false)
@@ -635,6 +703,28 @@ int sfb200_rollout_set_trace(void* trace_dev) {
 }
 
 int sfb200_rollout_last_form(void) { return g_rollout_form; }
+
+int sfb200_rollout_occupancy(int64_t n_envs, int K1, int H1, int H2, int A, int engine, int act, int* clusters_needed,
+                             int* clusters_resident) {
+    SFB_CHECK_ARG(n_envs > 0 && clusters_needed && clusters_resident, "rollout_occupancy: bad arguments");
+    SFB_CHECK_ARG(tc_rollout_mlp2_supported(nullptr, nullptr, K1, H1, H2, A, engine),
+                  "rollout_occupancy: model not covered (K1=%d H1=%d H2=%d A=%d engine=%d)", K1, H1, H2, A, engine);
+    // the instance a launch with registered fp16 twins and bounds takes
+    if (rollout_f16_enabled() && K1 % 64 == 0 && H1 % 64 == 0) {
+        switch (act) {
+            case SFB200_ACT_ELU: return rollout_occupancy<SFB200_ACT_ELU, true>(n_envs, H2, clusters_needed, clusters_resident);
+            case SFB200_ACT_RELU: return rollout_occupancy<SFB200_ACT_RELU, true>(n_envs, H2, clusters_needed, clusters_resident);
+            case SFB200_ACT_TANH: return rollout_occupancy<SFB200_ACT_TANH, true>(n_envs, H2, clusters_needed, clusters_resident);
+            default: return rollout_occupancy<SFB200_ACT_NONE, true>(n_envs, H2, clusters_needed, clusters_resident);
+        }
+    }
+    switch (act) {
+        case SFB200_ACT_ELU: return rollout_occupancy<SFB200_ACT_ELU, false>(n_envs, H2, clusters_needed, clusters_resident);
+        case SFB200_ACT_RELU: return rollout_occupancy<SFB200_ACT_RELU, false>(n_envs, H2, clusters_needed, clusters_resident);
+        case SFB200_ACT_TANH: return rollout_occupancy<SFB200_ACT_TANH, false>(n_envs, H2, clusters_needed, clusters_resident);
+        default: return rollout_occupancy<SFB200_ACT_NONE, false>(n_envs, H2, clusters_needed, clusters_resident);
+    }
+}
 
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine) {
     return tc_rollout_mlp2_supported(W1, W2, K1, H1, H2, A, engine);

@@ -162,8 +162,9 @@ __device__ __forceinline__ float act_bwd_ct(float h) {
 bool tc_init();
 bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
                uint32_t box1);
-// 3-D fp16 map over a [hi | lo] pair of row-major [rows][K] planes, lo_offset elements apart: box 64 k x 128 rows x both
-// planes with the 128B swizzle (the weights' registered twins; the rollout's split h1 scratch)
-bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows);
+// 3-D fp16 map over a [hi | lo] pair of row-major [rows][K] planes, lo_offset elements apart: box 64 k x box_rows rows x
+// both planes with the 128B swizzle (the weights' registered twins; the rollout's split h1 scratch)
+bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows,
+                         uint32_t box_rows);
 
 }  // namespace sfb

@@ -67,14 +67,14 @@ __device__ __forceinline__ float act_fwd_fast(float z, int act) {
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // raw tile (TMA, no swizzle) -> tf32 hi / lo halves in the swizzled K-major layout.  K-major raw: [rows][32 k];
-// MN-major raw: [32 k][rows] (transposed on the way).  ct = thread 0 .. 2*ROWS-1 (ROWS = 64: one warpgroup's rows of a
+// MN-major raw: [32 k][rows] (transposed on the way).  ct = thread 0 .. THREADS-1 (ROWS = 64: one warpgroup's rows of a
 // K-major tile, the pointers already offset to them).
-template <bool MN, bool SPLIT3, int ROWS = TBM>
+template <bool MN, bool SPLIT3, int ROWS = TBM, int THREADS = 2 * ROWS>
 __device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct) {
-    static_assert(!MN || ROWS == TBM, "MN-major tiles: whole tiles only");
+    static_assert(!MN || (ROWS == TBM && THREADS == 2 * TBM), "MN-major tiles: whole tiles only");
 #pragma unroll
-    for (int q = 0; q < (ROWS * TBK / 4) / (2 * ROWS); ++q) {
-        const int i = ct + 2 * ROWS * q;
+    for (int q = 0; q < (ROWS * TBK / 4) / THREADS; ++q) {
+        const int i = ct + THREADS * q;
         const float4 v = reinterpret_cast<const float4*>(raw)[i];
         const float e[4] = {v.x, v.y, v.z, v.w};
         if (!MN) {
@@ -116,13 +116,13 @@ __device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint
 // fp16-split engine: raw fp32 K-major tile [rows][64 k] -> scaled fp16 hi / lo halves (lo carries a 2^11 factor,
 // common.cuh) in the swizzled K-major [rows][64 fp16] layout.  (MN-major operands never take the fp16 form: the weight
 // operand of dX comes from its transposed twins instead, gemm_tc.cu.)
-// ct and ROWS as for split_tile.
-template <bool MN, int ROWS = TBM>
+// ct, ROWS and THREADS as for split_tile.
+template <bool MN, int ROWS = TBM, int THREADS = 2 * ROWS>
 __device__ __forceinline__ void split_tile_f16(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct, float scale) {
     static_assert(!MN, "fp16 split: K-major tiles only");
 #pragma unroll 4
-    for (int q = 0; q < (ROWS * 64 / 4) / (2 * ROWS); ++q) {
-        const int i = ct + 2 * ROWS * q;
+    for (int q = 0; q < (ROWS * 64 / 4) / THREADS; ++q) {
+        const int i = ct + THREADS * q;
         const float4 v = reinterpret_cast<const float4*>(raw)[i];
         const int r = i >> 4, c4 = i & 15;                         // row r, k = 4*c4 .. 4*c4+3
         const uint32_t off = (uint32_t)(r * 128 + ((((c4 >> 1) ^ r) & 7) << 4) + (c4 & 1) * 8);

@@ -6,7 +6,8 @@ computes anything itself and there is no CPU path -- a CPU tensor raises.
 """
 from __future__ import annotations
 
-from typing import Optional
+import ctypes
+from typing import Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -708,6 +709,15 @@ def rollout_mlp2_tape(T: int, W1: Tensor, b1: Tensor, W2: Tensor, b2: Tensor, ac
                None if fin_len is None else fin_len.data_ptr(), tr["obs"].data_ptr(), tr["obs"].stride(0), _p(rnn, F32),
                rnn.shape[1], tr["rnn_states"].data_ptr(), tr["rnn_states"].stride(0), _p(mean, F64), _p(var, F64), sub_mean,
                inv_scale, eps, clip, _stream())
+
+
+def rollout_occupancy(n_envs: int, K1: int, H1: int, H2: int, A: int, engine: int, act: int) -> Tuple[int, int]:
+    """(clusters needed, clusters resident at once) of a persistent-rollout launch over n_envs envs; needed > resident
+    means the launch runs in more than one wave"""
+    needed, resident = ctypes.c_int(0), ctypes.c_int(0)
+    lib().call("sfb200_rollout_occupancy", n_envs, K1, H1, H2, A, engine, act, ctypes.addressof(needed),
+               ctypes.addressof(resident))
+    return needed.value, resident.value
 
 
 def rollout_last_form() -> int:

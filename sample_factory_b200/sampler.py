@@ -114,8 +114,8 @@ class DeviceSampler:
                            not env.obs_uint8 and self.rnn is None and self.heads_plan.P > 0 and
                            not self.heads_plan.finish_in_gemm and not self.heads_plan.separate and
                            not spec.continuous and not spec.action_segments and not spec.action_heads)
-        # Whole rollout as ONE persistent kernel (csrc/rollout_fused.cu): clusters of H2/128 CTAs own a 128-env row block for
-        # all T steps.  Same conditions as the fused tail plus a two-layer MLP the kernel covers (one encoder: not the key
+        # Whole rollout as ONE persistent kernel (csrc/rollout_fused.cu): clusters of H2/256 CTAs own a 64-env row block for
+        # all T steps (H2 = 128: one CTA per 128-env block).  Same conditions as the fused tail plus a two-layer MLP the kernel covers (one encoder: not the key
         # encoders of a Dict model).  SFB200_ROLLOUT_FUSED=0 restores the per-step launches.
         self.fused_rollout = False
         if (self.fused_tail and os.environ.get("SFB200_ROLLOUT_FUSED", "1") != "0" and not deterministic and

@@ -6,6 +6,11 @@ boundaries of every step into a [T][16] buffer.  Prints, per step, the mean time
 last --iters rollouts (step 0 left out: it includes the launch ramp), with the GPU's name and power limit, and writes
 <out>/rollout_trace.json.  The stamps are one CTA's view; barrier phases include waiting for the cluster's slowest CTA.
 
+Every CTA also stamps its SM id and its entry / start (after the programmatic-dependency wait) / exit times: the tool
+prints the spread of the start times, how many CTAs started more than one step after the first (a second wave: the
+grid needs more clusters than the device holds at once, sfb200_rollout_occupancy), and the kernel's span against one
+CTA's span.
+
   python tools/rollout_trace.py --out DIR [--iters 5] [--warmup 3] [--engine auto]
 """
 from __future__ import annotations
@@ -25,6 +30,31 @@ import torch  # noqa: E402
 # (name, first stamp slot, last stamp slot) -- the RF_TRACE slots of the kernel
 PHASES = [("layer 1", 0, 3), ("barrier 1", 3, 4), ("layer 2 + heads", 4, 7), ("barrier 2", 7, 8), ("tail", 8, 9),
           ("barrier 3", 9, 10)]
+
+
+def cta_summary(ctas, step_us):
+    """per-CTA stamps of several rollouts -> start spread, late starters (more than a step after the first CTA), the
+    kernel's span and a CTA's median span (means over the rollouts), the last rollout's stamps relative to its first
+    start"""
+    spread = late = span = cta_span = 0.0
+    for rows in ctas:
+        t0 = min(r[2] for r in rows)
+        starts = [(r[2] - t0) / 1e3 for r in rows]
+        spans = sorted((r[3] - r[2]) / 1e3 for r in rows)
+        spread += max(starts)
+        late += sum(s > step_us for s in starts)
+        span += (max(r[3] for r in rows) - t0) / 1e3
+        cta_span += spans[len(spans) // 2]
+    n = len(ctas)
+    last = ctas[-1]
+    t0 = min(r[2] for r in last)
+    late_last = sorted(((r[0], (r[2] - t0) / 1e3, (r[3] - r[2]) / 1e3) for r in last if (r[2] - t0) / 1e3 > step_us),
+                       key=lambda x: x[1])
+    return {"count": len(last), "start_spread_us": round(spread / n, 2), "late_starts": round(late / n, 2),
+            "kernel_span_us": round(span / n, 1), "cta_span_us": round(cta_span / n, 1),
+            "late": [(sm, round(st, 1), round(sp, 1)) for sm, st, sp in late_last],
+            "last_rollout": [{"smid": r[0], "entry_us": round((r[1] - t0) / 1e3, 2), "start_us": round((r[2] - t0) / 1e3, 2),
+                              "exit_us": round((r[3] - t0) / 1e3, 2)} for r in last]}
 
 
 def main():
@@ -48,8 +78,9 @@ def main():
     gen = torch.Generator().manual_seed(1234)
     tape = torch.randn(bench.TAPE_LEN, bench.N_ENVS, bench.OBS_DIM, generator=gen).to(dev)
     register_env("synthetic_tape", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, bench.N_ACTIONS))
-    T = bench.ROLLOUT
-    trace = torch.zeros((T, 16), dtype=torch.int64, device=dev)
+    T, N, H = bench.ROLLOUT, bench.N_ENVS, bench.HIDDEN[-1]
+    n_words = T * 16 + 4 * (N // 32 + 4)   # phase stamps, then four words per CTA (include/sfb200.h)
+    trace = torch.zeros(n_words, dtype=torch.int64, device=dev)
     # set before the first rollout: the sampler's CUDA graph captures the kernel arguments, the trace pointer included
     lib().call("sfb200_rollout_set_trace", trace.data_ptr())
     try:
@@ -61,15 +92,22 @@ def main():
         torch.cuda.synchronize()
         sums = [0.0] * len(PHASES)
         count = 0
+        ctas = []   # per rollout: [(smid, entry, start, exit)] of every CTA that ran
         for _ in range(args.iters):
             trace.zero_()
             runner.iteration()
             torch.cuda.synchronize()
-            st = trace.cpu()
+            flat = trace.cpu()
+            st = flat[:T * 16].view(T, 16)
             for t in range(1, T):
                 for i, (_, a, b) in enumerate(PHASES):
                     sums[i] += (int(st[t, b]) - int(st[t, a])) / 1e3
                 count += 1
+            c = flat[T * 16:].view(-1, 4).tolist()
+            ctas.append([tuple(r) for r in c if r[2] != 0])
+        act = ops.ACT[runner.sampler.model.spec.nonlinearity]
+        needed, resident = ops.rollout_occupancy(N, bench.OBS_DIM, bench.HIDDEN[0], H, bench.N_ACTIONS,
+                                                 runner.sampler.engine, act)
     finally:
         lib().call("sfb200_rollout_set_trace", None)
     form = {1: "fp16 split", 0: "tf32 split"}.get(ops.rollout_last_form(), "?")
@@ -77,8 +115,10 @@ def main():
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     total = sum(per.values())
+    waves = cta_summary(ctas, total)
     result = {"gpu": gpu, "workload": bench.WORKLOAD, "form": form, "rollouts": args.iters, "steps_per_rollout": T,
-              "us_per_step": per, "us_per_step_total": round(total, 2)}
+              "us_per_step": per, "us_per_step_total": round(total, 2),
+              "occupancy": {"clusters_needed": needed, "clusters_resident": resident}, "ctas": waves}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "rollout_trace.json"), "w") as f:
         json.dump(result, f, indent=1)
@@ -86,6 +126,13 @@ def main():
     for name, v in per.items():
         print(f"  {name:16s} {v:8.2f}")
     print(f"  {'step':16s} {total:8.2f}")
+    print(f"occupancy: {needed} clusters needed, {resident} resident at once")
+    print(f"CTAs per rollout: {waves['count']}; start spread {waves['start_spread_us']:.2f} us; "
+          f"{waves['late_starts']} started more than a step ({total:.1f} us) after the first; "
+          f"kernel span {waves['kernel_span_us']:.1f} us vs one CTA's span {waves['cta_span_us']:.1f} us (means over "
+          f"{args.iters} rollouts)")
+    for sm, st, sp in waves["late"][:16]:
+        print(f"  late CTA on SM {sm}: started {st:.1f} us after the first, ran {sp:.1f} us")
 
 
 if __name__ == "__main__":
