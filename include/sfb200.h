@@ -625,7 +625,20 @@ int sfb200_heads_wide_backward(const float* h, int64_t ldh, int64_t rows, int H,
                                int accumulate, float* dWv, float* dbv, float* dba, float* db_prev, void* workspace,
                                void* stream);
 
+/* split-K slices sfb200_linear_backward gives dW [N,K] (reduced over M) on a device of sm_count SMs (<= 0: the current
+ * device's; 132 when there is none): with fewer output tiles than SMs, the most slices that still run in one wave */
+int sfb200_linear_backward_splits(int64_t M, int N, int K, int sm_count);
 int64_t sfb200_linear_backward_workspace_bytes(int64_t M, int N, int K);
+/* debug aids of the wgmma GEMM engine (tools/gemm_trace.py).
+ * sfb200_gemm_work_item: the tf32 form's work item `item` of C [M,N] = A.B^T over K in `splits` slices ->
+ *   out[0..5] = first row, first column, first k, k covered (whole 32-k stages), slice, number of work items.  The kernel
+ *   is persistent: CTA b of a grid of g runs items b, b + g, b + 2g, ...
+ * sfb200_gemm_set_trace: device buffer of n_words uint64 that the wgmma GEMMs the calling thread launches next fill, 16
+ *   words per work item: %smid, CTA, then %globaltimer (ns) at: item begun, its first stage landed, mainloop done,
+ *   epilogue done (one consumer thread), first / last load of the item issued (producer thread); words 8, 9 of the
+ *   CTA's first item: kernel entry, setup done.  A launch with more items than n_words / 16 fails.  NULL switches it off */
+int sfb200_gemm_work_item(int64_t item, int64_t M, int N, int K, int splits, int64_t* out);
+int sfb200_gemm_set_trace(void* trace_dev, int64_t n_words);
 /* backward of y = act(x.W^T + b) given dz = dL/d(pre-activation) [M,N]:
  *   dW[N,K] = dz^T . x  (skipped if dW == NULL) ;  (db is produced by the kernel that made dz)
  *   if dx != NULL: dx[M,K] = (dz . W) * act_prev'(x)     (x is the previous layer's OUTPUT, act_prev its activation;

@@ -191,7 +191,7 @@ int sm_count() {
             int n = 0;
             if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess) g_sm_count = n;
         }
-        if (g_sm_count <= 0) g_sm_count = 148;
+        if (g_sm_count <= 0) g_sm_count = 132;   // no device to ask (host-only callers sizing workspaces): the H100's
     }
     return g_sm_count;
 }

@@ -30,7 +30,8 @@ int tc_linear_backward(const float* dz, int64_t lddz, const float* x, int64_t ld
 
 namespace sfb {
 // shared with the SIMT engine (gemm_simt.cu)
-int choose_splits(int64_t M, int N, int K);
+int choose_splits(int64_t M, int N, int K, int sms);
+int choose_splits(int64_t M, int N, int K);   // on the current device
 int splitk_reduce(const float* part, int splits, int64_t M, int N, float* C, int64_t ldc, cudaStream_t st);
 int colsum_reduce(const float* part, int64_t groups, int N, float* out, cudaStream_t st);
 }  // namespace sfb

@@ -2,6 +2,8 @@
 // the fallback for shapes the wgmma engine does not take.  C[m,n] = sum_k A(m,k) * B(n,k) with either operand stored
 // K-contiguous ([rows, K]) or row-contiguous ([K, rows]); 128x128x16 CTA tile, 256 threads, 8x8 register micro-tile,
 // double-buffered shared memory, optional split-K (deterministic two-pass reduce).
+#include <cstdlib>
+
 #include "common.cuh"
 #include "gemm.h"
 
@@ -201,16 +203,33 @@ __global__ void colsum_reduce_kernel(const float* __restrict__ part, int groups,
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-int choose_splits(int64_t M, int N, int K) {
+// SFB200_SPLITK_LEGACY=1: the split-K rule this engine had before it was sized to the device (A/B comparison: dW sums
+// then group as they did, so results are bit-identical to that build's)
+static bool splitk_legacy() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("SFB200_SPLITK_LEGACY");
+        v = (e && e[0] == '1') ? 1 : 0;
+    }
+    return v == 1;
+}
+
+// Split-K slices of a GEMM with an M x N output reduced over K, on a device of `sms` SMs: fewer tiles than SMs -> as many
+// slices as still give every CTA an SM in one wave (tiles * s <= sms); otherwise none.  At least 128 k per slice, at
+// most 64 slices.
+int choose_splits(int64_t M, int N, int K, int sms) {
     const int64_t tiles = ceil_div(M, BM) * ceil_div(N, BN);
-    int64_t s = ceil_div(2 * (int64_t)148, tiles);
-    if (tiles >= 148) s = 1;
+    int64_t s = tiles < sms ? sms / tiles : 1;
+    if (splitk_legacy()) s = tiles >= 148 ? 1 : ceil_div(2 * (int64_t)148, tiles);
     const int64_t max_by_k = K / (BK * 8) > 0 ? K / (BK * 8) : 1;
     if (s > max_by_k) s = max_by_k;
     if (s > 64) s = 64;
     if (s < 1) s = 1;
     return (int)s;
 }
+// on the current device (sm_count(): 132, the H100's, when there is no device to ask, so that workspace sizes can be
+// computed without one)
+int choose_splits(int64_t M, int N, int K) { return choose_splits(M, N, K, sm_count()); }
 
 // C[M,N] = epilogue( sum_k A(m,k) B(n,k) ); ws needed only when splits > 1.
 int gemm_simt(bool a_kcont, const float* A, int64_t lda, bool b_kcont, const float* B, int64_t ldb, float* C, int64_t ldc,
@@ -338,6 +357,11 @@ int sfb200_linear_act_heads_forward(const float* x, int64_t ldx, const float* W,
                   "linear_act_heads_forward: shape/engine not covered (N=%d K=%d A=%d engine=%d); "
                   "sfb200_linear_heads_partials() tells when to use the separate calls", N, K, A, engine);
     return rc;
+}
+
+int sfb200_linear_backward_splits(int64_t M, int N, int K, int sm_count) {
+    const int m = (int)(M > 0x7fffffff ? 0x7fffffff : M);
+    return sm_count > 0 ? choose_splits(N, K, m, sm_count) : choose_splits(N, K, m);
 }
 
 int64_t sfb200_linear_backward_workspace_bytes(int64_t M, int N, int K) {

@@ -9,7 +9,11 @@
 // (Two accumulators keep the 2^-11 smaller cross terms apart from the large partial sums, which removes most of the
 // roundings applied to them.)
 //
-// One CTA per 128 x 128 output tile (x split-K slice), 384 threads = three warpgroups:
+// Work item = one 128 x 128 output tile (x split-K slice).  The kernel is persistent: the grid is the CTAs the device holds
+// at once (one per SM), CTA b runs items b, b + grid, b + 2 grid, ... (a fixed schedule; no result depends on it).  Barriers
+// are set up once per CTA, ring slots and mbarrier phases run on across items, and the producer does not wait for the
+// consumers' epilogue: it loads the first stages of item i+1 while the epilogue of item i runs.
+// 384 threads = three warpgroups:
 //   warpgroup 0   : TMA producer (one thread): raw fp32 A and B tiles -> 3-slot shared-memory rings, mbarrier complete_tx
 //   warpgroups 1-2: consumers.  Per k-block of 32 they split the raw tiles into tf32 hi / lo halves written K-major with the
 //                   128B swizzle wgmma reads, release the raw stage to the producer, then each issues the wgmmas of its
@@ -33,6 +37,11 @@
 namespace sfb {
 
 // ------------------------------------------------------------------------------------------------ the kernel
+// register budgets after the producer warpgroup hands its share to the consumers (the item loop's state does not fit
+// beside two 64-register accumulators in 168): 128 x 40 + 256 x 232 = the 384 x 168 the launch gets
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+
 // F16: the fp16-split engine (A K-major with a registered bound |A| <= a_bound[0], B a weight matrix with |w| < 255):
 // A * 2^a_shift is split into fp16 hi + lo * 2^-11 pairs (22 significand bits like the tf32 pair, on the fp16 MMA path at
 // twice the tf32 rate); B = W * 2^kF16WShift in the same form is the weight's registered fp16 twins, which tmap_b (a 3-D
@@ -47,8 +56,9 @@ template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false, bool 
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
-                  const float* __restrict__ a_bound) {
+                  const float* __restrict__ a_bound, unsigned long long* __restrict__ trace) {
     static_assert(!F16 || (!A_MN && SPLIT3), "fp16-split engine: K-major activations, 3-pass");
+    if (trace && threadIdx.x == 0) trace[blockIdx.x * kTraceWords + 8] = tc_now();
     using S = TcSmem<F16>;
     constexpr int KBK = S::KBK;
     constexpr int SA = S::A_STAGES, SB = S::B_STAGES;
@@ -65,7 +75,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int tiles_n = (N + TBN - 1) / TBN;
     const int tiles_per_z = tiles_n * (int)((M + TBM - 1) / TBM);
-    const TileCoord tc = tile_coord(blockIdx.x, tiles_n, tiles_per_z, K, k_chunk, KBK);
+    const int items = tiles_per_z * splits;
 
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap_a) : "memory");
@@ -85,130 +95,157 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // kernel; global memory is only touched after the wait
     pdl_wait();
     pdl_trigger();
+    if (trace && threadIdx.x == 0) trace[blockIdx.x * kTraceWords + 9] = tc_now();
 
+    // g0: stages of the CTA's earlier items -- stage g = g0 + kb uses ring slots g % SA, g % SB, conversion buffer g & 1
     if (warp < 4) {
         // ===================================================== TMA producer
-        if (threadIdx.x == 0) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (threadIdx.x != 0) return;
+        int g0 = 0;
+        for (int item = blockIdx.x; item < items; item += gridDim.x) {
+            const TileCoord tc = tile_coord(item, tiles_n, tiles_per_z, K, k_chunk, KBK);
             for (int kb = 0; kb < tc.num_kb; ++kb) {
                 const int k0 = tc.k_begin + kb * KBK;
-                const int sa = kb % SA, sb = kb % SB;
-                mbar_wait(&empty_a[sa], ((kb / SA) & 1) ^ 1);
+                const int g = g0 + kb;
+                const int sa = g % SA, sb = g % SB;
+                mbar_wait(&empty_a[sa], ((g / SA) & 1) ^ 1);
+                if (trace && kb == 0) trace[item * kTraceWords + 6] = tc_now();
                 mbar_expect_tx(&full_a[sa], S::A_RAW);
                 uint8_t* pa = smem + sa * S::A_RAW;
                 if (A_MN) tma_load_2d(pa, &tmap_a, &full_a[sa], (int)tc.m0, k0);
                 else tma_load_2d(pa, &tmap_a, &full_a[sa], k0, (int)tc.m0);
-                mbar_wait(&empty_b[sb], ((kb / SB) & 1) ^ 1);
+                mbar_wait(&empty_b[sb], ((g / SB) & 1) ^ 1);
                 mbar_expect_tx(&full_b[sb], S::B_SLOT);
                 uint8_t* pb = smem + S::B_RING + sb * S::B_SLOT;
                 if (F16) tma_load_3d(pb, &tmap_b, &full_b[sb], k0, tc.n0, 0);   // [hi | lo] twin tiles
                 else if (B_MN) tma_load_2d(pb, &tmap_b, &full_b[sb], tc.n0, k0);
                 else tma_load_2d(pb, &tmap_b, &full_b[sb], k0, tc.n0);
             }
+            if (trace) trace[item * kTraceWords + 7] = tc_now();
+            g0 += tc.num_kb;
         }
         return;
     }
 
     // ===================================================== consumers
+    setmaxnreg_inc<kConsumerRegs>();
     const int ct = threadIdx.x - 128;          // 0..255
     const int wg = ct >> 7;                    // 64-row half of the tile
 
     // fp16-split engine: binary shift of the A operand from its bound (written by an earlier kernel of the stream)
     const int a_shift = F16 ? f16_shift_for_bound(a_bound[0]) : 0;
     const float a_scale = pow2f_int(a_shift);
-    // split stage kb into conversion buffer kb & 1
-    auto split_stage = [&](int kb) {
-        const int sa = kb % SA, sb = kb % SB;
+    // split stage g into conversion buffer g & 1
+    auto split_stage = [&](int g) {
+        const int sa = g % SA, sb = g % SB;
         const uint8_t* pa = smem + sa * S::A_RAW;
-        uint8_t* cv = conv + (kb & 1) * S::CONV;
-        mbar_wait(&full_a[sa], (kb / SA) & 1);
+        uint8_t* cv = conv + (g & 1) * S::CONV;
+        mbar_wait(&full_a[sa], (g / SA) & 1);
         if constexpr (F16) {
             split_tile_f16<false>(pa, cv, cv + S::A_HALF, ct, a_scale);
         } else {
             split_tile<A_MN, SPLIT3>(pa, cv, cv + S::A_HALF, ct);
-            mbar_wait(&full_b[sb], (kb / SB) & 1);
+            mbar_wait(&full_b[sb], (g / SB) & 1);
             split_tile<B_MN, SPLIT3>(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct);
             mbar_arrive(&empty_b[sb]);
         }
         mbar_arrive(&empty_a[sa]);
         fence_proxy_async_smem();              // generic-proxy writes -> visible to the tensor core (async proxy)
     };
-    float acc[64], cross[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
-    split_stage(0);
-    consumer_sync();
-    for (int kb = 0; kb < tc.num_kb; ++kb) {
-        const int sb = kb % SB;
-        const uint8_t* cv = conv + (kb & 1) * S::CONV;
-        const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
-        const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
-        const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
-        const uint64_t db_hi = make_smem_desc(smem_u32(bt));
-        const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
-        if (F16) mbar_wait(&full_b[sb], (kb / SB) & 1);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < TBK / WG_K; ++k) {
-            const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step (8 tf32 or 16 fp16) inside the swizzle row
-            if constexpr (F16) {
-                wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, 1);
-                wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, 1);
-                wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
-            } else {
-                wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
-            }
-            if (SPLIT3 && !F16) {
-                wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, 1);
-                wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
-            }
+    int g0 = 0;
+    for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const TileCoord tc = tile_coord(item, tiles_n, tiles_per_z, K, k_chunk, KBK);
+        unsigned long long* tr = (trace && ct == 0) ? trace + item * kTraceWords : nullptr;
+        if (tr) {
+            tr[0] = tc_smid();
+            tr[1] = blockIdx.x;
+            tr[2] = tc_now();
+            mbar_wait(&full_a[g0 % SA], (g0 / SA) & 1);   // (split_stage waits again: it passes at once)
+            tr[3] = tc_now();
         }
-        wgmma_commit();
-        if (kb + 1 < tc.num_kb) split_stage(kb + 1);   // overlaps the wgmmas just issued
-        wgmma_wait_all();
-        if (F16) mbar_arrive(&empty_b[sb]);    // the wgmmas are done with the B twin tiles
-        consumer_sync();                       // split kb+1 complete, buffer kb & 1 free for kb+2, in both warpgroups
-    }
-    if (F16) {
-        // (main + cross * 2^-11) * 2^-(operand shifts): exact power-of-two scalings
-        const float out_scale = pow2f_int(-(a_shift + kF16WShift));
+        float acc[64], cross[64];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = fmaf(cross[i], 1.f / 2048.f, acc[i]) * out_scale;
-    } else if (SPLIT3) {
+        for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+        split_stage(g0);
+        consumer_sync();
+        for (int kb = 0; kb < tc.num_kb; ++kb) {
+            const int g = g0 + kb;
+            const int sb = g % SB;
+            const uint8_t* cv = conv + (g & 1) * S::CONV;
+            const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
+            const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
+            const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
+            const uint64_t db_hi = make_smem_desc(smem_u32(bt));
+            const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
+            if (F16) mbar_wait(&full_b[sb], (g / SB) & 1);
+            wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] += cross[i];
-    }
-
-    const int64_t row_base = tc.m0 + wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
-    if constexpr (HEADS) {
-        switch (epi.act) {
-            case SFB200_ACT_ELU: heads_tile<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-            case SFB200_ACT_RELU: heads_tile<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-            case SFB200_ACT_TANH: heads_tile<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-            default: heads_tile<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-        }
-        if (epi.fin_counters) {
-            // last-arriving n-tile CTA of this 128-row block finishes the heads (threadFenceReduction pattern)
-            const int mb = (int)(tc.m0 / TBM);
-            __threadfence();
-            consumer_sync();
-            if (ct == 0) *s_last = (atomicAdd(&epi.fin_counters[mb], 1) == tiles_n - 1) ? 1 : 0;
-            consumer_sync();
-            if (*s_last) {
-                __threadfence();
-                const float pv = epi.fin.pv_scalar ? *epi.fin.pv_scalar : 0.f;
-                const uint64_t offset = epi.fin.offset_host + (epi.fin.offset_dev ? (uint64_t)*epi.fin.offset_dev : 0ull);
-                for (int r = ct >> 5; r < TBM; r += 8) {
-                    const int64_t row = tc.m0 + r;
-                    if (row < M) heads_finish_row(epi.head_part, 2 * tiles_n, M, row, lane, epi.fin, pv, offset);
+            for (int k = 0; k < TBK / WG_K; ++k) {
+                const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step (8 tf32 or 16 fp16) inside the swizzle row
+                if constexpr (F16) {
+                    wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, 1);
+                    wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, 1);
+                    wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
+                } else {
+                    wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
                 }
-                if (ct == 0) epi.fin_counters[mb] = 0;
+                if (SPLIT3 && !F16) {
+                    wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, 1);
+                    wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
+                }
             }
+            wgmma_commit();
+            if (kb + 1 < tc.num_kb) split_stage(g + 1);    // overlaps the wgmmas just issued
+            wgmma_wait_all();
+            if (F16) mbar_arrive(&empty_b[sb]);    // the wgmmas are done with the B twin tiles
+            consumer_sync();                       // split g+1 complete, buffer g & 1 free for g+2, in both warpgroups
         }
-    } else if constexpr (RES) {
-        store_tile_residual(acc, tc, row_base, lane, C, ldc, M, N, epi);
-    } else {
-        float* Cz = C + (splits > 1 ? (int64_t)tc.z * M * ldc : 0);
-        store_tile(acc, tc, row_base, lane, Cz, ldc, M, N, splits == 1 ? epi.mode : 0, epi);
+        g0 += tc.num_kb;
+        if (tr) tr[4] = tc_now();
+        if (F16) {
+            // (main + cross * 2^-11) * 2^-(operand shifts): exact power-of-two scalings
+            const float out_scale = pow2f_int(-(a_shift + kF16WShift));
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = fmaf(cross[i], 1.f / 2048.f, acc[i]) * out_scale;
+        } else if (SPLIT3) {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] += cross[i];
+        }
+
+        const int64_t row_base = tc.m0 + wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
+        if constexpr (HEADS) {
+            switch (epi.act) {
+                case SFB200_ACT_ELU: heads_tile<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
+                case SFB200_ACT_RELU: heads_tile<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
+                case SFB200_ACT_TANH: heads_tile<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
+                default: heads_tile<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
+            }
+            if (epi.fin_counters) {
+                // last-arriving n-tile CTA of this 128-row block finishes the heads (threadFenceReduction pattern)
+                const int mb = (int)(tc.m0 / TBM);
+                __threadfence();
+                consumer_sync();
+                if (ct == 0) *s_last = (atomicAdd(&epi.fin_counters[mb], 1) == tiles_n - 1) ? 1 : 0;
+                consumer_sync();
+                if (*s_last) {
+                    __threadfence();
+                    const float pv = epi.fin.pv_scalar ? *epi.fin.pv_scalar : 0.f;
+                    const uint64_t offset = epi.fin.offset_host + (epi.fin.offset_dev ? (uint64_t)*epi.fin.offset_dev : 0ull);
+                    for (int r = ct >> 5; r < TBM; r += 8) {
+                        const int64_t row = tc.m0 + r;
+                        if (row < M) heads_finish_row(epi.head_part, 2 * tiles_n, M, row, lane, epi.fin, pv, offset);
+                    }
+                    if (ct == 0) epi.fin_counters[mb] = 0;
+                }
+            }
+        } else if constexpr (RES) {
+            store_tile_residual(acc, tc, row_base, lane, C, ldc, M, N, epi);
+        } else {
+            float* Cz = C + (splits > 1 ? (int64_t)tc.z * M * ldc : 0);
+            store_tile(acc, tc, row_base, lane, Cz, ldc, M, N, splits == 1 ? epi.mode : 0, epi);
+        }
+        if (tr) tr[5] = tc_now();
     }
 }
 
@@ -288,6 +325,10 @@ bool f16_check_enabled() {
     return v == 1;
 }
 
+// debug trace of the calling host thread (sfb200_gemm_set_trace): the wgmma launches that follow stamp into it
+static thread_local unsigned long long* g_gemm_trace = nullptr;
+static thread_local int64_t g_gemm_trace_words = 0;
+
 static bool operand_ok(const float* p, int64_t ld) {
     return ((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && (ld % 4 == 0) && ld > 0;
 }
@@ -297,16 +338,29 @@ static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int
                      int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr) {
     auto kern = gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES>;
     constexpr int smem = TcSmem<F16>::TOTAL;
-    static bool attr_set = false;
-    if (!attr_set) {
+    static int ctas_per_sm = 0;   // of this instantiation: 1 (shared memory), asked rather than assumed
+    if (!ctas_per_sm) {
         SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr_set = true;
+        SFB_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, kern, TC_THREADS, (size_t)smem));
+        SFB_CHECK_ARG(ctas_per_sm > 0, "gemm_wgmma_kernel does not fit on this device");
     }
-    const int64_t tiles = ceil_div(N, TBN) * ceil_div(M, TBM) * splits;
-    SFB_CUDA_OK(launch_pdl(kern, dim3((unsigned)tiles), dim3(TC_THREADS), (size_t)smem, st, ta, tb, C, ldc, M, N, K,
-                           k_chunk, splits, epi, a_bound));
+    const int64_t items = ceil_div(N, TBN) * ceil_div(M, TBM) * splits;
+    const int64_t resident = (int64_t)ctas_per_sm * sm_count();
+    SFB_CHECK_ARG(!g_gemm_trace || items * kTraceWords <= g_gemm_trace_words,
+                  "gemm trace buffer too small: %lld work items need %lld words", (long long)items,
+                  (long long)(items * kTraceWords));
+    SFB_CUDA_OK(launch_pdl(kern, dim3((unsigned)(items < resident ? items : resident)), dim3(TC_THREADS), (size_t)smem, st,
+                           ta, tb, C, ldc, M, N, K, k_chunk, splits, epi, a_bound, g_gemm_trace));
     SFB_LAUNCH_OK();
     return 0;
+}
+
+// k of one split-K slice: whole stages; *splits becomes the slices that leaves (none of them empty)
+static int split_k_chunk(int K, int* splits) {
+    if (*splits <= 1) return K;
+    const int k_chunk = (int)(ceil_div(ceil_div(K, *splits), TBK) * TBK);
+    *splits = (int)ceil_div(K, k_chunk);
+    return k_chunk;
 }
 
 // C[M,N] = epi( sum_k A(m,k) B(n,k) ). Returns SFB_TC_UNSUPPORTED when the shape/alignment is not covered.
@@ -348,11 +402,7 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
     else ok = ok && make_tmap(&tb, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, TBK, TBN);
     if (!ok) return SFB_TC_UNSUPPORTED;
 
-    int k_chunk = K;
-    if (splits > 1) {
-        k_chunk = (int)(ceil_div(ceil_div(K, splits), TBK) * TBK);
-        splits = (int)ceil_div(K, k_chunk);
-    }
+    const int k_chunk = split_k_chunk(K, &splits);
     if (splits > 1 && !ws) return SFB_TC_UNSUPPORTED;
     float* out = splits > 1 ? ws : C;
     const int64_t ld_out = splits > 1 ? N : ldc;
@@ -441,3 +491,21 @@ int tc_linear_backward(const float* dz, int64_t lddz, const float* x, int64_t ld
 }  // namespace sfb
 
 extern "C" int sfb200_tc_available(void) { return sfb::tc_init() ? 1 : 0; }
+
+extern "C" int sfb200_gemm_work_item(int64_t item, int64_t M, int N, int K, int splits, int64_t* out) {
+    SFB_CHECK_ARG(out && M > 0 && N > 0 && K > 0 && splits > 0, "gemm_work_item: bad arguments");
+    const int k_chunk = sfb::split_k_chunk(K, &splits);
+    const int tiles_n = (int)sfb::ceil_div(N, sfb::TBN);
+    const int tiles_per_z = tiles_n * (int)sfb::ceil_div(M, sfb::TBM);
+    SFB_CHECK_ARG(item >= 0 && item < (int64_t)tiles_per_z * splits, "gemm_work_item: item out of range");
+    const sfb::TileCoord t = sfb::tile_coord((int)item, tiles_n, tiles_per_z, K, k_chunk, sfb::TBK);
+    out[0] = t.m0, out[1] = t.n0, out[2] = t.k_begin, out[3] = t.num_kb * sfb::TBK, out[4] = t.z;
+    out[5] = (int64_t)tiles_per_z * splits;
+    return 0;
+}
+
+extern "C" int sfb200_gemm_set_trace(void* trace_dev, int64_t n_words) {
+    sfb::g_gemm_trace = (unsigned long long*)trace_dev;
+    sfb::g_gemm_trace_words = trace_dev ? n_words : 0;
+    return 0;
+}

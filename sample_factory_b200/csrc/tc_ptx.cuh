@@ -69,6 +69,19 @@ __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_grou
 // all but the most recently committed wgmma group of this warpgroup have completed
 __device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
+// gemm_wgmma_kernel's debug trace (sfb200_gemm_set_trace): %globaltimer in ns, %smid, 16 words per work item
+constexpr int kTraceWords = 16;
+__device__ __forceinline__ unsigned long long tc_now() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ uint32_t tc_smid() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+    return r;
+}
+
 // warpgroup-wide register budget hand-over (every warp of the warpgroup executes it)
 template <int REGS>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }

@@ -139,7 +139,9 @@ struct TileCoord {
     int n0, k_begin, num_kb, z;
 };
 
-__device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_n, int tiles_per_z, int K, int k_chunk, int kbk = TBK) {
+// work item -> tile and split-K slice: n fastest, then m, then the slice, so the CTAs that run at the same time (consecutive
+// items) share their A rows and the whole of B in L2
+__host__ __device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_n, int tiles_per_z, int K, int k_chunk, int kbk = TBK) {
     TileCoord t;
     t.z = tile / tiles_per_z;
     const int r = tile - t.z * tiles_per_z;

@@ -952,6 +952,31 @@ def linear_backward_workspace_bytes(M: int, N: int, K: int) -> int:
     return lib().query("sfb200_linear_backward_workspace_bytes", M, N, K)
 
 
+def linear_backward_splits(M: int, N: int, K: int, sm_count: int = 0) -> int:
+    """split-K slices linear_backward gives dW [N, K] on a device of sm_count SMs (0: the current device)"""
+    return lib().query("sfb200_linear_backward_splits", M, N, K, sm_count)
+
+
+def gemm_work_item(item: int, M: int, N: int, K: int, splits: int) -> Tuple[int, int, int, int, int, int]:
+    """(first row, first column, first k, k covered, slice, number of items) of work item `item` of the wgmma GEMM
+    C [M, N] over K in `splits` slices (tf32 form); CTA b of a grid of g runs items b, b + g, ..."""
+    out = (ctypes.c_int64 * 6)()
+    lib().call("sfb200_gemm_work_item", item, M, N, K, splits, ctypes.addressof(out))
+    return tuple(out)
+
+
+GEMM_TRACE_WORDS = 16   # int64 words per work item in a set_gemm_trace buffer (include/sfb200.h)
+
+
+def set_gemm_trace(trace: Optional[Tensor]) -> None:
+    """int64 device buffer the wgmma GEMMs this thread launches next stamp into (sfb200_gemm_set_trace); None: off"""
+    if trace is None:
+        lib().call("sfb200_gemm_set_trace", None, 0)
+    else:
+        assert trace.dtype == torch.int64 and trace.is_contiguous()
+        lib().call("sfb200_gemm_set_trace", trace.data_ptr(), trace.numel())
+
+
 def linear_backward(dz: Tensor, x: Tensor, W: Tensor, act_prev: int, dW: Optional[Tensor], dx: Optional[Tensor],
                     db_prev: Optional[Tensor], engine: int, workspace: Tensor) -> None:
     M, N = dz.shape
