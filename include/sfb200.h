@@ -454,7 +454,7 @@ int sfb200_vtrace(const float* ratio, const float* values, const float* rewards,
 #define SFB200_LS_KL_OLD_MAX 8
 #define SFB200_LS_ENTROPY_MEAN 9
 #define SFB200_LS_RATIO_MEAN_ABS_DEV 10 /* mean |1 - ratio| over valid */
-#define SFB200_LS_RATIO_MIN 11
+#define SFB200_LS_RATIO_MIN 11      /* over valid samples; +inf with none (KL_OLD_MAX and RATIO_MAX: -inf) */
 #define SFB200_LS_RATIO_MAX 12
 #define SFB200_LS_FRACTION_CLIPPED 13
 #define SFB200_LS_VALUE_MEAN 14

@@ -127,8 +127,10 @@ __global__ void __launch_bounds__(256) adv_stats_partial_kernel(const float* __r
 
 __device__ __forceinline__ void adv_finalize(double c, double s, double ss, double* stats) {
     const double mean = c > 0.0 ? s / c : 0.0;
-    // torch.std_mean default: unbiased (n-1); n == 1 gives NaN in torch too
-    const double var = (ss - s * mean) / (c - 1.0);
+    // torch.std_mean default: unbiased (n-1).  With one valid sample (or none) torch gives NaN, which would reach every
+    // weight; here the stddev is 0, clamped to 1e-7 by the loss, so the normalised advantage and the policy gradient are
+    // 0 while the value, exploration and KL terms still train (a deliberate deviation, DESIGN section 7)
+    const double var = c > 1.0 ? (ss - s * mean) / (c - 1.0) : 0.0;
     stats[SFB200_LS_NUM_VALID] = c;
     stats[SFB200_LS_ADV_MEAN] = (double)(float)mean;
     stats[SFB200_LS_ADV_STD] = (double)(float)sqrt(var > 0.0 ? var : 0.0);

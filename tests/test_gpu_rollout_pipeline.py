@@ -58,14 +58,15 @@ def _state(sampler, traj, env):
 
 
 def _check(obs_dim=64, hidden=512, num_actions=8, N=512, T=4, rollouts=2, train=False, graph=False, form=None,
-           normalize=True):
+           normalize=True, nonlinearity="elu"):
     """rollouts of both samplers compared after each one (train: learner.train on the persistent trajectories in between,
     so the weights, their fp16 twins and the h1 bound change); form: the operand form the kernel must have taken;
     normalize=False: a model without fp16 twins (every GEMM of both paths in the tf32 form)"""
     from sample_factory_b200 import ops
 
     ocfg = O.OracleCfg(obs_dim=obs_dim, num_actions=num_actions, encoder_mlp_layers=[hidden, hidden], rollout=T,
-                       recurrence=1, batch_size=N * T // 2, num_batches_per_epoch=2, normalize_input=normalize)
+                       recurrence=1, batch_size=N * T // 2, num_batches_per_epoch=2, normalize_input=normalize,
+                       nonlinearity=nonlinearity)
     model, learner, (ss, ts, es), (sp, tp, ep) = _pair(ocfg, N, seed=3 + hidden + obs_dim + N + T, graph=graph)
     ss.reset()
     sp.reset()
@@ -96,6 +97,21 @@ def test_bench_shape_tf32_form():
     """SFB200_TC_F16=0 is read once per process: the same check in a fresh one"""
     code = ("import sys; sys.path.insert(0, sys.argv[1]); from tests.test_gpu_rollout_pipeline import _check; "
             "_check(N=4096, T=32, form=0); print('ok')")
+    env = dict(os.environ, SFB200_TC_F16="0")
+    res = subprocess.run([sys.executable, "-c", code, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
+    assert res.returncode == 0 and "ok" in res.stdout, res.stdout[-3000:] + res.stderr[-3000:]
+
+
+@pytest.mark.parametrize("form", ["fp16", "tf32"])
+@pytest.mark.parametrize("act", ["relu", "tanh"])
+def test_activations(act, form):
+    """rollout_mlp2_tape_kernel<ACT, F16> for ReLU (unbounded: the fp16 form splits h1 by a bound that grows with the
+    weights) and tanh (h1 bound capped at 1 by linear_out_bound); the tf32 form in a fresh process, as above"""
+    if form == "fp16":
+        _check(N=1000, T=5, form=1, nonlinearity=act)
+        return
+    code = ("import sys; sys.path.insert(0, sys.argv[1]); from tests.test_gpu_rollout_pipeline import _check; "
+            f"_check(N=1000, T=5, form=0, nonlinearity={act!r}); print('ok')")
     env = dict(os.environ, SFB200_TC_F16="0")
     res = subprocess.run([sys.executable, "-c", code, ROOT], cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
     assert res.returncode == 0 and "ok" in res.stdout, res.stdout[-3000:] + res.stderr[-3000:]
