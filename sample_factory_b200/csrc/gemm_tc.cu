@@ -207,19 +207,23 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             // (main + cross * 2^-11) * 2^-(operand shifts): exact power-of-two scalings
             const float out_scale = pow2f_int(-(a_shift + kF16WShift));
 #pragma unroll
-            for (int i = 0; i < 64; ++i) acc[i] = fmaf(cross[i], 1.f / 2048.f, acc[i]) * out_scale;
+            // (a rounded product of its own: the straight-line epilogues must not contract it with their bias add)
+            for (int i = 0; i < 64; ++i) acc[i] = __fmul_rn(fmaf(cross[i], 1.f / 2048.f, acc[i]), out_scale);
         } else if (SPLIT3) {
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] += cross[i];
         }
+        if (tr) tr[10] = tc_now_after(acc[63]);
 
+        // the epilogue's mode and activation are chosen once per item; whole tiles (all of them at the learner's shapes)
+        // then run straight-line code
         const int64_t row_base = tc.m0 + wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
         if constexpr (HEADS) {
             switch (epi.act) {
-                case SFB200_ACT_ELU: heads_tile<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-                case SFB200_ACT_RELU: heads_tile<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-                case SFB200_ACT_TANH: heads_tile<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
-                default: heads_tile<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, N, epi); break;
+                case SFB200_ACT_ELU: heads_tile<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
+                case SFB200_ACT_RELU: heads_tile<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
+                case SFB200_ACT_TANH: heads_tile<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
+                default: heads_tile<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
             }
             if (epi.fin_counters) {
                 // last-arriving n-tile CTA of this 128-row block finishes the heads (threadFenceReduction pattern)
@@ -240,10 +244,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 }
             }
         } else if constexpr (RES) {
-            store_tile_residual(acc, tc, row_base, lane, C, ldc, M, N, epi);
+            if (tile_is_whole(tc, TBM, C, ldc, M, N, epi.aux, epi.ld_aux))
+                store_tile_whole<3, SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, epi, tr);
+            else
+                store_tile_residual(acc, tc, row_base, lane, C, ldc, M, N, epi);
         } else {
             float* Cz = C + (splits > 1 ? (int64_t)tc.z * M * ldc : 0);
-            store_tile(acc, tc, row_base, lane, Cz, ldc, M, N, splits == 1 ? epi.mode : 0, epi);
+            const int mode = splits == 1 ? epi.mode : 0;
+            if (!tile_is_whole(tc, TBM, Cz, ldc, M, N, mode == 2 ? epi.aux : nullptr, mode == 2 ? epi.ld_aux : 0))
+                store_tile(acc, tc, row_base, lane, Cz, ldc, M, N, mode, epi);
+            else if (mode == 1)
+                store_tile_whole_act<1>(acc, tc, row_base, lane, Cz, ldc, epi, tr);
+            else if (mode == 2)
+                store_tile_whole_act<2>(acc, tc, row_base, lane, Cz, ldc, epi, tr);
+            else
+                store_tile_whole<0, SFB200_ACT_NONE>(acc, tc, row_base, lane, Cz, ldc, epi, tr);
         }
         if (tr) tr[5] = tc_now();
     }

@@ -76,6 +76,21 @@ __device__ __forceinline__ unsigned long long tc_now() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
+// the time at which `dep` is in its register: the timer read is predicated on a test of dep, so the stamp waits for the
+// load (or the math) that produces it.  (0 for a NaN.)
+__device__ __forceinline__ unsigned long long tc_now_after(float dep) {
+    unsigned long long t;
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.num.f32 p, %1, %1;\n"
+        "mov.u64 %0, 0;\n"
+        "@p mov.u64 %0, %%globaltimer;\n"
+        "}\n"
+        : "=l"(t)
+        : "f"(dep));
+    return t;
+}
 __device__ __forceinline__ uint32_t tc_smid() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(r));

@@ -156,6 +156,8 @@ __host__ __device__ __forceinline__ TileCoord tile_coord(int tile, int tiles_n, 
 
 // Epilogue of one warpgroup's 64 x 128 accumulator: pair j (j = 0..31) of a thread is d[2j], d[2j+1] = columns
 // n0 + 8*(j/2) + 2*(lane%4) + {0, 1} of row  row_base + 8*(j%2).
+// store_tile guards every element and takes the mode at run time: the epilogue of ragged tiles (and of every tile of the
+// rollout's tf32 form).  Whole tiles of the GEMM engine take store_tile_whole below.
 __device__ __forceinline__ void store_tile(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
                                            int64_t ldc, int64_t M, int N, int mode, const TcEpilogue& epi) {
     const bool v2 = (ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(C) & 7u) == 0);
@@ -184,6 +186,78 @@ __device__ __forceinline__ void store_tile(const float (&acc)[64], const TileCoo
     }
 }
 
+// The tile lies wholly inside C (and inside aux, when the epilogue reads it) and every pair of a thread is one aligned
+// float2: the whole-tile epilogues below need no per-element guard.  rows = rows of the CTA's tile from tc.m0.
+__device__ __forceinline__ bool tile_is_whole(const TileCoord& tc, int rows, const float* C, int64_t ldc, int64_t M, int N,
+                                              const float* aux = nullptr, int64_t ld_aux = 0) {
+    return tc.m0 + rows <= M && tc.n0 + TBN <= N && ldc % 2 == 0 && ld_aux % 2 == 0 &&
+           ((reinterpret_cast<uintptr_t>(C) | reinterpret_cast<uintptr_t>(aux)) & 7u) == 0;
+}
+
+// A thread's 32 bias values (columns n0 + 8*c + 2*(lane%4) + {0, 1}, c = 0..15) in one batch of loads
+__device__ __forceinline__ void load_bias_pairs(const float* bias, int n0, int lane, float (&b)[32]) {
+    const float* p = bias + n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+        b[2 * c] = __ldg(p + 8 * c);
+        b[2 * c + 1] = __ldg(p + 8 * c + 1);
+    }
+}
+
+// store_tile for a whole tile (tile_is_whole) with the mode (TcEpilogue::mode, 3 = residual) and the activation fixed at
+// compile time: straight-line code, every global load of the thread (bias, the 32 float2 of aux) issued before the first
+// multiply, then 32 float2 stores.  Per element the expressions are store_tile's / store_tile_residual's, so the bits are
+// theirs.  tr: the traced thread's stamps (word 11: the loads have landed), else NULL.
+template <int MODE, int ACT>
+__device__ __forceinline__ void store_tile_whole(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane,
+                                                 float* C, int64_t ldc, const TcEpilogue& epi, unsigned long long* tr) {
+    const int nq = tc.n0 + 2 * (lane & 3);
+    float b[32];
+    float2 h[32];
+    if (MODE == 1 || MODE == 3) {
+        if (epi.bias) {
+            load_bias_pairs(epi.bias, tc.n0, lane, b);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) b[i] = 0.f;
+        }
+    }
+    if (MODE == 2 || MODE == 3) {
+        const float* ap = epi.aux + row_base * epi.ld_aux + nq;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) h[j] = *reinterpret_cast<const float2*>(ap + (j & 1) * 8 * epi.ld_aux + 8 * (j >> 1));
+    }
+    if (tr) tr[11] = tc_now_after(MODE == 0 ? 0.f : MODE == 1 ? b[31] : h[31].y);
+    float* cp = C + row_base * ldc + nq;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        float v0 = acc[2 * j], v1 = acc[2 * j + 1];
+        if (MODE == 1) {
+            v0 = act_fwd_fast(__fadd_rn(v0, b[j & ~1]), ACT);
+            v1 = act_fwd_fast(__fadd_rn(v1, b[j | 1]), ACT);
+        } else if (MODE == 2) {
+            v0 *= act_bwd_from_out(h[j].x, ACT);
+            v1 *= act_bwd_from_out(h[j].y, ACT);
+        } else if (MODE == 3) {
+            v0 = __fadd_rn(__fadd_rn(v0, b[j & ~1]), h[j].x);
+            v1 = __fadd_rn(__fadd_rn(v1, b[j | 1]), h[j].y);
+        }
+        *reinterpret_cast<float2*>(cp + (j & 1) * 8 * ldc + 8 * (j >> 1)) = make_float2(v0, v1);
+    }
+}
+
+// store_tile_whole with the activation chosen once per tile
+template <int MODE>
+__device__ __forceinline__ void store_tile_whole_act(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane,
+                                                     float* C, int64_t ldc, const TcEpilogue& epi, unsigned long long* tr) {
+    switch (epi.act) {
+        case SFB200_ACT_ELU: store_tile_whole<MODE, SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, epi, tr); break;
+        case SFB200_ACT_RELU: store_tile_whole<MODE, SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, epi, tr); break;
+        case SFB200_ACT_TANH: store_tile_whole<MODE, SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, epi, tr); break;
+        default: store_tile_whole<MODE, SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, epi, tr); break;
+    }
+}
+
 // Residual epilogue (a ResBlock's second conv plus its identity path, model/encoder.py:166-169): C = (acc + bias[n]) +
 // aux[m, n].  A separate instantiation (gemm_wgmma_kernel<..., RES = true>), so the other epilogues keep their code.
 __device__ __forceinline__ void store_tile_residual(const float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane,
@@ -204,51 +278,68 @@ __device__ __forceinline__ void store_tile_residual(const float (&acc)[64], cons
 // actor_critic.py:171-186): y = act(acc + bias) is formed in registers, optionally stored, and contracted with the (A+1)
 // head weight rows -- the separate heads kernel's re-read of y disappears.  Per 64-column half of the tile the four
 // threads of a quad hold a row's 64 values; a fixed-order quad reduction gives the partial.  Two partials per tile.
+// Loads come in batches ahead of the math that uses them: the thread's 32 bias values once, then per (half, head row) the
+// eight float2 of the weight row that both of the thread's rows (rs = 0, 1) multiply.  Each partial keeps its order of
+// operations: FMAs over jj = 0..7, then the quad sum over lanes ^ 1, ^ 2.
+// tr: the traced thread's stamps (11: bias landed, 12: y stored, 13: partials stored), else NULL.
 template <int ACT>
 __device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
-                                           int64_t ldc, int64_t M, int N, const TcEpilogue& epi) {
+                                           int64_t ldc, int64_t M, int N, const TcEpilogue& epi,
+                                           unsigned long long* tr = nullptr) {
     constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
+    const int nq = tc.n0 + 2 * (lane & 3);
+    float b[32];
+    load_bias_pairs(epi.bias, tc.n0, lane, b);
+    if (tr) tr[11] = tc_now_after(b[31]);
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
-        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
-        acc[2 * j] = act_fwd_ct<ACT>(acc[2 * j] + epi.bias[n]);
-        acc[2 * j + 1] = act_fwd_ct<ACT>(acc[2 * j + 1] + epi.bias[n + 1]);
+        acc[2 * j] = act_fwd_ct<ACT>(acc[2 * j] + b[j & ~1]);
+        acc[2 * j + 1] = act_fwd_ct<ACT>(acc[2 * j + 1] + b[j | 1]);
         const int64_t m = row_base + 8 * (j & 1);
-        if (C && m < M) *reinterpret_cast<float2*>(C + m * ldc + n) = make_float2(acc[2 * j], acc[2 * j + 1]);
+        if (C && m < M) *reinterpret_cast<float2*>(C + m * ldc + nq + 8 * (j >> 1)) = make_float2(acc[2 * j], acc[2 * j + 1]);
     }
+    if (tr) tr[12] = tc_now_after(acc[63]);
     const int p0 = (tc.n0 / TBN) * 2;
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
+        float hp[2][kHeadAP];
 #pragma unroll
-        for (int rs = 0; rs < 2; ++rs) {
-            float hp[kHeadAP];
+        for (int a = 0; a < kHeadAP; ++a) {
+            float s[2] = {0.f, 0.f};
+            if (a <= epi.head_A) {
+                const float* w = (a == 0 ? epi.head_wv : epi.head_wa + (int64_t)(a - 1) * N) + nq + 64 * half;
+                float2 wv[JP / 2];
 #pragma unroll
-            for (int a = 0; a < kHeadAP; ++a) {
-                float s = 0.f;
-                if (a <= epi.head_A) {
-                    const float* w = a == 0 ? epi.head_wv : epi.head_wa + (int64_t)(a - 1) * N;
+                for (int jj = 0; jj < JP / 2; ++jj) wv[jj] = __ldg(reinterpret_cast<const float2*>(w + 8 * jj));
 #pragma unroll
-                    for (int jj = 0; jj < JP / 2; ++jj) {
+                for (int jj = 0; jj < JP / 2; ++jj) {
+#pragma unroll
+                    for (int rs = 0; rs < 2; ++rs) {
                         const int j = JP * half + 2 * jj + rs;
-                        const int n = tc.n0 + 8 * (j >> 1) + 2 * (lane & 3);
-                        const float2 wv = __ldg(reinterpret_cast<const float2*>(w + n));
-                        s = fmaf(acc[2 * j], wv.x, s);
-                        s = fmaf(acc[2 * j + 1], wv.y, s);
+                        s[rs] = fmaf(acc[2 * j], wv[jj].x, s[rs]);
+                        s[rs] = fmaf(acc[2 * j + 1], wv[jj].y, s[rs]);
                     }
                 }
-                s += __shfl_xor_sync(0xffffffffu, s, 1);
-                s += __shfl_xor_sync(0xffffffffu, s, 2);
-                hp[a] = s;
             }
+#pragma unroll
+            for (int rs = 0; rs < 2; ++rs) {
+                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 1);
+                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 2);
+                hp[rs][a] = s[rs];
+            }
+        }
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
             const int64_t m = row_base + 8 * rs;
             if ((lane & 3) == 0 && m < M) {
                 float4* dst = reinterpret_cast<float4*>(epi.head_part + ((int64_t)(p0 + half) * M + m) * kHeadPad);
-                dst[0] = make_float4(hp[0], hp[1], hp[2], hp[3]);
-                dst[1] = make_float4(hp[4], hp[5], hp[6], hp[7]);
-                dst[2] = make_float4(hp[8], 0.f, 0.f, 0.f);
+                dst[0] = make_float4(hp[rs][0], hp[rs][1], hp[rs][2], hp[rs][3]);
+                dst[1] = make_float4(hp[rs][4], hp[rs][5], hp[rs][6], hp[rs][7]);
+                dst[2] = make_float4(hp[rs][8], 0.f, 0.f, 0.f);
             }
         }
     }
+    if (tr) tr[13] = tc_now();
 }
 
 }  // namespace sfb

@@ -3,9 +3,12 @@
 
 Switches the kernel's trace on (sfb200_gemm_set_trace: one consumer thread and the producer thread of every CTA stamp
 %globaltimer and %smid per work item) and runs, at M = 32768: the layer-2 forward with the heads folded in and dX
-(fp16 form, 512 x 512), dW2 (512 x 512) and dW1 (512 x 64) (tf32 form, split-K).  Prints per GEMM: CTAs, work items and
+(fp16 form, 512 x 512), the layer-1 forward (fp16 form, 512 x 64: one stage per item, so nearly all epilogue), dW2
+(512 x 512) and dW1 (512 x 64) (tf32 form, split-K).  Prints per GEMM: CTAs, work items and
 items per CTA, the mean microseconds of an item split into fill (item begun -> its first stage landed), mainloop and
-epilogue, the once-per-CTA setup (kernel entry -> barriers initialised and the programmatic-dependency wait passed), how
+epilogue, the epilogue split at the stamps inside it (a library without them leaves the words zero and the parts
+unprinted): accumulators combined, the epilogue's batch of global loads landed, and then either the stores issued, or for
+the fused heads: activated row stored, head partials stored, heads finished; the once-per-CTA setup (kernel entry -> barriers initialised and the programmatic-dependency wait passed), how
 far ahead of the consumers the producer issued an item's first load, and the kernel's span against the busiest CTA's sum
 of phases.  The stamps cost a few stores per item; the times are a profile, not a benchmark.
 
@@ -25,6 +28,20 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 M, H, OBS, A = 32768, 512, 64, 8
+
+
+def epilogue_parts(t, us):
+    """the epilogue between its stamps (words 10-13; 4 and 5 are its ends), whole-tile items only"""
+    t = t[(t[:, 10] != 0) & (t[:, 11] != 0)]
+    if t.shape[0] == 0:
+        return None
+    parts = {"combine": us(t[:, 10] - t[:, 4]), "loads": us(t[:, 11] - t[:, 10])}
+    if bool((t[:, 13] != 0).all()):
+        parts.update({"act_store": us(t[:, 12] - t[:, 11]), "head_partials": us(t[:, 13] - t[:, 12]),
+                      "heads_finish": us(t[:, 5] - t[:, 13])})
+    else:
+        parts["math_store"] = us(t[:, 5] - t[:, 11])
+    return parts
 
 
 def summarize(t):
@@ -50,6 +67,7 @@ def summarize(t):
         "fill_first_item_us": us(fill[first]),
         "fill_later_items_us": us(fill[later]) if bool(later.any()) else None,
         "mainloop_us": us(main), "epilogue_us": us(epi),
+        "epilogue_parts_us": epilogue_parts(t, us),
         "item_us": us(fill + main + epi),
         "producer_lead_us": us((t[:, 2] - t[:, 6])[later]) if bool(later.any()) else None,
         "kernel_span_us": float(t[:, 5].max() - t[:, 8][first].min()) / 1e3,
@@ -81,6 +99,8 @@ def main():
     flat = rnd(H * H) / math.sqrt(H)
     W2 = flat.view(H, H)
     W1 = (rnd(H, OBS) / math.sqrt(OBS)).contiguous()
+    flat1 = W1.view(-1)
+    b1 = rnd(H) * 0.1
     b2, Wv, Wa = rnd(H) * 0.1, rnd(H) * 0.1, (rnd(A, H) * 0.1).contiguous()
     h1, x0 = torch.nn.functional.elu(rnd(M, H)), rnd(M, OBS)
     dz = rnd(M, H) / M
@@ -92,15 +112,20 @@ def main():
     twinsT = torch.empty(2 * H * H, dtype=torch.float16, device=dev)
     ops.register_f16_twins(flat, twins)
     ops.register_f16_transposed(W2, twinsT)
-    bounds = [torch.full((1,), float(t.abs().max()), device=dev) for t in (h1, dz)]
+    twins1 = torch.empty(2 * H * OBS, dtype=torch.float16, device=dev)
+    ops.register_f16_twins(flat1, twins1)
+    bounds = [torch.full((1,), float(t.abs().max()), device=dev) for t in (h1, dz, x0)]
     ops.register_operand_bound(h1, bounds[0])
     ops.register_operand_bound(dz, bounds[1])
+    ops.register_operand_bound(x0, bounds[2])
 
     gemms = [
         ("forward + heads, fp16 form <0,0,1,1,1,0> [32768 x 512 x 512]",
          lambda: ops.linear_act_heads_forward(h1, W2, b2, y, ops.ACT["elu"], eng, Wv, Wa, part)),
         ("dX, fp16 form <0,1,1,0,1,0> [32768 x 512 x 512]",
          lambda: ops.linear_backward(dz, h1, W2, ops.ACT["elu"], None, dx, None, eng, ws)),
+        ("layer-1 forward, fp16 form <0,0,1,0,1,0> [32768 x 512 x 64]",
+         lambda: ops.linear_act_forward(x0, W1, b1, y, ops.ACT["elu"], eng)),
         ("dW2, tf32 form, split-K <1,1,1,0,0,0> [512 x 512, k = 32768]",
          lambda: ops.linear_backward(dz, h1, W2, ops.ACT["elu"], dW2, None, None, eng, ws)),
         ("dW1, tf32 form, split-K <1,1,1,0,0,0> [512 x 64, k = 32768]",
@@ -123,7 +148,10 @@ def main():
                 torch.cuda.synchronize()
                 rows.append(summarize(trace.cpu().view(-1, ops.GEMM_TRACE_WORDS)))
             ops.set_gemm_trace(None)
-            mean = {k: (None if rows[0][k] is None else round(sum(r[k] for r in rows) / len(rows), 2)) for k in rows[0]}
+            avg = lambda vs: None if vs[0] is None else round(sum(vs) / len(vs), 2)
+            mean = {k: avg([r[k] for r in rows]) for k in rows[0] if k != "epilogue_parts_us"}
+            parts = rows[0]["epilogue_parts_us"]
+            mean["epilogue_parts_us"] = parts and {k: avg([r["epilogue_parts_us"][k] for r in rows]) for k in parts}
             result["gemms"][name] = mean
             print(name)
             print(f"  {mean['items']:.0f} items on {mean['ctas']:.0f} CTAs ({mean['sms']:.0f} SMs), at most "
@@ -131,12 +159,16 @@ def main():
             print(f"  per CTA: setup {mean['setup_us']};  per item: fill {mean['fill_first_item_us']} (first) / "
                   f"{mean['fill_later_items_us']} (later), mainloop {mean['mainloop_us']}, epilogue {mean['epilogue_us']}, "
                   f"total {mean['item_us']}")
+            if mean["epilogue_parts_us"]:
+                print("  epilogue: " + ", ".join(f"{k} {v}" for k, v in mean["epilogue_parts_us"].items()))
             print(f"  producer issued a later item's first load {mean['producer_lead_us']} before the consumers began it")
             print(f"  kernel span {mean['kernel_span_us']} vs busiest CTA's sum {mean['busiest_cta_sum_us']}")
     finally:
         ops.set_gemm_trace(None)
         ops.unregister_operand_bound(h1)
         ops.unregister_operand_bound(dz)
+        ops.unregister_operand_bound(x0)
+        ops.unregister_f16_twins(flat1)
         ops.unregister_f16_transposed(W2)
         ops.unregister_f16_twins(flat)
     os.makedirs(args.out, exist_ok=True)
