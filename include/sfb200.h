@@ -73,9 +73,15 @@ int sfb200_linear_out_bound(const float* W, const float* b, int N, int K, const 
                             int act, void* stream);
 /* bound of the gradient sfb200_heads_backward writes for the last hidden layer (the activation operand of dX):
  * max_m (|dvalues[m]| + sum_a |dlogits[m][a]|) * max(|Wv|_inf, |Wa|_inf); act' <= 1 for every supported activation.
- * out_bound_dev: THREE 32-bit words [bound, scratch, counter], the last two zero on entry and on return. */
+ * out_bound_dev: THREE 32-bit words [bound, scratch, counter], the last two zero on entry and on return.
+ * With n_chain > 0 it also bounds the gradients of the n_chain hidden layers below (the operands of their dW / dX):
+ * chain_dev[4 i] = chain_dev[4 (i+1)] * factors_dev[4 (i+1)] for i = n_chain-1 .. 0, starting from the bound above, where
+ * factors_dev[4 j] is layer j's sfb200_linear_in_grad_bound. */
 int sfb200_heads_dz_bound(const float* dlogits, const float* dvalues, int64_t rows, int A, const float* Wv, const float* Wa,
-                          int H, float* out_bound_dev, void* stream);
+                          int H, float* out_bound_dev, const float* factors_dev, float* chain_dev, int n_chain, void* stream);
+/* max_k sum_n |W[n][k]| of a weight matrix W[N][K] (a hair of slack added): |dz . W| <= bound(dz) times it.  out_dev: FOUR
+ * 32-bit words [factor, scratch, counter, -], the middle two zero on entry and on return. */
+int sfb200_linear_in_grad_bound(const float* W, int N, int K, float* out_dev, void* stream);
 /* total number of CUDA kernels this library has launched (or recorded into a stream capture) in this process */
 uint64_t sfb200_launch_count(void);
 

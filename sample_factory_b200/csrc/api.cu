@@ -113,14 +113,48 @@ __global__ void __launch_bounds__(256) linear_out_bound_kernel(const float* __re
     }
 }
 
+// Gradient factor of a layer: max_k sum_n |W[n][k]|, so that |dz_in[m][k]| = |sum_n dz_out[m][n] W[n][k]| * |act'| <=
+// bound(dz_out) * factor (act' <= 1).  32 columns per block, each summed over the rows in a fixed order by 8 row phases;
+// block maxima meet as in linear_out_bound_kernel.  out = [factor, scratch bits, arrival counter, -].
+__global__ void __launch_bounds__(256) linear_in_grad_bound_kernel(const float* __restrict__ W, int N, int K,
+                                                                  float* __restrict__ out) {
+    __shared__ float s_p[8][33];
+    unsigned int* scratch = reinterpret_cast<unsigned int*>(out) + 1;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int k = blockIdx.x * 32 + tx;
+    float t = 0.f;
+    if (k < K)
+        for (int n = ty; n < N; n += 8) t += fabsf(W[(int64_t)n * K + k]);
+    s_p[ty][tx] = t;
+    __syncthreads();
+    if (ty == 0) {
+        for (int i = 1; i < 8; ++i) t += s_p[i][tx];
+        const float v = warp_max(t * 1.0001f);   // (the column sum is rounded: a hair of slack)
+        if (tx == 0) {
+            atomicMax(scratch, __float_as_uint(v));
+            __threadfence();
+            if (atomicAdd(scratch + 1, 1u) == gridDim.x - 1) {
+                __threadfence();
+                out[0] = __uint_as_float(*reinterpret_cast<volatile unsigned int*>(scratch));
+                scratch[0] = 0u;
+                scratch[1] = 0u;
+            }
+        }
+    }
+}
+
 // Upper bound of the gradient that heads_backward writes for the last hidden layer:
 // |dz[m][j]| = |dv[m] Wv[j] + sum_a dl[m][a] Wa[a][j]| * |act'| <= (|dv[m]| + sum_a |dl[m][a]|) * max(|Wv|_inf, |Wa|_inf),
 // act' <= 1 for ELU / ReLU / tanh.  1.2 MB of per-sample gradients at the cfg-2 minibatch: 64 blocks take the row maxima
 // (atomicMax on the bit pattern of a non-negative float), the block that arrives last folds in the weight maximum.
 // out = [bound, scratch bits, arrival counter]; scratch and counter are left at zero.
+// The last block also runs the chain down the hidden layers below: bound(dz[i]) = bound(dz[i+1]) * factor(W[i+1])
+// (linear_in_grad_bound_kernel) into chain[4 i], i = n_chain-1 .. 0, with factor(W[j]) at factors[4 j].
 __global__ void __launch_bounds__(256) heads_dz_bound_kernel(const float* __restrict__ dlogits, const float* __restrict__ dvalues,
                                                             int64_t rows, int A, const float* __restrict__ Wv,
-                                                            const float* __restrict__ Wa, int H, float* __restrict__ out) {
+                                                            const float* __restrict__ Wa, int H, float* __restrict__ out,
+                                                            const float* __restrict__ factors, float* __restrict__ chain,
+                                                            int n_chain) {
     __shared__ float s_r[8], s_w[8];
     unsigned int* scratch = reinterpret_cast<unsigned int*>(out) + 1;
     float r = 0.f, w = 0.f;
@@ -144,9 +178,14 @@ __global__ void __launch_bounds__(256) heads_dz_bound_kernel(const float* __rest
         __threadfence();
         if (atomicAdd(scratch + 1, 1u) == gridDim.x - 1) {
             __threadfence();
-            out[0] = __uint_as_float(*reinterpret_cast<volatile unsigned int*>(scratch));
+            float b = __uint_as_float(*reinterpret_cast<volatile unsigned int*>(scratch));
+            out[0] = b;
             scratch[0] = 0u;
             scratch[1] = 0u;
+            for (int i = n_chain - 1; i >= 0; --i) {
+                b = b * factors[4 * (i + 1)] * 1.0001f;   // (the product is rounded: a hair of slack)
+                chain[4 * i] = b;
+            }
         }
     }
 }
@@ -311,10 +350,20 @@ int sfb200_linear_out_bound(const float* W, const float* b, int N, int K, const 
     return 0;
 }
 
+int sfb200_linear_in_grad_bound(const float* W, int N, int K, float* out_dev, void* stream) {
+    SFB_CHECK_ARG(W && out_dev && N > 0 && K > 0, "linear_in_grad_bound: bad arguments");
+    sfb::linear_in_grad_bound_kernel<<<(unsigned)sfb::ceil_div(K, 32), 256, 0, (cudaStream_t)stream>>>(W, N, K, out_dev);
+    SFB_LAUNCH_OK();
+    return 0;
+}
+
 int sfb200_heads_dz_bound(const float* dlogits, const float* dvalues, int64_t rows, int A, const float* Wv, const float* Wa,
-                          int H, float* out_bound_dev, void* stream) {
-    SFB_CHECK_ARG(dlogits && dvalues && Wv && Wa && out_bound_dev && rows > 0 && A > 0 && H > 0, "heads_dz_bound: bad arguments");
-    sfb::heads_dz_bound_kernel<<<128, 256, 0, (cudaStream_t)stream>>>(dlogits, dvalues, rows, A, Wv, Wa, H, out_bound_dev);
+                          int H, float* out_bound_dev, const float* factors_dev, float* chain_dev, int n_chain, void* stream) {
+    SFB_CHECK_ARG(dlogits && dvalues && Wv && Wa && out_bound_dev && rows > 0 && A > 0 && H > 0 && n_chain >= 0 &&
+                      (n_chain == 0 || (factors_dev && chain_dev)),
+                  "heads_dz_bound: bad arguments");
+    sfb::heads_dz_bound_kernel<<<128, 256, 0, (cudaStream_t)stream>>>(dlogits, dvalues, rows, A, Wv, Wa, H, out_bound_dev,
+                                                                      factors_dev, chain_dev, n_chain);
     SFB_LAUNCH_OK();
     return 0;
 }

@@ -52,14 +52,20 @@ constexpr int kConsumerRegs = 232;
 // Mainloop: the split of stage kb+1 runs while the wgmmas of stage kb are in flight (two conversion buffers).  A and B
 // have their own TMA rings: a raw slot goes back to the producer as soon as it is split, an fp16 B slot (the twin tiles
 // the wgmmas read in place) once its wgmmas have completed.  Every accumulator receives the same wgmmas in the same k order as a serial loop would issue.
-template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false, bool RES = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
-                  const float* __restrict__ a_bound, unsigned long long* __restrict__ trace) {
+//
+// DW16: the fp16 form of dW = dz^T . x (gemm_dw_f16_kernel): both operands are MN-major activations with registered
+// bounds (a_bound, b_bound).  The raw fp32 tiles come through the tf32 form's 32-k rings; the consumers split both into
+// scaled fp16 hi / lo halves in the MN-major layout (split_tile_f16_mn, no transpose), which fp16 wgmma reads with its
+// transpose bits set; the three MMAs and the output scaling are the fp16 form's, the epilogue the plain one.
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16, bool RES, bool DW16>
+__device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, float* __restrict__ C,
+                                             int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits,
+                                             const TcEpilogue& epi, const float* __restrict__ a_bound,
+                                             const float* __restrict__ b_bound, unsigned long long* __restrict__ trace) {
     static_assert(!F16 || (!A_MN && SPLIT3), "fp16-split engine: K-major activations, 3-pass");
+    static_assert(!DW16 || (A_MN && B_MN && SPLIT3 && !HEADS && !F16 && !RES), "fp16 dW form: MN-major operands, plain epilogue");
     if (trace && threadIdx.x == 0) trace[blockIdx.x * kTraceWords + 8] = tc_now();
-    using S = TcSmem<F16>;
+    using S = TcSmem<F16, DW16>;
     constexpr int KBK = S::KBK;
     constexpr int SA = S::A_STAGES, SB = S::B_STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -134,8 +140,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int wg = ct >> 7;                    // 64-row half of the tile
 
     // fp16-split engine: binary shift of the A operand from its bound (written by an earlier kernel of the stream)
-    const int a_shift = F16 ? f16_shift_for_bound(a_bound[0]) : 0;
+    const int a_shift = (F16 || DW16) ? f16_shift_for_bound(a_bound[0]) : 0;
     const float a_scale = pow2f_int(a_shift);
+    const int b_shift = DW16 ? f16_shift_for_bound(b_bound[0]) : kF16WShift;
+    const float b_scale = pow2f_int(b_shift);
     // split stage g into conversion buffer g & 1
     auto split_stage = [&](int g) {
         const int sa = g % SA, sb = g % SB;
@@ -144,6 +152,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         mbar_wait(&full_a[sa], (g / SA) & 1);
         if constexpr (F16) {
             split_tile_f16<false>(pa, cv, cv + S::A_HALF, ct, a_scale);
+        } else if constexpr (DW16) {
+            split_tile_f16_mn(pa, cv, cv + S::A_HALF, ct, a_scale);
+            mbar_wait(&full_b[sb], (g / SB) & 1);
+            split_tile_f16_mn(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct, b_scale);
+            mbar_arrive(&empty_b[sb]);
         } else {
             split_tile<A_MN, SPLIT3>(pa, cv, cv + S::A_HALF, ct);
             mbar_wait(&full_b[sb], (g / SB) & 1);
@@ -173,26 +186,42 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             const int g = g0 + kb;
             const int sb = g % SB;
             const uint8_t* cv = conv + (g & 1) * S::CONV;
-            const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
-            const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
-            const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
-            const uint64_t db_hi = make_smem_desc(smem_u32(bt));
-            const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
-            if (F16) mbar_wait(&full_b[sb], (g / SB) & 1);
-            wgmma_fence();
+            if constexpr (DW16) {
+                // A: warpgroup wg's 64 rows are the wg-th 64-row atom column; a k-step of 16 is two 1024 B atoms
+                const uint64_t da_hi = make_smem_desc_mn(smem_u32(cv + wg * 4096));
+                const uint64_t da_lo = make_smem_desc_mn(smem_u32(cv + S::A_HALF + wg * 4096));
+                const uint64_t db_hi = make_smem_desc_mn(smem_u32(cv + 2 * S::A_HALF));
+                const uint64_t db_lo = make_smem_desc_mn(smem_u32(cv + 2 * S::A_HALF + S::B_HALF));
+                wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < TBK / WG_K; ++k) {
-                const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step (8 tf32 or 16 fp16) inside the swizzle row
-                if constexpr (F16) {
-                    wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, 1);
-                    wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, 1);
-                    wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
-                } else {
-                    wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
+                for (int k = 0; k < TBK / 16; ++k) {
+                    const uint64_t o = (uint64_t)(2048 >> 4) * k;
+                    wgmma_m64n128k16_f16_mn(acc, da_hi + o, db_hi + o, 1);
+                    wgmma_m64n128k16_f16_mn(cross, da_hi + o, db_lo + o, 1);
+                    wgmma_m64n128k16_f16_mn(cross, da_lo + o, db_hi + o, 1);
                 }
-                if (SPLIT3 && !F16) {
-                    wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, 1);
-                    wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
+            } else {
+                const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
+                const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
+                const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
+                const uint64_t db_hi = make_smem_desc(smem_u32(bt));
+                const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
+                if (F16) mbar_wait(&full_b[sb], (g / SB) & 1);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < TBK / WG_K; ++k) {
+                    const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step (8 tf32 or 16 fp16) inside the swizzle row
+                    if constexpr (F16) {
+                        wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, 1);
+                        wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, 1);
+                        wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
+                    } else {
+                        wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
+                    }
+                    if (SPLIT3 && !F16) {
+                        wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, 1);
+                        wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
+                    }
                 }
             }
             wgmma_commit();
@@ -203,9 +232,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
         g0 += tc.num_kb;
         if (tr) tr[4] = tc_now();
-        if (F16) {
+        if (F16 || DW16) {
             // (main + cross * 2^-11) * 2^-(operand shifts): exact power-of-two scalings
-            const float out_scale = pow2f_int(-(a_shift + kF16WShift));
+            const float out_scale = pow2f_int(-(a_shift + b_shift));
 #pragma unroll
             // (a rounded product of its own: the straight-line epilogues must not contract it with their bias add)
             for (int i = 0; i < 64; ++i) acc[i] = __fmul_rn(fmaf(cross[i], 1.f / 2048.f, acc[i]), out_scale);
@@ -262,6 +291,24 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         }
         if (tr) tr[5] = tc_now();
     }
+}
+
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16 = false, bool RES = false>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
+                  const float* __restrict__ a_bound, unsigned long long* __restrict__ trace) {
+    gemm_tc_body<A_MN, B_MN, SPLIT3, HEADS, F16, RES, false>(tmap_a, tmap_b, C, ldc, M, N, K, k_chunk, splits, epi, a_bound,
+                                                             nullptr, trace);
+}
+
+// dW = dz^T . x in the fp16 form (DW16 above); b_bound: the registered bound of x
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_dw_f16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   float* __restrict__ C, int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits, TcEpilogue epi,
+                   const float* __restrict__ a_bound, unsigned long long* __restrict__ trace, const float* __restrict__ b_bound) {
+    gemm_tc_body<true, true, true, false, false, false, true>(tmap_a, tmap_b, C, ldc, M, N, K, k_chunk, splits, epi, a_bound,
+                                                              b_bound, trace);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -348,11 +395,18 @@ static bool operand_ok(const float* p, int64_t ld) {
     return ((reinterpret_cast<uintptr_t>(p) & 15u) == 0) && (ld % 4 == 0) && ld > 0;
 }
 
-template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS = false, bool F16 = false, bool RES = false>
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16, bool RES, bool DW16>
+static auto tc_kernel() {
+    if constexpr (DW16) return gemm_dw_f16_kernel;
+    else return gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES>;
+}
+
+template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS = false, bool F16 = false, bool RES = false, bool DW16 = false>
 static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, int64_t M, int N, int K,
-                     int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr) {
-    auto kern = gemm_wgmma_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES>;
-    constexpr int smem = TcSmem<F16>::TOTAL;
+                     int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr,
+                     const float* b_bound = nullptr) {
+    auto kern = tc_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES, DW16>();
+    constexpr int smem = TcSmem<F16, DW16>::TOTAL;
     static int ctas_per_sm = 0;   // of this instantiation: 1 (shared memory), asked rather than assumed
     if (!ctas_per_sm) {
         SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -364,8 +418,13 @@ static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int
     SFB_CHECK_ARG(!g_gemm_trace || items * kTraceWords <= g_gemm_trace_words,
                   "gemm trace buffer too small: %lld work items need %lld words", (long long)items,
                   (long long)(items * kTraceWords));
-    SFB_CUDA_OK(launch_pdl(kern, dim3((unsigned)(items < resident ? items : resident)), dim3(TC_THREADS), (size_t)smem, st,
-                           ta, tb, C, ldc, M, N, K, k_chunk, splits, epi, a_bound, g_gemm_trace));
+    const dim3 grid((unsigned)(items < resident ? items : resident));
+    if constexpr (DW16)
+        SFB_CUDA_OK(launch_pdl(kern, grid, dim3(TC_THREADS), (size_t)smem, st, ta, tb, C, ldc, M, N, K, k_chunk, splits, epi,
+                               a_bound, g_gemm_trace, b_bound));
+    else
+        SFB_CUDA_OK(launch_pdl(kern, grid, dim3(TC_THREADS), (size_t)smem, st, ta, tb, C, ldc, M, N, K, k_chunk, splits, epi,
+                               a_bound, g_gemm_trace));
     SFB_LAUNCH_OK();
     return 0;
 }
@@ -434,10 +493,20 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
                     : launch_tc<false, false, false, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st);
         return rc;
     }
+    // fp16 form of dW = dz^T . x: both operands MN-major activations with registered bounds, split in the kernel
+    const float* a_bound = nullptr;
+    const float* b_bound = nullptr;
+    if (a_mn && b_mn && split3 && epi.mode == 0 && f16_enabled()) {
+        a_bound = operand_bound_lookup(A, ((int64_t)(K - 1) * lda + M) * (int64_t)sizeof(float));
+        if (a_bound) b_bound = operand_bound_lookup(B, ((int64_t)(K - 1) * ldb + N) * (int64_t)sizeof(float));
+    }
 #define SFB_TC(AM, BM_)                                                                                          \
     (split3 ? launch_tc<AM, BM_, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st)                 \
             : launch_tc<AM, BM_, false>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st))
-    if (!a_mn && !b_mn) rc = SFB_TC(false, false);
+    if (b_bound)
+        rc = launch_tc<true, true, true, false, false, false, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st,
+                                                                   a_bound, b_bound);
+    else if (!a_mn && !b_mn) rc = SFB_TC(false, false);
     else if (!a_mn && b_mn) rc = SFB_TC(false, true);
     else if (a_mn && b_mn) rc = SFB_TC(true, true);
     else rc = SFB_TC(true, false);

@@ -147,6 +147,27 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t de
         : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
+// The same with both operands MN-major (imm-trans-a = imm-trans-b = 1: A is [k][m], B is [k][n] in shared memory).
+__device__ __forceinline__ void wgmma_m64n128k16_f16_mn(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+        "%64, %65, p, 1, 1, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
+          "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]),
+          "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+          "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]),
+          "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
+          "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
+          "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+}
+
 // ------------------------------------------------------------------------------------------------ descriptors
 // wgmma shared-memory matrix descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout [62,64) (1 = 128B swizzle).
 // K-major tile [rows][32 fp32] with the 128B swizzle (16 B chunk index XOR row % 8, 8-row atoms of 1024 B): SBO = 1024
@@ -155,6 +176,16 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
     d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024u >> 4) << 32;
+    d |= (uint64_t)1 << 62;
+    return d;
+}
+// MN-major 16-bit tile with the 128B swizzle (split_tile_f16_mn): 1024 B atoms of [8 k][64 rows]; LBO = 4096 (next 64
+// rows), SBO = 1024 (next 8 k).  A k-step of 16 advances the start address by two atoms.
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
+    d |= (uint64_t)(4096u >> 4) << 16;
     d |= (uint64_t)(1024u >> 4) << 32;
     d |= (uint64_t)1 << 62;
     return d;

@@ -40,15 +40,18 @@ constexpr int TC_THREADS = 384;
 //   fp16 form: raw A fp32 tile of 64 k (32 KB, released once split); B = the weight tile's fp16 [hi | lo] twins, TMA-loaded
 //              in the swizzled layout wgmma reads (32 KB, released once its wgmmas completed); conversion buffer =
 //              [A hi | A lo] (32 KB)
-template <bool F16>
+//   fp16 dW form (DW16, gemm_dw_f16_kernel): raw MN-major A / B fp32 tiles of 32 k as in the tf32 form (16 KB each);
+//              conversion buffer = [A hi | A lo | B hi | B lo], each [32 k][128 rows] fp16 MN-major (8 KB): 160 KB in all
+template <bool F16, bool DW16 = false>
 struct TcSmem {
     static constexpr int KBK = F16 ? 64 : TBK;                    // k per stage
     static constexpr int A_STAGES = F16 ? 2 : 3;
     static constexpr int B_STAGES = 3;
     static constexpr int A_RAW = TBM * KBK * 4;
     static constexpr int B_SLOT = F16 ? 2 * TBN * 64 * 2 : TBN * TBK * 4;
-    static constexpr int A_HALF = TBM * 128;                      // one split half of A: [128 rows][128 B], swizzled K-major
-    static constexpr int B_HALF = TBN * 128;
+    // one split half of A: [128 rows][128 B] swizzled K-major; DW16: [32 k][128 rows] fp16 (split_tile_f16_mn)
+    static constexpr int A_HALF = DW16 ? TBM * TBK * 2 : TBM * 128;
+    static constexpr int B_HALF = DW16 ? TBN * TBK * 2 : TBN * 128;
     static constexpr int CONV = F16 ? 2 * A_HALF : 2 * A_HALF + 2 * B_HALF;
     static constexpr int B_RING = A_STAGES * A_RAW;               // offsets from the 1024-aligned base
     static constexpr int CONV_OFF = B_RING + B_STAGES * B_SLOT;
@@ -114,8 +117,8 @@ __device__ __forceinline__ void split_tile(const uint8_t* raw, uint8_t* hi, uint
 }
 
 // fp16-split engine: raw fp32 K-major tile [rows][64 k] -> scaled fp16 hi / lo halves (lo carries a 2^11 factor,
-// common.cuh) in the swizzled K-major [rows][64 fp16] layout.  (MN-major operands never take the fp16 form: the weight
-// operand of dX comes from its transposed twins instead, gemm_tc.cu.)
+// common.cuh) in the swizzled K-major [rows][64 fp16] layout.  (The weight operand of dX comes from its transposed twins,
+// gemm_tc.cu; dW's MN-major activations are split by split_tile_f16_mn below.)
 // ct, ROWS and THREADS as for split_tile.
 template <bool MN, int ROWS = TBM, int THREADS = 2 * ROWS>
 __device__ __forceinline__ void split_tile_f16(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct, float scale) {
@@ -126,6 +129,27 @@ __device__ __forceinline__ void split_tile_f16(const uint8_t* raw, uint8_t* hi, 
         const float4 v = reinterpret_cast<const float4*>(raw)[i];
         const int r = i >> 4, c4 = i & 15;                         // row r, k = 4*c4 .. 4*c4+3
         const uint32_t off = (uint32_t)(r * 128 + ((((c4 >> 1) ^ r) & 7) << 4) + (c4 & 1) * 8);
+        uint2 h, l;
+        f16_split2(v.x * scale, v.y * scale, h.x, l.x);
+        f16_split2(v.z * scale, v.w * scale, h.y, l.y);
+        *reinterpret_cast<uint2*>(hi + off) = h;
+        *reinterpret_cast<uint2*>(lo + off) = l;
+    }
+}
+
+// fp16 dW form: raw fp32 MN-major tile [32 k][128 rows] -> scaled fp16 hi / lo halves in the MN-major 128B-swizzled
+// layout fp16 wgmma reads with its transpose bit set (make_smem_desc_mn): per half, atom (k / 8, rows / 64) is 1024 B at
+// (rows / 64) * 4096 + (k / 8) * 1024, row k % 8 of it holds the 64 rows as eight 16 B chunks, chunk c at c ^ (k % 8).
+// No transpose: a thread turns four consecutive rows at one k into 8 B of hi and 8 B of lo (a half-warp writes one whole
+// 128 B row: no bank conflict).  ct = 0 .. 255.
+__device__ __forceinline__ void split_tile_f16_mn(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int ct, float scale) {
+#pragma unroll
+    for (int q = 0; q < (TBK * TBM / 4) / 256; ++q) {
+        const int i = ct + 256 * q;
+        const float4 v = reinterpret_cast<const float4*>(raw)[i];
+        const int k = i >> 5, r = (i & 31) * 4;                    // k, rows r .. r+3
+        const int c = (r >> 3) & 7;
+        const uint32_t off = (uint32_t)((r >> 6) * 4096 + (k >> 3) * 1024 + (k & 7) * 128 + ((c ^ (k & 7)) << 4) + (r & 4) * 2);
         uint2 h, l;
         f16_split2(v.x * scale, v.y * scale, h.x, l.x);
         f16_split2(v.z * scale, v.w * scale, h.y, l.y);

@@ -175,12 +175,15 @@ class Learner:
         self.h = [torch.empty((B, h), **f32) for h in spec.hidden]
         self.dz = [torch.empty((B, h), **f32) for h in spec.hidden]
         # fp16-split form of the GEMM engine (model._register_f16): tell the library the bounds of the activation buffers the
-        # forward GEMMs (normalised observations, hidden activations) and dX (gradient of the last hidden layer) read
+        # forward GEMMs (normalised observations, hidden activations), dX and dW (gradients of the hidden layers) read
         self.dz_bound = None
         if getattr(self.model, "f16_twins", None) is not None and self.engine == ops.GEMM_TC_3XTF32:
-            self.dz_bound = torch.zeros(4, **f32)        # [bound, scratch, counter, -] (sfb200_heads_dz_bound)
-            ops.register_operand_bounds(self, [(self.obs_flat_compact, self.model.bound_x), (self.dz[-1], self.dz_bound[0:1])] +
-                                        [(self.h[i], self.model.bound_h[4 * i: 4 * i + 1]) for i in range(len(spec.hidden) - 1)])
+            L = len(spec.hidden)
+            # [bound, scratch, counter, -] per hidden layer's dz (sfb200_heads_dz_bound: the last one, then the chain below)
+            self.dz_bound = torch.zeros(4 * L, **f32)
+            ops.register_operand_bounds(self, [(self.obs_flat_compact, self.model.bound_x)] +
+                                        [(self.dz[i], self.dz_bound[4 * i: 4 * i + 1]) for i in range(L)] +
+                                        [(self.h[i], self.model.bound_h[4 * i: 4 * i + 1]) for i in range(L - 1)])
             for i in range(1, len(spec.hidden)):            # layers whose input gradient is needed: dX reads W transposed
                 self.model.enable_f16_transposed(spec.fc_encoder_name(i, "weight"))
         self.mb_values = torch.empty(B, **f32)
@@ -594,7 +597,9 @@ class Learner:
         tail_dz = (self.dz[Le + Ld - 1] if Ld > 0 else d_enc) if tail_is_mlp else self.d_core
         tail_db = gdec[-1][1] if Ld > 0 else (None if rnn else db_enc)
         if self.dz_bound is not None and tail_is_mlp:
-            ops.heads_dz_bound(self.dlogits, self.dvalues, Wv, Wa, self.dz_bound)
+            L = len(spec.hidden)
+            ops.heads_dz_bound(self.dlogits, self.dvalues, Wv, Wa, self.dz_bound[4 * (L - 1):], m.grad_fac, self.dz_bound,
+                               L - 1)
         tail_act = self.act if tail_is_mlp else none
         if spec.wide_heads:
             # dWa = dlogits^T . x and tail_dz = (dlogits . Wa) * act'(x) on the GEMM engine, then the value term, the bias /

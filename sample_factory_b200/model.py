@@ -448,7 +448,7 @@ class PolicyModel:
         sp = self.spec
         self.f16_twins = None
         self.f16_T: Dict[str, Tensor] = {}
-        self.bound_x = self.bound_h = None
+        self.bound_x = self.bound_h = self.grad_fac = None
         ok = (self.flat.is_cuda and sp.normalize_input and sp.obs_shape is None and not sp.use_rnn and sp.share_weights
               and not sp.decoder_mlp_layers and not sp.dict_obs and len(sp.hidden) >= 1)
         if not ok:
@@ -459,19 +459,25 @@ class PolicyModel:
         ops.register_f16_twins(self.flat, self.f16_twins)
         self.bound_x = torch.full((1,), 5.0, dtype=torch.float32, device=self.device)
         self.bound_h = torch.zeros(4 * len(sp.hidden), dtype=torch.float32, device=self.device)   # [bound, scratch, counter, -] per layer
+        # per hidden layer i >= 1: max_k sum_n |W_i[n][k]|, the factor from the bound of dz[i] to that of dz[i-1] (same layout)
+        self.grad_fac = torch.zeros(4 * len(sp.hidden), dtype=torch.float32, device=self.device)
         self.refresh_bounds()
 
     def refresh_bounds(self) -> None:
-        """bounds of the hidden activations from the current weights (one tiny kernel per layer) + the transposed twins"""
+        """bounds of the hidden activations and gradient factors from the current weights (one tiny kernel per layer) + the
+        transposed twins"""
         if self.f16_twins is None:
             return
         from . import ops
 
         act = ops.ACT[self.spec.nonlinearity]
         inb = self.bound_x
-        for i, (W, b) in enumerate(self.hidden_layers()[:-1]):       # (the last hidden layer feeds the heads, not a GEMM)
+        layers = self.hidden_layers()
+        for i, (W, b) in enumerate(layers[:-1]):       # (the last hidden layer feeds the heads, not a GEMM)
             ops.linear_out_bound(W, b, inb, self.bound_h[4 * i: 4 * i + 4], act)
             inb = self.bound_h[4 * i: 4 * i + 1]
+        for i in range(1, len(layers)):                # layers whose input gradient the learner takes
+            ops.linear_in_grad_bound(layers[i][0], self.grad_fac[4 * i: 4 * i + 4])
         for name in self.f16_T:
             ops.refresh_f16_transposed(self.params[name])
 
@@ -563,6 +569,7 @@ class PolicyModel:
         if self.f16_twins is not None and other.f16_twins is not None:
             self.f16_twins.copy_(other.f16_twins)
             self.bound_h.copy_(other.bound_h)      # (scratch words are zero between launches)
+            self.grad_fac.copy_(other.grad_fac)
             self.refresh_cat_heads()
         else:
             self.weights_changed()

@@ -482,13 +482,25 @@ def linear_out_bound(W: Tensor, b: Optional[Tensor], in_bound: Tensor, out_bound
     lib().call("sfb200_linear_out_bound", _p(W, F32), _p(b, F32), N, K, _p(in_bound, F32), _p(out_bound, F32), act, _stream())
 
 
-def heads_dz_bound(dlogits: Tensor, dvalues: Tensor, Wv: Tensor, Wa: Tensor, out_bound: Tensor) -> None:
-    """out_bound = max_m (|dvalues[m]| + sum_a |dlogits[m][a]|) * max(|Wv|, |Wa|): bound of heads_backward's dz output"""
+def linear_in_grad_bound(W: Tensor, out: Tensor) -> None:
+    """out[0] = max_k sum_n |W[n][k]| (times 1.0001): |dz . W| <= bound(dz) * out[0]; out = four floats [factor, scratch,
+    counter, -], the middle two zero before and after"""
+    N, K = W.shape
+    assert W.is_contiguous() and out.numel() >= 4
+    lib().call("sfb200_linear_in_grad_bound", _p(W, F32), N, K, _p(out, F32), _stream())
+
+
+def heads_dz_bound(dlogits: Tensor, dvalues: Tensor, Wv: Tensor, Wa: Tensor, out_bound: Tensor,
+                   factors: Optional[Tensor] = None, chain: Optional[Tensor] = None, n_chain: int = 0) -> None:
+    """out_bound = max_m (|dvalues[m]| + sum_a |dlogits[m][a]|) * max(|Wv|, |Wa|): bound of heads_backward's dz output;
+    with n_chain > 0 also chain[4 i] = chain[4 (i+1)] * factors[4 (i+1)] for i = n_chain-1 .. 0 (linear_in_grad_bound
+    factors; the chain starts from out_bound)"""
     rows, A = dlogits.shape
     H = Wv.numel()
     assert Wa.numel() == A * H and dlogits.is_contiguous() and Wa.is_contiguous() and out_bound.numel() >= 3
+    assert n_chain == 0 or (factors.numel() >= 4 * (n_chain + 1) and chain.numel() >= 4 * n_chain)
     lib().call("sfb200_heads_dz_bound", _p(dlogits, F32), _p(dvalues, F32), rows, A, _p(Wv, F32), _p(Wa, F32), H,
-               _p(out_bound, F32), _stream())
+               _p(out_bound, F32), _p(factors, F32), _p(chain, F32), n_chain, _stream())
 
 
 def linear_heads_partials(N: int, A: int, engine: int) -> int:

@@ -53,3 +53,10 @@ for (M, N, K) in [(32768, 512, 512), (32768, 512, 64)]:
         ops.unregister_f16_transposed(W); ops.unregister_f16_twins(flat)
     ref = dz.double().t() @ x.double()
     print("   dW max abs err vs fp64:", float((dW.double() - ref).abs().max()), "of max", float(ref.abs().max()))
+    # dW with both operands' bounds registered: the fp16 form (dz^T and x split in the kernel)
+    bx = torch.full((1,), float(x.abs().max()), device=dev); bz = torch.full((1,), float(dz.abs().max()), device=dev)
+    ops.register_operand_bound(x, bx); ops.register_operand_bound(dz, bz)
+    t_dw16 = timeit(lambda: ops.linear_backward(dz, x, W, ops.ACT["elu"], dW, None, None, eng, ws))
+    ops.unregister_operand_bound(x); ops.unregister_operand_bound(dz)
+    print(f"M={M} N={N} K={K}: fp16-split dW {t_dw16:.1f} us ({2*M*N*K/t_dw16/1e6:.0f} TFLOP/s)")
+    print("   fp16-split dW max abs err vs fp64:", float((dW.double() - ref).abs().max()), "of max", float(ref.abs().max()))

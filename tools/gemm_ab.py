@@ -8,7 +8,8 @@ and dW (tf32 form, split-K), at the learner's size (M = 32768, 512 wide) and at 
 more, M < 128, N and K that are no multiples of the tile, a split-K whose last slice is short.  Outputs are stored as
 int32 bit patterns.  Forward and dX take no part in split-K, so they must not differ between builds that issue the same
 wgmmas in the same order; dW depends on the split-K rule (SFB200_SPLITK_LEGACY=1 pins the earlier one), so --compare
-lists it apart, and each run prints dW's largest error against an fp64 product."""
+lists it apart, and each run prints dW's largest error against an fp64 product.  dW is run twice: without bounds (the
+tf32 form) and with both operands' bounds registered (the fp16 form, not bit-identical to the tf32 one)."""
 from __future__ import annotations
 
 import argparse
@@ -84,11 +85,24 @@ def run(out_path):
                 ops.unregister_operand_bound(dz)
                 ops.unregister_f16_transposed(W)
                 ops.unregister_f16_twins(flat)
+        ref = dz.double().t() @ x.double()
         dW = torch.zeros(N, K, device=dev)
         ops.linear_backward(dz, x, W, ops.ACT["none"], dW, None, None, eng, ws)
         keep(f"dW/{M}x{N}x{K}", dW)
-        ref = dz.double().t() @ x.double()
         print(f"dW {M}x{N}x{K}: max |err| vs fp64 {float((dW.double() - ref).abs().max()):.3e} of max "
+              f"{float(ref.abs().max()):.3e}")
+        # dW with both operands' bounds registered: the fp16 form (a build without it runs the tf32 form again)
+        bx, bz = (torch.full((1,), float(t.abs().max()), device=dev) for t in (x, dz))
+        ops.register_operand_bound(x, bx)
+        ops.register_operand_bound(dz, bz)
+        try:
+            dW = torch.zeros(N, K, device=dev)
+            ops.linear_backward(dz, x, W, ops.ACT["none"], dW, None, None, eng, ws)
+        finally:
+            ops.unregister_operand_bound(x)
+            ops.unregister_operand_bound(dz)
+        keep(f"dW16/{M}x{N}x{K}", dW)
+        print(f"dW with bounds {M}x{N}x{K}: max |err| vs fp64 {float((dW.double() - ref).abs().max()):.3e} of max "
               f"{float(ref.abs().max()):.3e}")
     np.savez_compressed(out_path, **res)
     print(f"{len(res)} arrays -> {out_path}")
@@ -100,10 +114,12 @@ def compare(a_path, b_path):
     bad = [k for k in a.files if a[k].shape != b[k].shape or not np.array_equal(a[k], b[k])]
     for k in bad:
         print("DIFFERS", k, int((a[k] != b[k]).sum()), "of", a[k].size)
-    n_dw = sum(k.startswith("dW/") for k in a.files)
-    bad_dw = [k for k in bad if k.startswith("dW/")]
+    n_dw = sum(k.startswith("dW") for k in a.files)
+    bad_dw = [k for k in bad if k.startswith("dW")]
+    n_dw16 = sum(k.startswith("dW16/") for k in a.files)
+    bad_dw16 = sum(k.startswith("dW16/") for k in bad)
     print(f"forward / dX: {len(a.files) - n_dw - (len(bad) - len(bad_dw))} / {len(a.files) - n_dw} arrays bit-identical; "
-          f"dW: {n_dw - len(bad_dw)} / {n_dw}")
+          f"dW: {n_dw - n_dw16 - (len(bad_dw) - bad_dw16)} / {n_dw - n_dw16}; dW with bounds: {n_dw16 - bad_dw16} / {n_dw16}")
     return 1 if len(bad) > len(bad_dw) else 0
 
 

@@ -4,7 +4,8 @@
 Switches the kernel's trace on (sfb200_gemm_set_trace: one consumer thread and the producer thread of every CTA stamp
 %globaltimer and %smid per work item) and runs, at M = 32768: the layer-2 forward with the heads folded in and dX
 (fp16 form, 512 x 512), the layer-1 forward (fp16 form, 512 x 64: one stage per item, so nearly all epilogue), dW2
-(512 x 512) and dW1 (512 x 64) (tf32 form, split-K).  Prints per GEMM: CTAs, work items and
+(512 x 512) and dW1 (512 x 64) (split-K; both operands have registered bounds, so a library with the fp16 dW form runs
+that, gemm_dw_f16_kernel, and one without it the tf32 form).  Prints per GEMM: CTAs, work items and
 items per CTA, the mean microseconds of an item split into fill (item begun -> its first stage landed), mainloop and
 epilogue, the epilogue split at the stamps inside it (a library without them leaves the words zero and the parts
 unprinted): accumulators combined, the epilogue's batch of global loads landed, and then either the stores issued, or for
@@ -126,9 +127,9 @@ def main():
          lambda: ops.linear_backward(dz, h1, W2, ops.ACT["elu"], None, dx, None, eng, ws)),
         ("layer-1 forward, fp16 form <0,0,1,0,1,0> [32768 x 512 x 64]",
          lambda: ops.linear_act_forward(x0, W1, b1, y, ops.ACT["elu"], eng)),
-        ("dW2, tf32 form, split-K <1,1,1,0,0,0> [512 x 512, k = 32768]",
+        ("dW2, split-K [512 x 512, k = 32768]",
          lambda: ops.linear_backward(dz, h1, W2, ops.ACT["elu"], dW2, None, None, eng, ws)),
-        ("dW1, tf32 form, split-K <1,1,1,0,0,0> [512 x 64, k = 32768]",
+        ("dW1, split-K [512 x 64, k = 32768]",
          lambda: ops.linear_backward(dz, x0, W1, ops.ACT["none"], dW1, None, None, eng, ws)),
     ]
     trace = torch.zeros(4096 * ops.GEMM_TRACE_WORDS, dtype=torch.int64, device=dev)
