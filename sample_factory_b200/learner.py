@@ -21,7 +21,7 @@ from torch import Tensor
 
 from . import ops
 from .dist_utils import PeerComm, _ls_masks, peer_comm_wanted, pooled_moments_
-from .model import PolicyModel
+from .model import TOWERS, PolicyModel
 from .policy import HeadsPlan, forward_policy
 from .rnn_core import RnnCore
 
@@ -227,15 +227,28 @@ class Learner:
             lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(B, h, d) // 4 + 4)
             d = h
         self.rnn: Optional[RnnCore] = None
+        # separate actor / critic weights: one core per tower on its half of the state rows; the second tower's BPTT
+        # buffers share the first one's scratch and reset mask (the towers' backwards run one after the other)
+        self.tower_rnn: Optional[Dict[str, RnnCore]] = None
         if spec.use_rnn:
             # recurrent core (model/core.py): BPTT buffers for one minibatch + single-step buffers for the bootstrap value
-            self.rnn = RnnCore(model, engine)
-            self.rnn_bufs = self.rnn.alloc_bptt(B, cfg.recurrence)
-            self.rnn_boot = self.rnn.alloc_step(self.N)
+            if spec.share_weights:
+                self.rnn = RnnCore(model, engine)
+                self.rnn_bufs = self.rnn.alloc_bptt(B, cfg.recurrence)
+                self.rnn_boot = self.rnn.alloc_step(self.N)
+                core = self.rnn
+            else:
+                self.tower_rnn = {tw: RnnCore(model, engine, tw) for tw in TOWERS}
+                self.tower_rnn_bufs = {}
+                for tw in TOWERS:
+                    self.tower_rnn_bufs[tw] = self.tower_rnn[tw].alloc_bptt(B, cfg.recurrence,
+                                                                            self.tower_rnn_bufs.get(TOWERS[0]))
+                self.rnn_boot = self.tower_rnn[TOWERS[0]].alloc_step(self.N)     # (the towers step one after the other)
+                core = self.tower_rnn[TOWERS[0]]
             self.boot_state_out = torch.empty((self.N, spec.rnn_state_size), **f32)
             self.d_core = torch.empty((B, spec.rnn_size), **f32)
             self.rnn_states_flat = torch.empty((E, spec.rnn_state_size), **f32)
-            lin_ws = max(lin_ws, self.rnn.lin_ws_bytes(B, cfg.recurrence, d) // 4 + 4)
+            lin_ws = max(lin_ws, core.lin_ws_bytes(B, cfg.recurrence, d) // 4 + 4)
             d = spec.rnn_size
         for h in spec.decoder_mlp_layers:
             lin_ws = max(lin_ws, ops.linear_backward_workspace_bytes(B, h, d) // 4 + 4)
@@ -362,12 +375,15 @@ class Learner:
         else:
             ops.normalize_obs(obs2d, nobs2d, None, None, spec.obs_subtract_mean, inv_scale)
         # bootstrap value for step T (:965-967): forward on normalized_obs[:, T] in place (strided rows)
-        boot_rnn = None
+        boot_rnn = tower_boot = None
         if self.rnn is not None:
             boot_rnn = lambda head: self.rnn.step(head, batch["rnn_states"][:, T], self.boot_state_out, self.rnn_boot)
+        elif self.tower_rnn is not None:     # (both towers run; only the critic's half of the tail reaches the value)
+            tower_boot = {tw: (lambda head, c=c: c.step(head, batch["rnn_states"][:, T], self.boot_state_out, self.rnn_boot))
+                          for tw, c in self.tower_rnn.items()}
         forward_policy(m, self.normalized_obs[:, T], self.h_boot, self.act, self.engine, self.heads_plan,
                        dict(values=batch["values"][:, T], values_stride=batch["values"].stride(0)), boot_rnn,
-                       store_tail=False)
+                       store_tail=False, tower_rnn_fns=tower_boot)
         # :969-1003 fused
         ops.gae_returns(batch["rewards"], batch["dones"], batch["time_outs"], batch["values"], batch["valids"],
                         cfg.gamma, cfg.gae_lambda, cfg.value_bootstrap,
@@ -377,7 +393,7 @@ class Learner:
         ops.copy_rows(self.normalized_obs.view(N, (T + 1) * D)[:, : T * D], self.obs_flat_compact.view(N, T * D))
         ops.copy_rows(batch["values"][:, :T], self.values_old)
         ops.copy_rows_bytes(batch["valids"][:, :T], self.valids_flat)
-        if self.rnn is not None:
+        if spec.use_rnn:
             S = spec.rnn_state_size
             ops.copy_rows(batch["rnn_states"].view(N, (T + 1) * S)[:, : T * S], self.rnn_states_flat.view(N, T * S))
         if spec.normalize_returns and not cfg.with_vtrace:                                          # :1018-1019
@@ -438,7 +454,7 @@ class Learner:
                    lp_old=batch["log_prob_actions"].view(E, 1), logits_old=batch["action_logits"].view(E, spec.num_action_params),
                    valids=self.valids_flat.view(E, 1), v_old=self.values_old.view(E, 1), adv=self.advantages.view(E, 1),
                    ret=self.returns.view(E, 1), dones=batch["dones"].view(E, 1), rewards=batch["rewards"].view(E, 1))
-        if self.rnn is not None:
+        if spec.use_rnn:
             src["rnn"] = self.rnn_states_flat
         if self.shuffle:
             for k, v in src.items():
@@ -465,12 +481,16 @@ class Learner:
         valids = mbv["valids"][sl]
         v_old = mbv["v_old"][sl]
         # forward (:553-579)
-        mb_rnn = None
+        mb_rnn = mb_tower = None
         if self.rnn is not None:
             mb_rnn = lambda head: self.rnn.forward_bptt(head, mbv["rnn"][sl], mbv["dones"][sl], valids, self.rnn_bufs)
+        elif self.tower_rnn is not None:     # the first tower's core computes the minibatch's reset mask for both
+            mb_tower = {tw: (lambda head, tw=tw: self.tower_rnn[tw].forward_bptt(
+                head, mbv["rnn"][sl], mbv["dones"][sl] if tw == TOWERS[0] else None, valids, self.tower_rnn_bufs[tw]))
+                for tw in TOWERS}
         x = forward_policy(m, x0, self.h, self.act, self.engine, self.heads_plan,
                            dict(values=self.mb_values, values_stride=1, logits=self.mb_logits, logits_stride=A), mb_rnn,
-                           store_tail=True)
+                           store_tail=True, tower_rnn_fns=mb_tower)
         Wv, bv = m.critic
         Wa, ba = m.actor
         if cfg.with_vtrace:                                                                          # :602-640
@@ -670,42 +690,72 @@ class Learner:
 
     def _backward_separate(self, x0: Tensor) -> None:
         """backward of ActorCriticSeparateWeights: one heads-backward over the concatenated tail [B, 2H] (zero-padded head
-        weights route d(logits) into the actor half and d(value) into the critic half), then each tower's MLP chain."""
+        weights route d(logits) into the actor half and d(value) into the critic half), then per tower its decoder MLP
+        chain, its core's BPTT and its encoder MLP chain.  A tail that is a core's output has no activation and no bias."""
         m, spec, plan = self.model, self.model.spec, self.heads_plan
         B = x0.shape[0]
         H = spec.tail_input_size
         g = m.grads
         none = ops.ACT["none"]
+        tail_act = self.act if plan.tower_tail_is_mlp else none
+        db_cat = plan.db_cat if plan.tower_tail_is_mlp else None
         if spec.wide_heads:
             # logits GEMM backward on the actor half (Wa itself, not the zero-padded Wa_cat), then the critic half's value
             # term and the column sums of both halves
             Wv, Wa = m.critic[0], m.actor[0]
-            ops.linear_backward(self.dlogits, plan.tail_cat[:B, :H], Wa, self.act,
+            ops.linear_backward(self.dlogits, plan.tail_cat[:B, :H], Wa, tail_act,
                                 g["action_parameterization.distribution_linear.weight"], plan.dz_cat[:B, :H], None,
                                 self.engine, self.lin_ws)
-            ops.heads_wide_backward(plan.tail_cat[:B, H:], Wv, self.dlogits, self.dvalues, self.act, plan.dz_cat[:B], H,
+            ops.heads_wide_backward(plan.tail_cat[:B, H:], Wv, self.dlogits, self.dvalues, tail_act, plan.dz_cat[:B], H,
                                     False, g["critic_linear.weight"].view(-1), g["critic_linear.bias"],
-                                    g["action_parameterization.distribution_linear.bias"], plan.db_cat, self.heads_ws)
+                                    g["action_parameterization.distribution_linear.bias"], db_cat, self.heads_ws)
         else:
-            ops.heads_backward(plan.tail_cat[:B], m.Wv_cat, m.Wa_cat, self.dlogits, self.dvalues, self.act, plan.dz_cat[:B],
+            ops.heads_backward(plan.tail_cat[:B], m.Wv_cat, m.Wa_cat, self.dlogits, self.dvalues, tail_act, plan.dz_cat[:B],
                                plan.gWv_cat.view(-1), g["critic_linear.bias"], plan.gWa_cat,
-                               g["action_parameterization.distribution_linear.bias"], plan.db_cat, self.heads_ws)
+                               g["action_parameterization.distribution_linear.bias"], db_cat, self.heads_ws)
             g["critic_linear.weight"].copy_(plan.gWv_cat[:, H:])                                   # (the padded halves are
             g["action_parameterization.distribution_linear.weight"].copy_(plan.gWa_cat[:, :H])     #  not parameters: dropped)
-        for tw, col in (("actor_", 0), ("critic_", H)):
-            layers, glayers = m.tower_layers(tw), m.tower_layers(tw, grads=True)
-            L = len(layers)
-            glayers[L - 1][1].copy_(plan.db_cat[col: col + H])      # bias gradient of the tower's last layer
-            dz = plan.dz_cat[:B, col: col + H]
-            for k in range(L - 1, -1, -1):
-                W, dW = layers[k][0], glayers[k][0]
-                if k > 0:
-                    dx = plan.tower_dz[tw][k - 1][:B]
-                    ops.linear_backward(dz, plan.tower_h[tw][k - 1][:B], W, self.act, dW, dx, glayers[k - 1][1], self.engine,
-                                        self.lin_ws)
-                    dz = dx
-                else:
-                    ops.linear_backward(dz, x0, W, none, dW, None, None, self.engine, self.lin_ws)
+        for tw, col in zip(TOWERS, (0, H)):
+            enc, genc = m.tower_encoder_layers(tw), m.tower_encoder_layers(tw, grads=True)
+            dec, gdec = m.tower_decoder_layers(tw), m.tower_decoder_layers(tw, grads=True)
+            Le = len(enc)
+            layers, glayers = enc + dec, genc + gdec
+            acts = [plan.tail_cat[:B, col: col + H] if h is None else h[:B] for h in plan.tower_h[tw]]
+            dzs = [plan.dz_cat[:B, col: col + H] if dz is None else dz[:B] for dz in plan.tower_dz[tw]]
+            if plan.tower_tail_is_mlp:
+                glayers[-1][1].copy_(plan.db_cat[col: col + H])      # bias gradient of the tower's last layer
+            if self.tower_rnn is None:
+                self._mlp_chain_backward(layers, glayers, acts, dzs, 0, x0)
+                continue
+            # the encoder's output as the core reads it: (activations, activation, their gradient, its bias gradient)
+            if Le > 0:
+                x_enc, act_enc, d_enc, db_enc = acts[Le - 1], self.act, dzs[Le - 1], genc[-1][1]
+            else:
+                x_enc, act_enc, d_enc, db_enc = x0, none, None, None
+            core, bufs = self.tower_rnn[tw], self.tower_rnn_bufs[tw]
+            d_core = self.d_core if dec else plan.dz_cat[:B, col: col + H]
+            if dec:
+                self._mlp_chain_backward(layers, glayers, acts, dzs, Le, bufs["core_out"], none, d_core)
+            dgi_all = core.backward_bptt(d_core, bufs, self.lin_ws)
+            ops.linear_backward(dgi_all, x_enc, core._params()[0], act_enc, core._params(grads=True)[0], d_enc, db_enc,
+                                self.engine, self.lin_ws)
+            if Le > 0:
+                self._mlp_chain_backward(enc, genc, acts, dzs, 0, x0)
+
+    def _mlp_chain_backward(self, layers, glayers, acts, dzs, first: int, x_in: Tensor, act_in: Optional[int] = None,
+                            dx_in: Optional[Tensor] = None) -> None:
+        """backward of the MLP layers [first, len(layers)) whose output gradients dzs[i] of acts[i] are known from the top
+        one down: dW of every layer, and the gradient of every layer's input -- for layer `first` the input is x_in
+        (activation act_in, gradient dx_in, or none)"""
+        none = ops.ACT["none"]
+        for k in range(len(layers) - 1, first - 1, -1):
+            W, dW = layers[k][0], glayers[k][0]
+            if k > first:
+                ops.linear_backward(dzs[k], acts[k - 1], W, self.act, dW, dzs[k - 1], glayers[k - 1][1], self.engine,
+                                    self.lin_ws)
+            else:
+                ops.linear_backward(dzs[k], x_in, W, none if act_in is None else act_in, dW, dx_in, None, self.engine,
+                                    self.lin_ws)
 
     def exp_size_total_dev(self) -> Tensor:
         if not hasattr(self, "_exp_total"):

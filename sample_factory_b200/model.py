@@ -53,8 +53,10 @@ class ModelSpec:
     encoder_conv_architecture: str = "convnet_atari"
     encoder_conv_mlp_layers: List[int] = field(default_factory=lambda: [512])
     obs_uint8: bool = False              # dtype of the observation rows in the trajectory buffers
-    # False -> ActorCriticSeparateWeights (model/actor_critic.py:198-322): an actor tower (encoder + decoder MLP) feeding
-    # distribution_linear and a critic tower feeding critic_linear; vector observations, no recurrent core on this path
+    # False -> ActorCriticSeparateWeights (model/actor_critic.py:198-322): an actor tower (encoder MLP -> recurrent core
+    # if use_rnn -> decoder MLP) feeding distribution_linear and a critic tower feeding critic_linear.  Each tower's core
+    # owns one half of a state row, [actor state | critic state], each half laid out like a shared model's row.  Vector
+    # observations of one key only (conv / ResNet encoders and Dict observations raise ValueError)
     share_weights: bool = True
     # Dict observations of 1-D keys (MultiInputEncoder, model/encoder.py:33-70): [(key, d), ...] in sorted key order.  The
     # keys lie side by side in one packed row, key k in columns [c_k, c_k + d_k); every key has its own MlpEncoder with
@@ -248,6 +250,9 @@ class ModelSpec:
                                      f"{self.num_actions}")
         if self.obs_keys is not None:
             self._check_obs_keys()
+        if not self.share_weights and self.obs_shape is not None:
+            raise ValueError(f"separate actor / critic weights (actor_critic_share_weights=False) with an image encoder "
+                             f"({self.encoder_conv_architecture}) are not supported on the device path")
         tup = self.action_segments or self.action_heads
         if tup and len(tup) > self.MAX_TUPLE_HEADS:
             raise ValueError(f"Tuple action spaces are supported with at most {self.MAX_TUPLE_HEADS} heads, got "
@@ -312,6 +317,11 @@ class ModelSpec:
         """model/model_utils.py:11-24"""
         if not self.use_rnn:
             return 1 if self.share_weights else 2       # "actor and critic need separate states" (model_utils.py:20-22)
+        return self.rnn_tower_state_size * (1 if self.share_weights else 2)
+
+    @property
+    def rnn_tower_state_size(self) -> int:
+        """width of one core's columns of a state row (separate weights: [actor state | critic state], each this wide)"""
         return self.rnn_layer_state_size * self.rnn_num_layers
 
     @property
@@ -336,16 +346,19 @@ class ModelSpec:
         """(reference state_dict key, shape) in nn.Module.parameters() order."""
         out = []
         if not self.share_weights:
-            # registration order of ActorCriticSeparateWeights.__init__ (actor_critic.py:208-225)
-            assert self.obs_shape is None and not self.use_rnn, "separate actor / critic weights: MLP towers only"
-            for tw in ("actor_", "critic_"):
+            # registration order of ActorCriticSeparateWeights.__init__ (actor_critic.py:208-225): per tower its encoder
+            # then its core, then both decoders
+            for tw in TOWERS:
                 d = self.obs_dim
                 for i, h in enumerate(self.encoder_mlp_layers):
                     out.append((f"{tw}encoder.encoders.obs.mlp_head.{2 * i}.weight", (h, d)))
                     out.append((f"{tw}encoder.encoders.obs.mlp_head.{2 * i}.bias", (h,)))
                     d = h
+                if self.use_rnn:
+                    out += self._rnn_shapes(f"{tw}core.", d)
+                    d = self.rnn_size
             d_enc = d
-            for tw in ("actor_", "critic_"):
+            for tw in TOWERS:
                 d = d_enc
                 for i, h in enumerate(self.decoder_mlp_layers):
                     out.append((f"{tw}decoder.mlp.{2 * i}.weight", (h, d)))
@@ -373,11 +386,8 @@ class ModelSpec:
             out.append((self.fc_encoder_name(i, "bias"), (h,)))
             d = h
         if self.use_rnn:
-            G, H = self.rnn_gates, self.rnn_size
-            for k in range(self.rnn_num_layers):      # nn.GRU / nn.LSTM registration order: per layer ih, hh, biases
-                out += [(f"core.core.weight_ih_l{k}", (G * H, d)), (f"core.core.weight_hh_l{k}", (G * H, H)),
-                        (f"core.core.bias_ih_l{k}", (G * H,)), (f"core.core.bias_hh_l{k}", (G * H,))]
-                d = H
+            out += self._rnn_shapes("core.", d)
+            d = self.rnn_size
         for i, h in enumerate(self.decoder_mlp_layers):
             out.append((f"decoder.mlp.{2 * i}.weight", (h, d)))
             out.append((f"decoder.mlp.{2 * i}.bias", (h,)))
@@ -390,6 +400,20 @@ class ModelSpec:
         out.append(("action_parameterization.distribution_linear.weight", (self.num_linear_action_outputs, d)))
         out.append(("action_parameterization.distribution_linear.bias", (self.num_linear_action_outputs,)))
         return out
+
+    def _rnn_shapes(self, prefix: str, d: int) -> List[Tuple[str, Tuple[int, ...]]]:
+        """one core's parameters (prefix "core." / "actor_core." / "critic_core.", input width d), in nn.GRU / nn.LSTM
+        registration order: per layer ih, hh, biases"""
+        G, H = self.rnn_gates, self.rnn_size
+        out = []
+        for k in range(self.rnn_num_layers):
+            out += [(f"{prefix}core.weight_ih_l{k}", (G * H, d)), (f"{prefix}core.weight_hh_l{k}", (G * H, H)),
+                    (f"{prefix}core.bias_ih_l{k}", (G * H,)), (f"{prefix}core.bias_hh_l{k}", (G * H,))]
+            d = H
+        return out
+
+
+TOWERS = ("actor_", "critic_")      # separate actor / critic weights: the towers' state_dict prefixes, in state-row order
 
 
 def _align(n: int, a: int = 64) -> int:
@@ -530,7 +554,7 @@ class PolicyModel:
             p = self.params[name]
             if name == "action_parameterization.learned_stddev":
                 p.fill_(math.log(self.spec.initial_stddev))   # action_parameterization.py:59-61
-            elif name.startswith("core.core."):
+            elif ".core.weight_" in name or ".core.bias_" in name:
                 # RNNs keep the PyTorch default init U(-1/sqrt(H), 1/sqrt(H)) (actor_critic.py:83-88)
                 k = 1.0 / math.sqrt(self.spec.rnn_size)
                 p.copy_((torch.rand(p.shape, generator=g) * 2 - 1) * k)
@@ -597,12 +621,19 @@ class PolicyModel:
 
     def tower_layers(self, tower: str, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
         """separate actor / critic weights: [(W, b)] of one tower ("actor_" / "critic_"), encoder then decoder MLP"""
+        return self.tower_encoder_layers(tower, grads) + self.tower_decoder_layers(tower, grads)
+
+    def tower_encoder_layers(self, tower: str, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
+        """[(W, b)] of one tower's encoder MLP (the layers before its core)"""
         src = self.grads if grads else self.params
-        out = [(src[f"{tower}encoder.encoders.obs.mlp_head.{2 * i}.weight"], src[f"{tower}encoder.encoders.obs.mlp_head.{2 * i}.bias"])
-               for i in range(len(self.spec.encoder_mlp_layers))]
-        out += [(src[f"{tower}decoder.mlp.{2 * i}.weight"], src[f"{tower}decoder.mlp.{2 * i}.bias"])
+        return [(src[f"{tower}encoder.encoders.obs.mlp_head.{2 * i}.weight"], src[f"{tower}encoder.encoders.obs.mlp_head.{2 * i}.bias"])
+                for i in range(len(self.spec.encoder_mlp_layers))]
+
+    def tower_decoder_layers(self, tower: str, grads: bool = False) -> List[Tuple[Tensor, Tensor]]:
+        """[(W, b)] of one tower's decoder MLP (the layers after its core)"""
+        src = self.grads if grads else self.params
+        return [(src[f"{tower}decoder.mlp.{2 * i}.weight"], src[f"{tower}decoder.mlp.{2 * i}.bias"])
                 for i in range(len(self.spec.decoder_mlp_layers))]
-        return out
 
     def refresh_cat_heads(self) -> None:
         """separate weights: the heads kernels read ONE tail [M, 2H] = [actor tail | critic tail]; critic_linear and
@@ -627,12 +658,12 @@ class PolicyModel:
         return [(src[f"decoder.mlp.{2 * i}.weight"], src[f"decoder.mlp.{2 * i}.bias"])
                 for i in range(len(self.spec.decoder_mlp_layers))]
 
-    def rnn_params(self, grads: bool = False, layer: int = 0) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
-        """(W_ih [G*H, in], W_hh [G*H, H], b_ih, b_hh) of one layer of the GRU/LSTM core (in = H above layer 0)"""
+    def rnn_params(self, grads: bool = False, layer: int = 0, tower: str = "") -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """(W_ih [G*H, in], W_hh [G*H, H], b_ih, b_hh) of one layer of the GRU/LSTM core (in = H above layer 0); tower
+        "actor_" / "critic_" selects that tower's core of a separate-weights model"""
         src = self.grads if grads else self.params
-        k = layer
-        return (src[f"core.core.weight_ih_l{k}"], src[f"core.core.weight_hh_l{k}"], src[f"core.core.bias_ih_l{k}"],
-                src[f"core.core.bias_hh_l{k}"])
+        p, k = f"{tower}core.core.", layer
+        return (src[f"{p}weight_ih_l{k}"], src[f"{p}weight_hh_l{k}"], src[f"{p}bias_ih_l{k}"], src[f"{p}bias_hh_l{k}"])
 
     def hidden_layer_grads(self) -> List[Tuple[Tensor, Tensor]]:
         return self.encoder_layers(grads=True) + self.decoder_layers(grads=True)

@@ -24,7 +24,7 @@ import torch
 from torch import Tensor
 
 from . import ops
-from .model import PolicyModel
+from .model import TOWERS, PolicyModel
 
 
 class HeadsPlan:
@@ -58,17 +58,26 @@ class HeadsPlan:
         self.wide_logits: Optional[Tensor] = None
         if (self.wide or spec.action_heads) and not need_backward:
             self.wide_logits = torch.empty((max_rows, spec.num_action_params), dtype=torch.float32, device=model.device)
-        # separate actor / critic weights: per-tower activations and ONE concatenated tail [rows, 2H] = [actor | critic]
+        # separate actor / critic weights: per-tower activations and ONE concatenated tail [rows, 2H] = [actor | critic].
+        # tower_h[tw][i] / tower_dz[tw][i]: output of the tower's MLP layer i (encoder then decoder) and its gradient; the
+        # layer that feeds the heads writes its half of tail_cat instead (None here).  With a recurrent core and no decoder
+        # the core's output feeds the heads: every MLP layer keeps its buffer and the core output is copied into tail_cat.
         self.separate = not spec.share_weights
         if self.separate:
             f32 = dict(dtype=torch.float32, device=model.device)
             widths, H = spec.hidden, spec.tail_input_size
-            assert len(widths) > 0, "separate actor / critic weights need at least one MLP layer per tower"
-            self.tower_h = {tw: [torch.empty((max_rows, w), **f32) for w in widths[:-1]] for tw in ("actor_", "critic_")}
+            assert len(widths) > 0 or spec.use_rnn, "separate actor / critic weights need an MLP layer or a core per tower"
+            self.tower_tail_is_mlp = bool(spec.decoder_mlp_layers) or not spec.use_rnn
+            n_tail = 1 if self.tower_tail_is_mlp else 0
+
+            def per_layer():
+                return [torch.empty((max_rows, w), **f32) for w in widths[:len(widths) - n_tail]] + [None] * n_tail
+
+            self.tower_h = {tw: per_layer() for tw in TOWERS}
             self.tail_cat = torch.empty((max_rows, 2 * H), **f32)
             if need_backward:
                 A = spec.num_linear_action_outputs
-                self.tower_dz = {tw: [torch.empty((max_rows, w), **f32) for w in widths[:-1]] for tw in ("actor_", "critic_")}
+                self.tower_dz = {tw: per_layer() for tw in TOWERS}
                 self.dz_cat = torch.empty((max_rows, 2 * H), **f32)
                 self.db_cat = torch.empty(2 * H, **f32)
                 if not self.wide:     # (the wide backward writes the heads' gradients directly)
@@ -91,13 +100,15 @@ class HeadsPlan:
 
 def forward_policy(model: PolicyModel, x: Tensor, outs: List[Tensor], act: int, engine: int, plan: HeadsPlan,
                    heads_kwargs: Dict, rnn_fn: Optional[Callable[[Tensor], Tensor]] = None,
-                   store_tail: bool = True, finish_fn: Optional[Callable] = None) -> Tensor:
+                   store_tail: bool = True, finish_fn: Optional[Callable] = None,
+                   tower_rnn_fns: Optional[Dict[str, Callable[[Tensor], Tensor]]] = None) -> Tensor:
     """x [M, D] (rows may be strided) -> heads outputs described by `heads_kwargs` (the keyword arguments of
     ops.heads_forward after the weights).  outs: one [>=M, h] buffer per MLP layer.  Returns the tensor that fed the
-    heads (None if it was not stored)."""
+    heads (None if it was not stored).  Separate actor / critic weights with recurrent cores take one core function
+    per tower in tower_rnn_fns ({"actor_": fn, "critic_": fn}) instead of rnn_fn."""
     M = x.shape[0]
     if plan.separate:
-        return _forward_separate(model, x, act, engine, plan, heads_kwargs)
+        return _forward_separate(model, x, act, engine, plan, heads_kwargs, tower_rnn_fns)
     if plan.conv is not None:        # ConvEncoder: conv head first, its fully connected layers are `enc` below
         x = plan.conv.forward(x)
     if plan.keys:                    # MultiInputEncoder: the key encoders write the concatenation, `enc` below is empty
@@ -156,19 +167,26 @@ def _forward_keys(model: PolicyModel, x: Tensor, act: int, engine: int, plan: He
     return plan.enc_cat[:M]
 
 
-def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan: HeadsPlan, heads_kwargs: Dict) -> Tensor:
-    """ActorCriticSeparateWeights (model/actor_critic.py:283-318): two MLP towers on the same normalised observation; the
-    towers' last layers write the two halves of one [M, 2H] tail, and the heads read it through zero-padded weights
-    (PolicyModel.refresh_cat_heads), so value = critic half . Wv and logits = actor half . Wa^T."""
+def _forward_separate(model: PolicyModel, x: Tensor, act: int, engine: int, plan: HeadsPlan, heads_kwargs: Dict,
+                      tower_rnn_fns: Optional[Dict[str, Callable[[Tensor], Tensor]]] = None) -> Tensor:
+    """ActorCriticSeparateWeights (model/actor_critic.py:283-318): two towers (encoder MLP -> core -> decoder MLP) on the
+    same normalised observation; each tower's last stage writes its half of one [M, 2H] tail, and the heads read it
+    through zero-padded weights (PolicyModel.refresh_cat_heads), so value = critic half . Wv and logits = actor half .
+    Wa^T.  The last stage is the last MLP layer, or -- a recurrent core without a decoder -- the core, whose output (the
+    top layer's h, a slice of the state row or of the BPTT buffers) is copied into its half with one copy_rows."""
     M = x.shape[0]
     H = model.spec.tail_input_size
-    for tw, col in (("actor_", 0), ("critic_", H)):
+    for tw, col in zip(TOWERS, (0, H)):
         t = x
-        layers = model.tower_layers(tw)
-        for k, (W, b) in enumerate(layers):
-            out = plan.tail_cat[:M, col: col + H] if k == len(layers) - 1 else plan.tower_h[tw][k][:M]
+        enc, dec = model.tower_encoder_layers(tw), model.tower_decoder_layers(tw)
+        for k, (W, b) in enumerate(enc + dec):
+            if tower_rnn_fns is not None and k == len(enc):
+                t = tower_rnn_fns[tw](t)
+            out = plan.tail_cat[:M, col: col + H] if plan.tower_h[tw][k] is None else plan.tower_h[tw][k][:M]
             ops.linear_act_forward(t, W, b, out, act, engine)
             t = out
+        if not plan.tower_tail_is_mlp:      # a core without a decoder feeds the heads
+            ops.copy_rows(tower_rnn_fns[tw](t), plan.tail_cat[:M, col: col + H])
     Wv, bv = model.critic
     Wa, ba = model.actor
     tail = plan.tail_cat[:M]

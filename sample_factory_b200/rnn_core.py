@@ -15,6 +15,12 @@ h, so its x.W_ih^T is again one GEMM over all steps.  A state row is layer-major
 columns [k*Sl, (k+1)*Sl) with Sl = H (GRU, h) or 2H (LSTM, [h | c]); every kernel addresses its slice through a pointer
 offset and the full row stride.  A slice that starts off a 16-byte boundary (H % 4 != 0) is an operand TMA cannot
 describe, and the GEMM engine takes its SIMT path for it.
+
+Separate actor / critic weights (ActorCriticSeparateWeights._core_rnn, model/actor_critic.py:228-273) run one RnnCore
+per tower: it is bound to its parameters (prefix "actor_core." / "critic_core.") and to its half of the state row
+[actor state | critic state] by a column offset, so neither tower's state is split off or concatenated back.  The two
+towers' BPTT buffers keep what each backward reads back; the scratch one backward uses at a time and the reset mask are
+shared (alloc_bptt(shared=...)), since the towers run one after the other.
 """
 from __future__ import annotations
 
@@ -28,21 +34,28 @@ from .model import PolicyModel
 
 
 class RnnCore:
-    def __init__(self, model: PolicyModel, engine: int):
+    def __init__(self, model: PolicyModel, engine: int, tower: str = ""):
+        """tower: "" (the shared model's core), "actor_" or "critic_" (one tower of a separate-weights model)"""
         self.model = model
         self.spec = model.spec
         self.engine = engine
+        self.tower = tower
         self.H = self.spec.rnn_size
         self.G = self.spec.rnn_gates
-        self.S = self.spec.rnn_state_size
+        self.S = self.spec.rnn_state_size            # the full state row
         self.L = self.spec.rnn_num_layers
         self.Sl = self.spec.rnn_layer_state_size     # one layer's columns of a state row
+        self.col = self.spec.rnn_tower_state_size if tower == "critic_" else 0     # first column of this core's half
         self.is_lstm = self.spec.rnn_type == "lstm"
         self.none = ops.ACT["none"]
 
+    def _params(self, grads: bool = False, layer: int = 0):
+        return self.model.rnn_params(grads=grads, layer=layer, tower=self.tower)
+
     def _slice(self, state: Tensor, k: int) -> Tensor:
-        """layer k's columns of [rows, S] state rows"""
-        return state[:, k * self.Sl: (k + 1) * self.Sl]
+        """layer k's columns of this core in [rows, S] state rows"""
+        c = self.col + k * self.Sl
+        return state[:, c: c + self.Sl]
 
     # ------------------------------------------------------------------------------------------------ single step
     def alloc_step(self, M: int):
@@ -55,7 +68,7 @@ class RnnCore:
         (the top layer's new h)."""
         H = self.H
         for k in range(self.L):
-            W_ih, W_hh, b_ih, b_hh = self.model.rnn_params(layer=k)
+            W_ih, W_hh, b_ih, b_hh = self._params(layer=k)
             s_in, s_out = self._slice(state_in, k), self._slice(state_out, k)
             ops.linear_act_forward(x, W_ih, b_ih, bufs["gi"], self.none, self.engine)
             ops.linear_act_forward(s_in[:, :H], W_hh, b_hh, bufs["gh"], self.none, self.engine)
@@ -67,13 +80,16 @@ class RnnCore:
         return x
 
     # ------------------------------------------------------------------------------------------------ BPTT
-    def alloc_bptt(self, B: int, R: int):
+    def alloc_bptt(self, B: int, R: int, shared: Optional[dict] = None):
         """Per layer only what the backward reads back (gates, gh for the GRU, input / output states, core_out); the
-        GEMM outputs and gradient scratch that one layer uses at a time are shared by all layers."""
+        GEMM outputs and gradient scratch that one layer uses at a time are shared by all layers.  shared: the buffers of
+        the other tower's core -- its scratch and reset mask serve this core too."""
         dev, H, G, Sl = self.model.device, self.H, self.G, self.Sl
         n = B // R
         f32 = dict(dtype=torch.float32, device=dev)
-        gh_shared = None if not self.is_lstm else torch.empty((R, n, G * H), **f32)   # the LSTM backward never reads gh
+        gh_shared = None    # the LSTM backward never reads gh: one buffer serves every layer (and both towers)
+        if self.is_lstm:
+            gh_shared = shared["layers"][0]["gh"] if shared is not None else torch.empty((R, n, G * H), **f32)
         layers = []
         for _ in range(self.L):
             layers.append(dict(
@@ -83,9 +99,11 @@ class RnnCore:
                 state_out=torch.empty((R, n, Sl), **f32) if self.is_lstm else None,   # unmasked output state of step t
                 core_out=torch.empty((B, H), **f32),              # env-major: row c*R + t
             ))
-        b = dict(
-            n=n, R=R, layers=layers,
-            core_out=layers[-1]["core_out"],                  # the core's output: the top layer's h
+        b = dict(n=n, R=R, layers=layers, core_out=layers[-1]["core_out"])      # the core's output: the top layer's h
+        if shared is not None:
+            b.update({k: v for k, v in shared.items() if k not in b})
+            return b
+        b.update(
             gi_all=torch.empty((B, G * H), **f32),            # env-major: row c*R + t
             dgi_all=torch.empty((B, G * H), **f32),
             dgh=torch.empty((R, n, G * H), **f32),
@@ -98,15 +116,17 @@ class RnnCore:
         )
         return b
 
-    def forward_bptt(self, head: Tensor, rnn_states: Tensor, dones: Tensor, valids: Tensor, b) -> Tensor:
+    def forward_bptt(self, head: Tensor, rnn_states: Tensor, dones: Optional[Tensor], valids: Tensor, b) -> Tensor:
         """head [B, in] env-major (row c*R+t); rnn_states [B, S] stored states (only rows c*R are used);
-        dones / valids [B] bool.  Returns core_out [B, H] env-major."""
+        dones / valids [B] bool (dones None: the reset mask in b is already this minibatch's, computed by the other
+        tower's core).  Returns core_out [B, H] env-major."""
         n, R, H, G, S = b["n"], b["R"], self.H, self.G, self.S
-        torch.logical_or(dones.view(n, R), ~valids.view(n, R), out=b["doi"])      # done_or_invalid, learner.py:560
+        if dones is not None:
+            torch.logical_or(dones.view(n, R), ~valids.view(n, R), out=b["doi"])      # done_or_invalid, learner.py:560
         gi3 = b["gi_all"].view(n, R, G * H)
         x = head
         for k, lb in enumerate(b["layers"]):
-            W_ih, W_hh, b_ih, b_hh = self.model.rnn_params(layer=k)
+            W_ih, W_hh, b_ih, b_hh = self._params(layer=k)
             ops.linear_act_forward(x, W_ih, b_ih, b["gi_all"], self.none, self.engine)
             ops.copy_rows(self._slice(rnn_states.view(n, R * S), k), lb["state_in"][0])   # chunk-start states
             core3 = lb["core_out"].view(n, R, H)
@@ -133,8 +153,8 @@ class RnnCore:
         dgi3 = b["dgi_all"].view(n, R, G * H)
         for k in range(self.L - 1, -1, -1):
             lb = b["layers"][k]
-            W_ih, W_hh, b_ih, b_hh = self.model.rnn_params(layer=k)
-            dW_ih, dW_hh, db_ih, db_hh = self.model.rnn_params(grads=True, layer=k)
+            W_ih, W_hh, b_ih, b_hh = self._params(layer=k)
+            dW_ih, dW_hh, db_ih, db_hh = self._params(grads=True, layer=k)
             dcore3 = (d_core if k == self.L - 1 else b["d_core_below"]).view(n, R, H)
             carry_gemm: Optional[Tensor] = None
             carry_direct: Optional[Tensor] = None

@@ -23,7 +23,7 @@ import torch
 from torch import Tensor
 
 from . import ops
-from .model import PolicyModel
+from .model import TOWERS, PolicyModel
 from .policy import HeadsPlan, forward_policy
 from .rnn_core import RnnCore
 
@@ -71,10 +71,15 @@ class DeviceSampler:
         self.heads_plan = HeadsPlan(model, engine, self.N)
         self.last_rnn_state = torch.zeros((self.N, traj["rnn_states"].shape[2]), **f32)
         self.rnn: Optional[RnnCore] = None
+        self.tower_rnn: Optional[Dict[str, RnnCore]] = None      # separate weights: one core per tower, on its half of a row
         if spec.use_rnn:
             assert traj["rnn_states"].shape[2] == spec.rnn_state_size
-            self.rnn = RnnCore(model, engine)
-            self.rnn_step_bufs = self.rnn.alloc_step(self.N)
+            if spec.share_weights:
+                self.rnn = RnnCore(model, engine)
+            else:
+                self.tower_rnn = {tw: RnnCore(model, engine, tw) for tw in TOWERS}
+            # (the towers step one after the other: one set of step buffers serves both)
+            self.rnn_step_bufs = (self.rnn or self.tower_rnn[TOWERS[0]]).alloc_step(self.N)
             self.new_rnn_state = torch.zeros((self.N, spec.rnn_state_size), **f32)
         # policy version lives on the device so a captured graph always stamps the current one (inference_worker.py:332)
         self.policy_version = torch.zeros(1, **f32)
@@ -111,7 +116,7 @@ class DeviceSampler:
         from .envs import TapeVecEnv
         self.fused_tail = (os.environ.get("SFB200_TAIL_FUSED", "1") != "0" and type(env) is TapeVecEnv and
                            not env.continuous and not env.action_segments and not env.with_action_mask and
-                           not env.obs_uint8 and self.rnn is None and self.heads_plan.P > 0 and
+                           not env.obs_uint8 and not spec.use_rnn and self.heads_plan.P > 0 and
                            not self.heads_plan.finish_in_gemm and not self.heads_plan.separate and
                            not spec.continuous and not spec.action_segments and not spec.action_heads)
         # Whole rollout as ONE persistent kernel (csrc/rollout_fused.cu): clusters of H2/256 CTAs own a 64-env row block for
@@ -158,9 +163,12 @@ class DeviceSampler:
         """policy forward + sampling on the pre-step's x_norm; outputs go straight into traj[:, t].  fused_tail: the same
         launch that finishes the heads also steps the tape env and runs post-step(t) + pre-step(t+1)."""
         cfg, m, spec, tr = self.cfg, self.model, self.model.spec, self.traj
-        rnn_fn = None
+        rnn_fn = tower_fns = None
         if self.rnn is not None:   # ModelCoreRNN.forward (core.py:37-64), one step
             rnn_fn = lambda head: self.rnn.step(head, self.last_rnn_state, self.new_rnn_state, self.rnn_step_bufs)
+        elif self.tower_rnn is not None:   # ActorCriticSeparateWeights._core_rnn (actor_critic.py:259-271), one step per tower
+            tower_fns = {tw: (lambda head, c=c: c.step(head, self.last_rnn_state, self.new_rnn_state, self.rnn_step_bufs))
+                         for tw, c in self.tower_rnn.items()}
         noise_t = None if self.noise is None else self.noise[t]
         heads_kwargs = dict(
             values=tr["values"][:, t], values_stride=tr["values"].stride(0),
@@ -202,7 +210,7 @@ class DeviceSampler:
 
         try:
             forward_policy(m, self.x_norm, self.h, self.act, self.engine, self.heads_plan, heads_kwargs, rnn_fn,
-                           store_tail=False, finish_fn=finish_fn)
+                           store_tail=False, finish_fn=finish_fn, tower_rnn_fns=tower_fns)
         finally:
             if special:
                 ops.set_sampling_mode(None, False)
@@ -231,7 +239,7 @@ class DeviceSampler:
                      None if self.fin_return is None else self.fin_return[:, t],
                      None if self.fin_len is None else self.fin_len[:, t])
         last = t + 1 == self.T
-        if self.rnn is None:
+        if not spec.use_rnn:
             # non-recurrent core: new_rnn_states == rnn_states (core.py:76-77), times (1-done) stays zero
             mean = m.obs_mean if spec.normalize_input else None
             var = m.obs_var if spec.normalize_input else None
