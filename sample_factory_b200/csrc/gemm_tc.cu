@@ -49,14 +49,18 @@ constexpr int kConsumerRegs = 232;
 // B_MN only names the twin the host chose (the transposed one for dX = dz . W), so dX stays its own instantiation.
 // RES: the residual epilogue (store_tile_residual), forward layout only.
 //
-// Mainloop: the split of stage kb+1 runs while the wgmmas of stage kb are in flight (two conversion buffers).  A and B
-// have their own TMA rings: a raw slot goes back to the producer as soon as it is split, an fp16 B slot (the twin tiles
-// the wgmmas read in place) once its wgmmas have completed.  Every accumulator receives the same wgmmas in the same k order as a serial loop would issue.
+// Mainloop: tf32 form: the split of stage kb+1 runs while the wgmmas of stage kb are in flight (two conversion buffers).
+// fp16 forms: each warpgroup reads the raw fp32 A of its own 64 rows (128B-swizzled by TMA) straight into the register
+// fragments of the register-A form of fp16 wgmma, splitting them on the way, and keeps two groups of wgmmas (half a stage
+// each) in flight.  A and B have their own TMA rings: a raw slot goes back to the producer as soon as it is split or in
+// registers, an fp16 B slot (the twin tiles the wgmmas read in place) once its wgmmas have completed.  Every accumulator
+// receives the same wgmmas in the same k order as a serial loop would issue.
 //
 // DW16: the fp16 form of dW = dz^T . x (gemm_dw_f16_kernel): both operands are MN-major activations with registered
-// bounds (a_bound, b_bound).  The raw fp32 tiles come through the tf32 form's 32-k rings; the consumers split both into
-// scaled fp16 hi / lo halves in the MN-major layout (split_tile_f16_mn, no transpose), which fp16 wgmma reads with its
-// transpose bits set; the three MMAs and the output scaling are the fp16 form's, the epilogue the plain one.
+// bounds (a_bound, b_bound), in 32-k stages.  A goes into register fragments as in the fp16 form; the consumers split raw
+// B into scaled fp16 hi / lo halves in the MN-major layout (split_tile_f16_mn, no transpose, three conversion buffers),
+// which fp16 wgmma reads with its transpose bit set; the three MMAs and the output scaling are the fp16 form's, the
+// epilogue the plain one.
 template <bool A_MN, bool B_MN, bool SPLIT3, bool HEADS, bool F16, bool RES, bool DW16>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, float* __restrict__ C,
                                              int64_t ldc, int64_t M, int N, int K, int k_chunk, int splits,
@@ -73,7 +77,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
     uint8_t* conv = smem + S::CONV_OFF;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::BARS_OFF);
     uint64_t* full_a = bars;                // A slot landed (count 1 + tx)
-    uint64_t* empty_a = bars + SA;          // A slot split by every consumer thread (count 256)
+    uint64_t* empty_a = bars + SA;          // A slot split / in registers in every consumer thread (count 256)
     uint64_t* full_b = bars + 2 * SA;
     uint64_t* empty_b = bars + 2 * SA + SB; // B slot split (tf32) / read by the completed wgmmas (fp16), count 256
     int* s_last = reinterpret_cast<int*>(bars + 2 * (SA + SB));
@@ -103,7 +107,8 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
     pdl_trigger();
     if (trace && threadIdx.x == 0) trace[blockIdx.x * kTraceWords + 9] = tc_now();
 
-    // g0: stages of the CTA's earlier items -- stage g = g0 + kb uses ring slots g % SA, g % SB, conversion buffer g & 1
+    // g0: stages of the CTA's earlier items -- stage g = g0 + kb uses ring slots g % SA, g % SB (and conversion buffer g & 1
+    // in the tf32 form, g % 3 in DW16)
     if (warp < 4) {
         // ===================================================== TMA producer
         setmaxnreg_dec<kProducerRegs>();
@@ -119,8 +124,16 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
                 if (trace && kb == 0) trace[item * kTraceWords + 6] = tc_now();
                 mbar_expect_tx(&full_a[sa], S::A_RAW);
                 uint8_t* pa = smem + sa * S::A_RAW;
-                if (A_MN) tma_load_2d(pa, &tmap_a, &full_a[sa], (int)tc.m0, k0);
-                else tma_load_2d(pa, &tmap_a, &full_a[sa], k0, (int)tc.m0);
+                if (F16) {   // two swizzled [128 rows][32 k] boxes
+                    tma_load_2d(pa, &tmap_a, &full_a[sa], k0, (int)tc.m0);
+                    tma_load_2d(pa + TBM * 128, &tmap_a, &full_a[sa], k0 + 32, (int)tc.m0);
+                } else if (DW16) {   // four swizzled [32 k][32 rows] boxes
+                    for (int b = 0; b < TBM / 32; ++b) tma_load_2d(pa + b * 4096, &tmap_a, &full_a[sa], (int)tc.m0 + 32 * b, k0);
+                } else if (A_MN) {
+                    tma_load_2d(pa, &tmap_a, &full_a[sa], (int)tc.m0, k0);
+                } else {
+                    tma_load_2d(pa, &tmap_a, &full_a[sa], k0, (int)tc.m0);
+                }
                 mbar_wait(&empty_b[sb], ((g / SB) & 1) ^ 1);
                 mbar_expect_tx(&full_b[sb], S::B_SLOT);
                 uint8_t* pb = smem + S::B_RING + sb * S::B_SLOT;
@@ -144,27 +157,65 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
     const float a_scale = pow2f_int(a_shift);
     const int b_shift = DW16 ? f16_shift_for_bound(b_bound[0]) : kF16WShift;
     const float b_scale = pow2f_int(b_shift);
-    // split stage g into conversion buffer g & 1
+    // tf32 form: split stage g into conversion buffer g & 1
     auto split_stage = [&](int g) {
         const int sa = g % SA, sb = g % SB;
         const uint8_t* pa = smem + sa * S::A_RAW;
         uint8_t* cv = conv + (g & 1) * S::CONV;
         mbar_wait(&full_a[sa], (g / SA) & 1);
-        if constexpr (F16) {
-            split_tile_f16<false>(pa, cv, cv + S::A_HALF, ct, a_scale);
-        } else if constexpr (DW16) {
-            split_tile_f16_mn(pa, cv, cv + S::A_HALF, ct, a_scale);
-            mbar_wait(&full_b[sb], (g / SB) & 1);
-            split_tile_f16_mn(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct, b_scale);
-            mbar_arrive(&empty_b[sb]);
-        } else {
-            split_tile<A_MN, SPLIT3>(pa, cv, cv + S::A_HALF, ct);
-            mbar_wait(&full_b[sb], (g / SB) & 1);
-            split_tile<B_MN, SPLIT3>(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct);
-            mbar_arrive(&empty_b[sb]);
-        }
+        split_tile<A_MN, SPLIT3>(pa, cv, cv + S::A_HALF, ct);
+        mbar_wait(&full_b[sb], (g / SB) & 1);
+        split_tile<B_MN, SPLIT3>(smem + S::B_RING + sb * S::B_SLOT, cv + 2 * S::A_HALF, cv + 2 * S::A_HALF + S::B_HALF, ct);
+        mbar_arrive(&empty_b[sb]);
         mbar_arrive(&empty_a[sa]);
         fence_proxy_async_smem();              // generic-proxy writes -> visible to the tensor core (async proxy)
+    };
+    // fp16 forms: the A fragments of half h of stage g in registers (F16: 32 k, the h-th swizzled box; DW16: 16 k).  The
+    // A slot goes back to the producer once both halves are in registers.
+    constexpr int KS = KBK / 32;   // k16 steps per half stage
+    using Frags = F16Frags<KS>;
+    auto load_frags = [&](int g, int h, Frags& f) {
+        const int sa = g % SA;
+        const uint8_t* pa = smem + sa * S::A_RAW;
+        if (h == 0) mbar_wait(&full_a[sa], (g / SA) & 1);
+        if constexpr (F16) load_a_frags_f16(pa + h * (TBM * 128), wg * 64, ct & 127, a_scale, f);
+        else if constexpr (DW16) load_a_frags_f16_mn(pa, 16 * h, wg * 64, ct & 127, a_scale, f);
+        if (h == 1) mbar_arrive(&empty_a[sa]);
+    };
+    // DW16: split raw B stage g into conversion buffer g % 3 (its hi / lo halves, MN-major), release the raw slot
+    auto split_b = [&](int g) {
+        const int sb = g % SB;
+        uint8_t* cv = conv + (g % 3) * S::CONV;
+        mbar_wait(&full_b[sb], (g / SB) & 1);
+        split_tile_f16_mn(smem + S::B_RING + sb * S::B_SLOT, cv, cv + S::B_HALF, ct, b_scale);
+        mbar_arrive(&empty_b[sb]);
+        fence_proxy_async_smem();
+    };
+    // fp16 forms: the wgmmas of half h of stage g, A from the fragments f, as one committed group
+    auto issue_f16 = [&](int g, int h, const Frags& f, float (&acc)[64], float (&cross)[64]) {
+        if constexpr (F16) {
+            const int sb = g % SB;
+            const uint8_t* bt = smem + S::B_RING + sb * S::B_SLOT;
+            const uint64_t db_hi = make_smem_desc(smem_u32(bt)) + (uint64_t)(64 >> 4) * h;   // 64 B: 32 k of fp16
+            const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF)) + (uint64_t)(64 >> 4) * h;
+            if (h == 0) mbar_wait(&full_b[sb], (g / SB) & 1);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < KS; ++k) {
+                const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k16 inside the swizzle row
+                wgmma_m64n128k16_f16_rs<0>(acc, f.hi[k], db_hi + o);
+                wgmma_m64n128k16_f16_rs<0>(cross, f.hi[k], db_lo + o);
+                wgmma_m64n128k16_f16_rs<0>(cross, f.lo[k], db_hi + o);
+            }
+        } else {
+            const uint8_t* cv = conv + (g % 3) * S::CONV;
+            const uint64_t o = (uint64_t)(2048 >> 4) * h;   // a k-step of 16 is two 1024 B atoms
+            wgmma_fence();
+            wgmma_m64n128k16_f16_rs<1>(acc, f.hi[0], make_smem_desc_mn(smem_u32(cv)) + o);
+            wgmma_m64n128k16_f16_rs<1>(cross, f.hi[0], make_smem_desc_mn(smem_u32(cv + S::B_HALF)) + o);
+            wgmma_m64n128k16_f16_rs<1>(cross, f.lo[0], make_smem_desc_mn(smem_u32(cv)) + o);
+        }
+        wgmma_commit();
     };
     int g0 = 0;
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
@@ -178,57 +229,65 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
             tr[3] = tc_now();
         }
         float acc[64], cross[64];
-#pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
-        split_stage(g0);
-        consumer_sync();
-        for (int kb = 0; kb < tc.num_kb; ++kb) {
-            const int g = g0 + kb;
-            const int sb = g % SB;
-            const uint8_t* cv = conv + (g & 1) * S::CONV;
+        if constexpr (F16 || DW16) {
+            // Two groups of wgmmas in flight, a group being half a stage: half 0 of each stage is issued from the
+            // fragment set fa, half 1 from fb; after each issue wait_group 1 retires the group before, whose fragment
+            // set then takes the next half's A, and, when that group ended stage g-1, whose B slot (F16) goes back to
+            // the producer.  F16: the warpgroups share nothing but the mbarriers.  DW16: both warpgroups read the whole
+            // split B of a stage, so a consumer barrier follows each split (the wgmmas issued before keep running).
+            Frags fa, fb;
+            load_frags(g0, 0, fa);
             if constexpr (DW16) {
-                // A: warpgroup wg's 64 rows are the wg-th 64-row atom column; a k-step of 16 is two 1024 B atoms
-                const uint64_t da_hi = make_smem_desc_mn(smem_u32(cv + wg * 4096));
-                const uint64_t da_lo = make_smem_desc_mn(smem_u32(cv + S::A_HALF + wg * 4096));
-                const uint64_t db_hi = make_smem_desc_mn(smem_u32(cv + 2 * S::A_HALF));
-                const uint64_t db_lo = make_smem_desc_mn(smem_u32(cv + 2 * S::A_HALF + S::B_HALF));
-                wgmma_fence();
+                split_b(g0);
+                consumer_sync();
+            }
 #pragma unroll
-                for (int k = 0; k < TBK / 16; ++k) {
-                    const uint64_t o = (uint64_t)(2048 >> 4) * k;
-                    wgmma_m64n128k16_f16_mn(acc, da_hi + o, db_hi + o, 1);
-                    wgmma_m64n128k16_f16_mn(cross, da_hi + o, db_lo + o, 1);
-                    wgmma_m64n128k16_f16_mn(cross, da_lo + o, db_hi + o, 1);
+            for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+            for (int kb = 0; kb < tc.num_kb; ++kb) {
+                const int g = g0 + kb;
+                issue_f16(g, 0, fa, acc, cross);
+                wgmma_wait_1();
+                if (F16 && kb > 0) mbar_arrive(&empty_b[(g - 1) % SB]);   // stage g-1's wgmmas are done with its B twins
+                load_frags(g, 1, fb);
+                issue_f16(g, 1, fb, acc, cross);
+                wgmma_wait_1();
+                if (kb + 1 < tc.num_kb) {
+                    load_frags(g + 1, 0, fa);
+                    if constexpr (DW16) {
+                        split_b(g + 1);
+                        consumer_sync();
+                    }
                 }
-            } else {
+            }
+            wgmma_wait_all();
+            if (F16) mbar_arrive(&empty_b[(g0 + tc.num_kb - 1) % SB]);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = cross[i] = 0.f;
+            split_stage(g0);
+            consumer_sync();
+            for (int kb = 0; kb < tc.num_kb; ++kb) {
+                const int g = g0 + kb;
+                const uint8_t* cv = conv + (g & 1) * S::CONV;
                 const uint64_t da_hi = make_smem_desc(smem_u32(cv + wg * 64 * 128));
                 const uint64_t da_lo = make_smem_desc(smem_u32(cv + S::A_HALF + wg * 64 * 128));
-                const uint8_t* bt = F16 ? smem + S::B_RING + sb * S::B_SLOT : cv + 2 * S::A_HALF;
-                const uint64_t db_hi = make_smem_desc(smem_u32(bt));
-                const uint64_t db_lo = make_smem_desc(smem_u32(bt + S::B_HALF));
-                if (F16) mbar_wait(&full_b[sb], (g / SB) & 1);
+                const uint64_t db_hi = make_smem_desc(smem_u32(cv + 2 * S::A_HALF));
+                const uint64_t db_lo = make_smem_desc(smem_u32(cv + 2 * S::A_HALF + S::B_HALF));
                 wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < TBK / WG_K; ++k) {
-                    const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step (8 tf32 or 16 fp16) inside the swizzle row
-                    if constexpr (F16) {
-                        wgmma_m64n128k16_f16(acc, da_hi + o, db_hi + o, 1);
-                        wgmma_m64n128k16_f16(cross, da_hi + o, db_lo + o, 1);
-                        wgmma_m64n128k16_f16(cross, da_lo + o, db_hi + o, 1);
-                    } else {
-                        wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
-                    }
-                    if (SPLIT3 && !F16) {
+                    const uint64_t o = (uint64_t)(32 >> 4) * k;   // 32 B per k-step of 8 tf32 inside the swizzle row
+                    wgmma_m64n128k8_tf32(acc, da_hi + o, db_hi + o, 1);
+                    if (SPLIT3) {
                         wgmma_m64n128k8_tf32(cross, da_hi + o, db_lo + o, 1);
                         wgmma_m64n128k8_tf32(cross, da_lo + o, db_hi + o, 1);
                     }
                 }
+                wgmma_commit();
+                if (kb + 1 < tc.num_kb) split_stage(g + 1);    // overlaps the wgmmas just issued
+                wgmma_wait_all();
+                consumer_sync();                       // split g+1 complete, buffer g & 1 free for g+2, in both warpgroups
             }
-            wgmma_commit();
-            if (kb + 1 < tc.num_kb) split_stage(g + 1);    // overlaps the wgmmas just issued
-            wgmma_wait_all();
-            if (F16) mbar_arrive(&empty_b[sb]);    // the wgmmas are done with the B twin tiles
-            consumer_sync();                       // split g+1 complete, buffer g & 1 free for g+2, in both warpgroups
         }
         g0 += tc.num_kb;
         if (tr) tr[4] = tc_now();
@@ -336,16 +395,16 @@ bool tc_init() {
     return true;
 }
 
-// 2-D fp32 tensor map without swizzle. dim0 = contiguous dim.
+// 2-D fp32 tensor map, without swizzle or with the 128B swizzle (box0 * 4 = 128 B then). dim0 = contiguous dim.
 bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
-               uint32_t box1) {
+               uint32_t box1, bool swizzle128) {
     cuuint64_t gdim[2] = {dim0, dim1};
     cuuint64_t gstride[1] = {stride1_elems * sizeof(float)};
     cuuint32_t box[2] = {box0, box1};
     cuuint32_t estride[2] = {1, 1};
     CUresult r = g_encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estride,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
 
@@ -462,7 +521,7 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
                 const int rc_chk = b_mn ? f16_twins_check(B, tw, K, N, true, st) : f16_twins_check(B, tw, N, K, false, st);
                 if (rc_chk) return rc_chk;
             }
-            if (!make_tmap(&ta16, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, 64, TBM)) return SFB_TC_UNSUPPORTED;
+            if (!make_tmap(&ta16, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, 32, TBM, true)) return SFB_TC_UNSUPPORTED;
             if (epi.head_part) return launch_tc<false, false, true, true, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound);
             return b_mn ? launch_tc<false, true, true, false, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound)
                         : launch_tc<false, false, true, false, true>(ta16, tb16, C, ldc, M, N, K, K, 1, epi, st, a_bound);
@@ -503,9 +562,11 @@ static int gemm_tc(bool a_mn, const float* A, int64_t lda, bool b_mn, const floa
 #define SFB_TC(AM, BM_)                                                                                          \
     (split3 ? launch_tc<AM, BM_, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st)                 \
             : launch_tc<AM, BM_, false>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st))
+    CUtensorMap ta_sw;   // DW16: A in four swizzled [32 k][32 rows] boxes per stage
+    if (b_bound && !make_tmap(&ta_sw, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 32, TBK, true)) return SFB_TC_UNSUPPORTED;
     if (b_bound)
-        rc = launch_tc<true, true, true, false, false, false, true>(ta, tb, out, ld_out, M, N, K, k_chunk, splits, epi, st,
-                                                                   a_bound, b_bound);
+        rc = launch_tc<true, true, true, false, false, false, true>(ta_sw, tb, out, ld_out, M, N, K, k_chunk, splits, epi,
+                                                                   st, a_bound, b_bound);
     else if (!a_mn && !b_mn) rc = SFB_TC(false, false);
     else if (!a_mn && b_mn) rc = SFB_TC(false, true);
     else if (a_mn && b_mn) rc = SFB_TC(true, true);

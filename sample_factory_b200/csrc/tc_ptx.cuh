@@ -147,15 +147,18 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t de
         : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
-// The same with both operands MN-major (imm-trans-a = imm-trans-b = 1: A is [k][m], B is [k][n] in shared memory).
-__device__ __forceinline__ void wgmma_m64n128k16_f16_mn(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t scale_d) {
+// The same shape with the fp16 A operand in registers: a[4] is the thread's m64k16 fragment (warp w of the warpgroup
+// holds rows 16w .. 16w+15 in the mma.m16n8k16 A layout, F16Frags in wgmma_tile.cuh), B from shared memory, K-major
+// (TRANS_B = 0) or MN-major (TRANS_B = 1).
+template <int TRANS_B>
+__device__ __forceinline__ void wgmma_m64n128k16_f16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %66, 0;\n"
+        "setp.ne.b32 p, %70, 0;\n"
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
-        "%64, %65, p, 1, 1, 1, 1;\n"
+        "{%64, %65, %66, %67}, %68, p, 1, 1, %69;\n"
         "}\n"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
           "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),
@@ -165,7 +168,7 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16_mn(float (&d)[64], uint64_t
           "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
           "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
           "+f"(d[63])
-        : "l"(desc_a), "l"(desc_b), "r"(scale_d));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "n"(TRANS_B), "r"(1u));
 }
 
 // ------------------------------------------------------------------------------------------------ descriptors
@@ -217,10 +220,11 @@ __device__ __forceinline__ float act_bwd_ct(float h) {
 }
 
 // host side (gemm_tc.cu): driver entry point for cuTensorMapEncodeTiled resolved at run time; 2-D fp32 tensor maps
-// without swizzle (the engine re-lays the tiles out itself). dim0 = contiguous dimension.
+// without swizzle (the engine re-lays the tiles out itself), or with the 128B swizzle for tiles read straight into
+// wgmma register fragments (box0 = 32). dim0 = contiguous dimension.
 bool tc_init();
 bool make_tmap(CUtensorMap* out, const float* base, uint64_t dim0, uint64_t dim1, uint64_t stride1_elems, uint32_t box0,
-               uint32_t box1);
+               uint32_t box1, bool swizzle128 = false);
 // 3-D fp16 map over a [hi | lo] pair of row-major [rows][K] planes, lo_offset elements apart: box 64 k x box_rows rows x
 // both planes with the 128B swizzle (the weights' registered twins; the rollout's split h1 scratch)
 bool make_tmap_f16_twins(CUtensorMap* out, const uint16_t* hi, int64_t lo_offset, uint64_t K, uint64_t rows,

@@ -33,29 +33,35 @@ constexpr int kHeadPad = 12;   // floats per (partial, row): three 16 B stores
 constexpr int TC_THREADS = 384;
 
 // Shared memory of gemm_wgmma_kernel: a ring of A_STAGES TMA slots for the raw A tile, a ring of B_STAGES slots for the B
-// tile, two conversion buffers (the split of stage kb+1 is written into one while the wgmmas of stage kb read the other),
-// the mbarriers.
-//   tf32 form: raw A / raw B fp32 tiles of 32 k (16 KB each, both released once split); conversion buffer =
+// tile, CONV_BUFS conversion buffers (the split of stage kb+1 is written into one while the wgmmas of earlier stages read
+// the others), the mbarriers.
+//   tf32 form: raw A / raw B fp32 tiles of 32 k (16 KB each, both released once split); two conversion buffers =
 //              [A hi | A lo | B hi | B lo] (64 KB)
-//   fp16 form: raw A fp32 tile of 64 k (32 KB, released once split); B = the weight tile's fp16 [hi | lo] twins, TMA-loaded
-//              in the swizzled layout wgmma reads (32 KB, released once its wgmmas completed); conversion buffer =
-//              [A hi | A lo] (32 KB)
-//   fp16 dW form (DW16, gemm_dw_f16_kernel): raw MN-major A / B fp32 tiles of 32 k as in the tf32 form (16 KB each);
-//              conversion buffer = [A hi | A lo | B hi | B lo], each [32 k][128 rows] fp16 MN-major (8 KB): 160 KB in all
+//   fp16 form: raw A fp32 tile of 64 k as two 128B-swizzled [128 rows][32 k] boxes (32 KB, released once the consumers
+//              hold their fragments in registers); B = the weight tile's fp16 [hi | lo] twins, TMA-loaded in the swizzled
+//              layout wgmma reads (32 KB, released once its wgmmas completed); no conversion buffer: 3 A + 4 B slots,
+//              224 KB.  Four B slots: a warpgroup holds two (the stages in flight) while the producer fills the others.
+//   fp16 dW form (DW16, gemm_dw_f16_kernel): raw MN-major A fp32 tile of 32 k as four 128B-swizzled [32 k][32 rows]
+//              boxes (16 KB, released once in registers), raw MN-major B tile as in the tf32 form (16 KB, released once
+//              split); three conversion buffers [B hi | B lo], each [32 k][128 rows] fp16 MN-major (8 KB): with two
+//              stages of wgmmas in flight per warpgroup and the warpgroups up to a stage apart, three are read or
+//              written at once.  4 A + 4 B slots: 176 KB.
 template <bool F16, bool DW16 = false>
 struct TcSmem {
     static constexpr int KBK = F16 ? 64 : TBK;                    // k per stage
-    static constexpr int A_STAGES = F16 ? 2 : 3;
-    static constexpr int B_STAGES = 3;
+    static constexpr int A_STAGES = F16 ? 3 : DW16 ? 4 : 3;
+    static constexpr int B_STAGES = (F16 || DW16) ? 4 : 3;
     static constexpr int A_RAW = TBM * KBK * 4;
     static constexpr int B_SLOT = F16 ? 2 * TBN * 64 * 2 : TBN * TBK * 4;
-    // one split half of A: [128 rows][128 B] swizzled K-major; DW16: [32 k][128 rows] fp16 (split_tile_f16_mn)
-    static constexpr int A_HALF = DW16 ? TBM * TBK * 2 : TBM * 128;
+    // one split half of A (tf32 form): [128 rows][128 B] swizzled K-major
+    static constexpr int A_HALF = TBM * 128;
+    // one split half of B: tf32 form [128 rows][128 B] swizzled K-major; DW16 [32 k][128 rows] fp16 (split_tile_f16_mn)
     static constexpr int B_HALF = DW16 ? TBN * TBK * 2 : TBN * 128;
-    static constexpr int CONV = F16 ? 2 * A_HALF : 2 * A_HALF + 2 * B_HALF;
+    static constexpr int CONV = F16 ? 0 : DW16 ? 2 * B_HALF : 2 * A_HALF + 2 * B_HALF;
+    static constexpr int CONV_BUFS = F16 ? 0 : DW16 ? 3 : 2;
     static constexpr int B_RING = A_STAGES * A_RAW;               // offsets from the 1024-aligned base
     static constexpr int CONV_OFF = B_RING + B_STAGES * B_SLOT;
-    static constexpr int BARS_OFF = CONV_OFF + 2 * CONV;
+    static constexpr int BARS_OFF = CONV_OFF + CONV_BUFS * CONV;
     static constexpr int BARS = 2 * (A_STAGES + B_STAGES) * 8 + 16;
     static constexpr int TOTAL = 1024 /*align slack*/ + BARS_OFF + BARS;
     static_assert(TOTAL <= 227 * 1024, "shared memory");
@@ -155,6 +161,47 @@ __device__ __forceinline__ void split_tile_f16_mn(const uint8_t* raw, uint8_t* h
         f16_split2(v.z * scale, v.w * scale, h.y, l.y);
         *reinterpret_cast<uint2*>(hi + off) = h;
         *reinterpret_cast<uint2*>(lo + off) = l;
+    }
+}
+
+// A thread's fp16 A operand of half a stage in registers (the register-A form of fp16 wgmma): per k16 step the four
+// .f16x2 words of its m64k16 fragment, hi and lo halves.  Word j holds rows row + 8 * (j & 1), k = k16 + 2 * (lane % 4) +
+// 8 * (j / 2) + {0, 1} (element 0 in the low 16 bits), row = the warpgroup's first row + 16 * warp + lane / 4 -- the
+// mma.m16n8k16 A layout, one warp per 16 rows.
+template <int KS>
+struct F16Frags {
+    uint32_t hi[KS][4], lo[KS][4];
+};
+
+// fp16 form: fragments (32 k) of the rows from row0 (0 or 64) of a raw fp32 K-major [128 rows][32 k] box that TMA stored
+// with the 128B swizzle, times scale, split by f16_split2: the bits split_tile_f16 writes.  lt = thread of the warpgroup.
+// A warp's float2 loads cover eight rows of 32 B; the swizzle puts them in distinct 16 B columns pairwise, so each load
+// is the two wavefronts its 256 B need.
+__device__ __forceinline__ void load_a_frags_f16(const uint8_t* box, int row0, int lt, float scale, F16Frags<2>& f) {
+    const int r = row0 + 16 * (lt >> 5) + ((lt & 31) >> 2), q = lt & 3;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 x = *reinterpret_cast<const float2*>(box + sw128_offset(r + 8 * (j & 1), 16 * s + 2 * q + 8 * (j >> 1)));
+            f16_split2(x.x * scale, x.y * scale, f.hi[s][j], f.lo[s][j]);
+        }
+    }
+}
+
+// fp16 dW form: the fragments of k = k16 .. k16+15 from a raw fp32 MN-major tile [32 k][128 rows] that TMA stored as four
+// 128B-swizzled [32 k][32 rows] boxes (box b: rows 32b .. 32b+31; element (k, row) at b * 4096 + sw128_offset(k, row % 32)),
+// the bits split_tile_f16_mn writes.  Scalar loads: a warp reads eight rows at four k, which the swizzle spreads over 32
+// banks.
+__device__ __forceinline__ void load_a_frags_f16_mn(const uint8_t* raw, int k16, int row0, int lt, float scale, F16Frags<1>& f) {
+    const int r = row0 + 16 * (lt >> 5) + ((lt & 31) >> 2), q = lt & 3;
+    const float* p = reinterpret_cast<const float*>(raw);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int m = r + 8 * (j & 1), k = k16 + 2 * q + 8 * (j >> 1);
+        const float x0 = p[((m >> 5) * 4096 + sw128_offset(k, m & 31)) / 4];
+        const float x1 = p[((m >> 5) * 4096 + sw128_offset(k + 1, m & 31)) / 4];
+        f16_split2(x0 * scale, x1 * scale, f.hi[0][j], f.lo[0][j]);
     }
 }
 
