@@ -8,7 +8,14 @@
 // thread-block CLUSTER of CX = H2/BN CTAs owns a row block for the whole rollout and the only synchronisation is the
 // cluster barrier (three per step); there is no grid-wide barrier and no kernel boundary.  CTA c of the cluster computes
 // columns [BN c, BN c + BN) of h1, then of h2 (partial head products), then finishes rows [c BM/CX.., ) of the block.
-// h1 and the head partials cross between the CTAs of a cluster through global memory (L2-resident), read back by TMA.
+// Hand-offs between the phases of a step, by layout:
+//   h1, x_norm          every layout: global memory (L2-resident), read back by TMA.
+//   head partials       fp16 form (both layouts): written by the layer-2 epilogue straight into the shared memory of the
+//                       CTA that finishes the row (st.shared::cluster), summed from there by the tail; barrier 2 orders
+//                       writer and reader, and barriers 3 and 1 of the next step come between the tail's reads and the
+//                       next writes.  tf32 form: global memory.
+//   b1, b2, [Wv; Wa] rows, bv, ba   fp16 form: copied into shared memory once per launch (this CTA's BN columns), read
+//                       from there by both epilogues and the tail.  tf32 form (no room beside its 104 KB slots): global.
 // The CTA tile (rf_wide): BM x BN = 64 x 256 for H2 >= 256 (the two consumer warpgroups side by side on N over one 64-row
 // A tile), 128 x 128 for H2 = 128 (the warpgroups stacked on M).  At H2 = 512 that makes clusters of two: a TPC is two SMs,
 // so every GPC holds a whole number of them and the whole grid (64 clusters at 4096 envs) is resident at once.  Clusters
@@ -64,7 +71,10 @@ __host__ __device__ __forceinline__ int rf_bn(int H2) { return rf_wide(H2) ? 256
 //              (layer 2), B = the weight's [hi | lo] twin planes.  80 KB for 64 x 256, 64 KB for 128 x 128.
 //   tf32 form: [A raw BM x 128 B | B raw BN x 128 B | B hi | B lo].  104 KB for 64 x 256, 64 KB for 128 x 128.
 // Two slots: three 80 KB stages do not fit.  The conversion buffer [A hi | A lo] (BM x 256 B: the operands split in shared
-// memory) follows the slots, the mbarriers and the normaliser statistics follow the largest layout.
+// memory) follows the slots.  fp16 form: then the head partials of the rows this CTA finishes ([P][rows][kHeadPartPad]
+// floats, P * rows = H2 / 64 * BM / CX = 256 in every layout: 12 KB) and the step-invariant operands of the CTA's BN <= 256
+// columns: b1, b2, the [Wv; Wa] rows (RF_HEAD_AP x 256 floats), then bv, ba (16 floats).  The tf32 form has no room for
+// them (two 104 KB slots).  The mbarriers and the normaliser statistics follow the largest layout.
 template <bool F16>
 struct RfSmem {
     static constexpr int STAGES = 2;
@@ -73,11 +83,16 @@ struct RfSmem {
     __host__ __device__ static constexpr int a_bytes(int bm) { return bm * KBK * 4; }   // A of a stage; B starts here
     __host__ __device__ static constexpr int b_hi(int bm, int bn) { return F16 ? bm * 256 : (bm + bn) * 128; }
     __host__ __device__ static constexpr int stage_tx(int bm, int bn) { return (bm + bn) * KBK * 4; }
-    static constexpr int OFF_BARS = STAGES * slot(64, 256) + 64 * 256;   // full[STAGES], empty[STAGES]
+    static constexpr int OFF_PART = STAGES * slot(64, 256) + 64 * 256;
+    static constexpr int OFF_B1 = OFF_PART + (F16 ? 256 * kHeadPartPad * 4 : 0);
+    static constexpr int OFF_B2 = OFF_B1 + (F16 ? 256 * 4 : 0);
+    static constexpr int OFF_HW = OFF_B2 + (F16 ? 256 * 4 : 0);
+    static constexpr int OFF_HB = OFF_HW + (F16 ? RF_HEAD_AP * 256 * 4 : 0);
+    static constexpr int OFF_BARS = OFF_HB + (F16 ? 16 * 4 : 0);   // full[STAGES], empty[STAGES]
     static constexpr int OFF_CSTAT = OFF_BARS + 64;
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
     static_assert(2 * STAGES * 8 <= 64 && TOTAL + 64 <= 227 * 1024, "shared memory");
-    static_assert(STAGES * slot(128, 128) + 128 * 256 <= OFF_BARS, "the 128 x 128 layout fits below the barriers");
+    static_assert(STAGES * slot(128, 128) + 128 * 256 <= OFF_PART, "the 128 x 128 layout fits below the partials");
 };
 
 
@@ -123,6 +138,16 @@ __device__ __forceinline__ uint32_t smid() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
     return r;
+}
+// shared::cluster address of the same offset in the shared memory of CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
+    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+                 : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -204,9 +229,12 @@ __device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUte
 // conversion buffer (each warpgroup its own 64 rows of a 128-row tile; both together the one 64-row tile of the wide
 // layout, which both read); the tf32 form splits both operands.  3xTF32, or with F16 the fp16-split form of gemm_tc.cu
 // (A * 2^a_shift, weights * 2^kF16WShift, 64 k per stage).  Every accumulator receives its wgmmas in k order.
+// tr: the traced thread's stamps of this step, else NULL: slot s_land when the last stage has landed, s_split when its
+// split is done (tiles that split), s_done when the last wgmmas have completed.
 template <bool F16, bool SPLIT_A>
 __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& cu,
-                                        float (&acc)[64], float (&cross)[64], int ct, int a_shift) {
+                                        float (&acc)[64], float (&cross)[64], int ct, int a_shift, unsigned long long* tr,
+                                        int s_land, int s_split, int s_done) {
     using S = RfSmem<F16>;
     const int wg = ct >> 7, lt = ct & 127;
     const int bm = wide ? 64 : 128, bn = wide ? 256 : 128;
@@ -221,6 +249,7 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
         const int s = (int)(cu % S::STAGES);
         uint8_t* slot = smem + s * slot_bytes;
         mbar_wait(&full[s], (cu / S::STAGES) & 1);
+        if (tr && kb == nkb - 1) tr[s_land] = rf_now();
         const uint8_t* at = slot;
         if (SPLIT_A || !F16) {
             // the conversion buffer is read by the wgmmas in flight: this warpgroup's, and in the wide layout the other's
@@ -243,6 +272,7 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
             }
             fence_proxy_async_smem();
             consumer_sync();
+            if (tr && kb == nkb - 1) tr[s_split] = rf_now();
             at = conv;
         }
         const uint64_t da_hi = make_smem_desc(smem_u32(at + a_row * 128));
@@ -271,6 +301,7 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
         held = s;
     }
     wgmma_wait_all();
+    if (tr) tr[s_done] = rf_now();
     mbar_arrive(&empty[held]);
     if (F16) {
         const float out_scale = pow2f_int(-(a_shift + kF16WShift));
@@ -284,21 +315,93 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
 
 // Layer-1 epilogue of the fp16 form: h1 = act(acc + b1) exactly as store_tile forms it, times 2^shift_h, split by
 // f16_split2 into the hi plane (`hi`, [N][H1] halves) and the lo plane (lo_off halves later) -- the bits split_tile_f16
-// would make of the fp32 h1 tile.
+// would make of the fp32 h1 tile.  bias: b1 of column n0 (the CTA's copy in shared memory).  Straight-line: the thread's
+// 32 bias values are loaded before the first store (a load after a store to h1 could not be hoisted above it).
 __device__ __forceinline__ void store_h1_split(const float (&acc)[64], int n0, int64_t row_base, int lane, uint16_t* hi,
                                                int64_t lo_off, int64_t M, int H1, const float* bias, int act, float scale) {
+    float b[32];
+    const float* bp = bias + 2 * (lane & 3);
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+        b[2 * c] = bp[8 * c];
+        b[2 * c + 1] = bp[8 * c + 1];
+    }
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
         const int64_t m = row_base + 8 * (j & 1);
         const int n = n0 + 8 * (j >> 1) + 2 * (lane & 3);
         if (m >= M) continue;
-        const float v0 = act_fwd_fast(acc[2 * j] + bias[n], act);
-        const float v1 = act_fwd_fast(acc[2 * j + 1] + bias[n + 1], act);
+        const float v0 = act_fwd_fast(acc[2 * j] + b[j & ~1], act);
+        const float v1 = act_fwd_fast(acc[2 * j + 1] + b[j | 1], act);
         uint32_t h, l;
         f16_split2(v0 * scale, v1 * scale, h, l);
         uint16_t* dst = hi + m * H1 + n;
         *reinterpret_cast<uint32_t*>(dst) = h;
         *reinterpret_cast<uint32_t*>(dst + lo_off) = l;
+    }
+}
+
+// Layer-2 epilogue of the fp16 form: heads_tile's arithmetic (same expressions, same order of operations, so the same
+// bits) with b2 and the [Wv; Wa] rows read from the CTA's copies in shared memory (`b2`, `hw`: BN columns, rows of 256
+// floats), and each row's two partials written into the shared memory of the cluster CTA that finishes the row: rows
+// [c rpc, c rpc + rpc) of the block belong to CTA c, partial p of its row r at part + ((p * rpc + r) * kHeadPartPad) floats.
+// nl: the warpgroup's first column inside the CTA's tile; p0: its first partial (global column / 64); rb: the thread's
+// first row inside the block.
+template <int ACT>
+__device__ __forceinline__ void rf_heads_tile(float (&acc)[64], int nl, int p0, int rb, int lane, const float* b2,
+                                              const float* hw, int A, uint32_t part, int rpc) {
+    constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
+    const int nq = nl + 2 * (lane & 3);
+    float b[32];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+        b[2 * c] = b2[nq + 8 * c];
+        b[2 * c + 1] = b2[nq + 8 * c + 1];
+    }
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        acc[2 * j] = act_fwd_ct<ACT>(acc[2 * j] + b[j & ~1]);
+        acc[2 * j + 1] = act_fwd_ct<ACT>(acc[2 * j + 1] + b[j | 1]);
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        float hp[2][kHeadAP];
+#pragma unroll
+        for (int a = 0; a < kHeadAP; ++a) {
+            float s[2] = {0.f, 0.f};
+            if (a <= A) {
+                const float* w = hw + a * 256 + nq + 64 * half;
+                float2 wv[JP / 2];
+#pragma unroll
+                for (int jj = 0; jj < JP / 2; ++jj) wv[jj] = *reinterpret_cast<const float2*>(w + 8 * jj);
+#pragma unroll
+                for (int jj = 0; jj < JP / 2; ++jj) {
+#pragma unroll
+                    for (int rs = 0; rs < 2; ++rs) {
+                        const int j = JP * half + 2 * jj + rs;
+                        s[rs] = fmaf(acc[2 * j], wv[jj].x, s[rs]);
+                        s[rs] = fmaf(acc[2 * j + 1], wv[jj].y, s[rs]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int rs = 0; rs < 2; ++rs) {
+                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 1);
+                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 2);
+                hp[rs][a] = s[rs];
+            }
+        }
+        if ((lane & 3) == 0) {
+#pragma unroll
+            for (int rs = 0; rs < 2; ++rs) {
+                const int r = rb + 8 * rs;
+                const uint32_t dst =
+                    mapa_shared(part + (uint32_t)(((p0 + half) * rpc + r % rpc) * kHeadPartPad * 4), (uint32_t)(r / rpc));
+                st_cluster_f4(dst, make_float4(hp[rs][0], hp[rs][1], hp[rs][2], hp[rs][3]));
+                st_cluster_f4(dst + 16, make_float4(hp[rs][4], hp[rs][5], hp[rs][6], hp[rs][7]));
+                st_cluster_f4(dst + 32, make_float4(hp[rs][8], 0.f, 0.f, 0.f));
+            }
+        }
     }
 }
 
@@ -314,6 +417,12 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + S::OFF_BARS);   // [STAGES] slot landed (TMA)
     uint64_t* empty = full + S::STAGES;                                  // [STAGES] slot read by every consumer's wgmmas
     float* cstat = reinterpret_cast<float*>(smem + S::OFF_CSTAT);       // [2][K1]: mu, 1 / sigma of the observation normaliser
+    // fp16 form: the head partials of this CTA's rows, and its copies of the step-invariant operands (RfSmem)
+    float* s_part = reinterpret_cast<float*>(smem + S::OFF_PART);
+    float* s_b1 = reinterpret_cast<float*>(smem + S::OFF_B1);
+    float* s_b2 = reinterpret_cast<float*>(smem + S::OFF_B2);
+    float* s_hw = reinterpret_cast<float*>(smem + S::OFF_HW);           // [RF_HEAD_AP][256]: Wv, then the rows of Wa
+    float* s_hb = reinterpret_cast<float*>(smem + S::OFF_HB);           // bv, then ba
 
     // episode statistics of finished episodes: accumulated per CTA over the WHOLE rollout in shared memory, five global
     // atomics per CTA at the end (inside this kernel every cluster barrier's release would otherwise have to wait for
@@ -353,6 +462,15 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     if (cta_trace && threadIdx.x == 0) cta_trace[2] = rf_now();
     if (do_rms)
         for (int c = threadIdx.x; c < a.K1; c += RF_THREADS) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.K1 + c]);
+    if (F16) {   // the weights do not change inside a rollout: one copy per launch
+        for (int i = threadIdx.x; i < BN; i += RF_THREADS) {
+            s_b1[i] = a.b1[n0 + i];
+            s_b2[i] = a.b2[n0 + i];
+            s_hw[i] = a.wv[n0 + i];
+            for (int r = 0; r < a.A; ++r) s_hw[(r + 1) * 256 + i] = a.wa[(int64_t)r * a.H2 + n0 + i];
+        }
+        if (threadIdx.x <= a.A) s_hb[threadIdx.x] = threadIdx.x == 0 ? a.bv[0] : a.ba[threadIdx.x - 1];
+    }
     __syncthreads();
     const int64_t env_step0 = a.env_step[0];
     const uint64_t philox0 = a.sampler_step ? (uint64_t)*a.sampler_step : 0ull;
@@ -381,14 +499,16 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
 
         for (int t = 0; t < a.T; ++t) {
             RF_TRACE(0);
+            unsigned long long* const tr = tracer ? a.trace + (int64_t)t * 16 : nullptr;
             {
                 float acc[64], cross[64];
-                rf_tile<F16, true>(a.K1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_x);
+                rf_tile<F16, true>(a.K1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_x, tr, 1, 2, 5);
                 if (F16)
-                    store_h1_split(acc, tc.n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1, a.b1, ACT,
-                                   pow2f_int(shift_h));
+                    store_h1_split(acc, tc.n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1,
+                                   s_b1 + (tc.n0 - n0), ACT, pow2f_int(shift_h));
                 else
                     store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
+                RF_TRACE(6);               // epilogue stores issued
                 fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
                 RF_TRACE(3);
             }
@@ -396,8 +516,12 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
             RF_TRACE(4);
             {
                 float acc[64], cross[64];
-                rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h);
-                heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
+                rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h, tr, 11, 14, 12);
+                if (F16)
+                    rf_heads_tile<ACT>(acc, tc.n0 - n0, tc.n0 / 64, (int)(row_base - m0), lane, s_b2, s_hw, a.A,
+                                       smem_u32(s_part), BM / CX);
+                else
+                    heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);
                 RF_TRACE(7);
             }
             cluster_sync_all();   // all head partials of the row block written
@@ -433,10 +557,18 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                     int32_t el0 = 0;
                     const int cpl = a.K1 >> 3;                // observation columns per lane (K1 is a multiple of 32)
                     if (ok) {
-                        if (has_logit)
-                            for (int p = 0; p < P; ++p) x += a.part[((int64_t)p * a.N + row) * kHeadPartPad + 1 + act_idx];
-                        if (leader)
-                            for (int p = 0; p < P; ++p) val += a.part[((int64_t)p * a.N + row) * kHeadPartPad];
+                        // the fp16 form's partials are in this CTA's shared memory ([P][rpc] rows), the tf32 form's in L2
+                        if (F16) {
+                            if (has_logit)
+                                for (int p = 0; p < P; ++p) x += s_part[(p * rpc + rr) * kHeadPartPad + 1 + act_idx];
+                            if (leader)
+                                for (int p = 0; p < P; ++p) val += s_part[(p * rpc + rr) * kHeadPartPad];
+                        } else {
+                            if (has_logit)
+                                for (int p = 0; p < P; ++p) x += a.part[((int64_t)p * a.N + row) * kHeadPartPad + 1 + act_idx];
+                            if (leader)
+                                for (int p = 0; p < P; ++p) val += a.part[((int64_t)p * a.N + row) * kHeadPartPad];
+                        }
                         const float4* src4 = reinterpret_cast<const float4*>(src_step + row * a.K1 + g * cpl);
 #pragma unroll
                         for (int q = 0; q < RF_MAX_DIM / 32; ++q)
@@ -446,9 +578,10 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                             }
                         if (leader && a.ep_ret) { er0 = a.ep_ret[row]; el0 = a.ep_len[row]; mn0 = a.ep_min[row]; mx0 = a.ep_max[row]; }
                     }
+                    if (tr && base == 0) tr[13] = tc_now_after(val);   // partials landed
                     // ---- CategoricalActionDistribution on the group (action_distributions.py:110-148), as heads_row_tail
-                    x += has_logit ? a.ba[act_idx] : 0.f;
-                    val += a.bv[0];
+                    x += has_logit ? (F16 ? s_hb[1 + act_idx] : a.ba[act_idx]) : 0.f;
+                    val += F16 ? s_hb[0] : a.bv[0];
                     const float xl = has_logit ? x : -INFINITY;
                     float m = xl;
 #pragma unroll
@@ -477,6 +610,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                         if (ob_ > best || (ob_ == best && oi < idx)) { best = ob_; idx = oi; }
                     }
                     const float lp = __shfl_sync(0xffffffffu, logp, (grp << 3) | ((idx + 1) & 7));   // log_prob :145-148
+                    if (tr && base == 0) tr[15] = tc_now_after(lp);    // action sampled
                     (void)gmask;
                     if (!ok) continue;
                     // ---- trajectory slot t, env step, post step, pre step of t + 1

@@ -3,7 +3,8 @@
 Runs the headline workload (bench.make_cfg, the same synthetic tape env and sizes) through Runner with the kernel's
 phase trace switched on (sfb200_rollout_set_trace): CTA (0, 0)'s first consumer thread stamps %globaltimer at the phase
 boundaries of every step into a [T][16] buffer.  Prints, per step, the mean time of each phase over the steps of the
-last --iters rollouts (step 0 left out: it includes the launch ramp), with the GPU's name and power limit, and writes
+last --iters rollouts (step 0 left out: it includes the launch ramp), then of the sub-phases inside them (stages
+landed, split, wgmmas, epilogues, the tail's partial sums and sampling), with the GPU's name and power limit, and writes
 <out>/rollout_trace.json.  The stamps are one CTA's view; barrier phases include waiting for the cluster's slowest CTA.
 
 Every CTA also stamps its SM id and its entry / start (after the programmatic-dependency wait) / exit times: the tool
@@ -30,6 +31,12 @@ import torch  # noqa: E402
 # (name, first stamp slot, last stamp slot) -- the RF_TRACE slots of the kernel
 PHASES = [("layer 1", 0, 3), ("barrier 1", 3, 4), ("layer 2 + heads", 4, 7), ("barrier 2", 7, 8), ("tail", 8, 9),
           ("barrier 3", 9, 10)]
+# sub-phases inside them (slot 2: layer 1's split, 14: layer 2's split, stamped only by tiles that split in shared memory);
+# a sub-phase is averaged over the steps that stamped both ends
+SUBPHASES = [("L1 A landed", 0, 1), ("L1 split", 1, 2), ("L1 wgmmas", 2, 5), ("L1 wgmmas (no split)", 1, 5),
+             ("L1 epilogue", 5, 6), ("L1 fence", 6, 3), ("L2 stages", 4, 11), ("L2 last split", 11, 14),
+             ("L2 last wgmmas", 14, 12), ("L2 last wgmmas (no split)", 11, 12), ("L2 heads epilogue", 12, 7),
+             ("tail partials landed", 8, 13), ("tail sampling", 13, 15), ("tail stores", 15, 9)]
 
 
 def cta_summary(ctas, step_us):
@@ -92,6 +99,8 @@ def main():
         torch.cuda.synchronize()
         sums = [0.0] * len(PHASES)
         count = 0
+        sub_sums = [0.0] * len(SUBPHASES)
+        sub_counts = [0] * len(SUBPHASES)
         ctas = []   # per rollout: [(smid, entry, start, exit)] of every CTA that ran
         for _ in range(args.iters):
             trace.zero_()
@@ -103,6 +112,10 @@ def main():
                 for i, (_, a, b) in enumerate(PHASES):
                     sums[i] += (int(st[t, b]) - int(st[t, a])) / 1e3
                 count += 1
+                for i, (_, a, b) in enumerate(SUBPHASES):
+                    if int(st[t, a]) and int(st[t, b]):
+                        sub_sums[i] += (int(st[t, b]) - int(st[t, a])) / 1e3
+                        sub_counts[i] += 1
             c = flat[T * 16:].view(-1, 4).tolist()
             ctas.append([tuple(r) for r in c if r[2] != 0])
         act = ops.ACT[runner.sampler.model.spec.nonlinearity]
@@ -114,10 +127,11 @@ def main():
     per = {name: round(s / count, 2) for (name, _, _), s in zip(PHASES, sums)}
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
+    sub = {name: round(v / n, 2) for (name, _, _), v, n in zip(SUBPHASES, sub_sums, sub_counts) if n}
     total = sum(per.values())
     waves = cta_summary(ctas, total)
     result = {"gpu": gpu, "workload": bench.WORKLOAD, "form": form, "rollouts": args.iters, "steps_per_rollout": T,
-              "us_per_step": per, "us_per_step_total": round(total, 2),
+              "us_per_step": per, "us_per_step_total": round(total, 2), "us_per_step_sub": sub,
               "occupancy": {"clusters_needed": needed, "clusters_resident": resident}, "ctas": waves}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "rollout_trace.json"), "w") as f:
@@ -126,6 +140,9 @@ def main():
     for name, v in per.items():
         print(f"  {name:16s} {v:8.2f}")
     print(f"  {'step':16s} {total:8.2f}")
+    print("sub-phases, us per step:")
+    for name, v in sub.items():
+        print(f"  {name:26s} {v:8.2f}")
     print(f"occupancy: {needed} clusters needed, {resident} resident at once")
     print(f"CTAs per rollout: {waves['count']}; start spread {waves['start_spread_us']:.2f} us; "
           f"{waves['late_starts']} started more than a step ({total:.1f} us) after the first; "
