@@ -246,9 +246,9 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
  *   bounds (K1, H1 multiples of 64); the h1 scratch then holds h1 * 2^shift split into fp16 planes: hi [n_envs][H1] halves,
  *   then lo n_envs * H1 halves later (the same bytes).  Otherwise (tf32 form) it holds h1 as fp32 [n_envs][H1]. */
 int sfb200_rollout_mlp2_partials(const float* W1, const float* W2, int K1, int H1, int H2, int A, int engine);
-/* debug aid: device buffer of uint64 that the following rollouts fill with %globaltimer stamps: T x 16 phase stamps of one
+/* debug aid: device buffer of uint64 that the following rollouts fill with %globaltimer stamps: T x 32 phase stamps of one
  * CTA, then 4 words per CTA (index blockIdx.y * gridDim.x + blockIdx.x): %smid, entry, after the programmatic-dependency
- * wait, exit.  T x 16 + 4 x (n_envs / 32 + 4) words cover every launch shape; NULL switches it off */
+ * wait, exit.  T x 32 + 4 x (n_envs / 32 + 4) words cover every launch shape; NULL switches it off */
 int sfb200_rollout_set_trace(void* trace_dev);
 /* form the last sfb200_rollout_mlp2_tape call launched: 1 fp16 split, 0 tf32 split, -1 none yet */
 int sfb200_rollout_last_form(void);

@@ -9,7 +9,9 @@
 // cluster barrier (three per step); there is no grid-wide barrier and no kernel boundary.  CTA c of the cluster computes
 // columns [BN c, BN c + BN) of h1, then of h2 (partial head products), then finishes rows [c BM/CX.., ) of the block.
 // Hand-offs between the phases of a step, by layout:
-//   h1, x_norm          every layout: global memory (L2-resident), read back by TMA.
+//   h1, x_norm          every layout: global memory (L2-resident), read back by TMA.  fp16 form: h1 is written by TMA
+//                       tile stores from shared-memory staging (store_h1_tma).  Each CTA loads its A tiles itself:
+//                       multicasting them to both CTAs of a cluster measured slower (DESIGN §7).
 //   head partials       fp16 form (both layouts): written by the layer-2 epilogue straight into the shared memory of the
 //                       CTA that finishes the row (st.shared::cluster), summed from there by the tail; barrier 2 orders
 //                       writer and reader, and barriers 3 and 1 of the next step come between the tail's reads and the
@@ -35,7 +37,7 @@
 //               its wgmmas have completed.
 //
 // fp16-split form (weights with registered fp16 twins, bounded activations): a stage covers 64 k.  The weight tiles are
-// the twins, TMA-loaded in the swizzled layout wgmma reads.  The layer-1 epilogue writes h1 * 2^shift_h already split into
+// the twins, TMA-loaded in the swizzled layout wgmma reads.  The layer-1 epilogue stores h1 * 2^shift_h already split into
 // fp16 [hi | lo] planes (the h1 scratch holds the hi plane, then the lo plane N*H1 halves later), so layer 2 -- 8 of the 9
 // stages of a step at H1 = 512 -- is pure TMA -> wgmma.  Only x_norm (layer 1's A, written as fp32 by the step tail) is
 // split in shared memory.  Every wgmma receives the operands the fp32 buffers would give after split_tile_f16.
@@ -56,6 +58,7 @@ namespace sfb {
 constexpr int RF_THREADS = 384;
 constexpr int RF_HEAD_AP = 9;
 constexpr int RF_MAX_DIM = 128;
+constexpr int RF_TRACE_WORDS = 32;   // phase stamps per step (sfb200_rollout_set_trace)
 // register budgets after the hand-over: 128 x 40 + 256 x 232 = the 384 x 168 the launch gets
 constexpr int RF_PRODUCER_REGS = 40;
 constexpr int RF_CONSUMER_REGS = 232;
@@ -71,10 +74,11 @@ __host__ __device__ __forceinline__ int rf_bn(int H2) { return rf_wide(H2) ? 256
 //              (layer 2), B = the weight's [hi | lo] twin planes.  80 KB for 64 x 256, 64 KB for 128 x 128.
 //   tf32 form: [A raw BM x 128 B | B raw BN x 128 B | B hi | B lo].  104 KB for 64 x 256, 64 KB for 128 x 128.
 // Two slots: three 80 KB stages do not fit.  The conversion buffer [A hi | A lo] (BM x 256 B: the operands split in shared
-// memory) follows the slots.  fp16 form: then the head partials of the rows this CTA finishes ([P][rows][kHeadPartPad]
-// floats, P * rows = H2 / 64 * BM / CX = 256 in every layout: 12 KB) and the step-invariant operands of the CTA's BN <= 256
-// columns: b1, b2, the [Wv; Wa] rows (RF_HEAD_AP x 256 floats), then bv, ba (16 floats).  The tf32 form has no room for
-// them (two 104 KB slots).  The mbarriers and the normaliser statistics follow the largest layout.
+// memory) follows the slots.  fp16 form: then a 16 KB staging buffer of the h1 store (store_h1_tma), the head partials of
+// the rows this CTA finishes ([P][rows][kHeadPartPad] floats, P * rows = H2 / 64 * BM / CX = 256 in every layout: 12 KB)
+// and the step-invariant operands of the CTA's BN <= 256 columns: b1, b2, the [Wv; Wa] rows (RF_HEAD_AP x 256 floats),
+// then bv, ba (16 floats).  The tf32 form has no room for them (two 104 KB slots).  The mbarriers and the normaliser
+// statistics follow the largest layout.
 template <bool F16>
 struct RfSmem {
     static constexpr int STAGES = 2;
@@ -83,7 +87,8 @@ struct RfSmem {
     __host__ __device__ static constexpr int a_bytes(int bm) { return bm * KBK * 4; }   // A of a stage; B starts here
     __host__ __device__ static constexpr int b_hi(int bm, int bn) { return F16 ? bm * 256 : (bm + bn) * 128; }
     __host__ __device__ static constexpr int stage_tx(int bm, int bn) { return (bm + bn) * KBK * 4; }
-    static constexpr int OFF_PART = STAGES * slot(64, 256) + 64 * 256;
+    static constexpr int OFF_CONV_END = STAGES * slot(64, 256) + 64 * 256;   // the 64 x 256 layout's conversion buffer ends here
+    static constexpr int OFF_PART = OFF_CONV_END + (F16 ? 64 * 256 : 0);
     static constexpr int OFF_B1 = OFF_PART + (F16 ? 256 * kHeadPartPad * 4 : 0);
     static constexpr int OFF_B2 = OFF_B1 + (F16 ? 256 * 4 : 0);
     static constexpr int OFF_HW = OFF_B2 + (F16 ? 256 * 4 : 0);
@@ -93,6 +98,8 @@ struct RfSmem {
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
     static_assert(2 * STAGES * 8 <= 64 && TOTAL + 64 <= 227 * 1024, "shared memory");
     static_assert(STAGES * slot(128, 128) + 128 * 256 <= OFF_PART, "the 128 x 128 layout fits below the partials");
+    static_assert(a_bytes(64) % 1024 == 0 && slot(64, 256) % 1024 == 0 && OFF_CONV_END % 1024 == 0,
+                  "h1 staging boxes (slot A regions, conversion buffer, the buffer after it) on 1024 B swizzle atoms");
 };
 
 
@@ -114,8 +121,9 @@ struct RolloutArgs {
     float* traj_obs; int64_t traj_obs_rs; const float* rnn; int rnn_dim; float* traj_rnn; int64_t traj_rnn_rs;
     const double* mean; const double* var; float sub, inv_scale; int do_sub, do_scale; float eps, clip;
     unsigned int* ticket;
-    // debug, or NULL: [T][16] globaltimer stamps of CTA (0,0)'s first epilogue thread, then per CTA (blockIdx.y * gridDim.x
-    // + blockIdx.x) four words: %smid, globaltimer at entry, after the programmatic-dependency wait, at exit
+    // debug, or NULL: [T][RF_TRACE_WORDS] globaltimer stamps of CTA (0,0)'s first epilogue thread, then per CTA
+    // (blockIdx.y * gridDim.x + blockIdx.x) four words: %smid, globaltimer at entry, after the programmatic-dependency
+    // wait, at exit
     unsigned long long* trace;
     const float* bound_x; const float* bound_h1;   // fp16-split form: bounds of |x_norm| and |h1| (device floats), else NULL
 };
@@ -230,11 +238,12 @@ __device__ __forceinline__ void rf_produce(const CUtensorMap* tmap_x, const CUte
 // layout, which both read); the tf32 form splits both operands.  3xTF32, or with F16 the fp16-split form of gemm_tc.cu
 // (A * 2^a_shift, weights * 2^kF16WShift, 64 k per stage).  Every accumulator receives its wgmmas in k order.
 // tr: the traced thread's stamps of this step, else NULL: slot s_land when the last stage has landed, s_split when its
-// split is done (tiles that split), s_done when the last wgmmas have completed.
+// split is done (tiles that split), s_done when the last wgmmas have completed; s_each >= 0: slot s_each + kb when stage
+// kb < 16 has landed (A and B complete one full barrier, so they land together here).
 template <bool F16, bool SPLIT_A>
 __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& cu,
                                         float (&acc)[64], float (&cross)[64], int ct, int a_shift, unsigned long long* tr,
-                                        int s_land, int s_split, int s_done) {
+                                        int s_land, int s_split, int s_done, int s_each) {
     using S = RfSmem<F16>;
     const int wg = ct >> 7, lt = ct & 127;
     const int bm = wide ? 64 : 128, bn = wide ? 256 : 128;
@@ -249,7 +258,11 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
         const int s = (int)(cu % S::STAGES);
         uint8_t* slot = smem + s * slot_bytes;
         mbar_wait(&full[s], (cu / S::STAGES) & 1);
-        if (tr && kb == nkb - 1) tr[s_land] = rf_now();
+        if (tr) {
+            const unsigned long long now = rf_now();
+            if (kb == nkb - 1) tr[s_land] = now;
+            if (s_each >= 0 && kb < 16) tr[s_each + kb] = now;
+        }
         const uint8_t* at = slot;
         if (SPLIT_A || !F16) {
             // the conversion buffer is read by the wgmmas in flight: this warpgroup's, and in the wide layout the other's
@@ -314,11 +327,18 @@ __device__ __forceinline__ void rf_tile(int nkb, bool wide, uint8_t* smem, uint6
 }
 
 // Layer-1 epilogue of the fp16 form: h1 = act(acc + b1) exactly as store_tile forms it, times 2^shift_h, split by
-// f16_split2 into the hi plane (`hi`, [N][H1] halves) and the lo plane (lo_off halves later) -- the bits split_tile_f16
-// would make of the fp32 h1 tile.  bias: b1 of column n0 (the CTA's copy in shared memory).  Straight-line: the thread's
-// 32 bias values are loaded before the first store (a load after a store to h1 could not be hoisted above it).
-__device__ __forceinline__ void store_h1_split(const float (&acc)[64], int n0, int64_t row_base, int lane, uint16_t* hi,
-                                               int64_t lo_off, int64_t M, int H1, const float* bias, int act, float scale) {
+// f16_split2 into the hi and lo planes of the h1 scratch -- the bits split_tile_f16 would make of the fp32 h1 tile.  bias:
+// b1 of the warpgroup's first column n0 (the CTA's copy in shared memory).
+// The values go through shared memory: each 64-column box of tmap_h1 (the [hi | lo] x BM rows x 64 k box layer 2 loads,
+// 128B swizzle: the 16-byte chunk c of row r at chunk c ^ (r % 8), conflict-free for a warp's eight rows) is written in
+// the layer-2 A layout and stored by one thread with a TMA tile store, which writes whole 128-byte lines (a warp's direct
+// stores wrote eight 16-byte pieces) and clips the rows past N.  box[h]: the staging buffer of the warpgroup's box h
+// (columns n0 + 64 h); rt: the thread's first row inside the tile; `issuer` stores the boxes of its warpgroup (64 x 256:
+// each warpgroup its own two; 128 x 128: thread 0 the two boxes both warpgroups wrote).  Before box h is written, the
+// consumer barrier of box h - 1 has passed; before box 0, rf_tile's last barrier (after layer 1's split): see the caller.
+__device__ __forceinline__ void store_h1_tma(const float (&acc)[64], const CUtensorMap* tmap_h1, int n0, int m0, int rt,
+                                             int lane, uint8_t* const (&box)[2], int plane_bytes, bool issuer,
+                                             const float* bias, int act, float scale) {
     float b[32];
     const float* bp = bias + 2 * (lane & 3);
 #pragma unroll
@@ -327,17 +347,25 @@ __device__ __forceinline__ void store_h1_split(const float (&acc)[64], int n0, i
         b[2 * c + 1] = bp[8 * c + 1];
     }
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-        const int64_t m = row_base + 8 * (j & 1);
-        const int n = n0 + 8 * (j >> 1) + 2 * (lane & 3);
-        if (m >= M) continue;
-        const float v0 = act_fwd_fast(acc[2 * j] + b[j & ~1], act);
-        const float v1 = act_fwd_fast(acc[2 * j + 1] + b[j | 1], act);
-        uint32_t h, l;
-        f16_split2(v0 * scale, v1 * scale, h, l);
-        uint16_t* dst = hi + m * H1 + n;
-        *reinterpret_cast<uint32_t*>(dst) = h;
-        *reinterpret_cast<uint32_t*>(dst + lo_off) = l;
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+            const int j = 16 * h + jj;
+            const int r = rt + 8 * (j & 1), c = (j >> 1) & 7;
+            const float v0 = act_fwd_fast(acc[2 * j] + b[j & ~1], act);
+            const float v1 = act_fwd_fast(acc[2 * j + 1] + b[j | 1], act);
+            uint32_t hv, lv;
+            f16_split2(v0 * scale, v1 * scale, hv, lv);
+            uint8_t* dst = box[h] + r * 128 + (((c ^ r) & 7) << 4) + 4 * (lane & 3);
+            *reinterpret_cast<uint32_t*>(dst) = hv;
+            *reinterpret_cast<uint32_t*>(dst + plane_bytes) = lv;
+        }
+        fence_proxy_async_smem();   // these generic writes -> the TMA store's reads
+        consumer_sync();
+        if (issuer) {
+            tma_store_3d(tmap_h1, box[h], n0 + 64 * h, m0, 0);
+            bulk_commit();
+        }
     }
 }
 
@@ -439,7 +467,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     const int P = a.H2 / 64;                         // head partials per row: one per 64 columns
     const bool do_rms = a.mean != nullptr;
     unsigned long long* cta_trace =
-        a.trace ? a.trace + (int64_t)a.T * 16 + 4 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
+        a.trace ? a.trace + (int64_t)a.T * RF_TRACE_WORDS + 4 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
     if (cta_trace && threadIdx.x == 0) {
         cta_trace[0] = smid();
         cta_trace[1] = rf_now();
@@ -487,7 +515,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         const int shift_x = F16 ? f16_shift_for_bound(a.bound_x[0]) : 0;
         const int shift_h = F16 ? f16_shift_for_bound(a.bound_h1[0]) : 0;
         const bool tracer = a.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 128;
-#define RF_TRACE(slot) do { if (tracer) a.trace[(int64_t)t * 16 + (slot)] = rf_now(); } while (0)
+#define RF_TRACE(slot) do { if (tracer) a.trace[(int64_t)t * RF_TRACE_WORDS + (slot)] = rf_now(); } while (0)
         uint32_t cu = 0;
         const TcEpilogue epi_heads{1, ACT, a.b2, nullptr, 0, a.wv, a.wa, a.A, a.part};
         const TcEpilogue epi_h1{1, ACT, a.b1, nullptr, 0};
@@ -497,26 +525,45 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         TileCoord tc;
         tc.m0 = m0; tc.n0 = n0 + (wide ? (ct >> 7) * 128 : 0); tc.k_begin = 0; tc.num_kb = 0; tc.z = 0;
 
+        // fp16 form: the staging buffers of the warpgroup's two h1 boxes (store_h1_tma), BM x 256 B each.  Free from the end
+        // of layer 1's split to barrier 1: the A regions of the two ring slots (the x_norm tile was split out of its slot,
+        // and h1 tiles land only after barrier 1), and in the 64 x 256 layout, for warpgroup 0, the buffer after the
+        // conversion buffer and then the conversion buffer itself, which both warpgroups' layer-1 wgmmas read: the
+        // barrier after its first box comes after both warpgroups have waited for those wgmmas.
+        uint8_t* const conv = smem + S::STAGES * S::slot(BM, BN);
+        uint8_t* const h1_box[2] = {wide && ct < 128 ? conv + BM * 256 : smem,
+                                    wide && ct < 128 ? conv : smem + S::slot(BM, BN)};
+        const bool h1_issuer = wide ? (ct & 127) == 0 : ct == 0;
+
         for (int t = 0; t < a.T; ++t) {
             RF_TRACE(0);
-            unsigned long long* const tr = tracer ? a.trace + (int64_t)t * 16 : nullptr;
+            unsigned long long* const tr = tracer ? a.trace + (int64_t)t * RF_TRACE_WORDS : nullptr;
             {
                 float acc[64], cross[64];
-                rf_tile<F16, true>(a.K1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_x, tr, 1, 2, 5);
-                if (F16)
-                    store_h1_split(acc, tc.n0, row_base, lane, reinterpret_cast<uint16_t*>(a.h1), a.N * a.H1, a.N, a.H1,
-                                   s_b1 + (tc.n0 - n0), ACT, pow2f_int(shift_h));
-                else
+                rf_tile<F16, true>(a.K1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_x, tr, 1, 2, 5, -1);
+                if (F16) {
+                    store_h1_tma(acc, &tmap_h1, tc.n0, (int)m0, (int)(row_base - m0), lane, h1_box, BM * 128, h1_issuer,
+                                 s_b1 + (tc.n0 - n0), ACT, pow2f_int(shift_h));
+                    RF_TRACE(6);           // staging written, last box store issued
+                    // The h1 tiles were written by the async proxy (TMA stores), and the peers read them with TMA loads:
+                    // once an issuer's bulk groups have completed, its writes are performed and visible to it, and its
+                    // arrive (release) at barrier 1 below publishes them to the cluster (the loads follow the producers'
+                    // acquire).  Nothing generic is left to order, so no proxy fence here; the issuers must not arrive
+                    // before the wait.  The wait also frees the staging buffers (the next writes into the slot A regions
+                    // are the TMA loads after barrier 1).
+                    if (h1_issuer) bulk_wait_all();
+                } else {
                     store_tile(acc, tc, row_base, lane, a.h1, a.H1, a.N, a.H1, 1, epi_h1);
-                RF_TRACE(6);               // epilogue stores issued
-                fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
+                    RF_TRACE(6);               // epilogue stores issued
+                    fence_proxy_async_all();   // h1 stores -> the peers' TMA loads
+                }
                 RF_TRACE(3);
             }
             cluster_sync_all();   // h1 of the row block complete
             RF_TRACE(4);
             {
                 float acc[64], cross[64];
-                rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h, tr, 11, 14, 12);
+                rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h, tr, 11, 14, 12, 16);
                 if (F16)
                     rf_heads_tile<ACT>(acc, tc.n0 - n0, tc.n0 / 64, (int)(row_base - m0), lane, s_b2, s_hw, a.A,
                                        smem_u32(s_part), BM / CX);

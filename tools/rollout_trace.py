@@ -2,10 +2,16 @@
 
 Runs the headline workload (bench.make_cfg, the same synthetic tape env and sizes) through Runner with the kernel's
 phase trace switched on (sfb200_rollout_set_trace): CTA (0, 0)'s first consumer thread stamps %globaltimer at the phase
-boundaries of every step into a [T][16] buffer.  Prints, per step, the mean time of each phase over the steps of the
+boundaries of every step into a [T][32] buffer.  Prints, per step, the mean time of each phase over the steps of the
 last --iters rollouts (step 0 left out: it includes the launch ramp), then of the sub-phases inside them (stages
 landed, split, wgmmas, epilogues, the tail's partial sums and sampling), with the GPU's name and power limit, and writes
 <out>/rollout_trace.json.  The stamps are one CTA's view; barrier phases include waiting for the cluster's slowest CTA.
+
+In the fp16 form the layer-1 epilogue writes h1 into shared-memory staging boxes and stores them by TMA: "L1 epilogue"
+ends when the staging is written (and the last box store issued), "L1 store drained" when the traced thread's bulk
+stores have completed, just before it arrives at barrier 1.  (tf32 form: stores issued, then the proxy fence.)  Layer 2's
+stages are stamped one by one when the consumer's wait for the stage returns: A and B complete one barrier, so they
+are seen landing together; "L2 stage j landed" is the time since barrier 1 ended.
 
 Every CTA also stamps its SM id and its entry / start (after the programmatic-dependency wait) / exit times: the tool
 prints the spread of the start times, how many CTAs started more than one step after the first (a second wave: the
@@ -34,9 +40,12 @@ PHASES = [("layer 1", 0, 3), ("barrier 1", 3, 4), ("layer 2 + heads", 4, 7), ("b
 # sub-phases inside them (slot 2: layer 1's split, 14: layer 2's split, stamped only by tiles that split in shared memory);
 # a sub-phase is averaged over the steps that stamped both ends
 SUBPHASES = [("L1 A landed", 0, 1), ("L1 split", 1, 2), ("L1 wgmmas", 2, 5), ("L1 wgmmas (no split)", 1, 5),
-             ("L1 epilogue", 5, 6), ("L1 fence", 6, 3), ("L2 stages", 4, 11), ("L2 last split", 11, 14),
+             ("L1 epilogue", 5, 6), ("L1 store drained", 6, 3), ("L2 stages", 4, 11), ("L2 last split", 11, 14),
              ("L2 last wgmmas", 14, 12), ("L2 last wgmmas (no split)", 11, 12), ("L2 heads epilogue", 12, 7),
              ("tail partials landed", 8, 13), ("tail sampling", 13, 15), ("tail stores", 15, 9)]
+# slots 16 + j: layer-2 stage j landed (j < 16), reported relative to the end of barrier 1 (slot 4)
+WORDS = 32
+SUBPHASES += [(f"L2 stage {j} landed", 4, 16 + j) for j in range(16)]
 
 
 def cta_summary(ctas, step_us):
@@ -86,7 +95,7 @@ def main():
     tape = torch.randn(bench.TAPE_LEN, bench.N_ENVS, bench.OBS_DIM, generator=gen).to(dev)
     register_env("synthetic_tape", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, bench.N_ACTIONS))
     T, N, H = bench.ROLLOUT, bench.N_ENVS, bench.HIDDEN[-1]
-    n_words = T * 16 + 4 * (N // 32 + 4)   # phase stamps, then four words per CTA (include/sfb200.h)
+    n_words = T * WORDS + 4 * (N // 32 + 4)   # phase stamps, then four words per CTA (include/sfb200.h)
     trace = torch.zeros(n_words, dtype=torch.int64, device=dev)
     # set before the first rollout: the sampler's CUDA graph captures the kernel arguments, the trace pointer included
     lib().call("sfb200_rollout_set_trace", trace.data_ptr())
@@ -107,7 +116,7 @@ def main():
             runner.iteration()
             torch.cuda.synchronize()
             flat = trace.cpu()
-            st = flat[:T * 16].view(T, 16)
+            st = flat[:T * WORDS].view(T, WORDS)
             for t in range(1, T):
                 for i, (_, a, b) in enumerate(PHASES):
                     sums[i] += (int(st[t, b]) - int(st[t, a])) / 1e3
@@ -116,7 +125,7 @@ def main():
                     if int(st[t, a]) and int(st[t, b]):
                         sub_sums[i] += (int(st[t, b]) - int(st[t, a])) / 1e3
                         sub_counts[i] += 1
-            c = flat[T * 16:].view(-1, 4).tolist()
+            c = flat[T * WORDS:].view(-1, 4).tolist()
             ctas.append([tuple(r) for r in c if r[2] != 0])
         act = ops.ACT[runner.sampler.model.spec.nonlinearity]
         needed, resident = ops.rollout_occupancy(N, bench.OBS_DIM, bench.HIDDEN[0], H, bench.N_ACTIONS,
