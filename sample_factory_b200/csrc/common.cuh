@@ -156,27 +156,4 @@ __device__ __forceinline__ void f16_split1(float v, uint16_t& hi, uint16_t& lo) 
 
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
 
-// ---- obs normalisation ------------------------------------------------------------------------------------------
-// y = clamp(((x - sub) * inv_scale - mu) * (1/sqrt(var+eps)), +-clip), each op rounded separately (IEEE, no FMA
-// contraction) exactly like the reference's chain of in-place ATen ops (normalize.py:62-67,
-// running_mean_std.py:96-110).
-__device__ __forceinline__ float norm_one(float x, float sub, float inv_scale, bool do_sub, bool do_scale, bool do_rms,
-                                          float mu, float inv_sigma, float clip) {
-    if (do_sub) x = __fsub_rn(x, sub);
-    if (do_scale) x = __fmul_rn(x, inv_scale);
-    if (do_rms) {
-        x = __fmul_rn(__fsub_rn(x, mu), inv_sigma);
-        x = clampf(x, -clip, clip);
-    }
-    return x;
-}
-
-__device__ __forceinline__ void col_stats(const double* mean, const double* var, int c, float eps, float& mu,
-                                          float& inv_sigma) {
-    mu = (float)mean[c];
-    float sigma = __fsqrt_rn(__fadd_rn((float)var[c], eps));
-    inv_sigma = __fdiv_rn(1.0f, sigma);
-}
-
-
 }  // namespace sfb

@@ -2,6 +2,7 @@
 // All are streaming kernels: coalesced 128-bit accesses where alignment allows, grid sized in multiples of the SM
 // count, no shared-memory staging (no reuse).
 #include "common.cuh"
+#include "step_tail.cuh"
 
 namespace sfb {
 
@@ -12,14 +13,13 @@ struct NormArgs {
     float* y; int64_t ldy;               // the reference converts with .float() first, normalize.py:40-46)
     void* raw_copy; int64_t ld_copy;     // same element type as x
     int64_t rows; int dim;
-    const double* mean; const double* var;
-    float sub, inv_scale; int do_sub, do_scale; float eps, clip;
+    ObsNorm n;
     const float* rnn_src; int rnn_dim; float* rnn_dst; int64_t rnn_dst_stride; int64_t rnn_rows;
 };
 
 template <bool VEC4, bool U8>
 __device__ __forceinline__ void normalize_body(const NormArgs& a) {
-    const bool do_rms = a.mean != nullptr;
+    const bool do_rms = a.n.mean != nullptr;
     const int64_t tid0 = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     const int64_t nthr = (int64_t)gridDim.x * blockDim.x;
     if (a.rnn_src) {   // sampler pre-step: traj.rnn_states[:, t] <- rnn (tiny; folded in to save a launch)
@@ -54,8 +54,8 @@ __device__ __forceinline__ void normalize_body(const NormArgs& a) {
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
                     float mu = 0.f, is = 1.f;
-                    if (do_rms) col_stats(a.mean, a.var, c + k, a.eps, mu, is);
-                    out[k] = norm_one(in[k], a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, mu, is, a.clip);
+                    if (do_rms) col_stats(a.n.mean, a.n.var, c + k, a.n.eps, mu, is);
+                    out[k] = norm_one(in[k], a.n.sub, a.n.inv_scale, a.n.do_sub, a.n.do_scale, do_rms, mu, is, a.n.clip);
                 }
                 *reinterpret_cast<float4*>(a.y + r * a.ldy + c) = make_float4(out[0], out[1], out[2], out[3]);
             }
@@ -76,8 +76,8 @@ __device__ __forceinline__ void normalize_body(const NormArgs& a) {
             }
             if (a.y) {
                 float mu = 0.f, is = 1.f;
-                if (do_rms) col_stats(a.mean, a.var, c, a.eps, mu, is);
-                a.y[r * a.ldy + c] = norm_one(v, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, mu, is, a.clip);
+                if (do_rms) col_stats(a.n.mean, a.n.var, c, a.n.eps, mu, is);
+                a.y[r * a.ldy + c] = norm_one(v, a.n.sub, a.n.inv_scale, a.n.do_sub, a.n.do_scale, do_rms, mu, is, a.n.clip);
             }
         }
     }
@@ -96,8 +96,7 @@ static bool make_norm_args(NormArgs& a, const void* x, int64_t ldx, float* y, in
                            int64_t ld_copy, int64_t rows, int dim, const double* mean, const double* var, float sub_mean,
                            float inv_scale, float eps, float clip, const float* rnn_src, int rnn_dim, float* rnn_dst,
                            int64_t rnn_dst_stride, bool u8 = false) {
-    a = NormArgs{x, ldx, y, ldy, raw_copy, ld_copy, rows, dim, mean, var, sub_mean, inv_scale,
-                 fabsf(sub_mean) > 1e-8f, fabsf(inv_scale - 1.0f) > 1e-8f, eps, clip,
+    a = NormArgs{x, ldx, y, ldy, raw_copy, ld_copy, rows, dim, make_obs_norm(mean, var, sub_mean, inv_scale, eps, clip),
                  rnn_src, rnn_dim, rnn_dst, rnn_dst_stride, rows};
     const uintptr_t in_mask = u8 ? 3u : 15u;   // uchar4 vs float4 accesses on the input / raw-copy side
     return (dim % 4 == 0) && (ldx % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & in_mask) == 0) &&
@@ -175,10 +174,7 @@ __global__ void __launch_bounds__(256) copy_rows_bytes_kernel(const uint8_t* __r
 // ---- post env step -------------------------------------------------------------------------------------------------
 struct PostArgs {
     const float* rew; const uint8_t* term; const uint8_t* trunc; int64_t n;
-    float reward_scale, reward_clip; int32_t policy_id;
-    float* t_rew; uint8_t* t_done; uint8_t* t_to; int32_t* t_pid; int64_t stride;
-    float* ep_ret; int32_t* ep_len; float* ep_min; float* ep_max; int32_t len_inc;
-    double* stats; int64_t* step_counter; float* fin_ret; int32_t* fin_len;
+    EpisodeArgs e; int64_t* step_counter;
 };
 
 // All threads of the grid must call this (warp reductions inside); thread i < n handles env i.
@@ -187,38 +183,19 @@ __device__ __forceinline__ void post_step_body(const PostArgs& a) {
     if (a.step_counter && i == 0) *a.step_counter += 1;
     double c = 0.0, s_ret = 0.0, s_len = 0.0, s_min = 0.0, s_max = 0.0;
     if (i < a.n) {
-        const float r_raw = a.rew[i];
-        const bool tm = a.term[i] != 0, tr = a.trunc[i] != 0;
-        const bool done = tm || tr;                                   // batched_sampling.py:317
-        float r = __fmul_rn(r_raw, a.reward_scale);                     // :209
-        r = clampf(r, -a.reward_clip, a.reward_clip);                   // :210
-        a.t_rew[i * a.stride] = r;
-        a.t_done[i * a.stride] = done ? 1 : 0;
-        a.t_to[i * a.stride] = tr ? 1 : 0;                              // :328
-        a.t_pid[i * a.stride] = a.policy_id;
-        if (a.ep_ret) {
-            // _process_env_step :215-287 (episode accounting uses the RAW reward, :336 passes rewards_cpu)
-            float er = a.ep_ret[i] + r_raw;
-            int32_t el = a.ep_len[i] + a.len_inc;
-            float mn = fminf(a.ep_min[i], r_raw), mx = fmaxf(a.ep_max[i], r_raw);
-            if (a.fin_ret) {
-                a.fin_ret[i * a.stride] = done ? er : __int_as_float(0x7fc00000);
-                a.fin_len[i * a.stride] = done ? el : -1;
-            }
-            if (done) {
-                c = 1.0; s_ret = er; s_len = el; s_min = mn; s_max = mx;
-                er = 0.f; el = 0; mn = INFINITY; mx = -INFINITY;
-            }
-            a.ep_ret[i] = er; a.ep_len[i] = el; a.ep_min[i] = mn; a.ep_max[i] = mx;
+        const Episode ep = load_episode(a.e, i, true);
+        Episode fin;
+        if (post_step_env(a.e, i, i * a.e.stride, a.rew[i], a.term[i] != 0, a.trunc[i] != 0, ep, fin)) {
+            c = 1.0; s_ret = fin.ret; s_len = fin.len; s_min = fin.mn; s_max = fin.mx;
         }
     }
-    if (a.stats) {
+    if (a.e.stats) {
         c = warp_sum(c);
         if (c > 0.0) {   // warp-uniform after the reduction
             s_ret = warp_sum(s_ret); s_len = warp_sum(s_len); s_min = warp_sum(s_min); s_max = warp_sum(s_max);
             if ((threadIdx.x & 31) == 0) {
-                atomicAdd(a.stats + 0, c); atomicAdd(a.stats + 1, s_ret); atomicAdd(a.stats + 2, s_len);
-                atomicAdd(a.stats + 3, s_min); atomicAdd(a.stats + 4, s_max);
+                atomicAdd(a.e.stats + 0, c); atomicAdd(a.e.stats + 1, s_ret); atomicAdd(a.e.stats + 2, s_len);
+                atomicAdd(a.e.stats + 3, s_min); atomicAdd(a.e.stats + 4, s_max);
             }
         }
     }
@@ -241,7 +218,7 @@ __global__ void __launch_bounds__(256) tape_env_kernel(const int32_t* __restrict
                                                        const float* __restrict__ actions_f32, int act_dim, int64_t n,
                                                        int num_actions,
                                                        int64_t env_off, int term_period, int trunc_period,
-                                                       const int64_t* __restrict__ step_counter, int64_t step_host,
+                                                       int64_t* step_counter, int64_t step_host,
                                                        const float* __restrict__ tape, int64_t tape_len, int dim,
                                                        float* __restrict__ obs_out, float* __restrict__ rew,
                                                        uint8_t* __restrict__ term, uint8_t* __restrict__ trunc) {
@@ -254,8 +231,8 @@ __global__ void __launch_bounds__(256) tape_env_kernel(const int32_t* __restrict
         const int64_t env = env_off + tid;
         // Discrete: action / n ; Box: first action component clipped to [-1, 1] (same rules as the oracle's env)
         rew[tid] = actions_f32 ? clampf(actions_f32[tid * act_dim], -1.f, 1.f) : (float)actions[tid] / (float)num_actions;
-        const bool tm = ((step * 7 + env * 13) % term_period) == 0;
-        const bool tr = (((step + env) % trunc_period) == 0) && !tm;
+        bool tm, tr;
+        tape_done(step, env, term_period, trunc_period, tm, tr);
         term[tid] = tm; trunc[tid] = tr;
     }
     if (obs_out) {
@@ -270,16 +247,8 @@ __global__ void __launch_bounds__(256) tape_env_kernel(const int32_t* __restrict
         }
     }
     if (step_counter) {
-        // every block has read `step` before taking its ticket, so the last ticket holder may advance the counter
         __syncthreads();
-        if (threadIdx.x == 0) {
-            __threadfence();
-            unsigned long long* ticket = reinterpret_cast<unsigned long long*>(const_cast<int64_t*>(step_counter) + 1);
-            if (atomicAdd(ticket, 1ull) == (unsigned long long)gridDim.x - 1ull) {
-                *ticket = 0ull;
-                const_cast<int64_t*>(step_counter)[0] = step + 1;
-            }
-        }
+        if (threadIdx.x == 0) advance_step_counters(step_counter, step + 1, nullptr, 0, gridDim.x);
     }
 }
 
@@ -433,9 +402,11 @@ static int make_post_args(PostArgs& a, const float* rew, const uint8_t* terminat
     SFB_CHECK_ARG(rew && terminated && truncated && traj_rewards_t && traj_dones_t && traj_time_outs_t &&
                       traj_policy_id_t, "sampler_post_step: NULL argument");
     SFB_CHECK_ARG(!ep_return || (ep_len && ep_min_raw && ep_max_raw), "sampler_post_step: episode arrays incomplete");
-    a = PostArgs{rew, terminated, truncated, n_envs, reward_scale, reward_clip, policy_id, traj_rewards_t, traj_dones_t,
-                 traj_time_outs_t, traj_policy_id_t, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw,
-                 len_increment, ep_return ? stats : nullptr, step_counter, ep_return ? fin_return_t : nullptr, fin_len_t};
+    a = PostArgs{rew, terminated, truncated, n_envs,
+                 EpisodeArgs{reward_scale, reward_clip, policy_id, traj_rewards_t, traj_dones_t, traj_time_outs_t,
+                             traj_policy_id_t, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw, len_increment,
+                             ep_return ? stats : nullptr, ep_return ? fin_return_t : nullptr, fin_len_t},
+                 step_counter};
     return 0;
 }
 
@@ -545,7 +516,7 @@ static int tape_env_step_impl(const int32_t* actions, const float* actions_f32, 
     unsigned g = grid_for(work);
     if ((int64_t)g * 256 < n_envs) g = (unsigned)ceil_div(n_envs, 256);
     SFB_CUDA_OK(launch_pdl(tape_env_kernel, dim3(g), dim3(256), 0, st, actions, actions_f32, act_dim, n_envs, num_actions, env_index_offset,
-                           term_period, trunc_period, (const int64_t*)step_counter, step_host, tape, tape_len, dim, obs_out,
+                           term_period, trunc_period, step_counter, step_host, tape, tape_len, dim, obs_out,
                            rew, terminated, truncated));
     SFB_LAUNCH_OK();
     return 0;

@@ -3,6 +3,7 @@
 // (HBM-bound: 4*H bytes per row read, backward also writes 4*H).
 #include "gemm.h"
 #include "heads_tail.cuh"
+#include "step_tail.cuh"
 
 namespace sfb {
 
@@ -612,21 +613,17 @@ static int heads_from_partials_impl(const float* head_partials, int P, int64_t r
 
 // ---------------------------------------------------------------------------------------------------------------------
 // The rest of a sampler step after the policy GEMMs, for the synthetic tape env (envs.TapeVecEnv, BASELINE config 2), in
-// ONE launch: finish the heads + sample (heads_finish_row) -> env step (the rules of tape_env_kernel, elementwise.cu)
-// -> advance_rollouts part 2 (post_step_body: reward scale / clip, dones, episode accounting, batched_sampling.py:319-357)
-// -> generate_policy_request + normalisation of step t+1 (normalize_body).  Everything is per env, so one warp walks one
-// env through all four stages; the three kernel boundaries (and two of the five launches of a policy step) disappear.
-// Same device functions / same arithmetic as the separate kernels -> identical trajectories.
+// ONE launch: finish the heads + sample (heads_finish_row) -> env step -> advance_rollouts part 2 (post_step_env) ->
+// generate_policy_request + normalisation of step t+1, on the rules of step_tail.cuh.  Everything is per env, so one
+// warp walks one env through all four stages; the three kernel boundaries (and two of the five launches of a policy
+// step) disappear.
 struct TapeStepArgs {
     const float* tape; int64_t tape_len; int dim; int num_actions; int64_t env_off; int term_period, trunc_period;
     int64_t* env_step;                                   // [0] env step, [1] block ticket
     float* env_obs; float* env_rew; uint8_t* env_term; uint8_t* env_trunc;
-    float reward_scale, reward_clip; int32_t policy_id;
-    float* t_rew; uint8_t* t_done; uint8_t* t_to; int32_t* t_pid; int64_t stride;
-    float* ep_ret; int32_t* ep_len; float* ep_min; float* ep_max; int32_t len_inc; double* stats;
-    int64_t* sampler_step; float* fin_ret; int32_t* fin_len;
-    float* traj_obs_next; int64_t traj_obs_stride; float* x_norm; const double* mean; const double* var;
-    float sub, inv_scale; int do_sub, do_scale; float eps, clip;
+    EpisodeArgs e;
+    int64_t* sampler_step;
+    float* traj_obs_next; int64_t traj_obs_stride; float* x_norm; ObsNorm n;
     const float* rnn; int rnn_dim; float* traj_rnn_next; int64_t traj_rnn_stride;
 };
 
@@ -634,11 +631,11 @@ __global__ void __launch_bounds__(256) sampler_tail_tape_kernel(const float* __r
                                                                 const HeadsFinish f, const TapeStepArgs a) {
     // per-column normaliser constants once per block (instead of a double load + sqrt + divide per element)
     extern __shared__ float cstat[];   // [2][dim]: mu, 1 / sigma
-    const bool do_rms = a.mean != nullptr && a.x_norm != nullptr;
+    const bool do_rms = a.n.mean != nullptr && a.x_norm != nullptr;
     pdl_wait();
     pdl_trigger();
     if (do_rms) {
-        for (int c = threadIdx.x; c < a.dim; c += blockDim.x) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.dim + c]);
+        fill_col_stats(a.n, a.dim, cstat);
         __syncthreads();
     }
     const int lane = threadIdx.x & 31;
@@ -655,80 +652,45 @@ __global__ void __launch_bounds__(256) sampler_tail_tape_kernel(const float* __r
         const float* src = src_step + row * a.dim;
         float2 o2 = make_float2(0.f, 0.f);
         if (two) o2 = *reinterpret_cast<const float2*>(src + 2 * lane);
-        float er0 = 0.f, mn0 = 0.f, mx0 = 0.f;
-        int32_t el0 = 0;
-        if (lane == 0 && a.ep_ret) { er0 = a.ep_ret[row]; el0 = a.ep_len[row]; mn0 = a.ep_min[row]; mx0 = a.ep_max[row]; }
+        const Episode ep = load_episode(a.e, row, lane == 0);
         const int act = heads_finish_row(part, P, rows, row, lane, f, pv, offset);
-        // ---- env step
-        const int64_t env = a.env_off + row;
-        const float r_raw = (float)act / (float)a.num_actions;
-        const bool tm = ((step * 7 + env * 13) % a.term_period) == 0;
-        const bool tr = (((step + env) % a.trunc_period) == 0) && !tm;
         // ---- next observation: env buffer, trajectory slot t+1, normalised policy input
         if (two) {
             const int c = 2 * lane;
             *reinterpret_cast<float2*>(a.env_obs + row * a.dim + c) = o2;
             *reinterpret_cast<float2*>(a.traj_obs_next + row * a.traj_obs_stride + c) = o2;
-            if (a.x_norm) {
-                float2 y;
-                y.x = norm_one(o2.x, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c] : 0.f, do_rms ? cstat[a.dim + c] : 1.f, a.clip);
-                y.y = norm_one(o2.y, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 1] : 0.f, do_rms ? cstat[a.dim + c + 1] : 1.f, a.clip);
-                *reinterpret_cast<float2*>(a.x_norm + row * a.dim + c) = y;
-            }
+            if (a.x_norm)
+                *reinterpret_cast<float2*>(a.x_norm + row * a.dim + c) =
+                    make_float2(a.n.apply(o2.x, do_rms, cstat, a.dim, c), a.n.apply(o2.y, do_rms, cstat, a.dim, c + 1));
         } else {
             for (int c = lane; c < a.dim; c += 32) {
                 const float v = src[c];
                 a.env_obs[row * a.dim + c] = v;
                 a.traj_obs_next[row * a.traj_obs_stride + c] = v;
-                if (a.x_norm)
-                    a.x_norm[row * a.dim + c] = norm_one(v, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms,
-                                                         do_rms ? cstat[c] : 0.f, do_rms ? cstat[a.dim + c] : 1.f, a.clip);
+                if (a.x_norm) a.x_norm[row * a.dim + c] = a.n.apply(v, do_rms, cstat, a.dim, c);
             }
         }
         if (a.rnn)
             for (int j = lane; j < a.rnn_dim; j += 32) a.traj_rnn_next[row * a.traj_rnn_stride + j] = a.rnn[row * a.rnn_dim + j];
-        // ---- post step (lane 0 owns the env's scalars)
+        // ---- env step and post step (lane 0 owns the env's scalars)
         if (lane == 0) {
+            const float r_raw = (float)act / (float)a.num_actions;
+            bool tm, tr;
+            tape_done(step, a.env_off + row, a.term_period, a.trunc_period, tm, tr);
             a.env_rew[row] = r_raw;
             a.env_term[row] = tm;
             a.env_trunc[row] = tr;
-            const bool done = tm || tr;                                     // batched_sampling.py:317
-            float r = __fmul_rn(r_raw, a.reward_scale);                     // :209
-            r = clampf(r, -a.reward_clip, a.reward_clip);                   // :210
-            a.t_rew[row * a.stride] = r;
-            a.t_done[row * a.stride] = done ? 1 : 0;
-            a.t_to[row * a.stride] = tr ? 1 : 0;                            // :328
-            a.t_pid[row * a.stride] = a.policy_id;
-            if (a.ep_ret) {                                                 // _process_env_step :215-287 (raw reward)
-                float er = er0 + r_raw;
-                int32_t el = el0 + a.len_inc;
-                float mn = fminf(mn0, r_raw), mx = fmaxf(mx0, r_raw);
-                if (a.fin_ret) {
-                    a.fin_ret[row * a.stride] = done ? er : __int_as_float(0x7fc00000);
-                    a.fin_len[row * a.stride] = done ? el : -1;
-                }
-                if (done) {
-                    if (a.stats) {
-                        atomicAdd(a.stats + 0, 1.0); atomicAdd(a.stats + 1, (double)er); atomicAdd(a.stats + 2, (double)el);
-                        atomicAdd(a.stats + 3, (double)mn); atomicAdd(a.stats + 4, (double)mx);
-                    }
-                    er = 0.f; el = 0; mn = INFINITY; mx = -INFINITY;
-                }
-                a.ep_ret[row] = er; a.ep_len[row] = el; a.ep_min[row] = mn; a.ep_max[row] = mx;
+            Episode fin;
+            if (post_step_env(a.e, row, row * a.e.stride, r_raw, tm, tr, ep, fin) && a.e.stats) {
+                atomicAdd(a.e.stats + 0, 1.0); atomicAdd(a.e.stats + 1, (double)fin.ret);
+                atomicAdd(a.e.stats + 2, (double)fin.len); atomicAdd(a.e.stats + 3, (double)fin.mn);
+                atomicAdd(a.e.stats + 4, (double)fin.mx);
             }
         }
     }
-    // every block has read both counters before taking its ticket, so the last ticket holder may advance them
     __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        unsigned long long* ticket = reinterpret_cast<unsigned long long*>(a.env_step + 1);
-        if (atomicAdd(ticket, 1ull) == (unsigned long long)gridDim.x - 1ull) {
-            *ticket = 0ull;
-            a.env_step[0] = step + 1;
-            if (a.sampler_step) *a.sampler_step += 1;
-        }
-    }
+    if (threadIdx.x == 0)
+        advance_step_counters(a.env_step, step + 1, a.sampler_step, a.sampler_step ? *a.sampler_step + 1 : 0, gridDim.x);
 }
 
 // a Box action space on the heads of up to 31 distribution_linear rows
@@ -814,11 +776,12 @@ int sfb200_sampler_tail_tape_step(const float* head_partials, int P, int64_t n_e
     if (n_envs == 0) return 0;
     const bool with_rnn = rnn && traj_rnn_next && rnn_dim > 0;
     const TapeStepArgs a{tape, tape_len, dim, A, env_index_offset, term_period, trunc_period, env_step_counter, env_obs, env_rew,
-                         env_terminated, env_truncated, reward_scale, reward_clip, policy_id, traj_rewards_t, traj_dones_t,
-                         traj_time_outs_t, traj_policy_id_t, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw,
-                         len_increment, stats, sampler_step, fin_return_t, fin_len_t, traj_obs_next, traj_obs_stride, x_norm,
-                         mean, var, sub_mean, inv_scale, fabsf(sub_mean) > 1e-8f ? 1 : 0, fabsf(inv_scale - 1.0f) > 1e-8f ? 1 : 0,
-                         eps, clip, with_rnn ? rnn : nullptr, rnn_dim, traj_rnn_next, traj_rnn_stride};
+                         env_terminated, env_truncated,
+                         EpisodeArgs{reward_scale, reward_clip, policy_id, traj_rewards_t, traj_dones_t, traj_time_outs_t,
+                                     traj_policy_id_t, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw, len_increment,
+                                     stats, fin_return_t, fin_len_t},
+                         sampler_step, traj_obs_next, traj_obs_stride, x_norm, make_obs_norm(mean, var, sub_mean, inv_scale, eps, clip),
+                         with_rnn ? rnn : nullptr, rnn_dim, traj_rnn_next, traj_rnn_stride};
     const HeadsFinish fin{out, bv, ba, noise, philox_seed, 0ull, sampler_step, policy_version_scalar};
     int64_t blocks = ceil_div(n_envs, 8);
     const int64_t cap = (int64_t)sm_count() * 8;

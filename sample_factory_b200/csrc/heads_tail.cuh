@@ -47,14 +47,61 @@ int make_heads_layout(HeadsOut& out, int space, int A, int num_heads, const int3
 constexpr float kStddevMin = 1e-4f, kStddevMax = 1e4f;   // action_distributions.py:291-292
 constexpr float kHalfLog2Pi = 0.91893853320467274178f;   // log(sqrt(2 pi))
 
-// warp-wide argmax of (best, idx) pairs, first index on ties
+// argmax of (best, idx) pairs over an aligned group of G lanes (G = 32: the warp), first index on ties
+template <int G = 32>
 __device__ __forceinline__ void argmax_first(float& best, int& idx) {   // torch.multinomial(p, 1) == argmax(p / q)
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
+    for (int o = G / 2; o > 0; o >>= 1) {
         const float ob = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
         if (ob > best || (ob == best && oi < idx)) { best = ob; idx = oi; }
     }
+}
+
+// Draw number i of a row's noise: the explicit noise[i] if given, else Philox subsequence i at `offset`.
+// Exp(1) for the categorical race (curand_uniform is in (0, 1]), N(0, 1) for a Gaussian.
+__device__ __forceinline__ float exp1_draw(const float* __restrict__ noise, int64_t i, uint64_t seed, uint64_t offset) {
+    if (noise) return noise[i];
+    curandStatePhilox4_32_10_t st;
+    curand_init(seed, (unsigned long long)i, offset, &st);
+    return fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);
+}
+__device__ __forceinline__ float normal_draw(const float* __restrict__ noise, int64_t i, uint64_t seed, uint64_t offset) {
+    if (noise) return noise[i];
+    curandStatePhilox4_32_10_t st;
+    curand_init(seed, (unsigned long long)i, offset, &st);
+    return curand_normal(&st);
+}
+
+// CategoricalActionDistribution (action_distributions.py:110-148) of one row on an aligned group of G lanes, as
+// heads_row_tail runs it on a warp: the lane holding logit a (a < A, at group position (a + 1) % G) passes x = the logit
+// and its index a; the other lanes pass a >= A.  draw: sample with draw number row_draw0 + a (exp1_draw); otherwise
+// q = 1.  Returns the sampled index on every lane of the group, and its log-prob (:145-148) in lp.
+// The reductions are xor butterflies from G/2 down to 1.  G = 8 gives the bits of the 32-lane warp for up to 8 logits:
+// on 32 lanes (logit a on lane a + 1) the xor-16 and xor-8 steps only add exact zeros or take the max with -inf, after
+// which lane (a + 1) % 8 holds logit a -- the layout of an 8-lane group -- and the xor-4, 2, 1 steps associate the same
+// terms.
+template <int G>
+__device__ __forceinline__ int categorical_draw(float x_in, int a, int A, bool draw, const float* __restrict__ noise,
+                                                int64_t row_draw0, uint64_t seed, uint64_t offset, float& lp) {
+    const bool is_logit = a < A;
+    const float x = is_logit ? x_in : -INFINITY;
+    float m = x;
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    const float e = is_logit ? expf(x - m) : 0.f;
+    float s = e;
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    const float p = __fdiv_rn(e, s);                    // softmax :116
+    const float logp = (x - m) - logf(s);               // log_softmax :125
+    const float q = (is_logit && draw) ? exp1_draw(noise, row_draw0 + a, seed, offset) : 1.f;
+    // torch.multinomial(p, 1, True) == argmax(p / q) (first index on ties)
+    float best = is_logit ? __fdiv_rn(p, q) : -INFINITY;
+    int idx = is_logit ? a : 0x7fffffff;
+    argmax_first<G>(best, idx);
+    lp = __shfl_sync(0xffffffffu, logp, (idx + 1) & (G - 1), G);
+    return idx;
 }
 
 // Slot k of lane l holds element (32k + l - S) mod 32*LPL of the row.  S = 1 leaves lane 0 free for the value: up to
@@ -135,15 +182,7 @@ __device__ __forceinline__ int row_tail(const float (&x)[LPL], int lane, int64_t
             for (int k = 0; k < LPL; ++k) {
                 const int j = slot_elem<LPL, S>(k, lane) - po;
                 if ((unsigned)j >= (unsigned)n) continue;
-                float q = 1.f;
-                if (!L.deterministic) {
-                    if (noise) q = noise[row * L.m.Wn + no + j];
-                    else {
-                        curandStatePhilox4_32_10_t st;
-                        curand_init(seed, (unsigned long long)(row * L.m.Wn + no + j), offset, &st);
-                        q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);          // Exp(1); uniform is in (0, 1]
-                    }
-                }
+                const float q = L.deterministic ? 1.f : exp1_draw(noise, row * L.m.Wn + no + j, seed, offset);
                 const float r = __fdiv_rn(p[k], q);
                 if (k == 0 || r > best || (r == best && j < idx)) { best = r; idx = j; }
             }
@@ -182,15 +221,7 @@ __device__ __forceinline__ int row_tail(const float (&x)[LPL], int lane, int64_t
                 }
                 if (out.actions_f32 == nullptr) continue;   // distribution parameters only (warp-uniform)
                 const float sd = clampf(expf(log_std), kStddevMin, kStddevMax);
-                float eps = 0.f;
-                if (!L.deterministic) {
-                    if (noise) eps = noise[row * L.m.Wn + no + j];
-                    else {
-                        curandStatePhilox4_32_10_t st;
-                        curand_init(seed, (unsigned long long)(row * L.m.Wn + no + j), offset, &st);
-                        eps = curand_normal(&st);
-                    }
-                }
+                const float eps = L.deterministic ? 0.f : normal_draw(noise, row * L.m.Wn + no + j, seed, offset);
                 // Normal.sample(): eps * std + mean, product and sum rounded separately (SURVEY App.C)
                 const float a = __fadd_rn(__fmul_rn(eps, sd), mean);
                 const float d = a - mean;
@@ -237,15 +268,7 @@ __device__ __forceinline__ void gaussian_row_tail(float mine, int lane, int64_t 
     }
     if (out.actions_f32 == nullptr) return;   // values / distribution parameters only (warp-uniform)
     const float sd = clampf(expf(log_std), kStddevMin, kStddevMax);
-    float eps = 0.f;
-    if (is_dim && !L.deterministic) {
-        if (noise) eps = noise[row * Ad + (lane - 1)];
-        else {
-            curandStatePhilox4_32_10_t st;
-            curand_init(seed, (unsigned long long)(row * Ad + (lane - 1)), offset, &st);
-            eps = curand_normal(&st);
-        }
-    }
+    const float eps = (is_dim && !L.deterministic) ? normal_draw(noise, row * Ad + (lane - 1), seed, offset) : 0.f;
     // Normal.sample(): eps * std + mean, product and sum rounded separately (SURVEY App.C)
     const float a = __fadd_rn(__fmul_rn(eps, sd), mean);
     const float d = a - mean;
@@ -267,15 +290,7 @@ __device__ __forceinline__ void tuple_row_tail(float mine, int lane, int A, int6
                                                const float* __restrict__ noise, uint64_t seed, uint64_t offset, float pv) {
     const ActionLayout& L = out.lay;
     const bool is_logit = lane >= 1 && lane <= A;
-    float q = 1.f;
-    if (is_logit && !L.deterministic) {
-        if (noise) q = noise[row * A + (lane - 1)];
-        else {
-            curandStatePhilox4_32_10_t st;
-            curand_init(seed, (unsigned long long)(row * A + (lane - 1)), offset, &st);
-            q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);
-        }
-    }
+    const float q = (is_logit && !L.deterministic) ? exp1_draw(noise, row * A + (lane - 1), seed, offset) : 1.f;
     float lp_total = 0.f;
     int start = 0;
     const int K = L.m.K;
@@ -337,16 +352,7 @@ __device__ __forceinline__ int heads_row_tail(float mine, int lane, int A, int64
         p = __fdiv_rn(p, __fadd_rn(warp_sum(p), 1.0e-13f));                // :89
         if (__ballot_sync(0xffffffffu, p > 0.f) == 0u) p = 1.0e-6f;        // :137-140 nothing allowed: uniform fallback
     }
-    float q = 1.f;
-    if (is_logit && !L.deterministic) {
-        if (noise) q = noise[row * A + (lane - 1)];
-        else {
-            curandStatePhilox4_32_10_t st;
-            curand_init(seed, (unsigned long long)(row * A + (lane - 1)), offset, &st);
-            q = -logf(curand_uniform(&st));             // Exp(1); uniform is in (0, 1]
-            q = fmaxf(q, 1.0e-30f);
-        }
-    }
+    const float q = (is_logit && !L.deterministic) ? exp1_draw(noise, row * A + (lane - 1), seed, offset) : 1.f;
     // torch.multinomial(p, 1, True) == argmax(p / q) (first index on ties)
     float best = is_logit ? __fdiv_rn(p, q) : -INFINITY;
     int idx = is_logit ? (lane - 1) : 0x7fffffff;

@@ -25,7 +25,8 @@
 // old 128 x 128 decomposition were resident, and the last two ran as a second wave after the first.
 //
 // Each GEMM tile is the wgmma tile of gemm_tc.cu (3-pass split operands, main | cross accumulators in registers); the step
-// tail is the code of sampler_tail_tape_kernel (heads.cu).
+// tail samples with categorical_draw (heads_tail.cuh) and steps the env on the rules of step_tail.cuh, as
+// sampler_tail_tape_kernel (heads.cu) does.
 //
 //   warps 0-3   TMA producer (one elected thread; the warpgroup gives its registers to the consumers).  It walks the
 //               same sequence of ring uses as the consumers and puts the weight tiles, which do not depend on the step,
@@ -50,6 +51,7 @@
 #include "common.cuh"
 #include "gemm.h"
 #include "heads_tail.cuh"
+#include "step_tail.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma_tile.cuh"
 
@@ -114,13 +116,10 @@ struct RolloutArgs {
     // tape env
     const float* tape; int64_t tape_len; int64_t env_off; int term_period, trunc_period; int64_t* env_step;
     float* env_obs; float* env_rew; uint8_t* env_term; uint8_t* env_trunc;
-    // post step
-    float reward_scale, reward_clip; int32_t policy_id; float* t_rew; uint8_t* t_done; uint8_t* t_to; int32_t* t_pid; int64_t stride;
-    float* ep_ret; int32_t* ep_len; float* ep_min; float* ep_max; int32_t len_inc; double* stats; float* fin_ret; int32_t* fin_len;
+    EpisodeArgs e;   // post step; the trajectory pointers at step 0 (slot t = + t)
     // pre step
     float* traj_obs; int64_t traj_obs_rs; const float* rnn; int rnn_dim; float* traj_rnn; int64_t traj_rnn_rs;
-    const double* mean; const double* var; float sub, inv_scale; int do_sub, do_scale; float eps, clip;
-    unsigned int* ticket;
+    ObsNorm n;
     // debug, or NULL: [T][RF_TRACE_WORDS] globaltimer stamps of CTA (0,0)'s first epilogue thread, then per CTA
     // (blockIdx.y * gridDim.x + blockIdx.x) four words: %smid, globaltimer at entry, after the programmatic-dependency
     // wait, at exit
@@ -465,7 +464,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     const int n0 = cx * BN;
     const int64_t m0 = (int64_t)blockIdx.y * BM;
     const int P = a.H2 / 64;                         // head partials per row: one per 64 columns
-    const bool do_rms = a.mean != nullptr;
+    const bool do_rms = a.n.mean != nullptr;
     unsigned long long* cta_trace =
         a.trace ? a.trace + (int64_t)a.T * RF_TRACE_WORDS + 4 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) : nullptr;
     if (cta_trace && threadIdx.x == 0) {
@@ -488,8 +487,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     pdl_wait();
     pdl_trigger();
     if (cta_trace && threadIdx.x == 0) cta_trace[2] = rf_now();
-    if (do_rms)
-        for (int c = threadIdx.x; c < a.K1; c += RF_THREADS) col_stats(a.mean, a.var, c, a.eps, cstat[c], cstat[a.K1 + c]);
+    if (do_rms) fill_col_stats(a.n, a.K1, cstat);
     if (F16) {   // the weights do not change inside a rollout: one copy per launch
         for (int i = threadIdx.x; i < BN; i += RF_THREADS) {
             s_b1[i] = a.b1[n0 + i];
@@ -578,8 +576,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
             // FOUR rows per warp at a time: an 8-lane group owns a row (one lane per action logit, the group leader also the value
             // and the env's scalars), so the 32 rows of a CTA are ONE pass of eight warps -- the per-row dependency chain (partial
             // sums from L2 -> softmax -> Philox -> argmax -> env rule -> stores, ~4.7 us measured) is paid once per step, not once
-            // per row a warp owns.  Bit-identical to heads_row_tail: logit a sits at group position (a + 1) % 8, which reproduces
-            // the association order of the 32-lane butterfly sums there (lanes 1..8 after the xor-16 / xor-8 steps).
+            // per row a warp owns.
             {
                 const int g = lane & 7;                       // position inside the 8-lane group
                 const int grp = lane >> 3;                    // which of the warp's four rows
@@ -592,7 +589,6 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                 const float* src_step = a.tape + ((step + 1) % a.tape_len) * a.N * a.K1;
                 const float* noise_t = a.noise ? a.noise + (int64_t)t * a.N * a.A : nullptr;
                 const int rpc = BM / CX;                      // rows of the block this CTA finishes
-                const unsigned gmask = 0xffu << (grp * 8);
                 for (int base = 0; base < rpc; base += 32) {
                     const int rr = base + (warp - 4) * 4 + grp;
                     const int64_t row = m0 + cx * rpc + rr;
@@ -600,8 +596,6 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                     // ---- loads first: head partials, next observation (K1 / 8 floats per lane), episode accumulators
                     float x = 0.f, val = 0.f;
                     float ob[RF_MAX_DIM / 8];
-                    float er0 = 0.f, mn0 = 0.f, mx0 = 0.f;
-                    int32_t el0 = 0;
                     const int cpl = a.K1 >> 3;                // observation columns per lane (K1 is a multiple of 32)
                     if (ok) {
                         // the fp16 form's partials are in this CTA's shared memory ([P][rpc] rows), the tf32 form's in L2
@@ -623,49 +617,17 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                                 const float4 f4 = src4[q];
                                 ob[4 * q] = f4.x; ob[4 * q + 1] = f4.y; ob[4 * q + 2] = f4.z; ob[4 * q + 3] = f4.w;
                             }
-                        if (leader && a.ep_ret) { er0 = a.ep_ret[row]; el0 = a.ep_len[row]; mn0 = a.ep_min[row]; mx0 = a.ep_max[row]; }
                     }
+                    const Episode ep = load_episode(a.e, row, ok && leader);
                     if (tr && base == 0) tr[13] = tc_now_after(val);   // partials landed
-                    // ---- CategoricalActionDistribution on the group (action_distributions.py:110-148), as heads_row_tail
                     x += has_logit ? (F16 ? s_hb[1 + act_idx] : a.ba[act_idx]) : 0.f;
                     val += F16 ? s_hb[0] : a.bv[0];
-                    const float xl = has_logit ? x : -INFINITY;
-                    float m = xl;
-#pragma unroll
-                    for (int o = 4; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-                    const float ex = has_logit ? expf(xl - m) : 0.f;
-                    float ssum = ex;
-#pragma unroll
-                    for (int o = 4; o > 0; o >>= 1) ssum += __shfl_xor_sync(0xffffffffu, ssum, o);
-                    const float pr = __fdiv_rn(ex, ssum);                       // softmax :116
-                    const float logp = (xl - m) - logf(ssum);                   // log_softmax :125
-                    float q = 1.f;
-                    if (ok && has_logit) {
-                        if (noise_t) q = noise_t[row * a.A + act_idx];
-                        else {
-                            curandStatePhilox4_32_10_t st;
-                            curand_init(a.seed, (unsigned long long)(row * a.A + act_idx), offset, &st);
-                            q = fmaxf(-logf(curand_uniform(&st)), 1.0e-30f);    // Exp(1)
-                        }
-                    }
-                    float best = has_logit ? __fdiv_rn(pr, q) : -INFINITY;      // multinomial == argmax(p / q), first index on ties
-                    int idx = has_logit ? act_idx : 0x7fffffff;
-#pragma unroll
-                    for (int o = 4; o > 0; o >>= 1) {
-                        const float ob_ = __shfl_xor_sync(0xffffffffu, best, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-                        if (ob_ > best || (ob_ == best && oi < idx)) { best = ob_; idx = oi; }
-                    }
-                    const float lp = __shfl_sync(0xffffffffu, logp, (grp << 3) | ((idx + 1) & 7));   // log_prob :145-148
+                    float lp;
+                    const int idx = categorical_draw<8>(x, act_idx, a.A, ok, noise_t, row * a.A, a.seed, offset, lp);
                     if (tr && base == 0) tr[15] = tc_now_after(lp);    // action sampled
-                    (void)gmask;
                     if (!ok) continue;
                     // ---- trajectory slot t, env step, post step, pre step of t + 1
                     if (has_logit) a.logits[row * a.logits_rs + (int64_t)t * a.A + act_idx] = x;
-                    const int64_t env = a.env_off + row;
-                    const float r_raw = (float)idx / (float)a.A;
-                    const bool tm = ((step * 7 + env * 13) % a.term_period) == 0;
-                    const bool tr = (((step + env) % a.trunc_period) == 0) && !tm;
                     float* obs_next = a.traj_obs + row * a.traj_obs_rs + (int64_t)(t + 1) * a.K1 + g * cpl;
                     float* env_o = a.env_obs + row * a.K1 + g * cpl;
                     float* xn = a.x_norm + row * a.K1 + g * cpl;
@@ -677,18 +639,18 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                             reinterpret_cast<float4*>(obs_next)[q4] = f4;
                             if (!last) {
                                 const int c = g * cpl + 4 * q4;
-                                float4 y;
-                                y.x = norm_one(f4.x, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c] : 0.f, do_rms ? cstat[a.K1 + c] : 1.f, a.clip);
-                                y.y = norm_one(f4.y, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 1] : 0.f, do_rms ? cstat[a.K1 + c + 1] : 1.f, a.clip);
-                                y.z = norm_one(f4.z, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 2] : 0.f, do_rms ? cstat[a.K1 + c + 2] : 1.f, a.clip);
-                                y.w = norm_one(f4.w, a.sub, a.inv_scale, a.do_sub, a.do_scale, do_rms, do_rms ? cstat[c + 3] : 0.f, do_rms ? cstat[a.K1 + c + 3] : 1.f, a.clip);
-                                reinterpret_cast<float4*>(xn)[q4] = y;
+                                reinterpret_cast<float4*>(xn)[q4] =
+                                    make_float4(a.n.apply(f4.x, do_rms, cstat, a.K1, c), a.n.apply(f4.y, do_rms, cstat, a.K1, c + 1),
+                                                a.n.apply(f4.z, do_rms, cstat, a.K1, c + 2), a.n.apply(f4.w, do_rms, cstat, a.K1, c + 3));
                             }
                         }
                     if (a.rnn)
                         for (int j = g; j < a.rnn_dim; j += 8)
                             a.traj_rnn[row * a.traj_rnn_rs + (int64_t)(t + 1) * a.rnn_dim + j] = a.rnn[row * a.rnn_dim + j];
                     if (leader) {
+                        const float r_raw = (float)idx / (float)a.A;
+                        bool tm, to;
+                        tape_done(step, a.env_off + row, a.term_period, a.trunc_period, tm, to);
                         a.values[row * a.values_rs + t] = val;
                         a.actions[row * a.actions_rs + t] = (float)idx;
                         a.env_actions[row] = idx;
@@ -696,30 +658,12 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                         a.pv_out[row * a.pv_rs + t] = pv;
                         a.env_rew[row] = r_raw;
                         a.env_term[row] = tm;
-                        a.env_trunc[row] = tr;
-                        const bool done = tm || tr;                                     // batched_sampling.py:317
-                        float r = __fmul_rn(r_raw, a.reward_scale);                     // :209
-                        r = clampf(r, -a.reward_clip, a.reward_clip);                   // :210
-                        a.t_rew[row * a.stride + t] = r;
-                        a.t_done[row * a.stride + t] = done ? 1 : 0;
-                        a.t_to[row * a.stride + t] = tr ? 1 : 0;                        // :328
-                        a.t_pid[row * a.stride + t] = a.policy_id;
-                        if (a.ep_ret) {                                                 // _process_env_step :215-287 (raw reward)
-                            float er = er0 + r_raw;
-                            int32_t el = el0 + a.len_inc;
-                            float mn = fminf(mn0, r_raw), mx = fmaxf(mx0, r_raw);
-                            if (a.fin_ret) {
-                                a.fin_ret[row * a.stride + t] = done ? er : __int_as_float(0x7fc00000);
-                                a.fin_len[row * a.stride + t] = done ? el : -1;
-                            }
-                            if (done) {
-                                if (a.stats) {
-                                    atomicAdd(&s_stats[0], 1.0); atomicAdd(&s_stats[1], (double)er); atomicAdd(&s_stats[2], (double)el);
-                                    atomicAdd(&s_stats[3], (double)mn); atomicAdd(&s_stats[4], (double)mx);
-                                }
-                                er = 0.f; el = 0; mn = INFINITY; mx = -INFINITY;
-                            }
-                            a.ep_ret[row] = er; a.ep_len[row] = el; a.ep_min[row] = mn; a.ep_max[row] = mx;
+                        a.env_trunc[row] = to;
+                        Episode fin;
+                        if (post_step_env(a.e, row, row * a.e.stride + t, r_raw, tm, to, ep, fin) && a.e.stats) {
+                            atomicAdd(&s_stats[0], 1.0); atomicAdd(&s_stats[1], (double)fin.ret);
+                            atomicAdd(&s_stats[2], (double)fin.len); atomicAdd(&s_stats[3], (double)fin.mn);
+                            atomicAdd(&s_stats[4], (double)fin.mx);
                         }
                     }
                 }
@@ -735,15 +679,10 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
 
     // every block has read the two step counters at its start; the last one to finish advances them by T
     __syncthreads();
-    if (threadIdx.x < 5 && a.stats && s_stats[0] > 0.0) atomicAdd(a.stats + threadIdx.x, s_stats[threadIdx.x]);
+    if (threadIdx.x < 5 && a.e.stats && s_stats[0] > 0.0) atomicAdd(a.e.stats + threadIdx.x, s_stats[threadIdx.x]);
     if (threadIdx.x == 0) {
         if (cta_trace) cta_trace[3] = rf_now();
-        __threadfence();
-        if (atomicAdd(a.ticket, 1u) == gridDim.x * gridDim.y - 1u) {
-            *a.ticket = 0u;
-            a.env_step[0] = env_step0 + a.T;
-            if (a.sampler_step) *a.sampler_step = (int64_t)philox0 + a.T;
-        }
+        advance_step_counters(a.env_step, env_step0 + a.T, a.sampler_step, (int64_t)philox0 + a.T, gridDim.x * gridDim.y);
     }
 }
 
@@ -940,17 +879,16 @@ int sfb200_rollout_mlp2_tape(int64_t n_envs, int T, int K1, const float* W1, con
     SFB_CHECK_ARG((reinterpret_cast<uintptr_t>(h1_scratch) & 15u) == 0 && (reinterpret_cast<uintptr_t>(x_norm) & 15u) == 0 &&
                       (reinterpret_cast<uintptr_t>(head_partials) & 15u) == 0, "rollout_mlp2_tape: scratch buffers must be 16-byte aligned");
     const bool with_rnn = rnn && traj_rnn_0 && rnn_dim > 0;
-    // the block ticket lives in the second word pair of the env's step counter (int64 [2]: step, ticket)
-    unsigned int* ticket = reinterpret_cast<unsigned int*>(env_step_counter + 1);
     const RolloutArgs a{n_envs, T, K1, H1, H2, b1, b2, Wv, Wa, A, bv, ba, h1_scratch, head_partials, x_norm,
                         values_0, values_stride, logits_0, logits_stride, actions_0, actions_stride, env_actions, log_prob_0,
                         log_prob_stride, policy_version_0, pv_stride, policy_version_scalar, noise, philox_seed, sampler_step,
                         tape, tape_len, env_index_offset, term_period, trunc_period, env_step_counter, env_obs, env_rew,
-                        env_terminated, env_truncated, reward_scale, reward_clip, policy_id, traj_rewards_0, traj_dones_0,
-                        traj_time_outs_0, traj_policy_id_0, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw, len_increment,
-                        stats, fin_return_0, fin_len_0, traj_obs_0, traj_obs_stride, with_rnn ? rnn : nullptr, rnn_dim, traj_rnn_0,
-                        traj_rnn_stride, mean, var, sub_mean, inv_scale, fabsf(sub_mean) > 1e-8f ? 1 : 0,
-                        fabsf(inv_scale - 1.0f) > 1e-8f ? 1 : 0, eps, clip, ticket, g_rollout_trace, nullptr, nullptr};
+                        env_terminated, env_truncated,
+                        EpisodeArgs{reward_scale, reward_clip, policy_id, traj_rewards_0, traj_dones_0, traj_time_outs_0,
+                                    traj_policy_id_0, traj_stride, ep_return, ep_len, ep_min_raw, ep_max_raw, len_increment, stats,
+                                    fin_return_0, fin_len_0},
+                        traj_obs_0, traj_obs_stride, with_rnn ? rnn : nullptr, rnn_dim, traj_rnn_0, traj_rnn_stride,
+                        make_obs_norm(mean, var, sub_mean, inv_scale, eps, clip), g_rollout_trace, nullptr, nullptr};
     const int rc = tc_rollout_mlp2_tape(W1, W2, act, engine, a, (cudaStream_t)stream);
     SFB_CHECK_ARG(rc != SFB_TC_UNSUPPORTED, "rollout_mlp2_tape: model not covered (K1=%d H1=%d H2=%d A=%d engine=%d); "
                   "sfb200_rollout_mlp2_partials() tells when to use the per-step calls", K1, H1, H2, A, engine);

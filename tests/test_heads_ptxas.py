@@ -1,7 +1,7 @@
 """Register spills of the heads kernels do not grow (the Makefile writes each object's ptxas -v report to
 csrc/build/<name>.ptxas.log); the figures are nvcc 12.9's for sm_90a.  The GEMMs that finish the heads in their epilogue (HEADS = true) sit at the
-384-thread register cap, so they must stay at 168 registers or fewer without spilling, and heads_from_partials_kernel,
-which runs on the learner's path, keeps to 48 registers."""
+384-thread register cap, so they must stay at 168 registers or fewer without spilling; heads_from_partials_kernel,
+which runs on the learner's path, keeps to 48 registers, and sampler_tail_tape_kernel to 128."""
 import os
 import re
 import subprocess
@@ -11,9 +11,7 @@ BUILD = os.path.join(ROOT, "sample_factory_b200", "csrc", "build")
 
 # demangled kernel -> (spill store, spill load) bytes allowed; kernels not listed: none
 SPILLS = {
-    "sfb::sampler_tail_tape_kernel": (8, 8),
     "void sfb::heads_forward_kernel<32, 1, true>": (20, 12),
-    "void sfb::heads_forward_kernel<9, 4, false>": (12, 48),
 }
 NARROW = {"heads_forward_kernel": 7, "heads_from_partials_kernel": 1, "sampler_tail_tape_kernel": 1}
 
@@ -42,6 +40,8 @@ def test_narrow_heads_kernels_spill_no_more_than_listed():
     _check(found)
     regs = [r for name, _, _, r in found if name == "sfb::heads_from_partials_kernel"]
     assert regs[0] <= 48, regs
+    regs = [r for name, _, _, r in found if name == "sfb::sampler_tail_tape_kernel"]
+    assert regs[0] <= 128, regs
 
 
 def test_stored_row_tail_does_not_spill():

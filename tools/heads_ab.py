@@ -7,7 +7,14 @@ Runs heads_forward (every instantiation the dispatch picks), heads_from_partials
 Tuple entry points on seeded inputs: Discrete (masked, with an all-masked row), Tuple, Box adaptive and learned
 (tanh_scale 0 and 1.5), each with explicit noise, Philox and deterministic sampling, plus the values-only and
 params-only modes.  Every output (values, params rows, actions, env actions, log-prob, policy-version stamp) is stored
-as int32 bit patterns, so -0.0 and NaN payloads count."""
+as int32 bit patterns, so -0.0 and NaN payloads count.
+
+The step-tail section runs the entry points after the heads -- sampler_tail_tape_step, sampler_post_step,
+sampler_post_pre_step, tape_env_step(_continuous) and the persistent rollout_mlp2_tape (tf32 form: no fp16 twins are
+registered here) -- over N = 4000 envs (a partial last row block), K1 in {32, 64, 96, 128} and H in {128, 256, 512},
+with explicit noise and Philox, with and without the normaliser's running statistics and with and without the episode,
+fin_* and stats buffers.  Every env, trajectory, episode and counter buffer is compared bit for bit, except the episode
+statistics (keys ending in /stats): sums of double atomics in a run-dependent order, compared with rtol 1e-12."""
 from __future__ import annotations
 
 import argparse
@@ -213,17 +220,147 @@ def run(out_path):
                      log_prob=o["log_prob"], pv=o["policy_version_out"],
                      **{f"env{i}": e for i, e in enumerate(env)})
     ops.set_sampling_mode(None, False)
+    step_tail(ops, dev, g, rnd, keep)
+    res.update(res_stats)
     np.savez_compressed(out_path, **res)
     print(f"{len(res)} arrays -> {out_path}")
+
+
+def step_tail(ops, dev, g, rnd, keep):
+    import torch
+
+    from sample_factory_b200.envs import TapeVecEnv
+    from sample_factory_b200.trajectory import alloc_trajectory_tensors
+
+    N, A, T, R = 4000, 6, 5, 16
+
+    def episode(full):
+        """episode accumulators, stats and fin_* buffers (all None when not full)"""
+        if not full:
+            return dict(ep_return=None, ep_len=None, ep_min_raw=None, ep_max_raw=None, stats=None)
+        return dict(ep_return=rnd(N), ep_len=torch.randint(0, 50, (N,), generator=g, dtype=torch.int32).to(dev),
+                    ep_min_raw=rnd(N), ep_max_raw=rnd(N), stats=torch.zeros(8, dtype=torch.float64, device=dev))
+
+    def fin(full, t_=T):
+        if not full:
+            return None, None
+        return torch.full((N, t_), -7.0, device=dev), torch.full((N, t_), -7, dtype=torch.int32, device=dev)
+
+    def keep_tail(name, env, ep, traj, **more):
+        """the env, episode and trajectory buffers a step-tail entry point writes; the episode statistics aside"""
+        out = dict(env_obs=env.obs, env_rew=env.rew, env_term=env.terminated, env_trunc=env.truncated,
+                   env_step=env.step_counter, **{k: v for k, v in ep.items() if k != "stats"}, **traj, **more)
+        keep(name, **{k: v.int() if v is not None and v.dtype == torch.bool else v for k, v in out.items()})
+        if ep["stats"] is not None:
+            res_stats[f"{name}/stats"] = ep["stats"].cpu().numpy()
+
+    def norm(rms, dim):
+        if not rms:
+            return dict(mean=None, var=None, sub_mean=0.0, inv_scale=1.0)
+        return dict(mean=rnd(dim, scale=0.3).double(), var=(rnd(dim).abs() + 0.5).double(), sub_mean=0.25, inv_scale=0.5)
+
+    for K1 in (32, 64, 96, 128):
+        tape = rnd(2 * T + 1, N, K1)
+        for full in (True, False):
+            for rms in (True, False):
+                tag = f"{K1}/{'ep' if full else 'noep'}/{'rms' if rms else 'norms'}"
+                # ---- per-stage kernels: env step (Discrete and Box), post step, post + pre step
+                env = TapeVecEnv(tape, A)
+                env.step_counter[0] = 3
+                acts = torch.randint(0, A, (N,), generator=g, dtype=torch.int32).to(dev)
+                ops.tape_env_step(acts, A, 5, env.term_period, env.trunc_period, env.step_counter, 0, tape, env.obs, env.rew,
+                                  env.terminated, env.truncated)
+                keep(f"tail/env/{tag}", obs=env.obs, rew=env.rew, term=env.terminated.int(), trunc=env.truncated.int(),
+                     step=env.step_counter)
+                acts_f = rnd(N, 3)
+                ops.tape_env_step_continuous(acts_f, 5, env.term_period, env.trunc_period, None, 7, None, None, env.rew,
+                                             env.terminated, env.truncated)
+                keep(f"tail/env_box/{tag}", rew=env.rew, term=env.terminated.int(), trunc=env.truncated.int())
+                traj = alloc_trajectory_tensors(K1, A, N, T, dev, rnn_size=R)
+                ep = episode(full)
+                fr, fl = fin(full)
+                pstep = torch.zeros(1, dtype=torch.int64, device=dev)
+                ops.sampler_post_step(env.rew, env.terminated, env.truncated, 0.5, 0.3, 2, traj["rewards"][:, 0],
+                                      traj["dones"][:, 0], traj["time_outs"][:, 0], traj["policy_id"][:, 0], ep["ep_return"],
+                                      ep["ep_len"], ep["ep_min_raw"], ep["ep_max_raw"], 2, ep["stats"], pstep,
+                                      None if fr is None else fr[:, 0], None if fl is None else fl[:, 0])
+                rnn = rnd(N, R)
+                x_norm = torch.full((N, K1), -7.0, device=dev)
+                ops.sampler_post_pre_step(env.rew, env.terminated, env.truncated, 1.0, 10.0, 1, traj["rewards"][:, 1],
+                                          traj["dones"][:, 1], traj["time_outs"][:, 1], traj["policy_id"][:, 1],
+                                          ep["ep_return"], ep["ep_len"], ep["ep_min_raw"], ep["ep_max_raw"], 1, ep["stats"],
+                                          pstep, None if fr is None else fr[:, 1], None if fl is None else fl[:, 1],
+                                          obs=env.obs, traj_obs_next=traj["obs"][:, 2], rnn=rnn,
+                                          traj_rnn_next=traj["rnn_states"][:, 2], x_norm=x_norm, **norm(rms, K1))
+                keep_tail(f"tail/post/{tag}", env, ep, traj, pstep=pstep, x_norm=x_norm, fin_ret=fr, fin_len=fl)
+                for mode in ("noise", "philox"):
+                    noise = torch.rand(T, N, A, generator=g).clamp_min(1e-6).to(dev) if mode == "noise" else None
+                    # ---- fused step tail (heads.cu): T steps on random partials
+                    env = TapeVecEnv(tape, A, env_index_offset=11)
+                    traj = alloc_trajectory_tensors(K1, A, N, T, dev, rnn_size=R)
+                    ep = episode(full)
+                    fr, fl = fin(full)
+                    sstep = torch.full((1,), 4, dtype=torch.int64, device=dev)
+                    env_actions = torch.full((N,), -7, dtype=torch.int32, device=dev)
+                    x_norm = torch.full((N, K1), -7.0, device=dev)
+                    bv, ba, P = rnd(1), rnd(A), 3
+                    pv = torch.tensor([2.0], device=dev)
+                    tr = traj
+                    for t in range(T):
+                        part = rnd(P, N, 12)
+                        ops.sampler_tail_tape_step(
+                            part, P, N, bv, ba, values=tr["values"][:, t], values_stride=tr["values"].stride(0),
+                            logits=tr["action_logits"][:, t], logits_stride=tr["action_logits"].stride(0),
+                            noise=None if noise is None else noise[t], philox_seed=77, sampler_step=sstep,
+                            actions_f32=tr["actions"][:, t], actions_stride=tr["actions"].stride(0),
+                            env_actions=env_actions,
+                            log_prob=tr["log_prob_actions"][:, t], log_prob_stride=tr["log_prob_actions"].stride(0),
+                            policy_version_scalar=pv, policy_version_out=tr["policy_version"][:, t],
+                            pv_stride=tr["policy_version"].stride(0), env=env, reward_scale=0.5, reward_clip=0.3,
+                            policy_id=1, traj_rewards=tr["rewards"][:, t], traj_dones=tr["dones"][:, t],
+                            traj_time_outs=tr["time_outs"][:, t], traj_policy_id=tr["policy_id"][:, t], len_increment=2,
+                            fin_return=None if fr is None else fr[:, t], fin_len=None if fl is None else fl[:, t],
+                            traj_obs_next=tr["obs"][:, t + 1], rnn=rnn, traj_rnn_next=tr["rnn_states"][:, t + 1],
+                            x_norm=None if t == T - 1 else x_norm, **ep, **norm(rms, K1))
+                    keep_tail(f"tail/fused/{tag}/{mode}", env, ep, traj, x_norm=x_norm, fin_ret=fr, fin_len=fl,
+                              env_actions=env_actions, sstep=sstep)
+                    # ---- persistent rollout (rollout_fused.cu)
+                    for H in (128, 256, 512):
+                        W1, b1, W2, b2 = rnd(H, K1, scale=0.1), rnd(H, scale=0.1), rnd(H, H, scale=0.05), rnd(H, scale=0.1)
+                        Wv, bv, Wa, ba = rnd(H, scale=0.1), rnd(1), rnd(A, H, scale=0.1), rnd(A)
+                        assert ops.rollout_mlp2_partials(W1, W2, A, ops.GEMM_TC_3XTF32)
+                        env = TapeVecEnv(tape, A, env_index_offset=11)
+                        env.step_counter[0] = 2
+                        traj = alloc_trajectory_tensors(K1, A, N, T, dev, rnn_size=R)
+                        ep = episode(full)
+                        fr, fl = fin(full)
+                        sstep = torch.full((1,), 9, dtype=torch.int64, device=dev)
+                        env_actions = torch.full((N,), -7, dtype=torch.int32, device=dev)
+                        x_norm = rnd(N, K1)
+                        h1 = torch.zeros(N, H, device=dev)
+                        part = torch.zeros(H // 64, N, 12, device=dev)
+                        ops.rollout_mlp2_tape(T, W1, b1, W2, b2, ops.ACT["elu"], ops.GEMM_TC_3XTF32, Wv, bv, Wa, ba, h1,
+                                              part, x_norm, traj, env, noise, 55, sstep, env_actions, pv, 0.5, 0.3, 1,
+                                              ep["ep_return"], ep["ep_len"], ep["ep_min_raw"], ep["ep_max_raw"], 2,
+                                              ep["stats"], fr, fl, rnn, **norm(rms, K1))
+                        keep_tail(f"tail/rollout/{H}/{tag}/{mode}", env, ep, traj, x_norm=x_norm, fin_ret=fr, fin_len=fl,
+                                  env_actions=env_actions, sstep=sstep)
+
+
+res_stats = {}   # episode statistics of the step-tail section: float64, compared with rtol 1e-12
 
 
 def compare(a_path, b_path):
     a, b = np.load(a_path), np.load(b_path)
     assert sorted(a.files) == sorted(b.files), set(a.files) ^ set(b.files)
-    bad = [k for k in a.files if a[k].shape != b[k].shape or not np.array_equal(a[k], b[k])]
+    stats = [k for k in a.files if k.endswith("/stats")]
+    for k in stats:
+        np.testing.assert_allclose(a[k], b[k], rtol=1e-12, err_msg=k)
+    bad = [k for k in a.files if k not in stats and (a[k].shape != b[k].shape or not np.array_equal(a[k], b[k]))]
     for k in bad[:20]:
         print("DIFFERS", k, int((a[k] != b[k]).sum()) if a[k].shape == b[k].shape else "shape")
-    print(f"{len(a.files) - len(bad)} / {len(a.files)} arrays bit-identical")
+    print(f"{len(a.files) - len(stats) - len(bad)} / {len(a.files) - len(stats)} arrays bit-identical, "
+          f"{len(stats)} episode statistics within rtol 1e-12")
     return 1 if bad else 0
 
 
