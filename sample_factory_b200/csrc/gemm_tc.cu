@@ -69,7 +69,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
     static_assert(!F16 || (!A_MN && SPLIT3), "fp16-split engine: K-major activations, 3-pass");
     static_assert(!DW16 || (A_MN && B_MN && SPLIT3 && !HEADS && !F16 && !RES), "fp16 dW form: MN-major operands, plain epilogue");
     if (trace && threadIdx.x == 0) trace[blockIdx.x * kTraceWords + 8] = tc_now();
-    using S = TcSmem<F16, DW16>;
+    using S = TcSmem<F16, DW16, HEADS>;
     constexpr int KBK = S::KBK;
     constexpr int SA = S::A_STAGES, SB = S::B_STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -151,6 +151,12 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
     setmaxnreg_inc<kConsumerRegs>();
     const int ct = threadIdx.x - 128;          // 0..255
     const int wg = ct >> 7;                    // 64-row half of the tile
+    if constexpr (HEADS && F16) {
+        // the [Wv; Wa] operand of the head partials, all N columns: written once, read by every item's epilogue
+        fill_head_weights_f16(smem + S::HW_OFF, epi.head_wv, epi.head_wa, epi.head_A, N, 0, N, ct, 256);
+        fence_proxy_async_smem();
+        consumer_sync();
+    }
 
     // fp16-split engine: binary shift of the A operand from its bound (written by an earlier kernel of the stream)
     const int a_shift = (F16 || DW16) ? f16_shift_for_bound(a_bound[0]) : 0;
@@ -306,13 +312,23 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap& tmap_a, const CU
         // the epilogue's mode and activation are chosen once per item; whole tiles (all of them at the learner's shapes)
         // then run straight-line code
         const int64_t row_base = tc.m0 + wg * 64 + ((ct >> 5) & 3) * 16 + (lane >> 2);
-        if constexpr (HEADS) {
+        if constexpr (HEADS && F16) {
+            const uint32_t hw = smem_u32(smem + S::HW_OFF);
+            switch (epi.act) {
+                case SFB200_ACT_ELU: heads_tile_f16<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, epi, hw, tr); break;
+                case SFB200_ACT_RELU: heads_tile_f16<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, epi, hw, tr); break;
+                case SFB200_ACT_TANH: heads_tile_f16<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, epi, hw, tr); break;
+                default: heads_tile_f16<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, epi, hw, tr); break;
+            }
+        } else if constexpr (HEADS) {
             switch (epi.act) {
                 case SFB200_ACT_ELU: heads_tile<SFB200_ACT_ELU>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
                 case SFB200_ACT_RELU: heads_tile<SFB200_ACT_RELU>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
                 case SFB200_ACT_TANH: heads_tile<SFB200_ACT_TANH>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
                 default: heads_tile<SFB200_ACT_NONE>(acc, tc, row_base, lane, C, ldc, M, N, epi, tr); break;
             }
+        }
+        if constexpr (HEADS) {
             if (epi.fin_counters) {
                 // last-arriving n-tile CTA of this 128-row block finishes the heads (threadFenceReduction pattern)
                 const int mb = (int)(tc.m0 / TBM);
@@ -465,7 +481,7 @@ static int launch_tc(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int
                      int k_chunk, int splits, const TcEpilogue& epi, cudaStream_t st, const float* a_bound = nullptr,
                      const float* b_bound = nullptr) {
     auto kern = tc_kernel<A_MN, B_MN, SPLIT3, HEADS, F16, RES, DW16>();
-    constexpr int smem = TcSmem<F16, DW16>::TOTAL;
+    constexpr int smem = TcSmem<F16, DW16, HEADS>::TOTAL;
     static int ctas_per_sm = 0;   // of this instantiation: 1 (shared memory), asked rather than assumed
     if (!ctas_per_sm) {
         SFB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));

@@ -16,8 +16,9 @@
 //                       CTA that finishes the row (st.shared::cluster), summed from there by the tail; barrier 2 orders
 //                       writer and reader, and barriers 3 and 1 of the next step come between the tail's reads and the
 //                       next writes.  tf32 form: global memory.
-//   b1, b2, [Wv; Wa] rows, bv, ba   fp16 form: copied into shared memory once per launch (this CTA's BN columns), read
-//                       from there by both epilogues and the tail.  tf32 form (no room beside its 104 KB slots): global.
+//   b1, b2, [Wv; Wa] rows, bv, ba   fp16 form: copied into shared memory once per launch (this CTA's BN columns; [Wv; Wa]
+//                       as the fp16 B operand of the tensor-core head partials), read from there by both epilogues and
+//                       the tail.  tf32 form (no room beside its 104 KB slots): global.
 // The CTA tile (rf_wide): BM x BN = 64 x 256 for H2 >= 256 (the two consumer warpgroups side by side on N over one 64-row
 // A tile), 128 x 128 for H2 = 128 (the warpgroups stacked on M).  At H2 = 512 that makes clusters of two: a TPC is two SMs,
 // so every GPC holds a whole number of them and the whole grid (64 clusters at 4096 envs) is resident at once.  Clusters
@@ -61,9 +62,10 @@ constexpr int RF_THREADS = 384;
 constexpr int RF_HEAD_AP = 9;
 constexpr int RF_MAX_DIM = 128;
 constexpr int RF_TRACE_WORDS = 32;   // phase stamps per step (sfb200_rollout_set_trace)
-// register budgets after the hand-over: 128 x 40 + 256 x 232 = the 384 x 168 the launch gets
-constexpr int RF_PRODUCER_REGS = 40;
-constexpr int RF_CONSUMER_REGS = 232;
+// register budgets after the hand-over: 128 x 24 + 256 x 240 = the 384 x 168 the launch gets (the consumers hold the
+// tensor-core head partials beside the step loop's state; the producer issues TMA loads only)
+constexpr int RF_PRODUCER_REGS = 24;
+constexpr int RF_CONSUMER_REGS = 240;
 
 // CTA tile of a layer: BM x BN = 64 x 256 (warpgroup w: columns n0 + 128 w of the same 64 rows) for H2 >= 256, else
 // 128 x 128 (warpgroup w: rows m0 + 64 w).  Same rule on the host (launch shape, TMA boxes) and in the kernel.
@@ -78,9 +80,9 @@ __host__ __device__ __forceinline__ int rf_bn(int H2) { return rf_wide(H2) ? 256
 // Two slots: three 80 KB stages do not fit.  The conversion buffer [A hi | A lo] (BM x 256 B: the operands split in shared
 // memory) follows the slots.  fp16 form: then a 16 KB staging buffer of the h1 store (store_h1_tma), the head partials of
 // the rows this CTA finishes ([P][rows][kHeadPartPad] floats, P * rows = H2 / 64 * BM / CX = 256 in every layout: 12 KB)
-// and the step-invariant operands of the CTA's BN <= 256 columns: b1, b2, the [Wv; Wa] rows (RF_HEAD_AP x 256 floats),
-// then bv, ba (16 floats).  The tf32 form has no room for them (two 104 KB slots).  The mbarriers and the normaliser
-// statistics follow the largest layout.
+// and the step-invariant operands of the CTA's BN <= 256 columns: b1, b2, the [Wv; Wa] operand of the head partials
+// (fill_head_weights_f16: 16 rows x 256 columns, hi and lo planes, 16 KB), then bv, ba (16 floats).  The tf32 form has
+// no room for them (two 104 KB slots).  The mbarriers and the normaliser statistics follow the largest layout.
 template <bool F16>
 struct RfSmem {
     static constexpr int STAGES = 2;
@@ -94,7 +96,7 @@ struct RfSmem {
     static constexpr int OFF_B1 = OFF_PART + (F16 ? 256 * kHeadPartPad * 4 : 0);
     static constexpr int OFF_B2 = OFF_B1 + (F16 ? 256 * 4 : 0);
     static constexpr int OFF_HW = OFF_B2 + (F16 ? 256 * 4 : 0);
-    static constexpr int OFF_HB = OFF_HW + (F16 ? RF_HEAD_AP * 256 * 4 : 0);
+    static constexpr int OFF_HB = OFF_HW + (F16 ? (256 / TBN) * kHeadTileBytes : 0);
     static constexpr int OFF_BARS = OFF_HB + (F16 ? 16 * 4 : 0);   // full[STAGES], empty[STAGES]
     static constexpr int OFF_CSTAT = OFF_BARS + 64;
     static constexpr int TOTAL = OFF_CSTAT + 2 * RF_MAX_DIM * 4 + 1024 /*align slack*/;
@@ -102,6 +104,7 @@ struct RfSmem {
     static_assert(STAGES * slot(128, 128) + 128 * 256 <= OFF_PART, "the 128 x 128 layout fits below the partials");
     static_assert(a_bytes(64) % 1024 == 0 && slot(64, 256) % 1024 == 0 && OFF_CONV_END % 1024 == 0,
                   "h1 staging boxes (slot A regions, conversion buffer, the buffer after it) on 1024 B swizzle atoms");
+    static_assert(OFF_HW % 1024 == 0, "the head operand on 1024 B swizzle atoms");
 };
 
 
@@ -152,9 +155,8 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
     return r;
 }
-__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
-    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                 : "memory");
+__device__ __forceinline__ void st_cluster_f2(uint32_t addr, float2 v) {
+    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -368,17 +370,16 @@ __device__ __forceinline__ void store_h1_tma(const float (&acc)[64], const CUten
     }
 }
 
-// Layer-2 epilogue of the fp16 form: heads_tile's arithmetic (same expressions, same order of operations, so the same
-// bits) with b2 and the [Wv; Wa] rows read from the CTA's copies in shared memory (`b2`, `hw`: BN columns, rows of 256
-// floats), and each row's two partials written into the shared memory of the cluster CTA that finishes the row: rows
-// [c rpc, c rpc + rpc) of the block belong to CTA c, partial p of its row r at part + ((p * rpc + r) * kHeadPartPad) floats.
-// nl: the warpgroup's first column inside the CTA's tile; p0: its first partial (global column / 64); rb: the thread's
-// first row inside the block.
+// Layer-2 epilogue of the fp16 form: heads_tile_f16's arithmetic (same y, same head_partials_f16, so the same bits) with
+// b2 and the [Wv; Wa] operand read from the CTA's copies in shared memory (`b2`: BN columns; `hw`: fill_head_weights_f16
+// from the CTA's first column), and each row's two partials written into the shared memory of the cluster CTA that
+// finishes the row: rows [c rpc, c rpc + rpc) of the block belong to CTA c, partial p of its row r at
+// part + ((p * rpc + r) * kHeadPartPad) floats.  nl: the warpgroup's first column inside the CTA's tile; p0: its first
+// partial (global column / 64); rb: the thread's first row inside the block.
 template <int ACT>
 __device__ __forceinline__ void rf_heads_tile(float (&acc)[64], int nl, int p0, int rb, int lane, const float* b2,
-                                              const float* hw, int A, uint32_t part, int rpc) {
-    constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
-    const int nq = nl + 2 * (lane & 3);
+                                              uint32_t hw, uint32_t part, int rpc) {
+    const int q = lane & 3, nq = nl + 2 * q;
     float b[32];
 #pragma unroll
     for (int c = 0; c < 16; ++c) {
@@ -390,46 +391,18 @@ __device__ __forceinline__ void rf_heads_tile(float (&acc)[64], int nl, int p0, 
         acc[2 * j] = act_fwd_ct<ACT>(acc[2 * j] + b[j & ~1]);
         acc[2 * j + 1] = act_fwd_ct<ACT>(acc[2 * j + 1] + b[j | 1]);
     }
+    float hp[2][8];
+    head_partials_f16<64>(acc, hw + (uint32_t)(nl / TBN) * kHeadTileBytes, hp);
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-        float hp[2][kHeadAP];
+    for (int half = 0; half < 2; ++half)
 #pragma unroll
-        for (int a = 0; a < kHeadAP; ++a) {
-            float s[2] = {0.f, 0.f};
-            if (a <= A) {
-                const float* w = hw + a * 256 + nq + 64 * half;
-                float2 wv[JP / 2];
-#pragma unroll
-                for (int jj = 0; jj < JP / 2; ++jj) wv[jj] = *reinterpret_cast<const float2*>(w + 8 * jj);
-#pragma unroll
-                for (int jj = 0; jj < JP / 2; ++jj) {
-#pragma unroll
-                    for (int rs = 0; rs < 2; ++rs) {
-                        const int j = JP * half + 2 * jj + rs;
-                        s[rs] = fmaf(acc[2 * j], wv[jj].x, s[rs]);
-                        s[rs] = fmaf(acc[2 * j + 1], wv[jj].y, s[rs]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int rs = 0; rs < 2; ++rs) {
-                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 1);
-                s[rs] += __shfl_xor_sync(0xffffffffu, s[rs], 2);
-                hp[rs][a] = s[rs];
-            }
+        for (int rs = 0; rs < 2; ++rs) {
+            const int r = rb + 8 * rs;
+            const uint32_t dst = mapa_shared(part + (uint32_t)((((p0 + half) * rpc + r % rpc) * kHeadPartPad + 2 * q) * 4),
+                                             (uint32_t)(r / rpc));
+            st_cluster_f2(dst, make_float2(hp[half][2 * rs], hp[half][2 * rs + 1]));
+            if (q < 2) st_cluster_f2(dst + 32, make_float2(hp[half][4 + 2 * rs], hp[half][5 + 2 * rs]));
         }
-        if ((lane & 3) == 0) {
-#pragma unroll
-            for (int rs = 0; rs < 2; ++rs) {
-                const int r = rb + 8 * rs;
-                const uint32_t dst =
-                    mapa_shared(part + (uint32_t)(((p0 + half) * rpc + r % rpc) * kHeadPartPad * 4), (uint32_t)(r / rpc));
-                st_cluster_f4(dst, make_float4(hp[rs][0], hp[rs][1], hp[rs][2], hp[rs][3]));
-                st_cluster_f4(dst + 16, make_float4(hp[rs][4], hp[rs][5], hp[rs][6], hp[rs][7]));
-                st_cluster_f4(dst + 32, make_float4(hp[rs][8], 0.f, 0.f, 0.f));
-            }
-        }
-    }
 }
 
 template <int ACT, bool F16>
@@ -448,7 +421,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
     float* s_part = reinterpret_cast<float*>(smem + S::OFF_PART);
     float* s_b1 = reinterpret_cast<float*>(smem + S::OFF_B1);
     float* s_b2 = reinterpret_cast<float*>(smem + S::OFF_B2);
-    float* s_hw = reinterpret_cast<float*>(smem + S::OFF_HW);           // [RF_HEAD_AP][256]: Wv, then the rows of Wa
+    uint8_t* s_hw = smem + S::OFF_HW;                                   // [Wv; Wa] operand of the head partials
     float* s_hb = reinterpret_cast<float*>(smem + S::OFF_HB);           // bv, then ba
 
     // episode statistics of finished episodes: accumulated per CTA over the WHOLE rollout in shared memory, five global
@@ -492,9 +465,9 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
         for (int i = threadIdx.x; i < BN; i += RF_THREADS) {
             s_b1[i] = a.b1[n0 + i];
             s_b2[i] = a.b2[n0 + i];
-            s_hw[i] = a.wv[n0 + i];
-            for (int r = 0; r < a.A; ++r) s_hw[(r + 1) * 256 + i] = a.wa[(int64_t)r * a.H2 + n0 + i];
         }
+        fill_head_weights_f16(s_hw, a.wv, a.wa, a.A, a.H2, n0, BN, threadIdx.x, RF_THREADS);
+        fence_proxy_async_smem();   // -> the head partials' wgmmas
         if (threadIdx.x <= a.A) s_hb[threadIdx.x] = threadIdx.x == 0 ? a.bv[0] : a.ba[threadIdx.x - 1];
     }
     __syncthreads();
@@ -563,7 +536,7 @@ rollout_mlp2_tape_kernel(const __grid_constant__ CUtensorMap tmap_x, const __gri
                 float acc[64], cross[64];
                 rf_tile<F16, !F16>(a.H1 / KBK, wide, smem, full, empty, cu, acc, cross, ct, shift_h, tr, 11, 14, 12, 16);
                 if (F16)
-                    rf_heads_tile<ACT>(acc, tc.n0 - n0, tc.n0 / 64, (int)(row_base - m0), lane, s_b2, s_hw, a.A,
+                    rf_heads_tile<ACT>(acc, tc.n0 - n0, tc.n0 / 64, (int)(row_base - m0), lane, s_b2, smem_u32(s_hw),
                                        smem_u32(s_part), BM / CX);
                 else
                     heads_tile<ACT>(acc, tc, row_base, lane, nullptr, 0, a.N, a.H2, epi_heads);

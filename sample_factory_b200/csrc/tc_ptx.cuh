@@ -159,9 +159,10 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t de
 
 // The same shape with the fp16 A operand in registers: a[4] is the thread's m64k16 fragment (warp w of the warpgroup
 // holds rows 16w .. 16w+15 in the mma.m16n8k16 A layout, F16Frags in wgmma_tile.cuh), B from shared memory, K-major
-// (TRANS_B = 0) or MN-major (TRANS_B = 1).
+// (TRANS_B = 0) or MN-major (TRANS_B = 1).  scale_d = 0 overwrites D.
 template <int TRANS_B>
-__device__ __forceinline__ void wgmma_m64n128k16_f16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b) {
+__device__ __forceinline__ void wgmma_m64n128k16_f16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b,
+                                                        uint32_t scale_d = 1) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
@@ -178,7 +179,23 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16_rs(float (&d)[64], const ui
           "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]),
           "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),
           "+f"(d[63])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "n"(TRANS_B), "r"(1u));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "n"(TRANS_B), "r"(scale_d));
+}
+
+// m64n64k16 with the fp16 A operand in registers (as above) and B MN-major (transpose bit set); scale_d = 0 overwrites D.
+// Accumulator fragment: d[i] at row 16*(t/32) + (t%32)/4 + 8*((i/2)%2), column 8*(i/4) + 2*(t%4) + i%2.
+__device__ __forceinline__ void wgmma_m64n64k16_f16_rs_mn(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b,
+                                                          uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
 
 // ------------------------------------------------------------------------------------------------ descriptors
@@ -194,11 +211,12 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     return d;
 }
 // MN-major 16-bit tile with the 128B swizzle (split_tile_f16_mn): 1024 B atoms of [8 k][64 rows]; LBO = 4096 (next 64
-// rows), SBO = 1024 (next 8 k).  A k-step of 16 advances the start address by two atoms.
-__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
+// rows), SBO = 1024 (next 8 k).  A k-step of 16 advances the start address by two atoms.  (lbo = 0: rows 64 .. 127 read
+// the atoms of rows 0 .. 63 again -- head_partials_f16, whose B has 64 rows.)
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr, uint32_t lbo = 4096) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)(4096u >> 4) << 16;
+    d |= (uint64_t)(lbo >> 4) << 16;
     d |= (uint64_t)(1024u >> 4) << 32;
     d |= (uint64_t)1 << 62;
     return d;

@@ -31,6 +31,8 @@ struct TcEpilogue {
 constexpr int kHeadAP = 9;     // value + up to 8 action outputs
 constexpr int kHeadPad = 12;   // floats per (partial, row): three 16 B stores
 constexpr int TC_THREADS = 384;
+// fp16 form of the head partials: the B operand for 128 columns of [Wv; Wa] (fill_head_weights_f16)
+constexpr int kHeadTileBytes = 8192;
 
 // Shared memory of gemm_wgmma_kernel: a ring of A_STAGES TMA slots for the raw A tile, a ring of B_STAGES slots for the B
 // tile, CONV_BUFS conversion buffers (the split of stage kb+1 is written into one while the wgmmas of earlier stages read
@@ -41,15 +43,19 @@ constexpr int TC_THREADS = 384;
 //              hold their fragments in registers); B = the weight tile's fp16 [hi | lo] twins, TMA-loaded in the swizzled
 //              layout wgmma reads (32 KB, released once its wgmmas completed); no conversion buffer: 3 A + 4 B slots,
 //              224 KB.  Four B slots: a warpgroup holds two (the stages in flight) while the producer fills the others.
+//              With the heads folded in (HEADS): 2 A slots (an A slot is free once both halves are in registers) and
+//              the [Wv; Wa] operand of the head partials (fill_head_weights_f16, N <= 512 columns: 32 KB), written once
+//              per CTA: 224 KB.  (3 A + 3 B slots gave outputs that changed from launch to launch in rows of later items
+//              even without the partials' wgmmas; the cause was not found, so the B ring keeps its four slots.)
 //   fp16 dW form (DW16, gemm_dw_f16_kernel): raw MN-major A fp32 tile of 32 k as four 128B-swizzled [32 k][32 rows]
 //              boxes (16 KB, released once in registers), raw MN-major B tile as in the tf32 form (16 KB, released once
 //              split); three conversion buffers [B hi | B lo], each [32 k][128 rows] fp16 MN-major (8 KB): with two
 //              stages of wgmmas in flight per warpgroup and the warpgroups up to a stage apart, three are read or
 //              written at once.  4 A + 4 B slots: 176 KB.
-template <bool F16, bool DW16 = false>
+template <bool F16, bool DW16 = false, bool HEADS = false>
 struct TcSmem {
     static constexpr int KBK = F16 ? 64 : TBK;                    // k per stage
-    static constexpr int A_STAGES = F16 ? 3 : DW16 ? 4 : 3;
+    static constexpr int A_STAGES = (F16 && HEADS) ? 2 : F16 ? 3 : DW16 ? 4 : 3;
     static constexpr int B_STAGES = (F16 || DW16) ? 4 : 3;
     static constexpr int A_RAW = TBM * KBK * 4;
     static constexpr int B_SLOT = F16 ? 2 * TBN * 64 * 2 : TBN * TBK * 4;
@@ -61,7 +67,8 @@ struct TcSmem {
     static constexpr int CONV_BUFS = F16 ? 0 : DW16 ? 3 : 2;
     static constexpr int B_RING = A_STAGES * A_RAW;               // offsets from the 1024-aligned base
     static constexpr int CONV_OFF = B_RING + B_STAGES * B_SLOT;
-    static constexpr int BARS_OFF = CONV_OFF + CONV_BUFS * CONV;
+    static constexpr int HW_OFF = CONV_OFF + CONV_BUFS * CONV;   // fp16 form with heads: fill_head_weights_f16's layout
+    static constexpr int BARS_OFF = HW_OFF + ((F16 && HEADS) ? (512 / TBN) * kHeadTileBytes : 0);
     static constexpr int BARS = 2 * (A_STAGES + B_STAGES) * 8 + 16;
     static constexpr int TOTAL = 1024 /*align slack*/ + BARS_OFF + BARS;
     static_assert(TOTAL <= 227 * 1024, "shared memory");
@@ -353,11 +360,10 @@ __device__ __forceinline__ void store_tile_residual(const float (&acc)[64], cons
 // eight float2 of the weight row that both of the thread's rows (rs = 0, 1) multiply.  Each partial keeps its order of
 // operations: FMAs over jj = 0..7, then the quad sum over lanes ^ 1, ^ 2.
 // tr: the traced thread's stamps (11: bias landed, 12: y stored, 13: partials stored), else NULL.
+// y = act(acc + bias) in place, stored into C (when not NULL) -- the first half of both heads epilogues
 template <int ACT>
-__device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
-                                           int64_t ldc, int64_t M, int N, const TcEpilogue& epi,
-                                           unsigned long long* tr = nullptr) {
-    constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
+__device__ __forceinline__ void heads_act_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
+                                               int64_t ldc, int64_t M, const TcEpilogue& epi, unsigned long long* tr) {
     const int nq = tc.n0 + 2 * (lane & 3);
     float b[32];
     load_bias_pairs(epi.bias, tc.n0, lane, b);
@@ -370,6 +376,15 @@ __device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc
         if (C && m < M) *reinterpret_cast<float2*>(C + m * ldc + nq + 8 * (j >> 1)) = make_float2(acc[2 * j], acc[2 * j + 1]);
     }
     if (tr) tr[12] = tc_now_after(acc[63]);
+}
+
+template <int ACT>
+__device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
+                                           int64_t ldc, int64_t M, int N, const TcEpilogue& epi,
+                                           unsigned long long* tr = nullptr) {
+    constexpr int JP = 16;   // accumulator pairs of a thread per partial (per 64 columns)
+    const int nq = tc.n0 + 2 * (lane & 3);
+    heads_act_tile<ACT>(acc, tc, row_base, lane, C, ldc, M, epi, tr);
     const int p0 = (tc.n0 / TBN) * 2;
 #pragma unroll
     for (int half = 0; half < 2; ++half) {
@@ -410,6 +425,132 @@ __device__ __forceinline__ void heads_tile(float (&acc)[64], const TileCoord& tc
             }
         }
     }
+    if (tr) tr[13] = tc_now();
+}
+
+// ---- the head partials on the tensor cores (fp16 form) -------------------------------------------------------------
+// The B operand of head_partials_f16 for columns [n_begin, n_begin + cols) of [Wv; Wa] (Wa's rows ld_wa floats apart),
+// split as the weights' fp16 twins hold them (f16_split1 of w * 2^kF16WShift: the same bits).  Per 128-column tile
+// (kHeadTileBytes at dst + (column / 128) * kHeadTileBytes) and k16 step kk (the tile's columns 64 h + 16 kk .. + 15 of
+// both halves h): two MN-major 128B-swizzled atoms [8 k][64 n] (k = 0..7, then 8..15; the layout of split_tile_f16_mn)
+// whose 64 n are, for half h, 32 h + a = hi and 32 h + 16 + a = lo of output row a (a = 0 .. 15, rows A+1 .. 15 zero).
+// Threads t = 0 .. nthreads-1 of the caller share the work, a column each, its (up to kHeadAP) loads issued together; it
+// is followed by fence_proxy_async_smem and a barrier before the first wgmma reads it.  cols: a multiple of 128.
+__device__ __forceinline__ void fill_head_weights_f16(uint8_t* dst, const float* wv, const float* wa, int A, int64_t ld_wa,
+                                                      int n_begin, int cols, int t, int nthreads) {
+    for (int n = t; n < cols; n += nthreads) {
+        float w[16];
+#pragma unroll
+        for (int a = 0; a < 16; ++a)
+            w[a] = a == 0 ? wv[n_begin + n] : (a < kHeadAP && a <= A) ? wa[(int64_t)(a - 1) * ld_wa + n_begin + n] : 0.f;
+        const int h = (n >> 6) & 1, kr = n & 7;   // half; k row inside the atom
+        uint8_t* row = dst + (n >> 7) * kHeadTileBytes + ((n >> 4) & 3) * 2048 + ((n >> 3) & 1) * 1024 + kr * 128;
+#pragma unroll
+        for (int a = 0; a < 16; ++a) {
+            uint16_t hi, lo;
+            f16_split1(w[a] * (float)(1 << kF16WShift), hi, lo);
+            const int nh = 32 * h + a, nl = nh + 16;
+            *reinterpret_cast<uint16_t*>(row + ((((nh >> 3) ^ kr) & 7) << 4) + (nh & 7) * 2) = hi;
+            *reinterpret_cast<uint16_t*>(row + ((((nl >> 3) ^ kr) & 7) << 4) + (nl & 7) * 2) = lo;
+        }
+    }
+}
+
+// The two head partials of a warpgroup's 64 x 128 tile of activated values y (a thread's 64 accumulator values, in the
+// wgmma layout) in the 3-pass fp16 form: y * 2^s split into hi + lo * 2^-11 in registers -- the accumulator pairs of two
+// adjacent n8 blocks are the register-A fragment of one k16 step -- times the [Wv; Wa] hi / lo operand at hw
+// (fill_head_weights_f16, the tile's 8 KB), ((main + c1 * 2^-11) + c2 * 2^-11) * 2^-(s + kF16WShift) with main = y_hi . w_hi,
+// c1 = y_hi . w_lo, c2 = y_lo . w_hi.  s is chosen per row and half from the row's own max |y| over the 64 columns
+// (f16_shift_for_bound), so no bound has to be known and the bits of a row's partial depend on its 64 values and the
+// weights only, whatever the tile shape around them.  Columns A+1 .. 15 come out 0.
+// The MMAs are register-A wgmmas with B MN-major over the 64 rows of the operand: N = 128 is the GEMM engine's m64n128k16
+// (LBO 0: columns 64 .. 127 repeat 0 .. 63 and are not read), N = 64 the m64n64k16 of the persistent rollout, whose
+// larger live state across the step loop leaves no room for a 64-register accumulator; columns 0 .. 63 come out the
+// same either way.  Per half, four k16 steps of y_hi give main in columns 32 h + 0..15 and y_hi . w_lo in 32 h + 16..31, then
+// four of y_lo, from a fresh accumulator, give y_lo . w_hi in 32 h + 0..15.  Every pass writes junk into the other
+// columns (the other half's weights), so the four passes run one after the other through one accumulator.
+// hp[half][i]: row + 8 * ((i / 2) % 2), column 8 * (i / 4) + 2 * (lane % 4) + i % 2.  Every thread of the warpgroup calls it (wgmma is warpgroup-wide).
+template <int N>
+__device__ __forceinline__ void head_partials_f16(const float (&y)[64], uint32_t hw, float (&hp)[2][8]) {
+    static_assert(N == 64 || N == 128, "m64n64k16 or m64n128k16");
+    int shift[2][2];   // per half and row (rs: row + 8 rs)
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+            float mx = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+                const int i = 32 * h + 4 * jj + 2 * rs;
+                mx = fmaxf(mx, fmaxf(fabsf(y[i]), fabsf(y[i + 1])));
+            }
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));   // the quad holds the row's 64 columns
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            shift[h][rs] = f16_shift_for_bound(mx);
+        }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        F16Frags<4> f;   // the half's k16 steps (split here: the other half stays 32 values of y meanwhile)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int i = 32 * h + 8 * kk + 2 * j;
+                const float sc = pow2f_int(shift[h][j & 1]);
+                f16_split2(y[i] * sc, y[i + 1] * sc, f.hi[kk][j], f.lo[kk][j]);
+            }
+        // Nothing may write a register the asynchronous wgmmas below read or accumulate into while they run: the
+        // fragments are pinned complete before the fence (register arithmetic is not ordered by its memory clobber), and
+        // the accumulator is not zero-filled but overwritten by the first wgmma of each pass (scale-d 0) -- a zero-fill the
+        // compiler placed among the wgmmas corrupted whole rows of partials.
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(f.hi[k][j]), "+r"(f.lo[k][j]));
+        float d[N / 2];
+        float (&part)[8] = hp[h];   // main + (y_hi . w_lo) * 2^-11, then + (y_lo . w_hi) * 2^-11, then scaled
+#pragma unroll
+        for (int pass = 0; pass < 2; ++pass) {
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                const uint64_t db = make_smem_desc_mn(hw + kk * 2048, 0);
+                if constexpr (N == 128) wgmma_m64n128k16_f16_rs<1>(d, pass ? f.lo[kk] : f.hi[kk], db, kk != 0);
+                else wgmma_m64n64k16_f16_rs_mn(d, pass ? f.lo[kk] : f.hi[kk], db, kk != 0);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                if (pass == 0) part[i] = fmaf(d[16 * h + 8 + i], 1.f / 2048.f, d[16 * h + i]);
+                else part[i] = __fmul_rn(fmaf(d[16 * h + i], 1.f / 2048.f, part[i]),
+                                         pow2f_int(-(shift[h][(i >> 1) & 1] + kF16WShift)));
+            }
+        }
+    }
+}
+
+// heads_tile of the fp16 form: y as there, the partials from head_partials_f16 (hw: the [Wv; Wa] operand of the whole
+// layer, fill_head_weights_f16 from column 0).  A thread writes its columns of the kHeadPad row: 2q, 2q+1 and, for q < 2,
+// 8 + 2q, 9 + 2q (q = lane % 4).
+template <int ACT>
+__device__ __forceinline__ void heads_tile_f16(float (&acc)[64], const TileCoord& tc, int64_t row_base, int lane, float* C,
+                                               int64_t ldc, int64_t M, const TcEpilogue& epi, uint32_t hw,
+                                               unsigned long long* tr) {
+    heads_act_tile<ACT>(acc, tc, row_base, lane, C, ldc, M, epi, tr);
+    const int p0 = (tc.n0 / TBN) * 2, q = lane & 3;
+    float hp[2][8];
+    head_partials_f16<128>(acc, hw + (uint32_t)(tc.n0 / TBN) * kHeadTileBytes, hp);
+#pragma unroll
+    for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int rs = 0; rs < 2; ++rs) {
+            const int64_t m = row_base + 8 * rs;
+            if (m >= M) continue;
+            float* dst = epi.head_part + ((int64_t)(p0 + half) * M + m) * kHeadPad + 2 * q;
+            *reinterpret_cast<float2*>(dst) = make_float2(hp[half][2 * rs], hp[half][2 * rs + 1]);
+            if (q < 2) *reinterpret_cast<float2*>(dst + 8) = make_float2(hp[half][4 + 2 * rs], hp[half][5 + 2 * rs]);
+        }
     if (tr) tr[13] = tc_now();
 }
 
