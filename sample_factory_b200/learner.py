@@ -139,11 +139,6 @@ class Learner:
         # device, and ONE gather pass per train() rearranges every per-sample array the minibatch steps read; the steps then
         # run on contiguous slices exactly as in the unshuffled case.
         self.shuffle = bool(cfg.shuffle_minibatches) and cfg.num_batches_per_epoch > 1
-        assert len(spec.hidden) > 0 or spec.use_rnn or (spec.dict_obs and spec.encoder_mlp_layers), (
-            "the device path needs at least one hidden layer or an RNN core")
-        assert spec.obs_shape is None or len(spec.fc_encoder_layers) > 0, (
-            "ConvEncoder on the device path needs at least one fully connected layer after the conv head "
-            "(encoder_conv_mlp_layers, reference default [512])")
         if spec.use_rnn:
             assert cfg.rollout % cfg.recurrence == 0, "rollout must be a multiple of recurrence (learner.py:500)"
             assert cfg.batch_size % cfg.recurrence == 0
@@ -208,7 +203,7 @@ class Learner:
         # every epoch.  (V-trace advantages depend on the current policy: they keep the per-step path.)
         self.mb_partials = torch.zeros((cfg.num_batches_per_epoch, 3), dtype=torch.float64, device=dev)
         self.loss_ws = torch.empty(ops.loss_workspace_bytes(max(B, E)) // 8 + 8, dtype=torch.float64, device=dev)
-        tail_w = spec.tail_input_size * (1 if spec.share_weights else 2)     # separate weights: [actor tail | critic tail]
+        tail_w = spec.tail_input_size * (2 if spec.separate_towers else 1)     # separate weights: [actor tail | critic tail]
         lin_ws = 4
         if spec.wide_heads:
             # heads wider than 31 rows: linear_backward for dWa / dz, sfb200_heads_wide_backward for the rest
@@ -257,6 +252,9 @@ class Learner:
         self.heads_plan = HeadsPlan(model, engine, max(B, self.N), need_backward=True)
         # image observations: gradient w.r.t. the conv head's output (pre-activation of its last layer, (C,H,W) order)
         self.dfeat = torch.empty((B, spec.conv_out_size), **f32) if spec.obs_shape is not None else None
+        # linear policy: the heads backward writes the gradient w.r.t. the normalised observation rows here; nothing reads it
+        # (the [B, obs_dim] store is as wide as the rows the kernel reads anyway)
+        self.dobs = torch.empty((B, D), **f32) if spec.heads_read_input else None
         self.adam_ws = torch.empty(1024, **f32)
         assert cfg.optimizer in ("adam", "lamb"), f"Unknown optimizer {cfg.optimizer}"    # learner.py:228-230
         if cfg.optimizer == "lamb":
@@ -611,16 +609,20 @@ class Learner:
             x_enc, act_enc, d_enc, db_enc = plan.enc_cat[:B], self.act, plan.denc_cat[:B], plan.db_enc_cat
         elif Le > 0:
             x_enc, act_enc, d_enc, db_enc = self.h[Le - 1], self.act, self.dz[Le - 1], genc[-1][1]
+        elif plan.conv is not None:      # conv head without fully connected layers: its activated features, bias in the head
+            x_enc, act_enc, d_enc, db_enc = plan.conv.feat[:B], self.act, self.dfeat, None
         else:
             x_enc, act_enc, d_enc, db_enc = x0, none, None, None
-        tail_is_mlp = Ld > 0 or not rnn            # is the tensor feeding the heads an activated MLP output?
+        tail_is_mlp = Ld > 0 or not rnn            # is the tensor feeding the heads the decoder's or the encoder's output?
         tail_dz = (self.dz[Le + Ld - 1] if Ld > 0 else d_enc) if tail_is_mlp else self.d_core
+        if tail_dz is None:                        # linear policy: the input gradient goes to a scratch nobody reads
+            tail_dz = self.dobs
         tail_db = gdec[-1][1] if Ld > 0 else (None if rnn else db_enc)
         if self.dz_bound is not None and tail_is_mlp:
             L = len(spec.hidden)
             ops.heads_dz_bound(self.dlogits, self.dvalues, Wv, Wa, self.dz_bound[4 * (L - 1):], m.grad_fac, self.dz_bound,
                                L - 1)
-        tail_act = self.act if tail_is_mlp else none
+        tail_act = (self.act if Ld > 0 else act_enc) if tail_is_mlp else none
         if spec.wide_heads:
             # dWa = dlogits^T . x and tail_dz = (dlogits . Wa) * act'(x) on the GEMM engine, then the value term, the bias /
             # value gradients and db_prev (the bound above covers the sum: the formula holds for any number of rows)
@@ -650,6 +652,8 @@ class Learner:
             ops.linear_backward(dgi_all, x_enc, W_ih, act_enc, dW_ih, d_enc, db_enc, self.engine, self.lin_ws)
         if plan.keys:
             self._backward_keys(x0)
+        if Le == 0 and plan.conv is not None:
+            plan.conv.backward(self.dfeat)
         for li in range(Le - 1, -1, -1):
             W, dW = enc[li][0], genc[li][0]
             if li > 0:

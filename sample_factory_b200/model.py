@@ -56,7 +56,8 @@ class ModelSpec:
     # False -> ActorCriticSeparateWeights (model/actor_critic.py:198-322): an actor tower (encoder MLP -> recurrent core
     # if use_rnn -> decoder MLP) feeding distribution_linear and a critic tower feeding critic_linear.  Each tower's core
     # owns one half of a state row, [actor state | critic state], each half laid out like a shared model's row.  Vector
-    # observations of one key only (conv / ResNet encoders and Dict observations raise ValueError)
+    # observations of one key only (conv / ResNet encoders and Dict observations raise ValueError).  Towers with no layer
+    # and no core run as the shared identity model (separate_towers)
     share_weights: bool = True
     # Dict observations of 1-D keys (MultiInputEncoder, model/encoder.py:33-70): [(key, d), ...] in sorted key order.  The
     # keys lie side by side in one packed row, key k in columns [c_k, c_k + d_k); every key has its own MlpEncoder with
@@ -222,14 +223,32 @@ class ModelSpec:
         return 2 * self.num_actions if self.adaptive_stddev else self.num_actions
 
     NARROW_HEADS_MAX = 31      # rows the warp-per-row heads kernels hold (lane 0 = value, lanes 1..A = logits)
+    NARROW_HEADS_SMEM = 200 * 1024     # bytes of [critic_linear | distribution_linear] the narrow heads forward stages
     MAX_LINEAR_ACTION_OUTPUTS = 1024
     MAX_TUPLE_HEADS = 8
 
     @property
     def wide_heads(self) -> bool:
-        """distribution_linear has more than 31 rows: the heads run as a GEMM on the regular engine plus
+        """distribution_linear has more than 31 rows, or its rows and critic_linear's do not fit the narrow heads forward's
+        shared memory (heads reading conv features thousands wide): the heads run as a GEMM on the regular engine plus
         sfb200_heads_tail_wide instead of the fused warp-per-row heads kernels"""
-        return self.num_linear_action_outputs > self.NARROW_HEADS_MAX
+        A = self.num_linear_action_outputs
+        width = self.tail_input_size * (2 if self.separate_towers else 1)     # what the narrow kernels read per row
+        return A > self.NARROW_HEADS_MAX or (A + 1) * width * 4 > self.NARROW_HEADS_SMEM
+
+    @property
+    def separate_towers(self) -> bool:
+        """separate actor / critic weights whose towers hold an MLP layer or a core.  Towers that are identities own no
+        parameters (ActorCriticSeparateWeights then has only the heads, actor_critic.py:198-322): such a model runs as
+        the shared-weights identity model and differs from it only in the width of its state rows"""
+        return not self.share_weights and (bool(self.hidden) or self.use_rnn)
+
+    @property
+    def heads_read_input(self) -> bool:
+        """a linear policy: no MLP layer and no core, the heads read the normalised observation rows (the concatenated
+        key rows of a Dict model with identity key encoders)"""
+        return not self.hidden and not self.use_rnn and self.obs_shape is None and not (
+            self.dict_obs and self.encoder_mlp_layers)
 
     def __post_init__(self) -> None:
         if self.use_rnn and self.rnn_num_layers < 1:
@@ -638,7 +657,7 @@ class PolicyModel:
     def refresh_cat_heads(self) -> None:
         """separate weights: the heads kernels read ONE tail [M, 2H] = [actor tail | critic tail]; critic_linear and
         distribution_linear are embedded in zero-padded [., 2H] matrices (value <- critic half, logits <- actor half)."""
-        if self.spec.share_weights:
+        if not self.spec.separate_towers:
             return
         H = self.spec.tail_input_size
         if not hasattr(self, "Wv_cat"):

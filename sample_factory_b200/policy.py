@@ -11,7 +11,11 @@ Dict observations with several keys (MultiInputEncoder) start with a key encoder
 slice of the normalised rows and its last layer writes its block of one concatenated buffer, which then feeds the
 recurrent core, the decoder MLP or (unfused) the heads like the output of a single encoder would.
 
-Models whose distribution_linear has more than 31 rows (ModelSpec.wide_heads) store the last hidden layer, run
+Encoders without fully connected layers hand their input on unchanged: the heads (or the decoder / core) read the
+normalised rows of a linear policy, or the conv head's features, through the unfused heads kernels.
+
+Models whose distribution_linear has more than 31 rows, or whose rows do not fit the narrow heads forward's shared memory
+(ModelSpec.wide_heads), store the last hidden layer, run
 distribution_linear as a GEMM on the same engine straight into the logits' final place, and finish with
 sfb200_heads_tail_wide (value head + distribution tail, one warp per row).
 """
@@ -62,11 +66,10 @@ class HeadsPlan:
         # tower_h[tw][i] / tower_dz[tw][i]: output of the tower's MLP layer i (encoder then decoder) and its gradient; the
         # layer that feeds the heads writes its half of tail_cat instead (None here).  With a recurrent core and no decoder
         # the core's output feeds the heads: every MLP layer keeps its buffer and the core output is copied into tail_cat.
-        self.separate = not spec.share_weights
+        self.separate = spec.separate_towers
         if self.separate:
             f32 = dict(dtype=torch.float32, device=model.device)
             widths, H = spec.hidden, spec.tail_input_size
-            assert len(widths) > 0 or spec.use_rnn, "separate actor / critic weights need an MLP layer or a core per tower"
             self.tower_tail_is_mlp = bool(spec.decoder_mlp_layers) or not spec.use_rnn
             n_tail = 1 if self.tower_tail_is_mlp else 0
 
