@@ -420,6 +420,34 @@ int sfb200_tape_env_step_continuous(const float* actions_f32, int act_dim, int64
                                     const float* tape, int64_t tape_len, int dim, float* obs_out, float* rew,
                                     uint8_t* terminated, uint8_t* truncated, void* stream);
 
+/* Batched tensor envs (IsaacGym / Brax style: one env with num_agents = N whose reset() / step() return tensors batched
+ * along dim 0, in their own dtypes; algo/utils/make_env.py:172-237 hands them through unchanged, inference_worker.py:324-331
+ * pops the "action_mask" key): ONE launch converts every tensor of a step into the sampler's static buffers.
+ * desc_host: n_desc (<= SFB200_INGEST_MAX) entries of SFB200_INGEST_FIELDS int64 each, in HOST memory:
+ *   {src, src_dtype, src_row_stride, cols, dst, dst_row_stride, dst_kind}
+ * entry k: dst[r * dst_row_stride + c] = convert(src[r * src_row_stride + c]) for r < rows, c < cols (element strides of the
+ * source / destination type; src and dst are device addresses, dst already at the entry's first column; each row's cols
+ * elements are dense).  src_dtype: SFB200_DT_*.  dst_kind:
+ *   SFB200_INGEST_F32   float32, bit-equal to torch's .to(torch.float32) (round to nearest even)
+ *   SFB200_INGEST_U8    uint8 copy (uint8 sources only: image observations)
+ *   SFB200_INGEST_BOOL  bool (1 byte) = (x != 0) evaluated in the source type */
+#define SFB200_DT_F32 0
+#define SFB200_DT_F16 1
+#define SFB200_DT_BF16 2
+#define SFB200_DT_F64 3
+#define SFB200_DT_I8 4
+#define SFB200_DT_I16 5
+#define SFB200_DT_I32 6
+#define SFB200_DT_I64 7
+#define SFB200_DT_U8 8
+#define SFB200_DT_BOOL 9
+#define SFB200_INGEST_F32 0
+#define SFB200_INGEST_U8 1
+#define SFB200_INGEST_BOOL 2
+#define SFB200_INGEST_FIELDS 7
+#define SFB200_INGEST_MAX 16
+int sfb200_env_ingest(const int64_t* desc_host, int n_desc, int64_t rows, void* stream);
+
 /* ------------------------------------------------------------- learner: batch prep ---- */
 /* learner.py:950-955: valids[:, :T] = (policy_id == this_policy) & (train_step - policy_version < max_lag);
  * valids[:, T] = valids[:, T-1]. */

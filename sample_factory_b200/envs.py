@@ -1,5 +1,8 @@
-"""Environment boundary: registry (reference envs/env_utils.py:12-31, envs/create_env.py:13-46) and the batched
-GPU-env contract the device sampler drives (what the reference's BatchedVecEnv guarantees, make_env.py:147-237):
+"""Environment boundary: registry (reference envs/env_utils.py:12-31, envs/create_env.py:13-46) and the two env contracts
+the engine accepts.
+
+1. The engine's batched GPU-env contract, which the device sampler drives directly (what the reference's BatchedVecEnv
+   guarantees, make_env.py:147-237):
 
     env.num_agents : int
     env.obs_dim / env.num_actions
@@ -12,6 +15,12 @@ GPU-env contract the device sampler drives (what the reference's BatchedVecEnv g
     env.obs_keys (optional): a Dict observation of 1-D keys, [(key, d), ...] in sorted key order.  Each obs row is then the
         keys laid side by side as float32 (key k in columns [c_k, c_k + d_k), obs_dim = sum(d)), and the model builds one
         encoder per key (MultiInputEncoder).  An "action_mask" key is not part of the row.
+
+2. The reference's gymnasium-API contracts, adapted by host_env.create_batched_env: a plain (single- or multi-agent) env
+   is wrapped into host_env.BatchedHostEnv; a batched tensor env (IsaacGym / Brax style: one env with num_agents = N,
+   reset() -> (obs, info), step(actions) -> (obs, rew, terminated, truncated, infos), torch tensors batched along dim 0 on
+   the GPU or the CPU, obs a tensor or a dict of tensors described by observation_space) into
+   host_env.BatchedTensorEnvAdapter, which converts each step's tensors into static buffers with one kernel.
 
 `TapeVecEnv` is the synthetic env of BASELINE.json config 2 (Box(64) obs, Discrete(8)): GPU-resident, one CUDA kernel
 per step, buffers reused across steps so a whole rollout can be captured in a CUDA graph.  `HostTapeVecEnv` is the

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -779,6 +780,29 @@ def tape_env_step_continuous(actions_f32: Tensor, env_index_offset: int, term_pe
     lib().call("sfb200_tape_env_step_continuous", _p(actions_f32, F32), act_dim, n, env_index_offset, term_period,
                trunc_period, _p(step_counter, I64), step_host, _p(tape, F32), tape_len, dim, _p(obs_out, F32),
                _p(rew, F32), _p(terminated, U8), _p(truncated, U8), _stream())
+
+
+INGEST_DTYPES = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2, torch.float64: 3, torch.int8: 4, torch.int16: 5,
+                 torch.int32: 6, torch.int64: 7, torch.uint8: 8, torch.bool: 9}
+INGEST_F32, INGEST_U8, INGEST_BOOL = 0, 1, 2
+INGEST_MAX = 16
+
+
+def env_ingest(entries, rows: int) -> None:
+    """One launch over entries (src, src_row_stride, cols, dst, dst_col, kind): dst[r, dst_col + c] = convert(src row r's
+    element c) for r < rows, c < cols.  src: CUDA tensor of any INGEST_DTYPES dtype whose rows hold cols dense elements
+    (src_row_stride in elements); dst: a 2-D float32 (INGEST_F32) or uint8 / bool (INGEST_U8 / INGEST_BOOL) CUDA tensor
+    with dense rows."""
+    assert 0 < len(entries) <= INGEST_MAX
+    desc = np.empty((len(entries), 7), dtype=np.int64)
+    for k, (src, src_stride, cols, dst, dst_col, kind) in enumerate(entries):
+        if not (src.is_cuda and dst.is_cuda):
+            raise RuntimeError("sample_factory_b200 ops need CUDA tensors (there is no CPU path)")
+        assert dst.dim() == 2 and dst.stride(1) == 1 and dst_col + cols <= dst.shape[1] and dst.shape[0] >= rows
+        assert dst.dtype == (F32 if kind == INGEST_F32 else BYTE if kind == INGEST_U8 else U8)
+        desc[k] = (src.data_ptr(), INGEST_DTYPES[src.dtype], src_stride, cols,
+                   dst.data_ptr() + dst_col * dst.element_size(), dst.stride(0), kind)
+    lib().call("sfb200_env_ingest", desc.ctypes.data, len(entries), rows, _stream())
 
 
 # ------------------------------------------------------------------------------------------------ learner: prep
