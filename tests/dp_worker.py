@@ -24,7 +24,7 @@ from sample_factory_b200.dist_utils import init_from_env  # noqa: E402
 from sample_factory_b200.learner import Learner  # noqa: E402
 from sample_factory_b200.model import ModelSpec, PolicyModel  # noqa: E402
 from sample_factory_b200.trajectory import alloc_trajectory_tensors  # noqa: E402
-from tests.test_gpu_engine import make_cfg  # noqa: E402
+from tests.device_harness import make_cfg  # noqa: E402
 
 N, T, NMB = 512, 16, 4
 SUMMED = ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "kl_old_mean", "entropy_mean", "value_mean",

@@ -49,6 +49,17 @@ def load_case(name):
     return z, meta, cfg
 
 
+def load_mixed_case(name):
+    """a fixture of tests/golden/make_golden_mixed.py -> (npz, meta, MixedCfg)"""
+    import dataclasses
+
+    from tests import mixed_oracle as MO
+
+    z, meta, cfg = load_case(name)
+    MO.install()
+    return z, meta, MO.MixedCfg(**dataclasses.asdict(cfg), action_heads=[tuple(h) for h in meta["action_heads"]])
+
+
 def state_from(z, prefix):
     """prefix 'init/' or 'it0/state/' -> dict of torch tensors keyed by reference state_dict names."""
     st = {k[len(prefix):]: torch.from_numpy(z[k].copy()) for k in z.files if k.startswith(prefix)}

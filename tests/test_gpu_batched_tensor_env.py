@@ -10,19 +10,11 @@ import torch
 
 from gymnasium import spaces
 from oracle import appo_oracle as O
-from tests import test_gpu_engine as E
-from tests.golden_utils import load_case, state_from
+from tests import dict_obs_oracle as DO
+from tests.device_harness import DEV, TOL, build, build_case, make_cfg, ops_for
+from tests.golden_utils import load_case, load_mixed_case, state_from
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-TOL = 1e-5
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    ops.bind_device(DEV)
-    return ops
 
 
 # ------------------------------------------------------------------------------------------------ kernel
@@ -60,7 +52,7 @@ DTYPES = [torch.float32, torch.float16, torch.bfloat16, torch.float64, torch.int
 def test_ingest_matches_torch_conversions(dtype, n):
     """keys of 3 / 5 / 1 / 9 / 16 columns at odd column offsets, with dense, strided (padded or misaligned) and 3-D rows;
     a dense reward-like vector; a bool x != 0 mask -- bit-equal to .to(torch.float32) and != 0"""
-    ops = _ops()
+    ops = ops_for()
     gen = torch.Generator().manual_seed(n * 31 + DTYPES.index(dtype))
     keys = []
     for i, cols in enumerate([3, 5, 1, 9, 16]):
@@ -185,22 +177,9 @@ GOLDEN = ["tiny_gae", "tiny_gauss", "tiny_tuple", "tiny_conv", "tiny_mask", "tin
 
 def _golden_setup(name):
     """(z, meta, ocfg, cfg, model, traj, native tape env, learner) of a reference-executed fixture"""
-    if name == "tiny_mixed":
-        from tests import test_gpu_mixed_tuple as MT
-
-        z, meta, ocfg, model, traj, sampler, learner = MT._build_fixture(name, "simt")
-        return z, meta, ocfg, sampler.cfg, model, traj, sampler.env, learner
-    if name == "tiny_dict":
-        from tests import dict_obs_oracle as DO
-        from tests import test_gpu_dict_obs as D
-
-        z, meta, ocfg = DO.load_dict_case(name)
-        cfg, model, traj, sampler, learner = D._build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]),
-                                                      "simt")
-        return z, meta, ocfg, cfg, model, traj, sampler.env, learner
-    z, meta, ocfg = load_case(name)
-    cfg, model, traj, env, sampler, learner = E.build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]),
-                                                      DEV)
+    load = {"tiny_mixed": load_mixed_case, "tiny_dict": DO.load_dict_case}.get(name, load_case)
+    z, meta, ocfg = case = load(name)
+    cfg, model, traj, env, sampler, learner = build_case(case, "simt")
     return z, meta, ocfg, cfg, model, traj, env, learner
 
 
@@ -211,7 +190,7 @@ def test_adapter_matches_reference_golden(name, where):
     post-Adam weights: Discrete actions bit-exact, policy outputs 1e-5, weights 2e-5"""
     from sample_factory_b200.sampler import DeviceSampler
 
-    ops = _ops()
+    ops = ops_for()
     z, meta, ocfg, cfg, model, traj, native, learner = _golden_setup(name)
     env = _adapter(native, where == "cpu", obs_dtype=torch.float64 if name == "tiny_gae" else torch.float32)
     assert (env.obs_dim, env.num_actions, env.obs_uint8) == (model.spec.obs_dim, model.spec.num_actions, model.spec.obs_uint8)
@@ -282,10 +261,10 @@ def test_adapter_rollouts_are_bit_identical_to_the_native_env(where, monkeypatch
     from sample_factory_b200.sampler import DeviceSampler, SplitSampler
 
     monkeypatch.setenv("SFB200_TAIL_FUSED", "0")
-    ops = _ops()
+    ops = ops_for()
     N, T = 256, 16
     ocfg, tape = _cfg2_small(N, T)
-    cfg, model, traj, _, _, _ = E.build(ocfg, N, O.init_state(ocfg, seed=8), tape.cpu(), DEV)
+    cfg, model, traj, _, _, _ = build(ocfg, N, O.init_state(ocfg, seed=8), tape.cpu())
     kw = dict(engine=ops.GEMM_SIMT, philox_seed=3)
     native = _collect(DeviceSampler(cfg, TapeVecEnv(tape, ocfg.num_actions), model, traj, **kw), traj, 3)
     for graph in (False, True):
@@ -314,7 +293,7 @@ def test_async_runner_over_the_adapter_matches_the_native_env(tmp_path, monkeypa
     register_env("bt_tensor", lambda n, c, e, render_mode=None: TensorTapeEnv(TapeVecEnv(tape, ocfg.num_actions)))
     runs = []
     for name in ("bt_native", "bt_tensor"):
-        cfg = E.make_cfg(ocfg, env=name, train_dir=str(tmp_path), experiment=name, cuda_graph=False, seed=0,
+        cfg = make_cfg(ocfg, env=name, train_dir=str(tmp_path), experiment=name, cuda_graph=False, seed=0,
                          gemm_engine="simt", async_rl=True, restart_behavior="overwrite", env_gpu_actions=True)
         r = Runner(cfg)
         assert r.init() == 0
@@ -334,10 +313,10 @@ def test_cuda_env_with_gpu_actions_never_synchronises_the_host():
     from sample_factory_b200.envs import TapeVecEnv
     from sample_factory_b200.sampler import DeviceSampler
 
-    ops = _ops()
+    ops = ops_for()
     N, T = 256, 16
     ocfg, tape = _cfg2_small(N, T)
-    cfg, model, traj, _, _, _ = E.build(ocfg, N, O.init_state(ocfg, seed=8), tape.cpu(), DEV)
+    cfg, model, traj, _, _, _ = build(ocfg, N, O.init_state(ocfg, seed=8), tape.cpu())
     for graph in (False, True):
         s = DeviceSampler(cfg, _adapter(TapeVecEnv(tape, ocfg.num_actions), False), model, traj, engine=ops.GEMM_SIMT,
                           use_cuda_graph=graph)
@@ -404,7 +383,7 @@ def test_torch_cartpole_trains_through_run_rl_and_enjoys(tmp_path):
     from sample_factory_b200.host_env import BatchedTensorEnvAdapter
     from sample_factory_b200.train import make_runner
 
-    _ops()
+    ops_for()
     register_env("TorchCartPole-v0", lambda name, cfg, env_config, render_mode=None: TorchCartPole())
     iters = 150
     argv = ["--env=TorchCartPole-v0", "--experiment=torch_cartpole", f"--train_dir={tmp_path}", "--restart_behavior=overwrite",

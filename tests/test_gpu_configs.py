@@ -2,39 +2,12 @@
 size-independent properties only (the numerics of each ingredient are pinned by the reference goldens at small sizes:
 tiny_gauss, tiny_conv, tiny_gru / tiny_lstm).  These runs catch what small cases cannot: workspace sizing, 32-bit
 index overflow, kernel shape limits, memory footprint."""
-import numpy as np
 import pytest
 import torch
 
+from tests.device_harness import check_finite, runner
+
 pytestmark = pytest.mark.gpu
-
-
-def _runner(env_name, make_env, argv_extra):
-    from sample_factory_b200.cfg import parse_full_cfg, parse_sf_args
-    from sample_factory_b200.envs import register_env
-    from sample_factory_b200.train import Runner
-
-    register_env(env_name, make_env)
-    argv = [f"--env={env_name}", "--experiment=cfg_test", "--train_dir=/tmp/sfb200_tests", "--restart_behavior=overwrite",
-            "--batched_sampling=True", "--num_workers=1", "--num_envs_per_worker=1", "--worker_num_splits=1", "--seed=0",
-            "--save_every_sec=100000", "--experiment_summaries_interval=100000"] + argv_extra
-    parser, _ = parse_sf_args(argv)
-    cfg = parse_full_cfg(parser, argv)
-    r = Runner(cfg)
-    r.init()
-    return r
-
-
-def _check_finite(runner, n_iter, expect_steps):
-    for _ in range(n_iter):
-        runner.iteration()
-    torch.cuda.synchronize()
-    st = runner.learner.fetch_stats()
-    bad = {k: v for k, v in st.items() if isinstance(v, float) and not np.isfinite(v)}
-    assert not bad, bad
-    assert torch.isfinite(runner.model.flat).all()
-    assert runner.env_steps == expect_steps
-    return st
 
 
 def test_cfg3_continuous_async_2048_envs():
@@ -45,14 +18,14 @@ def test_cfg3_continuous_async_2048_envs():
     dev = torch.device("cuda", 0)
     N, T = 2048, 64
     tape = torch.randn(2 * T + 1, N, 27, generator=torch.Generator().manual_seed(0)).to(dev)
-    r = _runner("synthetic_ant", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8, continuous=True),
+    r = runner("synthetic_ant", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8, continuous=True),
                 ["--use_rnn=False", "--async_rl=True", f"--rollout={T}", "--recurrence=1", "--batch_size=32768",
                  "--num_batches_per_epoch=4", "--num_epochs=2", "--encoder_mlp_layers", "64", "64", "--nonlinearity=tanh",
                  "--adaptive_stddev=False", "--kl_loss_coeff=0.1", "--value_loss_coeff=1.3", "--max_grad_norm=3.5",
                  "--exploration_loss_coeff=0.0", "--ppo_clip_ratio=0.2", "--learning_rate=0.00295", "--value_bootstrap=True",
                  "--policy_initialization=torch_default"])
     assert r.async_rl and r.model.spec.continuous and not r.model.spec.adaptive_stddev
-    st = _check_finite(r, 4, 4 * N * T)
+    st = check_finite(r, 4, 4 * N * T)
     # async: the samples are one iteration (8 SGD steps) old when trained on (policy lag recorded per sample)
     assert st["version_diff_min"] >= 8 and st["version_diff_max"] <= 16, st
     a = r.traj["actions"]
@@ -70,7 +43,7 @@ def test_cfg4_atari_conv_1024_envs():
     dev = torch.device("cuda", 0)
     N, T = 1024, 16
     tape = torch.randint(0, 256, (T + 1, N, 4 * 84 * 84), dtype=torch.uint8, generator=torch.Generator().manual_seed(1)).to(dev)
-    r = _runner("synthetic_atari", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
+    r = runner("synthetic_atari", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
                 ["--use_rnn=False", "--async_rl=False", f"--rollout={T}", "--recurrence=1", "--batch_size=4096",
                  "--num_batches_per_epoch=4", "--num_epochs=1", "--encoder_conv_architecture=convnet_atari",
                  "--encoder_conv_mlp_layers", "512", "--nonlinearity=relu", "--obs_scale=255.0",
@@ -78,7 +51,7 @@ def test_cfg4_atari_conv_1024_envs():
     sp = r.model.spec
     assert sp.obs_uint8 and sp.conv_out_size == 64 * 7 * 7 and r.traj["obs"].dtype == torch.uint8
     before = r.model.params["encoder.encoders.obs.enc.conv_head.0.weight"].clone()
-    _check_finite(r, 2, 2 * N * T)
+    check_finite(r, 2, 2 * N * T)
     assert not torch.equal(before, r.model.params["encoder.encoders.obs.enc.conv_head.0.weight"])
     # per-pixel input statistics after two updates: mean of uniform 0..255 frames / 255 is ~0.5
     assert abs(r.model.obs_mean.mean().item() - 0.5) < 0.02 and r.model.obs_count.item() == 1 + 2 * N * (T + 1)
@@ -92,14 +65,14 @@ def test_cfg5_lstm_4096_envs_per_gpu():
     dev = torch.device("cuda", 0)
     N, T = 4096, 16
     tape = torch.randn(2 * T + 1, N, 256, generator=torch.Generator().manual_seed(2)).to(dev)
-    r = _runner("synthetic_isaac", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
+    r = runner("synthetic_isaac", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
                 ["--use_rnn=True", "--rnn_type=lstm", "--rnn_size=512", "--async_rl=False", f"--rollout={T}",
                  f"--recurrence={T}", "--batch_size=32768", "--num_batches_per_epoch=2", "--num_epochs=2",
                  "--encoder_mlp_layers", "512", "256", "128", "--value_bootstrap=True", "--reward_scale=0.01",
                  "--lr_schedule=kl_adaptive_epoch", "--lr_schedule_kl_threshold=0.016", "--max_grad_norm=1.0"])
     assert r.model.spec.rnn_state_size == 1024 and r.traj["rnn_states"].shape == (N, T + 1, 1024)
     lr0 = r.learner.curr_lr
-    st = _check_finite(r, 3, 3 * N * T)
+    st = check_finite(r, 3, 3 * N * T)
     assert st["num_valid"] == 32768
     assert r.learner.curr_lr != lr0         # the KL-adaptive scheduler moved the learning rate
     hs = r.traj["rnn_states"]

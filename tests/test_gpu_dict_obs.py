@@ -10,50 +10,10 @@ import torch
 
 from oracle import appo_oracle as O
 from tests import dict_obs_oracle as DO
-from tests.golden_utils import state_from
-from tests.test_gpu_engine import make_cfg
+from tests.device_harness import (DEV, ENGINES, TOL, build, build_case, check_finite, ops_for, replay_learner,
+                                  replay_sampler, runner)
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-ENGINES = ["simt", "3xtf32"]
-
-
-def _ops(engine="simt"):
-    from sample_factory_b200 import ops
-
-    ops.bind_device(torch.device("cuda", 0))
-    if engine != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return ops
-
-
-def _spec(ocfg):
-    from sample_factory_b200.model import ModelSpec
-
-    return ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), list(ocfg.decoder_mlp_layers),
-                     ocfg.nonlinearity, ocfg.normalize_input, ocfg.normalize_returns, ocfg.obs_subtract_mean,
-                     ocfg.obs_scale, ocfg.use_rnn, ocfg.rnn_type, ocfg.rnn_size, continuous=ocfg.continuous,
-                     obs_keys=ocfg.obs_keys)
-
-
-def _build(ocfg, N, state, tape, engine, graph=False, **over):
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-
-    ops = _ops(engine)
-    dev = torch.device("cuda", 0)
-    cfg = make_cfg(ocfg, **over)
-    model = PolicyModel(_spec(ocfg), dev)
-    model.load_state_dict(state, strict=False)
-    traj = alloc_for_spec(model.spec, N, ocfg.rollout, dev)
-    env = TapeVecEnv(tape.to(dev).contiguous(), ocfg.num_actions, continuous=ocfg.continuous,
-                     with_action_mask=ocfg.action_mask, obs_keys=ocfg.obs_keys)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine], use_cuda_graph=graph)
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
-    return cfg, model, traj, sampler, learner
 
 
 # ------------------------------------------------------------------------------------------------ vs torch autograd
@@ -75,8 +35,8 @@ def test_key_encoders_match_torch_autograd(layout, decoder, engine):
     st = O.init_state(ocfg, seed=3)
     tape = torch.randn(T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(8)) * 1.5 + 0.3
     noise = torch.empty(T, N, 5).exponential_(generator=torch.Generator().manual_seed(9))
-    dev = torch.device("cuda", 0)
-    cfg, model, traj, sampler, learner = _build(ocfg, N, st, tape, engine)
+    dev = DEV
+    cfg, model, traj, _, sampler, learner = build(ocfg, N, st, tape, engine)
     assert model.spec.dict_obs and learner.heads_plan.keys and not sampler.fused_rollout
     if not decoder:     # the concatenation feeds the heads directly: unfused heads
         assert learner.heads_plan.P == 0 and sampler.heads_plan.P == 0
@@ -111,67 +71,15 @@ GOLDEN = ["tiny_dict", "tiny_dict_lstm", "tiny_dict_mask"]
 @pytest.mark.parametrize("name", GOLDEN)
 def test_sampler_matches_reference_golden(name, engine):
     """the sampler on the reference's weights, packed obs tape and noise: Discrete actions bit-exact, policy outputs 1e-5"""
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = DO.load_dict_case(name)
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]),
-                                                engine)
-    sampler.reset()
-    for it in range(meta["iters"]):
-        st = state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/")
-        model.load_state_dict(st, strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(dev).contiguous()
-        sampler.rollout()
-        got = {k: v.cpu() for k, v in traj.items()}
-        ref = {k: torch.from_numpy(z[f"it{it}/traj/{k}"]) for k in
-               ["obs", "actions", "action_logits", "log_prob_actions", "values", "rewards", "dones", "rnn_states"]}
-        assert torch.equal(got["obs"].view(ref["obs"].shape), ref["obs"])
-        assert torch.equal(got["dones"].view(ref["dones"].shape), ref["dones"])
-        if ocfg.continuous:
-            for k in ("actions", "rewards"):
-                np.testing.assert_allclose(got[k].view(ref[k].shape).numpy(), ref[k].numpy(), atol=TOL, err_msg=k)
-        else:
-            assert torch.equal(got["actions"].view(ref["actions"].shape), ref["actions"]), "actions must be bit-exact"
-            assert torch.equal(got["rewards"].view(ref["rewards"].shape), ref["rewards"])
-        np.testing.assert_allclose(got["rnn_states"].numpy(), ref["rnn_states"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["action_logits"].numpy(), ref["action_logits"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), ref["values"][:, :-1].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), ref["log_prob_actions"].numpy(), atol=TOL)
+    case = DO.load_dict_case(name)
+    replay_sampler(case, build_case(case, engine), exact=("obs", "dones", "rewards", "actions"))
 
 
 def _learner_vs_golden(name, engine, graph):
-    from sample_factory_b200 import ops
-
-    z, meta, ocfg = DO.load_dict_case(name)
-    over = dict(learner_cuda_graph=graph)
-    shuffle = any(k.endswith("/mb_indices") for k in z.files)
-    if shuffle:
-        over["shuffle_minibatches"] = True
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]),
-                                                engine, **over)
-    assert learner.use_graph == graph and learner.shuffle == shuffle
-    for it in range(meta["iters"]):
-        assert learner.train_step == int(z[f"it{it}/train_step_before"])
-        for k, v in DO.traj_from(z, it, ocfg).items():
-            traj[k].copy_(v.view(traj[k].shape))
-        if shuffle:
-            learner.set_minibatch_permutation(z[f"it{it}/mb_indices"])
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        p = f"it{it}/prep/"
-        assert torch.equal(learner.valids_flat.view(-1).cpu(), torch.from_numpy(z[p + "valids"]))
-        np.testing.assert_allclose(traj["values"][:, -1].cpu().numpy(), z[p + "bootstrap_values"], atol=TOL)
-        np.testing.assert_allclose(learner.advantages.view(-1).cpu().numpy(), z[p + "advantages"], atol=TOL)
-        np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), z[p + "returns"], atol=TOL)
-        log = learner.minibatch_log().numpy()
-        assert log.shape[0] == len(z[f"it{it}/loss/policy_loss"])
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=TOL, rtol=1e-5, err_msg=key)
-        got_state = model.state_dict()
-        for k, v in state_from(z, f"it{it}/state/").items():
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * TOL
-            np.testing.assert_allclose(got_state[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = DO.load_dict_case(name)
+    rig = build_case(case, engine, learner_cuda_graph=graph)
+    assert rig.learner.use_graph == graph
+    replay_learner(case, rig, traj_of=DO.traj_from)
 
 
 @pytest.mark.parametrize("engine", ENGINES)
@@ -277,7 +185,7 @@ def test_host_env_dict_rows_run_rl_and_enjoy(tmp_path, multi_agent):
     from sample_factory_b200.host_env import BatchedHostEnv
     from sample_factory_b200.train import run_rl
 
-    _ops()
+    ops_for()
     dev = torch.device("cuda", 0)
     cls = GoalMultiAgentEnv if multi_agent else GoalEnv
     env = BatchedHostEnv(cls, 4, dev)
@@ -319,8 +227,6 @@ def test_dict_goal_env_4096_envs_full_size():
     """keys (25, 3, 3) with MLP [512, 512] per key through Runner: 4096 envs, T = 32, 4 x 32768 minibatches.  Peak
     allocated memory stays under 1.5 GiB (0.99 GiB measured by this test on an H100 80GB HBM3); the large items: per key
     one [32768, 512] hidden activation and its gradient, the [32768, 1536] concatenation and its gradient, the trajectories."""
-    from tests.test_gpu_configs import _check_finite, _runner
-
     from sample_factory_b200.envs import TapeVecEnv
 
     dev = torch.device("cuda", 0)
@@ -330,13 +236,13 @@ def test_dict_goal_env_4096_envs_full_size():
     base = torch.cuda.memory_allocated()
     keys = [("achieved_goal", 3), ("desired_goal", 3), ("observation", 25)]
     tape = torch.randn(2 * T + 1, N, 31, generator=torch.Generator().manual_seed(2)).to(dev)
-    r = _runner("synthetic_goal_dict", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8, obs_keys=keys),
+    r = runner("synthetic_goal_dict", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8, obs_keys=keys),
                 ["--use_rnn=False", "--async_rl=False", f"--rollout={T}", "--recurrence=1", "--batch_size=32768", "--num_batches_per_epoch=4",
                  "--encoder_mlp_layers", "512", "512"])
     assert r.model.spec.obs_keys == keys and r.model.spec.fc_encoder_input == 1536
     assert not getattr(r.sampler, "fused_rollout", False)
     w = r.model.params["encoder.encoders.desired_goal.mlp_head.0.weight"].clone()
-    st = _check_finite(r, 2, 2 * N * T)
+    st = check_finite(r, 2, 2 * N * T)
     assert st["num_valid"] == 32768
     assert not torch.equal(w, r.model.params["encoder.encoders.desired_goal.mlp_head.0.weight"])
     peak = (torch.cuda.max_memory_allocated() - base) / 2**30

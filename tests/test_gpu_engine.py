@@ -7,74 +7,11 @@ import pytest
 import torch
 
 from oracle import appo_oracle as O
-from tests.golden_utils import load_case, state_from, traj_from
+from tests.device_harness import (DEV, ENGINES, TOL, build, build_case, compare_rollout_runs, graphed_sampler_matches_eager,
+                                  make_cfg, need, ops_for, replay_learner, replay_sampler)
+from tests.golden_utils import load_case
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-
-
-def make_cfg(ocfg: O.OracleCfg, **over):
-    from sample_factory_b200.cfg import default_cfg
-
-    cfg = default_cfg()
-    for k in ["rollout", "recurrence", "batch_size", "num_batches_per_epoch", "num_epochs", "gamma", "gae_lambda",
-              "ppo_clip_ratio", "ppo_clip_value", "exploration_loss_coeff", "value_loss_coeff", "kl_loss_coeff",
-              "max_grad_norm", "learning_rate", "adam_eps", "adam_beta1", "adam_beta2", "normalize_input",
-              "normalize_returns", "value_bootstrap", "with_vtrace", "vtrace_rho", "vtrace_c", "reward_scale",
-              "reward_clip", "max_policy_lag", "nonlinearity", "obs_subtract_mean", "obs_scale", "use_rnn", "rnn_type",
-              "rnn_size", "adaptive_stddev", "continuous_tanh_scale", "initial_stddev", "exploration_loss", "optimizer", "actor_critic_share_weights"]:
-        setattr(cfg, k, getattr(ocfg, k))
-    cfg.encoder_mlp_layers = list(ocfg.encoder_mlp_layers)
-    cfg.decoder_mlp_layers = list(ocfg.decoder_mlp_layers)
-    cfg.encoder_conv_architecture = ocfg.encoder_conv_architecture
-    cfg.encoder_conv_mlp_layers = list(ocfg.encoder_conv_mlp_layers)
-    cfg.async_rl = False
-    for k, v in over.items():
-        setattr(cfg, k, v)
-    return cfg
-
-
-def build(ocfg: O.OracleCfg, N: int, state, tape, dev, engine="simt", graph=False):
-    from sample_factory_b200 import ops
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import ModelSpec, PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-
-    ops.bind_device(dev)
-    cfg = make_cfg(ocfg)
-    spec = ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), list(ocfg.decoder_mlp_layers),
-                     ocfg.nonlinearity, ocfg.normalize_input, ocfg.normalize_returns, ocfg.obs_subtract_mean,
-                     ocfg.obs_scale, ocfg.use_rnn, ocfg.rnn_type, ocfg.rnn_size, continuous=ocfg.continuous,
-                     adaptive_stddev=ocfg.adaptive_stddev, continuous_tanh_scale=ocfg.continuous_tanh_scale,
-                     initial_stddev=ocfg.initial_stddev, obs_shape=ocfg.obs_shape,
-                     encoder_conv_architecture=ocfg.encoder_conv_architecture,
-                     encoder_conv_mlp_layers=list(ocfg.encoder_conv_mlp_layers), obs_uint8=tape.dtype == torch.uint8,
-                     action_segments=ocfg.action_segments, share_weights=ocfg.actor_critic_share_weights)
-    model = PolicyModel(spec, dev)
-    model.load_state_dict(state, strict=False)
-    traj = alloc_for_spec(spec, N, ocfg.rollout, dev)
-    env = TapeVecEnv(tape.to(dev).contiguous(), ocfg.num_actions, continuous=ocfg.continuous, obs_shape=ocfg.obs_shape,
-                     action_segments=ocfg.action_segments, with_action_mask=ocfg.action_mask)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine], use_cuda_graph=graph)
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
-    return cfg, model, traj, env, sampler, learner
-
-
-def upload_traj(traj_dev, traj_cpu):
-    for k, v in traj_cpu.items():
-        traj_dev[k].copy_(v.view(traj_dev[k].shape))
-
-
-ENGINES = ["simt", "3xtf32"]
-
-
-def _need(engine):
-    from sample_factory_b200 import ops
-
-    if engine != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
 
 
 GOLDEN_CASES = ["tiny_gae", "tiny_vtrace", "tiny_gru", "tiny_lstm", "cfg2_small", "tiny_gauss", "tiny_gauss_adaptive", "tiny_conv", "tiny_symkl", "tiny_lamb", "tiny_tuple", "tiny_separate", "tiny_mask"]
@@ -84,42 +21,8 @@ GOLDEN_CASES = ["tiny_gae", "tiny_vtrace", "tiny_gru", "tiny_lstm", "cfg2_small"
 @pytest.mark.parametrize("name", GOLDEN_CASES)
 def test_rollout_matches_reference_golden(name, engine):
     """Sampler vs the REFERENCE's own trajectories (same weights, same obs tape, same Exp(1) noise)."""
-    _need(engine)
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = load_case(name)
-    tape = torch.from_numpy(z["tape"])
-    cfg, model, traj, env, sampler, learner = build(ocfg, meta["N"], state_from(z, "init/"), tape, dev, engine=engine)
-    sampler.reset()
-    for it in range(meta["iters"]):
-        st = state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/")
-        model.load_state_dict(st, strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(dev).contiguous()
-        sampler.rollout()
-        poisoned = meta["poison"] and it == meta["iters"] - 1
-        got = {k: v.cpu() for k, v in traj.items()}
-        ref = {k: torch.from_numpy(z[f"it{it}/traj/{k}"]) for k in
-               ["obs", "actions", "action_logits", "log_prob_actions", "values", "policy_version", "rewards", "dones",
-                "time_outs", "policy_id", "rnn_states"]}
-        for k in ["obs", "rewards", "dones", "time_outs"]:
-            if k == "rewards" and ocfg.continuous:   # reward = f(float action): tolerance, not bit-exactness
-                np.testing.assert_allclose(got[k].numpy(), ref[k].numpy(), atol=TOL)
-                continue
-            assert torch.equal(got[k].view(ref[k].shape), ref[k]), k
-        np.testing.assert_allclose(got["rnn_states"].numpy(), ref["rnn_states"].numpy(), atol=TOL)
-        if not poisoned:
-            assert torch.equal(got["policy_id"], ref["policy_id"])
-            assert torch.equal(got["policy_version"], ref["policy_version"])
-        np.testing.assert_allclose(got["action_logits"].numpy(), ref["action_logits"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), ref["values"][:, :-1].numpy(), atol=TOL)
-        if ocfg.continuous:
-            # Box actions are floats: a = eps*std + mean inherits the 1e-6-level differences of means / log_std
-            np.testing.assert_allclose(got["actions"].numpy(), ref["actions"].numpy(), atol=TOL)
-        else:
-            # action indices: bit-exact (BASELINE.json). A flip would need p_i/q_i == p_j/q_j to within the 1e-6 logit
-            # difference -- none occurs on these seeded inputs.
-            assert torch.equal(got["actions"].view(ref["actions"].shape), ref["actions"]), "action indices must be bit-exact"
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), ref["log_prob_actions"].numpy(), atol=TOL)
+    case = load_case(name)
+    replay_sampler(case, build_case(case, engine))
 
 
 @pytest.mark.parametrize("engine", ENGINES)
@@ -127,40 +30,8 @@ def test_rollout_matches_reference_golden(name, engine):
 def test_learner_matches_reference_golden(name, engine):
     """Learner.train on the REFERENCE's trajectories: returns / advantages / loss terms / post-Adam weights /
     normalizer statistics against what the reference itself computed."""
-    from sample_factory_b200 import ops
-
-    _need(engine)
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = load_case(name)
-    tape = torch.from_numpy(z["tape"])
-    cfg, model, traj, env, sampler, learner = build(ocfg, meta["N"], state_from(z, "init/"), tape, dev, engine=engine)
-    for it in range(meta["iters"]):
-        assert learner.train_step == int(z[f"it{it}/train_step_before"])
-        upload_traj(traj, traj_from(z, it, ocfg))
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        p = f"it{it}/prep/"
-        assert torch.equal(learner.valids_flat.view(-1).cpu(), torch.from_numpy(z[p + "valids"]))
-        np.testing.assert_allclose(traj["values"][:, -1].cpu().numpy(), z[p + "bootstrap_values"], atol=TOL)
-        np.testing.assert_allclose(traj["rewards"].view(-1).cpu().numpy(), z[p + "rewards"], atol=1e-6)
-        if not ocfg.with_vtrace:
-            np.testing.assert_allclose(learner.advantages.view(-1).cpu().numpy(), z[p + "advantages"], atol=TOL)
-            np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), z[p + "returns"], atol=TOL)
-        log = learner.minibatch_log().numpy()
-        n_ref = len(z[f"it{it}/loss/policy_loss"])
-        assert log.shape[0] == n_ref
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=TOL, rtol=1e-5, err_msg=key)
-        ref_state = state_from(z, f"it{it}/state/")
-        got_state = model.state_dict()
-        for k, v in ref_state.items():
-            # float64 normaliser state: the obs statistics are functions of exact inputs (1e-8); the returns statistics
-            # are moments of fp32 returns that themselves carry the 1e-5 tolerance (1e-6 on the moments)
-            # post-Adam weights: an element whose gradient is comparable to adam_eps moves by lr * g / (|g| + eps), which
-            # amplifies a 1e-6 gradient difference to ~1e-5 on the weight (seen on 2 of 8192 conv weights) -> 2e-5
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * TOL
-            np.testing.assert_allclose(got_state[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = load_case(name)
+    replay_learner(case, build_case(case, engine), rewards=True)
 
 
 @pytest.mark.parametrize("engine", ENGINES)
@@ -169,14 +40,13 @@ def test_closed_loop_vs_oracle_cfg2_shape(engine):
     tape / noise / initial weights (the tape env keeps both rollouts aligned)."""
     from sample_factory_b200 import ops
 
-    dev = torch.device("cuda", 0)
     N, T = 256, 32
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T // 4, num_batches_per_epoch=4, num_epochs=1)
     st0 = O.init_state(ocfg, seed=3)
     gen = torch.Generator().manual_seed(11)
     tape = torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=gen) * 1.2 - 0.2
-    _need(engine)
-    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, dev, engine=engine)
+    need(engine)
+    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, engine=engine)
     olearner = O.OracleLearner(ocfg, st0)
     oenv = O.TapeVecEnv(tape, ocfg.num_actions)
     olast = oenv.reset()
@@ -185,7 +55,7 @@ def test_closed_loop_vs_oracle_cfg2_shape(engine):
         noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=gen)
         otraj = O.alloc_trajectories(ocfg, N)
         olast = O.rollout(ocfg, olearner.st, oenv, olast, otraj, noise, olearner.train_step)
-        sampler.noise = noise.to(dev)
+        sampler.noise = noise.to(DEV)
         sampler.set_policy_version(learner.train_step)
         sampler.rollout()
         got = {k: v.cpu() for k, v in traj.items()}
@@ -218,26 +88,13 @@ def test_full_size_properties_and_graph_replay():
     * a training iteration changes the weights, keeps everything finite, and leaves padding untouched."""
     from sample_factory_b200 import ops
 
-    dev = torch.device("cuda", 0)
     N, T = 4096, 32
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T // 4, num_batches_per_epoch=4)
     st0 = O.init_state(ocfg, seed=5)
     tape = torch.randn(3 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(12))
-    cfgA, modelA, trajA, envA, samplerA, learnerA = build(ocfg, N, st0, tape, dev, graph=False)
-    cfgB, modelB, trajB, envB, samplerB, learnerB = build(ocfg, N, st0, tape, dev, graph=True)
-    samplerA.reset()
-    samplerB.reset()
-    samplerA.rollout()
-    samplerB.rollout()   # warm-up + capture + first replay start from the same counters? -> compare second rollouts
-    # Graph capture runs the rollout eagerly once (warm-up) before replaying, so B is ahead; re-align both and compare
-    for s, e in ((samplerA, envA), (samplerB, envB)):
-        s.reset()
-        s.step_counter.zero_()
-    samplerA.rollout()
-    samplerB.rollout()
-    torch.cuda.synchronize()
-    for k in trajA:
-        assert torch.equal(trajA[k], trajB[k]), f"graph replay differs from eager for {k}"
+    A = build(ocfg, N, st0, tape)
+    graphed_sampler_matches_eager(A, build(ocfg, N, st0, tape, graph=True))
+    modelA, trajA, learnerA = A.model, A.traj, A.learner
     a = trajA["actions"]
     assert a.min().item() >= 0 and a.max().item() <= ocfg.num_actions - 1
     assert torch.all(trajA["policy_id"] == 0) and torch.isfinite(trajA["action_logits"]).all()
@@ -245,15 +102,15 @@ def test_full_size_properties_and_graph_replay():
     assert freq.min().item() > 0.01, "every action should be sampled under near-uniform initial logits"
 
     # GAE linearity at full size
-    r1 = torch.randn(N, T, device=dev)
-    r2 = torch.randn(N, T, device=dev)
+    r1 = torch.randn(N, T, device=DEV)
+    r2 = torch.randn(N, T, device=DEV)
     dones = trajA["dones"]
-    zeros_v = torch.zeros(N, T + 1, device=dev)
-    ones_valid = torch.ones(N, T + 1, dtype=torch.bool, device=dev)
+    zeros_v = torch.zeros(N, T + 1, device=DEV)
+    ones_valid = torch.ones(N, T + 1, dtype=torch.bool, device=DEV)
     outs = []
     for r in (r1, r2, r1 + r2):
-        adv = torch.empty(N, T, device=dev)
-        ret = torch.empty(N, T, device=dev)
+        adv = torch.empty(N, T, device=DEV)
+        ret = torch.empty(N, T, device=DEV)
         ops.gae_returns(r.clone(), dones, trajA["time_outs"], zeros_v, ones_valid, 0.99, 0.95, False, None, None, adv, ret)
         outs.append(adv)
         assert torch.equal(adv, ret)   # values == 0 -> returns == advantages
@@ -279,25 +136,15 @@ def test_action_mask_graph_replay_and_mask_respected():
     """Action-mask env (obs dict) under the production path: in-kernel Philox noise, CUDA-graph replay == eager, every
     sampled action is allowed by the mask of its step (rows that allow nothing excepted), and the fused GEMM + heads path
     (hidden 128) honours the mask too."""
-    dev = torch.device("cuda", 0)
     N, T = 512, 16
     ocfg = O.OracleCfg(obs_dim=32, num_actions=8, encoder_mlp_layers=[128, 128], rollout=T, recurrence=1,
                        batch_size=N * T // 2, num_batches_per_epoch=2, action_mask=True)
     st0 = O.init_state(ocfg, seed=6)
     tape = torch.randn(3 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(13))
-    engine = "3xtf32" if _tc() else "simt"
-    _, _, trajA, envA, samplerA, _ = build(ocfg, N, st0, tape, dev, engine=engine, graph=False)
-    _, _, trajB, envB, samplerB, _ = build(ocfg, N, st0, tape, dev, engine=engine, graph=True)
-    for s in (samplerA, samplerB):
-        s.reset()
-        s.rollout()
-    for s in (samplerA, samplerB):
-        s.reset()
-        s.step_counter.zero_()
-        s.rollout()
-    torch.cuda.synchronize()
-    for k in trajA:
-        assert torch.equal(trajA[k], trajB[k]), f"graph replay differs from eager for {k}"
+    engine = "3xtf32" if ops_for().tc_available() else "simt"
+    B = build(ocfg, N, st0, tape, engine, graph=True)
+    graphed_sampler_matches_eager(build(ocfg, N, st0, tape, engine), B)
+    trajB = B.traj
     a = trajB["actions"][:, :, 0].cpu().long()
     env_idx = torch.arange(N)
     some_allowed = torch.zeros(N, T, dtype=torch.bool)
@@ -314,12 +161,6 @@ def test_action_mask_graph_replay_and_mask_respected():
     np.testing.assert_allclose(trajB["log_prob_actions"].cpu()[~some_allowed].numpy(), -np.log(ocfg.num_actions), atol=1e-6)
 
 
-def _tc():
-    from sample_factory_b200 import ops
-
-    return ops.tc_available()
-
-
 def test_async_double_buffered_runner_matches_lagged_oracle(tmp_path):
     """async_rl=True (train.py): the sampler collects rollout i+1 on its own stream with a weight snapshot while the
     learner trains on rollout i.  The schedule is deterministic, so the oracle can replay it: rollout r is sampled
@@ -331,7 +172,6 @@ def test_async_double_buffered_runner_matches_lagged_oracle(tmp_path):
     from sample_factory_b200.envs import TapeVecEnv, register_env
     from sample_factory_b200.train import Runner
 
-    dev = torch.device("cuda", 0)
     N, T, ITERS = 128, 16, 3
     ocfg = O.OracleCfg(obs_dim=32, num_actions=8, encoder_mlp_layers=[128, 128], rollout=T, recurrence=1,
                        batch_size=N * T // 4, num_batches_per_epoch=4, num_epochs=1)
@@ -339,13 +179,13 @@ def test_async_double_buffered_runner_matches_lagged_oracle(tmp_path):
     gen = torch.Generator().manual_seed(17)
     tape = torch.randn((ITERS + 1) * T + 1, N, ocfg.obs_dim, generator=gen)
     noises = [torch.empty(T, N, ocfg.num_actions).exponential_(generator=gen) for _ in range(ITERS + 1)]
-    register_env("async_tape", lambda n, c, e, render_mode=None: TapeVecEnv(tape.to(dev).contiguous(), ocfg.num_actions))
+    register_env("async_tape", lambda n, c, e, render_mode=None: TapeVecEnv(tape.to(DEV).contiguous(), ocfg.num_actions))
     cfg = make_cfg(ocfg, env="async_tape", train_dir=str(tmp_path), experiment="async", cuda_graph=False, seed=0,
                    gemm_engine="simt", async_rl=True, restart_behavior="overwrite")
     runner = Runner(cfg)
     assert runner.init() == 0
     runner.load_state_dict(st0)
-    runner.rollout_hook = lambda r: setattr(runner.sampler, "noise", noises[r].to(dev))
+    runner.rollout_hook = lambda r: setattr(runner.sampler, "noise", noises[r].to(DEV))
 
     olearner = O.OracleLearner(ocfg, copy.deepcopy(st0))
     oenv = O.TapeVecEnv(tape, ocfg.num_actions)
@@ -383,14 +223,13 @@ def test_split_sampler_matches_single_sampler():
     from sample_factory_b200.envs import TapeVecEnv
     from sample_factory_b200.sampler import DeviceSampler, SplitSampler
 
-    dev = torch.device("cuda", 0)
     N, T = 256, 8
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T, num_batches_per_epoch=1, encoder_mlp_layers=[128, 128])
     st0 = O.init_state(ocfg, seed=8)
-    tape = (torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(5)) * 1.1).to(dev)
-    cfg, model, traj, env, sampler, _ = build(ocfg, N, st0, tape.cpu(), dev, engine="3xtf32" if ops.tc_available() else "simt")
+    tape = (torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(5)) * 1.1).to(DEV)
+    cfg, model, traj, env, sampler, _ = build(ocfg, N, st0, tape.cpu(), engine="3xtf32" if ops.tc_available() else "simt")
     eng = sampler.engine
-    noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=torch.Generator().manual_seed(9)).to(dev)
+    noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=torch.Generator().manual_seed(9)).to(DEV)
     sampler.reset()
     sampler.noise = noise
     sampler.rollout()
@@ -443,17 +282,16 @@ def test_double_buffered_host_sampling_matches_one_group_after_the_other(use_gra
     from sample_factory_b200.envs import HostTapeVecEnv
     from sample_factory_b200.sampler import SplitSampler
 
-    dev = torch.device("cuda", 0)
     N, T = 256, 8
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T, num_batches_per_epoch=1, encoder_mlp_layers=[128, 128])
     st0 = O.init_state(ocfg, seed=8)
     tape = torch.randn(5 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(5)) * 1.1
-    cfg, model, traj, env, sampler, _ = build(ocfg, N, st0, tape, dev, engine="3xtf32" if ops.tc_available() else "simt")
+    cfg, model, traj, env, sampler, _ = build(ocfg, N, st0, tape, engine="3xtf32" if ops.tc_available() else "simt")
     h = N // 2
 
     def run(interleaved, n):
-        es = [HostTapeVecEnv(tape[:, :h].contiguous().numpy(), ocfg.num_actions, dev, env_index_offset=0),
-              HostTapeVecEnv(tape[:, h:].contiguous().numpy(), ocfg.num_actions, dev, env_index_offset=h)]
+        es = [HostTapeVecEnv(tape[:, :h].contiguous().numpy(), ocfg.num_actions, DEV, env_index_offset=0),
+              HostTapeVecEnv(tape[:, h:].contiguous().numpy(), ocfg.num_actions, DEV, env_index_offset=h)]
         sp = SplitSampler(cfg, es, model, traj, engine=sampler.engine, use_cuda_graph=use_graph, philox_seed=3)
         assert sp.host_interleaved
         if not interleaved:
@@ -483,22 +321,17 @@ def test_graphed_learner_matches_eager():
     same parameters, Adam moments and loss statistics as the launch-by-launch learner, iteration after iteration."""
     from sample_factory_b200 import ops
 
-    dev = torch.device("cuda", 0)
     N, T = 128, 8
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T // 2, num_batches_per_epoch=2, encoder_mlp_layers=[128, 128])
     st0 = O.init_state(ocfg, seed=2)
     tape = torch.randn(6 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(3))
     eng = "3xtf32" if ops.tc_available() else "simt"
-    cfgA, modelA, trajA, envA, samplerA, learnerA = build(ocfg, N, st0, tape, dev, engine=eng)
-    cfgB, modelB, trajB, envB, samplerB, _ = build(ocfg, N, st0, tape, dev, engine=eng)
-    from sample_factory_b200.learner import Learner
-
-    cfgB.learner_cuda_graph = True
-    learnerB = Learner(cfgB, modelB, N, engine=ops.ENGINES[eng])
+    cfgA, modelA, trajA, envA, samplerA, learnerA = build(ocfg, N, st0, tape, engine=eng)
+    cfgB, modelB, trajB, envB, samplerB, learnerB = build(ocfg, N, st0, tape, engine=eng, learner_cuda_graph=True)
     assert learnerB.use_graph and not learnerA.use_graph
     samplerA.reset()
     for it in range(5):
-        noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=torch.Generator().manual_seed(20 + it)).to(dev)
+        noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=torch.Generator().manual_seed(20 + it)).to(DEV)
         samplerA.noise = noise
         samplerA.set_policy_version(learnerA.train_step)
         samplerA.rollout()
@@ -523,19 +356,18 @@ def test_fused_tail_and_rollout_match_separate_launches(explicit_noise, monkeypa
     (csrc/rollout_fused.cu), produce the same trajectories, episode statistics, env state and next policy input as the
     per-layer / per-stage launches: bit-identical for everything downstream of the logits (same device functions),
     logits / values at rounding level."""
-    _need("3xtf32")
-    dev = torch.device("cuda", 0)
+    need("3xtf32")
     N, T = 1000, 12
     ocfg = O.OracleCfg(rollout=T, recurrence=1, batch_size=N * T // 4, num_batches_per_epoch=4)
     st0 = O.init_state(ocfg, seed=9)
     gen = torch.Generator().manual_seed(3)
     tape = torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=gen)
-    noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=gen).to(dev)
+    noise = torch.empty(T, N, ocfg.num_actions).exponential_(generator=gen).to(DEV)
     runs = {}
     for mode in ("separate", "tail", "persistent"):
         monkeypatch.setenv("SFB200_TAIL_FUSED", "0" if mode == "separate" else "1")
         monkeypatch.setenv("SFB200_ROLLOUT_FUSED", "1" if mode == "persistent" else "0")
-        cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, dev, engine="3xtf32")
+        cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, engine="3xtf32")
         assert sampler.fused_tail == (mode != "separate")
         assert sampler.fused_rollout == (mode == "persistent")
         sampler.reset()
@@ -555,21 +387,7 @@ def test_fused_tail_and_rollout_match_separate_launches(explicit_noise, monkeypa
     assert launches["separate"] > launches["tail"] > launches["persistent"], launches
     assert launches["persistent"] == 2, launches     # pre-step(0) + ONE kernel for T steps
     for other in ("tail", "persistent"):
-        _compare_rollout_runs(runs["separate"], runs[other], other)
-
-
-def _compare_rollout_runs(a, b, what):
-    # logits, values and log-probs agree to ~2 ulp of their size; everything else is bit-identical
-    for ta, tb in zip(a["traj"], b["traj"]):
-        for k in ta:
-            if k in ("action_logits", "values", "log_prob_actions"):
-                np.testing.assert_allclose(ta[k].cpu().numpy(), tb[k].cpu().numpy(), rtol=0, atol=2e-6, err_msg=f"{what} {k}")
-            elif k != "valids":
-                assert torch.equal(ta[k], tb[k]), (what, k)
-    for k in ("obs", "rew", "term", "step", "pstep"):
-        assert torch.equal(a[k], b[k]), (what, k)
-    np.testing.assert_allclose(a["stats"].cpu().numpy(), b["stats"].cpu().numpy(), rtol=1e-12)
-    assert torch.equal(a["ep"][0], b["ep"][0]) and torch.equal(a["ep"][1], b["ep"][1])
+        compare_rollout_runs(runs["separate"], runs[other], other)
 
 
 @pytest.mark.parametrize("rnn", [False, True])
@@ -580,8 +398,7 @@ def test_shuffle_minibatches_matches_oracle(engine, rnn):
     chunks keep their BPTT structure."""
     from sample_factory_b200 import ops
 
-    _need(engine)
-    dev = torch.device("cuda", 0)
+    need(engine)
     N, T = 64, 16
     R = 8 if rnn else 1
     kw = dict(use_rnn=True, rnn_type="gru", rnn_size=64, recurrence=R) if rnn else dict(recurrence=1)
@@ -590,11 +407,7 @@ def test_shuffle_minibatches_matches_oracle(engine, rnn):
     st0 = O.init_state(ocfg, seed=2)
     gen = torch.Generator().manual_seed(8)
     tape = torch.randn(T + 1, N, ocfg.obs_dim, generator=gen)
-    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, dev, engine=engine)
-    # (build() copies the oracle cfg; switch shuffling on in a fresh learner)
-    from sample_factory_b200.learner import Learner
-    cfg.shuffle_minibatches = True
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
+    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, engine=engine, shuffle_minibatches=True)
     assert learner.shuffle
     olearner = O.OracleLearner(ocfg, st0)
     oenv = O.TapeVecEnv(tape, ocfg.num_actions)

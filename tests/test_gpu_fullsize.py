@@ -18,10 +18,9 @@ import pytest
 import torch
 
 from oracle import appo_oracle as O
-from tests.test_gpu_engine import build
+from tests.device_harness import DEV, TOL, build, need
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
 
 CASES = {
     # BASELINE.json configs[1]: exact size
@@ -54,11 +53,9 @@ CASES = {
 def test_full_size_parity_vs_oracle(name):
     from sample_factory_b200 import ops
 
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
+    need("3xtf32")
     case = CASES[name]
     N, T = case["N"], case["T"]
-    dev = torch.device("cuda", 0)
     ocfg = O.OracleCfg(**case["ocfg"])
     st0 = O.init_state(ocfg, seed=5)
     gen = torch.Generator().manual_seed(23)
@@ -66,7 +63,7 @@ def test_full_size_parity_vs_oracle(name):
         tape = torch.randint(0, 256, (case["iters"] * T + 1, N, ocfg.obs_dim), dtype=torch.uint8, generator=gen)
     else:
         tape = torch.randn(case["iters"] * T + 1, N, ocfg.obs_dim, generator=gen) * 1.2 - 0.2
-    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, dev, engine="3xtf32")
+    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, "3xtf32")
     olearner = O.OracleLearner(ocfg, st0)
     oenv = O.TapeVecEnv(tape, ocfg.num_actions)
     olast = oenv.reset()
@@ -79,7 +76,7 @@ def test_full_size_parity_vs_oracle(name):
             noise = torch.empty(T, N, A).exponential_(generator=gen)
         otraj = O.alloc_trajectories(ocfg, N)
         olast = O.rollout(ocfg, olearner.st, oenv, olast, otraj, noise, olearner.train_step)
-        sampler.noise = noise.to(dev)
+        sampler.noise = noise.to(DEV)
         sampler.set_policy_version(learner.train_step)
         sampler.rollout()
         got = {k: v.cpu() for k, v in traj.items()}

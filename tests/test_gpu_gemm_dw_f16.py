@@ -12,42 +12,9 @@ import sys
 import pytest
 import torch
 
-from tests.test_gpu_gemm_pipeline import _ops, g
+from tests.device_harness import g, mlp_learner, ops_for, tc_dev, tc_dw  # noqa: F401  (tc_dev: the `dev` fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    ops = _ops()
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return d
-
-
-def _dw(dev, dz, x, bounds=None):
-    """dW = dz^T x; bounds = (bound of dz, bound of x) registered for the call, or None (the tf32 form)"""
-    ops = _ops()
-    M, N = dz.shape
-    K = x.shape[1]
-    W = torch.zeros(N, K, device=dev)
-    ws = torch.empty(ops.linear_backward_workspace_bytes(M, N, K) // 4 + 4, device=dev)
-    dW = torch.full((N, K), float("nan"), device=dev)
-    keep = []
-    if bounds is not None:
-        for t, b in zip((dz, x), bounds):
-            keep.append(torch.full((1,), float(b), device=dev))
-            ops.register_operand_bound(t, keep[-1])
-    try:
-        ops.linear_backward(dz, x, W, ops.ACT["none"], dW, None, None, ops.GEMM_TC_3XTF32, ws)
-        torch.cuda.synchronize()
-    finally:
-        if bounds is not None:
-            ops.unregister_operand_bound(dz)
-            ops.unregister_operand_bound(x)
-    return dW
 
 
 # dW2 and dW1 at the learner's shapes, a short last split-K slice (17000), one 32-k stage, ragged tiles; operands scaled
@@ -61,8 +28,8 @@ CASES = [(32768, 512, 512, 1.0, 1.0, 1.0), (32768, 512, 64, 1.0, 1.0, 1.0), (170
 def test_dw_f16_error_against_fp64(dev, M, N, K, sz, sx, looser):
     dz = (torch.randn(M, N, generator=g(70)) * sz).to(dev)
     x = (torch.nn.functional.elu(torch.randn(M, K, generator=g(71))) * sx).to(dev)
-    dw16 = _dw(dev, dz, x, (float(dz.abs().max()) * looser, float(x.abs().max()) * looser))
-    dw32 = _dw(dev, dz, x)
+    dw16 = tc_dw(dev, dz, x, (float(dz.abs().max()) * looser, float(x.abs().max()) * looser))
+    dw32 = tc_dw(dev, dz, x)
     ref = dz.double().t() @ x.double()
     top = float((dz.double().abs().t() @ x.double().abs()).max())
     err16 = float((dw16.double() - ref).abs().max())
@@ -74,50 +41,28 @@ def test_dw_f16_error_against_fp64(dev, M, N, K, sz, sx, looser):
 
 def test_dw_f16_needs_both_bounds(dev):
     """one operand without a bound keeps the tf32 form (bit for bit)"""
-    ops = _ops()
+    ops = ops_for()
     M, N, K = 4096, 256, 128
     dz = torch.randn(M, N, generator=g(72)).to(dev)
     x = torch.randn(M, K, generator=g(73)).to(dev)
-    dw32 = _dw(dev, dz, x)
+    dw32 = tc_dw(dev, dz, x)
     bound = torch.full((1,), float(dz.abs().max()), device=dev)
     ops.register_operand_bound(dz, bound)
     try:
-        only_dz = _dw(dev, dz, x)
+        only_dz = tc_dw(dev, dz, x)
     finally:
         ops.unregister_operand_bound(dz)
     assert torch.equal(only_dz, dw32)
 
 
-def _learner(dev, hidden, N=512, T=16):
-    from sample_factory_b200.cfg import default_cfg
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import ModelSpec, PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_trajectory_tensors
-
-    ops = _ops()
-    cfg = default_cfg()
-    cfg.use_rnn, cfg.async_rl = False, False
-    cfg.encoder_mlp_layers = list(hidden)
-    cfg.rollout, cfg.recurrence, cfg.batch_size, cfg.num_batches_per_epoch = T, 1, N * T // 2, 2
-    model = PolicyModel(ModelSpec(64, 8, list(hidden)), dev)
-    traj = alloc_trajectory_tensors(64, 8, N, T, dev)
-    tape = torch.randn(T + 1, N, 64, generator=g(74)).to(dev)
-    sampler = DeviceSampler(cfg, TapeVecEnv(tape, 8), model, traj, engine=ops.GEMM_TC_3XTF32)
-    learner = Learner(cfg, model, N, engine=ops.GEMM_TC_3XTF32)
-    sampler.reset()
-    return model, sampler, learner, traj
-
-
 _PROFILE_STEP = """
 import torch
 from torch.profiler import ProfilerActivity, profile
-from tests.test_gpu_gemm_dw_f16 import _learner
+from tests.device_harness import mlp_learner
 dev = torch.device("cuda", 0)
 from sample_factory_b200 import ops
 ops.bind_device(dev)
-model, sampler, learner, traj = _learner(dev, (512, 512))
+model, sampler, learner, traj = mlp_learner(dev, (512, 512))
 sampler.rollout()
 learner.train(traj)
 sampler.rollout()
@@ -149,7 +94,7 @@ def test_learner_runs_dw_f16_for_both_layers(dev):
 def test_hidden_gradient_bounds_hold(dev):
     """after several learner steps, |dz[i]| <= its bound, and the bound is bound(dz[i+1]) * max_k sum_n |W_{i+1}[n][k]|
     within 1.001 (three hidden layers: a chain of two products)"""
-    model, sampler, learner, traj = _learner(dev, (256, 256, 256))
+    model, sampler, learner, traj = mlp_learner(dev, (256, 256, 256))
     L = 3
     for _ in range(3):
         sampler.rollout()

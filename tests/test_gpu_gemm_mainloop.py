@@ -8,20 +8,9 @@ import math
 import pytest
 import torch
 
-from tests.test_gpu_gemm_dw_f16 import _dw
-from tests.test_gpu_gemm_pipeline import _ops, g
+from tests.device_harness import g, ops_for, tc_dev, tc_dw  # noqa: F401  (tc_dev: the `dev` fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    ops = _ops()
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return d
 
 
 # (M, N, K, amplitude of the activations): K / 64 stages of the forward, N / 64 of dX
@@ -31,7 +20,7 @@ FWD_CASES = [(300, 512, 64, 1.0), (2048, 512, 128, 1.0), (1000, 200, 192, 1.0), 
 
 @pytest.mark.parametrize("M,N,K,amp", FWD_CASES)
 def test_fp16_forward_and_dx_against_fp64(dev, M, N, K, amp):
-    ops = _ops()
+    ops = ops_for()
     x = (torch.randn(M, K, generator=g(270)) * amp).to(dev)
     W = (torch.randn(N, K, generator=g(271)) / math.sqrt(K)).to(dev).contiguous()
     b = (torch.randn(N, generator=g(272)) * 0.1 * amp).to(dev)
@@ -81,9 +70,9 @@ def test_fp16_dw_against_fp64(dev, M, N, K, sz, sx):
     dz = (torch.randn(M, N, generator=g(275)) * sz).to(dev)
     x = (torch.nn.functional.elu(torch.randn(M, K, generator=g(276))) * sx).to(dev)
     bounds = (float(dz.abs().max()), float(x.abs().max()))
-    dw = _dw(dev, dz, x, bounds)
+    dw = tc_dw(dev, dz, x, bounds)
     ref = dz.double().t() @ x.double()
     top = float((dz.double().abs().t() @ x.double().abs()).max())
     err = float((dw.double() - ref).abs().max())
     assert err < 3e-6 * top, (err, top)
-    assert torch.equal(dw, _dw(dev, dz, x, bounds))
+    assert torch.equal(dw, tc_dw(dev, dz, x, bounds))

@@ -9,19 +9,9 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_gemm_pipeline import Registered, _ops, g
+from tests.device_harness import Registered, g, ops_for, tc_dev  # noqa: F401  (tc_dev: the `dev` fixture)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    ops = _ops()
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return d
 
 
 # many items per CTA; ragged N and K; M < 128 (one item); fewer items than SMs; a few more items than SMs
@@ -31,7 +21,7 @@ SHAPES = [(32768, 512, 512), (1000, 72, 200), (100, 128, 64), (4096, 256, 192), 
 @pytest.mark.parametrize("M,N,K", SHAPES)
 @pytest.mark.parametrize("form", ["fp16", "tf32"])
 def test_forward_epilogues_and_dx(dev, M, N, K, form):
-    ops = _ops()
+    ops = ops_for()
     eng = ops.GEMM_TC_3XTF32
     if form == "fp16" and K % 64 != 0:
         pytest.skip("the fp16 form takes K in multiples of 64")
@@ -81,7 +71,7 @@ def test_forward_epilogues_and_dx(dev, M, N, K, form):
 # split, 144 items on the H100's 132 SMs), one tile with ragged edges
 @pytest.mark.parametrize("M,N,K", [(32768, 512, 512), (32768, 512, 64), (17000, 512, 128), (2048, 1536, 1536), (1000, 72, 200)])
 def test_dw_with_device_sized_split_k(dev, M, N, K):
-    ops = _ops()
+    ops = ops_for()
     dz = (torch.randn(M, N, generator=g(50)) / M).to(dev)
     x = torch.randn(M, K, generator=g(51)).to(dev)
     W = (torch.randn(N, K, generator=g(52)) / math.sqrt(K)).to(dev)
@@ -97,7 +87,7 @@ def test_dw_with_device_sized_split_k(dev, M, N, K):
 
 @pytest.mark.parametrize("M,N,K", [(32768, 512, 512), (1000, 72, 200), (100, 128, 64)])
 def test_trace_shows_every_item_once_on_its_cta(dev, M, N, K):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(M, K, generator=g(60)).to(dev)
     W = (torch.randn(N, K, generator=g(61)) / math.sqrt(K)).to(dev).contiguous()
     b = (torch.randn(N, generator=g(62)) * 0.1).to(dev)

@@ -8,28 +8,9 @@ import numpy as np
 import pytest
 import torch
 
+from tests.device_harness import Registered, g, ops_for, tc_dev  # noqa: F401  (tc_dev: the `dev` fixture)
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def dev():
-    from sample_factory_b200 import ops
-
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return d
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    return ops
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 def torch_twins(w):
@@ -40,39 +21,11 @@ def torch_twins(w):
     return hi, lo
 
 
-class Registered:
-    """fp16 twins + transposed twins of W, bounds of x and dz, registered for the duration of a block"""
-
-    def __init__(self, W, x=None, dz=None):
-        ops = _ops()
-        self.W, self.x, self.dz = W, x, dz
-        self.twins = torch.empty(2 * W.numel(), dtype=torch.float16, device=W.device)
-        self.twinsT = torch.empty(2 * W.numel(), dtype=torch.float16, device=W.device)
-        ops.register_f16_twins(W.view(-1), self.twins)
-        ops.register_f16_transposed(W, self.twinsT)
-        self.bounds = []                                 # (the library keeps the bound's address: keep it alive)
-        for t in (x, dz):
-            if t is not None:
-                self.bounds.append(torch.full((1,), float(t.abs().max().item()), device=W.device))
-                ops.register_operand_bound(t, self.bounds[-1])
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        ops = _ops()
-        for t in (self.x, self.dz):
-            if t is not None:
-                ops.unregister_operand_bound(t)
-        ops.unregister_f16_transposed(self.W)
-        ops.unregister_f16_twins(self.W.view(-1))
-
-
 def test_fp16_form_reads_the_weight_twins(dev, monkeypatch):
     """Perturbing one element W[n][k] of the hi twin changes the forward output in column n only, and the same element
     of the transposed hi twin changes dX in column k only: the kernel's B operand is the twin, not a re-split of W."""
     monkeypatch.delenv("SFB200_CHECK_F16", raising=False)
-    ops = _ops()
+    ops = ops_for()
     M, N, K = 512, 256, 192
     x = torch.randn(M, K, generator=g(1)).to(dev)
     W = (torch.randn(N, K, generator=g(2)) / math.sqrt(K)).to(dev).contiguous()
@@ -125,7 +78,7 @@ def test_twins_follow_every_weight_write(dev):
     from sample_factory_b200.sampler import DeviceSampler
     from sample_factory_b200.trajectory import alloc_trajectory_tensors
 
-    ops = _ops()
+    ops = ops_for()
     N, T = 256, 8
     spec = ModelSpec(64, 8, [128, 128])
     for optimizer in ("adam", "lamb"):
@@ -175,7 +128,7 @@ def _fp64_forward(x, W, b, act):
 @pytest.mark.parametrize("M,N,K", [(300, 64, 64), (1000, 96, 192), (129, 200, 320), (4096, 512, 64)])
 @pytest.mark.parametrize("form", ["fp16", "tf32"])
 def test_forward_and_dx_pipeline_edges(dev, M, N, K, form):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(M, K, generator=g(20)).to(dev)
     W = (torch.randn(N, K, generator=g(21)) / math.sqrt(K)).to(dev).contiguous()
     b = (torch.randn(N, generator=g(22)) * 0.1).to(dev)
@@ -208,7 +161,7 @@ def test_forward_and_dx_pipeline_edges(dev, M, N, K, form):
 # dW = dz^T x on the tf32 form (both operands MN-major, split-K): one 32-k stage, odd stage counts, uneven last chunk
 @pytest.mark.parametrize("M,N,K", [(32, 64, 64), (96, 130, 40), (1000, 70, 200), (4000, 512, 64), (32768, 512, 512)])
 def test_dw_pipeline_edges(dev, M, N, K):
-    ops = _ops()
+    ops = ops_for()
     dz = (torch.randn(M, N, generator=g(30)) / M).to(dev)
     x = torch.randn(M, K, generator=g(31)).to(dev)
     W = (torch.randn(N, K, generator=g(32)) / math.sqrt(K)).to(dev)

@@ -12,25 +12,16 @@ import numpy as np
 import pytest
 import torch
 
+from tests.device_harness import ops_for
+
 pytestmark = pytest.mark.gpu
-
-
-def _ops():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    from sample_factory_b200 import ops
-
-    ops.bind_device(torch.device("cuda", 0))
-    if not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return ops
 
 
 @pytest.mark.parametrize("scale", [1.0, 1e-6, 300.0])
 @pytest.mark.parametrize("act", ["elu", "relu", "tanh", "none"])
 @pytest.mark.parametrize("M,A", [(32768, 8), (1000, 1), (4133, 8)])
 def test_partials_against_float64(M, A, act, scale):
-    ops = _ops()
+    ops = ops_for("3xtf32")
     dev = torch.device("cuda", 0)
     K = N = 512
     g = torch.Generator().manual_seed(M + 31 * A + 7 * len(act) + int(math.log10(scale) + 10))

@@ -2,53 +2,14 @@
 device sampler -- the plumbing of BASELINE.json config 1 (CartPole-v1, 64 envs).  The env here is a small CartPole
 re-implementation (gymnasium is not installed in this image); the check is semantic equivalence with the oracle's
 rollout over a CPU batched wrapper with the reference's auto-reset rule (make_env.py:89-94)."""
-import math
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import appo_oracle as O
+from tests.device_harness import MiniCartPole, make_cfg
 
 pytestmark = pytest.mark.gpu
-
-
-class _Space:
-    def __init__(self, shape=None, n=None, dtype=np.float32):
-        self.shape, self.dtype = shape, dtype
-        if n is not None:
-            self.n = n
-
-
-class MiniCartPole:
-    """classic cart-pole dynamics (Barto, Sutton & Anderson), float64 state, float32 observations"""
-
-    def __init__(self, max_steps=40):
-        self.observation_space = _Space(shape=(4,))
-        self.action_space = _Space(shape=(), n=2)
-        self.max_steps = max_steps
-        self.rng = np.random.RandomState(0)
-        self.s, self.t = None, 0
-
-    def reset(self, seed=None):
-        if seed is not None:
-            self.rng = np.random.RandomState(seed)
-        self.s = self.rng.uniform(-0.05, 0.05, size=4)
-        self.t = 0
-        return self.s.astype(np.float32), {}
-
-    def step(self, a):
-        x, xd, th, thd = self.s
-        f = 10.0 if a == 1 else -10.0
-        ct, st = math.cos(th), math.sin(th)
-        tmp = (f + 0.05 * thd * thd * st) / 1.1
-        tha = (9.8 * st - ct * tmp) / (0.5 * (4.0 / 3.0 - 0.1 * ct * ct / 1.1))
-        xa = tmp - 0.05 * tha * ct / 1.1
-        self.s = np.array([x + 0.02 * xd, xd + 0.02 * xa, th + 0.02 * thd, thd + 0.02 * tha])
-        self.t += 1
-        terminated = bool(abs(self.s[0]) > 2.4 or abs(self.s[2]) > 12 * math.pi / 180)
-        truncated = bool(self.t >= self.max_steps and not terminated)
-        return self.s.astype(np.float32), 1.0, terminated, truncated, {"t": self.t}
 
 
 class CpuBatched:
@@ -78,7 +39,6 @@ def test_host_env_rollout_matches_oracle():
     from sample_factory_b200.model import ModelSpec, PolicyModel
     from sample_factory_b200.sampler import DeviceSampler
     from sample_factory_b200.trajectory import alloc_for_spec
-    from tests.test_gpu_engine import make_cfg
 
     dev = torch.device("cuda", 0)
     ops.bind_device(dev)

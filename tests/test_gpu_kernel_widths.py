@@ -28,14 +28,10 @@ import torch
 
 from oracle import appo_oracle as O
 from tests import mixed_oracle as MO
+from tests.device_harness import DEV, g, masked_rows, ops_for, wide_tail
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "sample_factory_b200", "csrc", "build")
-DEV = torch.device("cuda", 0)
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 # ----------------------------------------------------------------------------------------------- the table
@@ -205,13 +201,6 @@ def test_every_instantiation_has_a_case():
 
 
 # ----------------------------------------------------------------------------------------------- helpers
-def _ops():
-    from sample_factory_b200 import ops
-
-    ops.bind_device(DEV)
-    return ops
-
-
 def _launched(fn):
     """the templated sfb kernels fn launches.  The profiler keeps only device records whose time stamps fall inside its
     capture window, so the window is padded on both sides.  fn is idempotent and launches at least one kernel: a
@@ -365,7 +354,7 @@ def _loss_reference(space, layout, expl, d):
 
 
 def _run_loss(space, layout, expl, valid, kernels):
-    ops = _ops()
+    ops = ops_for()
     d = _loss_inputs(space, layout, seed=7 * len(_lid(layout)) + MO.rows_of(_heads_of(space, layout)), valid=valid)
     heads = d["heads"]
     A = MO.rows_of(heads)
@@ -507,9 +496,7 @@ def test_loss_single_valid_row(space, layout, kernels):
 def test_heads_tail_wide(space, layout, mode, kernels):
     """sfb200_heads_tail_wide over stored rows: values against float64, actions bit-exact against the oracle's sampling
     of the same rows (Box actions up to the rounding of expf), log-probs against the oracle"""
-    from tests.test_gpu_wide_heads import _masked_rows, _tail
-
-    ops = _ops()
+    ops = ops_for()
     M, H = 300, 96
     gen = g(11 + len(_lid(layout)))
     h = torch.randn(M, H, generator=gen)
@@ -526,7 +513,7 @@ def test_heads_tail_wide(space, layout, mode, kernels):
         kw = dict(noise=eps.to(DEV), deterministic=det, continuous=True, act_dim=ad, adaptive_stddev=adaptive,
                   learned_log_std=None if adaptive else learned.to(DEV), tanh_scale=0.0 if adaptive else TS)
         res = []
-        _check_launched(lambda: res.append(_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, **kw)), kernels)
+        _check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, **kw)), kernels)
         v, act, lp, env = res[0]
         means = raw[:, :ad] if adaptive else torch.tanh(raw[:, :ad] / TS) * TS
         log_std = raw[:, ad:] if adaptive else learned.expand(M, ad)
@@ -546,13 +533,13 @@ def test_heads_tail_wide(space, layout, mode, kernels):
         logits = torch.randn(M, A, generator=gen) * 2
         logits[::17] *= 100.0                               # probabilities exactly 0
         q = torch.empty(M, A).exponential_(generator=gen)
-        mask = _masked_rows(M, A, 5) if mode == "mask" else None
+        mask = masked_rows(M, A, 5) if mode == "mask" else None
         ld = logits.clone().to(DEV)
         kw = dict(noise=q.to(DEV), mask=None if mask is None else mask.to(DEV), deterministic=det)
         if space == "tuple":
             kw["head_sizes"] = segs
         res = []
-        _check_launched(lambda: res.append(_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, **kw)), kernels)
+        _check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, **kw)), kernels)
         v, act, lp, env = res[0]
         assert torch.equal(ld.cpu(), logits)
         qq = torch.ones_like(q) if det else q
@@ -575,7 +562,7 @@ def test_heads_tail_wide(space, layout, mode, kernels):
 @pytest.mark.parametrize("layout,kernels", [pytest.param(*c, id=_lid(c[0])) for c in MIXED_TAIL_CASES])
 @pytest.mark.parametrize("deterministic", [False, True])
 def test_heads_tail_wide_mixed(layout, kernels, deterministic):
-    ops = _ops()
+    ops = ops_for()
     heads = list(layout)
     A, W = MO.rows_of(heads), MO.width_of(heads)
     M, H = 300, 64
@@ -639,7 +626,7 @@ def test_heads_tail_wide_mixed(layout, kernels, deterministic):
 def test_heads_forward(rows, H, ldh, A, mode, kernels):
     """sfb200_heads_forward: values and logits against float64, actions bit-exact against the oracle's sampling of the
     kernel's logits (ldh > H: rows that are not 16-byte aligned)"""
-    ops = _ops()
+    ops = ops_for()
     gen = g(rows + H + A)
     base = torch.randn(rows, ldh, generator=gen)
     h = base[:, ldh - H:]
@@ -688,7 +675,7 @@ def test_heads_forward(rows, H, ldh, A, mode, kernels):
 @pytest.mark.parametrize("rows,H,A,act,kernels", [pytest.param(*c, id=f"{c[0]}x{c[1]}-A{c[2]}-{c[3]}")
                                                   for c in BACKWARD_CASES])
 def test_heads_backward(rows, H, A, act, kernels):
-    ops = _ops()
+    ops = ops_for()
     gen = g(rows + H + A)
     pre = torch.randn(rows, H, generator=gen)
     fn = {"elu": torch.nn.functional.elu, "relu": torch.relu, "tanh": torch.tanh, "none": lambda t: t}[act]

@@ -10,34 +10,15 @@ import torch
 
 from oracle import appo_oracle as O
 
+from tests.device_harness import TOL, dev, g, ops_for  # noqa: F401  (dev: fixture)
+
 pytestmark = pytest.mark.gpu
-
-TOL = 1e-5
-
-
-@pytest.fixture(scope="module")
-def dev():
-    from sample_factory_b200 import ops
-
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    return d
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    return ops
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 # ----------------------------------------------------------------------------------------------- normalizers
 @pytest.mark.parametrize("rows,dim", [(1, 4), (257, 64), (1000, 27), (4096, 64)])
 def test_normalize_obs_bit_exact(dev, rows, dim):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(rows, dim, generator=g(0)) * 3 + 1
     mean = torch.randn(dim, generator=g(1), dtype=torch.float64)
     var = torch.rand(dim, generator=g(2), dtype=torch.float64) * 4 + 0.01
@@ -56,7 +37,7 @@ def test_normalize_obs_bit_exact(dev, rows, dim):
 
 @pytest.mark.parametrize("rows,dim", [(33, 1), (1056, 16), (135168, 64), (5000, 27), (300, 300)])
 def test_moments_and_merge(dev, rows, dim):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(rows, dim, generator=g(3)) * 2 + 5
     mean = torch.zeros(dim, dtype=torch.float64)
     var = torch.ones(dim, dtype=torch.float64)
@@ -79,7 +60,7 @@ def test_moments_and_merge(dev, rows, dim):
 
 def test_returns_normalizer_roundtrip(dev):
     """reference tests/algo/test_rms.py:11-68: normalize -> denormalize round trip (atol 1e-6 x scale)."""
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(100000, generator=g(4)) * 0.8 + 0.3
     mean = torch.tensor([0.25], dtype=torch.float64)
     var = torch.tensor([0.7], dtype=torch.float64)
@@ -101,7 +82,7 @@ def test_returns_normalizer_roundtrip(dev):
                                        (128, 64, 16, "none")])
 @pytest.mark.parametrize("engine", ["simt", "3xtf32"])
 def test_linear_act_forward(dev, M, N, K, act, engine):
-    ops = _ops()
+    ops = ops_for()
     if engine != "simt" and not ops.tc_available():
         pytest.skip("wgmma engine not built")
     x = torch.randn(M, K, generator=g(5))
@@ -119,7 +100,7 @@ def test_linear_act_forward(dev, M, N, K, act, engine):
 def test_tc_engine_precision_classes(dev):
     """wgmma engine: the 3xTF32 split must be fp32-grade (same error class as the exact-fp32 CUDA-core engine),
     the single-pass TF32 mode must be visibly coarser (proves the tensor-core path really ran and the split matters)."""
-    ops = _ops()
+    ops = ops_for()
     if not ops.tc_available():
         pytest.skip("wgmma engine not available")
     M, N, K = 2048, 512, 512
@@ -144,7 +125,7 @@ def test_fp16_split_engine_is_fp32_grade(dev, M, N, K, amp):
     """The fp16-split form of the 3-pass engine (registered fp16 weight twins + a registered activation bound): same
     accuracy class as 3xTF32 against fp64 -- forward (with bias / ELU), and dX through the transposed twins -- for
     activations of very different magnitudes (the bound sets the power-of-two operand shift) and a loose bound."""
-    ops = _ops()
+    ops = ops_for()
     if not ops.tc_available():
         pytest.skip("wgmma engine not available")
     x = (torch.randn(M, K, generator=g(170)) * amp).to(dev)
@@ -200,7 +181,7 @@ def test_fp16_split_engine_is_fp32_grade(dev, M, N, K, amp):
 
 
 def test_linear_out_bound(dev):
-    ops = _ops()
+    ops = ops_for()
     W = torch.randn(96, 40, generator=g(180)).to(dev)
     b = torch.randn(96, generator=g(181)).to(dev)
     inb = torch.full((1,), 5.0, device=dev)
@@ -229,7 +210,7 @@ def test_linear_out_bound(dev):
 
 def test_linear_forward_strided_input(dev):
     """The learner feeds obs[:, T] rows in place: x row stride != K."""
-    ops = _ops()
+    ops = ops_for()
     base = torch.randn(64, 9, 32, generator=g(8))
     x = base[:, 8]
     W = torch.randn(48, 32, generator=g(9)) / 6
@@ -246,7 +227,7 @@ def test_linear_forward_strided_input(dev):
                                             (8192, 128, 384, "relu")])
 @pytest.mark.parametrize("engine", ["simt", "3xtf32"])
 def test_linear_backward(dev, M, N, K, act_prev, engine):
-    ops = _ops()
+    ops = ops_for()
     if engine != "simt" and not ops.tc_available():
         pytest.skip("wgmma engine not built")
     dz = torch.randn(M, N, generator=g(10)) / M
@@ -280,7 +261,7 @@ def test_linear_backward(dev, M, N, K, act_prev, engine):
 # ----------------------------------------------------------------------------------------------- heads
 @pytest.mark.parametrize("rows,H,A", [(5, 64, 8), (4096, 512, 8), (1001, 96, 3), (257, 128, 17), (64, 512, 31)])
 def test_heads_forward_and_sampling(dev, rows, H, A):
-    ops = _ops()
+    ops = ops_for()
     h = torch.randn(rows, H, generator=g(13))
     Wv = torch.randn(1, H, generator=g(14)) / math.sqrt(H)
     bv = torch.randn(1, generator=g(15))
@@ -317,7 +298,7 @@ def test_heads_forward_and_sampling(dev, rows, H, A):
 def test_heads_action_mask_and_deterministic(dev, rows, H, A):
     """masked_softmax / masked_log_softmax sampling (action_distributions.py:84-95,135-143) incl. rows that allow nothing,
     and deterministic (argmax) actions (enjoy.py:165-171), through both heads entry points."""
-    ops = _ops()
+    ops = ops_for()
     h = torch.randn(rows, H, generator=g(113))
     Wv = torch.randn(1, H, generator=g(114)) / math.sqrt(H)
     bv = torch.randn(1, generator=g(115))
@@ -379,7 +360,7 @@ def test_heads_action_mask_and_deterministic(dev, rows, H, A):
 
 
 def test_heads_deterministic_continuous_and_mask_errors(dev):
-    ops = _ops()
+    ops = ops_for()
     rows, H, Ad = 300, 64, 5
     h = torch.randn(rows, H, generator=g(120)).to(dev)
     Wv = (torch.randn(1, H, generator=g(121)) / 8).to(dev)
@@ -405,7 +386,7 @@ def test_heads_deterministic_continuous_and_mask_errors(dev):
 
 def test_heads_philox_sampling_distribution(dev):
     """Production path: in-kernel Philox Exp(1) noise. Empirical action frequencies must match softmax(logits)."""
-    ops = _ops()
+    ops = ops_for()
     rows, H, A = 200000, 32, 8
     h = torch.zeros(rows, H)
     h[:, 0] = 1.0
@@ -432,7 +413,7 @@ def test_heads_philox_sampling_distribution(dev):
                                           (20011, 256, 8, "relu"), (16500, 128, 5, "tanh"), (16384, 512, 2, "elu"),
                                           (555, 300, 17, "tanh")])
 def test_heads_backward(dev, rows, H, A, act):
-    ops = _ops()
+    ops = ops_for()
     cfg = O.OracleCfg(nonlinearity=act)
     pre = torch.randn(rows, H, generator=g(19))
     h = O._act(cfg, pre)
@@ -467,7 +448,7 @@ def test_heads_backward(dev, rows, H, A, act):
 
 # ----------------------------------------------------------------------------------------------- sampler steps
 def test_sampler_pre_post_step_and_env(dev):
-    ops = _ops()
+    ops = ops_for()
     N, D, T, A = 300, 16, 5, 8
     obs = torch.randn(N, D, generator=g(24))
     mean = torch.randn(D, generator=g(25), dtype=torch.float64)
@@ -532,7 +513,7 @@ def test_sampler_pre_post_step_and_env(dev):
 
 
 def test_compute_valids(dev):
-    ops = _ops()
+    ops = ops_for()
     N, T = 200, 9
     pid = torch.randint(-1, 2, (N, T), generator=g(28), dtype=torch.int32)
     pver = torch.randint(0, 50, (N, T), generator=g(29)).float()
@@ -548,7 +529,7 @@ def test_compute_valids(dev):
 @pytest.mark.parametrize("N,T", [(7, 1), (257, 8), (4096, 32), (100, 50), (33, 128)])
 @pytest.mark.parametrize("bootstrap,denorm", [(False, False), (True, True)])
 def test_gae_returns(dev, N, T, bootstrap, denorm):
-    ops = _ops()
+    ops = ops_for()
     rewards = torch.randn(N, T, generator=g(30))
     dones = torch.rand(N, T, generator=g(31)) < 0.1
     time_outs = dones & (torch.rand(N, T, generator=g(32)) < 0.5)
@@ -577,7 +558,7 @@ def test_gae_returns(dev, N, T, bootstrap, denorm):
 
 @pytest.mark.parametrize("n,R", [(5, 2), (300, 8), (1024, 32), (50, 40)])
 def test_vtrace(dev, n, R):
-    ops = _ops()
+    ops = ops_for()
     cfg = O.OracleCfg(gamma=0.99, vtrace_rho=1.0, vtrace_c=0.9)
     ratio = torch.exp(torch.randn(n * R, generator=g(35)) * 0.3).clamp(0.05, 20)
     values = torch.randn(n * R, generator=g(36))
@@ -597,7 +578,7 @@ def test_vtrace(dev, n, R):
 @pytest.mark.parametrize("B,A,frac_invalid,kl_coeff", [(64, 8, 0.0, 0.0), (1000, 8, 0.2, 0.1), (32768, 8, 0.0, 0.0),
                                                        (777, 3, 0.3, 0.5), (513, 17, 0.1, 0.2)])
 def test_ppo_loss_fwd_bwd(dev, B, A, frac_invalid, kl_coeff, expl):
-    ops = _ops()
+    ops = ops_for()
     cfg = O.OracleCfg(num_actions=A, kl_loss_coeff=kl_coeff, ppo_clip_ratio=0.1, ppo_clip_value=0.2, exploration_loss=expl,
                       exploration_loss_coeff=0.003 if expl == "entropy" else 0.02)
     logits = (torch.randn(B, A, generator=g(39)) * 1.5).requires_grad_(True)
@@ -658,7 +639,7 @@ def test_ppo_loss_fwd_bwd(dev, B, A, frac_invalid, kl_coeff, expl):
 
 
 def test_action_ratio(dev):
-    ops = _ops()
+    ops = ops_for()
     B, A = 1000, 8
     logits = torch.randn(B, A, generator=g(48))
     actions = torch.randint(0, A, (B, 1), generator=g(49)).float()
@@ -672,7 +653,7 @@ def test_action_ratio(dev):
 # ----------------------------------------------------------------------------------------------- optimizer
 @pytest.mark.parametrize("n,max_norm", [(1000, 4.0), (300553, 4.0), (300553, 0.0), (4097, 1e-3)])
 def test_clip_adam_step(dev, n, max_norm):
-    ops = _ops()
+    ops = ops_for()
     p = torch.randn(n, generator=g(51))
     m = torch.zeros(n)
     v = torch.zeros(n)
@@ -703,7 +684,7 @@ def test_rnn_cell_forward_backward(dev, rnn_type, M, H, IN):
     """One recurrent step (cell kernels + the two gate GEMMs) against the oracle's written-out nn.GRU / nn.LSTM cell
     (oracle.rnn_cell, pinned to the reference's PackedSequence path by the tiny_gru / tiny_lstm goldens) incl. autograd
     gradients, with a reset mask on the outgoing state and carried gradients from a fictitious next step."""
-    ops = _ops()
+    ops = ops_for()
     ocfg = O.OracleCfg(obs_dim=IN, num_actions=4, encoder_mlp_layers=[IN], use_rnn=True, rnn_type=rnn_type, rnn_size=H)
     st = O.init_state(ocfg, seed=2)
     G = 4 if rnn_type == "lstm" else 3
@@ -771,7 +752,7 @@ def test_bptt_matches_loopy_torch_rnn(dev, T, N, D, random_dones, rnn_type, engi
     """The reference's own recurrent-core check (tests/algo/test_rnn.py:10-75: T in {5,27,37}, N in {1,64}, D in {1,10,42},
     dones every 7th step or random) against the device BPTT: a step-by-step torch nn.GRU / nn.LSTM loop that zeroes the
     state after a done is the ground truth for the forward outputs AND, through autograd, for every gradient."""
-    ops = _ops()
+    ops = ops_for()
     from sample_factory_b200.model import ModelSpec, PolicyModel
     from sample_factory_b200.rnn_core import RnnCore
 
@@ -830,7 +811,7 @@ def test_bptt_matches_loopy_torch_rnn(dev, T, N, D, random_dones, rnn_type, engi
 
 def test_bad_arguments_raise(dev):
     """Error behaviour: argument violations surface as Python exceptions carrying the library message."""
-    ops = _ops()
+    ops = ops_for()
     from sample_factory_b200._lib import SfbError
 
     x = torch.zeros(4, 4, device=dev)
@@ -846,7 +827,7 @@ def test_bad_arguments_raise(dev):
 def test_linear_heads_fused_matches_separate(dev, engine_name, M, K, N, A, act):
     """sfb200_linear_act_heads_forward + sfb200_heads_from_partials == sfb200_linear_act_forward + sfb200_heads_forward
     (same GEMM accumulators -> identical y; head dot products differ only in summation order) and == the oracle."""
-    ops = _ops()
+    ops = ops_for()
     engine = {"3xtf32": ops.GEMM_TC_3XTF32, "tf32": ops.GEMM_TC_TF32}[engine_name]
     P = ops.linear_heads_partials(N, A, engine)
     assert P == 2 * (N // 128), "fused path must cover these shapes on an H100"
@@ -923,7 +904,7 @@ def test_linear_heads_fused_matches_separate(dev, engine_name, M, K, N, A, act):
 
 def test_sampler_post_pre_step_fused_matches_separate(dev):
     """sfb200_sampler_post_pre_step == sfb200_sampler_post_step(t) then sfb200_sampler_pre_step(t+1), bit for bit."""
-    ops = _ops()
+    ops = ops_for()
     N, D, T = 1000, 64, 4
     mean = torch.randn(D, generator=g(70), dtype=torch.float64).to(dev)
     var = (torch.rand(D, generator=g(71), dtype=torch.float64) + 0.1).to(dev)
@@ -974,7 +955,7 @@ def test_sampler_post_pre_step_fused_matches_separate(dev):
 def test_heads_forward_continuous(dev, rows, H, Ad, adaptive, tanh_scale):
     """sfb200_heads_forward_continuous vs the oracle's ContinuousActionDistribution restatement (pinned to the reference
     by the tiny_gauss goldens): distribution parameters, sampled actions, log-probs."""
-    ops = _ops()
+    ops = ops_for()
     ocfg = O.OracleCfg(obs_dim=H, num_actions=Ad, encoder_mlp_layers=[], continuous=True, adaptive_stddev=adaptive,
                        continuous_tanh_scale=tanh_scale)
     n_lin = O.num_linear_action_outputs(ocfg)
@@ -1029,7 +1010,7 @@ def test_heads_forward_continuous(dev, rows, H, Ad, adaptive, tanh_scale):
 def test_ppo_loss_fwd_bwd_continuous(dev, B, Ad, adaptive, tanh_scale, frac_invalid, kl_coeff):
     """Gaussian PPO loss forward + backward vs autograd through the oracle's distribution formulas; the leaves are the
     distribution_linear outputs z (and the learned log-stddev vector when adaptive_stddev=False)."""
-    ops = _ops()
+    ops = ops_for()
     cfg = O.OracleCfg(num_actions=Ad, kl_loss_coeff=kl_coeff, ppo_clip_ratio=0.2, ppo_clip_value=0.2, continuous=True,
                       exploration_loss_coeff=0.003)
     n_lin = 2 * Ad if adaptive else Ad
@@ -1109,7 +1090,7 @@ def test_ppo_loss_fwd_bwd_continuous(dev, B, Ad, adaptive, tanh_scale, frac_inva
 def test_conv_head_forward_backward(dev, B, shape, arch, engine_name):
     """ConvHead (im2col + GEMM engine + col2im) vs torch.nn.functional.conv2d + autograd on the CPU (the arithmetic the
     reference's ConvEncoderImpl executes, model/encoder.py:88-118): features, conv weight / bias gradients."""
-    ops = _ops()
+    ops = ops_for()
     if engine_name != "simt" and not ops.tc_available():
         pytest.skip("wgmma engine not available")
     from sample_factory_b200.conv_encoder import ConvHead
@@ -1150,7 +1131,7 @@ def test_conv_head_forward_backward(dev, B, shape, arch, engine_name):
 
 def test_normalize_obs_uint8(dev):
     """uint8 observation rows: .float() -> scale -> running-mean-std (utils/normalize.py:40-67), bit-exact"""
-    ops = _ops()
+    ops = ops_for()
     rows, dim = 77, 4 * 12 * 12
     x = torch.randint(0, 256, (rows, dim), generator=g(160), dtype=torch.uint8)
     mean = torch.rand(dim, generator=g(161), dtype=torch.float64)
@@ -1184,7 +1165,7 @@ def test_normalize_obs_uint8(dev):
 def test_clip_lamb_step(dev):
     """sfb200_clip_lamb_step vs the oracle's restatement of algo/utils/optimizers.py (pinned by the tiny_lamb golden):
     three steps on a padded flat buffer with tensors of very different norms (trust ratio clamped at both ends)."""
-    ops = _ops()
+    ops = ops_for()
     shapes = [(64, 16), (64,), (5, 64), (5,), (1, 64), (1,)]
     numels = [int(np.prod(sh)) for sh in shapes]
     offs, off = [], 0
@@ -1235,7 +1216,7 @@ def test_clip_lamb_step(dev):
                                                           (4096, [3, 3, 3, 3, 3, 3, 3, 3], 0.1, 0.3), (513, [17, 2, 5], 0.3, 0.2)])
 def test_ppo_loss_fwd_bwd_tuple(dev, B, segs, frac_invalid, kl_coeff, expl):
     """Tuple-of-Discretes PPO loss forward + backward vs autograd through the oracle's TupleActionDistribution formulas"""
-    ops = _ops()
+    ops = ops_for()
     A = sum(segs)
     cfg = O.OracleCfg(num_actions=A, action_segments=list(segs), kl_loss_coeff=kl_coeff, ppo_clip_ratio=0.1,
                       ppo_clip_value=0.2, exploration_loss=expl, exploration_loss_coeff=0.003 if expl == "entropy" else 0.02)
@@ -1294,7 +1275,7 @@ def test_ppo_loss_fwd_bwd_tuple(dev, B, segs, frac_invalid, kl_coeff, expl):
 
 def test_heads_forward_tuple(dev):
     """Tuple heads: per-head sampling / log-prob sums vs the oracle, both the dot-product kernel and the from-partials one"""
-    ops = _ops()
+    ops = ops_for()
     rows, H, segs = 777, 96, [3, 2, 4]
     A = sum(segs)
     cfg = O.OracleCfg(num_actions=A, action_segments=segs)

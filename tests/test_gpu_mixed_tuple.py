@@ -8,23 +8,14 @@ import numpy as np
 import pytest
 import torch
 
-import tests.test_gpu_engine as E
 from oracle import appo_oracle as O
 from tests import mixed_oracle as MO
+from tests.device_harness import (DEV, ENGINES, build_case, discrete_cols, g, graphed_learner_matches_eager,
+                                  graphed_sampler_matches_eager, mixed_closed_loop_vs_oracle, mixed_rig, ops_for,
+                                  replay_learner, replay_sampler, sampled_feed)
+from tests.golden_utils import load_mixed_case
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    ops.bind_device(DEV)
-    return ops
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 def _model(heads, hidden=(64, 128), seed=0, obs_dim=16):
@@ -45,7 +36,7 @@ def _policy(model, engine, x, noise=None, deterministic=False):
     """forward_policy with sampling outputs; returns (plan, values, params, actions, log_prob, env actions, pv_out)"""
     from sample_factory_b200.policy import HeadsPlan, forward_policy
 
-    ops = _ops()
+    ops = ops_for()
     sp = model.spec
     M = x.shape[0]
     plan = HeadsPlan(model, engine, M)
@@ -90,7 +81,7 @@ WIDE = [[("discrete", 24), ("box", 8), ("discrete", 5)], [("box", 300), ("discre
                          [(h, "wide") for h in WIDE])
 @pytest.mark.parametrize("deterministic", [False, True])
 def test_mixed_tail_matches_torch(heads, path, deterministic):
-    ops = _ops()
+    ops = ops_for()
     if path == "partials" and not ops.tc_available():
         pytest.skip("wgmma engine not available")
     engine = ops.GEMM_TC_3XTF32 if path == "partials" else ops.GEMM_SIMT
@@ -109,7 +100,7 @@ def test_mixed_tail_matches_torch(heads, path, deterministic):
     # actions from the kernel's own params: Discrete indices bit-exact, Box values eps * std + mean up to the last bits
     # of expf (the stddev), means exactly in deterministic mode
     want_a = MO.mixed_sample(heads, params, noise, deterministic=deterministic)
-    dcols = _discrete_cols(heads)
+    dcols = discrete_cols(heads)
     assert torch.equal(actions[:, dcols], want_a[:, dcols])
     if deterministic:
         assert torch.equal(actions, want_a)
@@ -122,7 +113,7 @@ def test_mixed_tail_matches_torch(heads, path, deterministic):
 
 def test_mixed_philox_statistics():
     """Philox draws: categorical frequencies follow the softmax, (a - mean) / std of a Box member is N(0, 1) per dim"""
-    ops = _ops()
+    ops = ops_for()
     heads = [("discrete", 5), ("box", 3), ("discrete", 3)]
     model = _model(heads, seed=3)
     M = 1 << 16
@@ -156,7 +147,7 @@ def _torch_ppo(lp, lp_old, ent, kl, values, v_old, targets, adv, valids, c_ent, 
 @pytest.mark.parametrize("heads", NARROW + WIDE)
 @pytest.mark.parametrize("c_kl", [0.0, 0.05])
 def test_mixed_loss_and_ratio_match_autograd(heads, c_kl):
-    ops = _ops()
+    ops = ops_for()
     B = 600
     A = MO.rows_of(heads)
     gen = g(A)
@@ -229,201 +220,41 @@ CASES = {
 }
 
 
-def _build(case, N, T, st_seed, engine, graph=False):
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import ModelSpec, PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-
-    ops = _ops()
-    heads = CASES[case]["heads"]
-    kw = dict(rollout=T, recurrence=T if CASES[case]["kw"].get("with_vtrace") else 1, batch_size=N * T // 2,
-              num_batches_per_epoch=2, encoder_mlp_layers=[64, 128], obs_dim=24)
-    kw.update(CASES[case]["kw"])
-    ocfg = MO.MixedCfg(num_actions=MO.rows_of(heads), action_heads=heads, **kw)
-    MO.install()
-    st0 = O.init_state(ocfg, seed=st_seed)
-    cfg = E.make_cfg(ocfg)
-    spec = ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), [], ocfg.nonlinearity,
-                     action_heads=heads)
-    model = PolicyModel(spec, DEV)
-    model.load_state_dict(st0, strict=False)
-    traj = alloc_for_spec(spec, N, T, DEV)
-    tape = torch.randn(4 * T + 1, N, ocfg.obs_dim, generator=g(st_seed + 10)) * 1.3 - 0.1
-    env = TapeVecEnv(tape.to(DEV).contiguous(), ocfg.num_actions, action_heads=heads)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine], use_cuda_graph=graph)
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
-    return ocfg, st0, tape, cfg, model, traj, env, sampler, learner
-
-
-def _noise(heads, T, N, gen):
-    return torch.cat([torch.empty(T, N, n).exponential_(generator=gen) if k == "discrete" else
-                      torch.randn(T, N, n, generator=gen) for k, n in heads], 2)
-
-
-def _discrete_cols(heads):
-    cols, c = [], 0
-    for k, n in heads:
-        if k == "discrete":
-            cols.append(c)
-        c += 1 if k == "discrete" else n
-    return cols
-
-
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("case", list(CASES))
 def test_mixed_closed_loop_vs_oracle(case, engine):
     """sampler + learner for 3 iterations against the torch restatement on the same tape, noise and initial weights"""
-    ops = _ops()
-    E._need(engine)
-    N, T = 64, 8
-    ocfg, st0, tape, cfg, model, traj, env, sampler, learner = _build(case, N, T, 3, engine)
-    heads = ocfg.action_heads
-    assert (sampler.heads_plan.P > 0) == (case == "mixed_fused" and engine != "simt")
-    olearner = O.OracleLearner(ocfg, st0)
-    oenv = O.TapeVecEnv(tape, ocfg.num_actions)
-    olast = oenv.reset()
-    sampler.reset()
-    gen = g(21)
-    dcols = _discrete_cols(heads)
-    for it in range(3):
-        noise = _noise(heads, T, N, gen)
-        otraj = O.alloc_trajectories(ocfg, N)
-        olast = MO.rollout(ocfg, olearner.st, oenv, olast, otraj, noise, olearner.train_step)
-        sampler.noise = noise.to(DEV)
-        sampler.set_policy_version(learner.train_step)
-        sampler.rollout()
-        got = {k: v.cpu() for k, v in traj.items()}
-        assert torch.equal(got["actions"][:, :, dcols], otraj["actions"][:, :, dcols]), it
-        # Box actions eps * std + mean inherit the 1e-7-relative differences of the params
-        np.testing.assert_allclose(got["actions"].numpy(), otraj["actions"].numpy(), rtol=2e-5, atol=E.TOL)
-        for k in ["obs", "dones", "time_outs", "policy_id", "policy_version"]:
-            assert torch.equal(got[k], otraj[k]), k
-        np.testing.assert_allclose(got["rewards"].numpy(), otraj["rewards"].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["action_logits"].numpy(), otraj["action_logits"].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), otraj["values"][:, :-1].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), otraj["log_prob_actions"].numpy(), atol=E.TOL)
-        n0 = len(olearner.log)
-        olearner.train(otraj)
-        learner.train(traj)
-        log = learner.minibatch_log().numpy()
-        for j, d in enumerate(olearner.log[n0:]):
-            for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss"]:
-                assert abs(log[j, ops.LS[key]] - d[key]) < E.TOL, (it, j, key, log[j, ops.LS[key]], d[key])
-        sd = model.state_dict()
-        for k in O.param_names(ocfg):
-            np.testing.assert_allclose(sd[k].cpu().numpy(), olearner.st[k].numpy(), atol=2e-5, err_msg=k)
+    mixed_closed_loop_vs_oracle(CASES[case]["heads"], CASES[case]["kw"], engine,
+                                partials=case == "mixed_fused" and engine != "simt")
 
 
 @pytest.mark.parametrize("case", ["mixed", "wide_mixed"])
 def test_mixed_graphed_learner_and_sampler_match_eager(case):
-    ops = _ops()
-    from sample_factory_b200.learner import Learner
-
-    N, T = 64, 8
-    eng = "3xtf32" if ops.tc_available() else "simt"
-    _, _, _, _, modelA, trajA, _, samplerA, learnerA = _build(case, N, T, 5, eng)
-    _, _, _, cfgB, modelB, trajB, _, samplerB, _ = _build(case, N, T, 5, eng, graph=True)
-    assert samplerB.use_cuda_graph
-    cfgB.learner_cuda_graph = True
-    learnerB = Learner(cfgB, modelB, N, engine=ops.ENGINES[eng])
-    assert learnerB.use_graph
-    for smp in (samplerA, samplerB):
-        smp.reset()
-        smp.rollout()
-    for smp in (samplerA, samplerB):
-        smp.reset()
-        smp.step_counter.zero_()
-        smp.rollout()
-    torch.cuda.synchronize()
-    for k in trajA:
-        assert torch.equal(trajA[k], trajB[k]), f"graphed sampler differs from eager for {k}"
-    for it in range(3):
-        samplerA.set_policy_version(learnerA.train_step)
-        samplerA.rollout()
-        for k in trajA:
-            trajB[k].copy_(trajA[k])
-        learnerA.train(trajA)
-        learnerB.train(trajB)
-        torch.cuda.synchronize()
-        assert torch.equal(modelA.flat, modelB.flat), it
-        assert torch.equal(learnerA.minibatch_log(), learnerB.minibatch_log())
+    eng = "3xtf32" if ops_for().tc_available() else "simt"
+    heads, kw = CASES[case]["heads"], CASES[case]["kw"]
+    a = mixed_rig(heads, kw, 64, 8, 5, eng)[3]
+    b = mixed_rig(heads, kw, 64, 8, 5, eng, graph=True, learner_cuda_graph=True)[3]
+    assert b.sampler.use_cuda_graph
+    graphed_sampler_matches_eager(a, b)
+    graphed_learner_matches_eager(a, b, sampled_feed(a, b), iters=3)
 
 
 # ----------------------------------------------------------------------------------------------- reference fixtures
-def _build_fixture(name, engine):
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import ModelSpec, PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-    from tests.golden_utils import state_from
-    from tests.test_mixed_tuple_cpu import load_mixed_case
-
-    ops = _ops()
-    z, meta, ocfg = load_mixed_case(name)
-    cfg = E.make_cfg(ocfg)
-    spec = ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), [], ocfg.nonlinearity,
-                     action_heads=ocfg.action_heads)
-    model = PolicyModel(spec, DEV)
-    model.load_state_dict(state_from(z, "init/"), strict=False)
-    traj = alloc_for_spec(spec, meta["N"], ocfg.rollout, DEV)
-    env = TapeVecEnv(torch.from_numpy(z["tape"]).to(DEV).contiguous(), ocfg.num_actions, action_heads=ocfg.action_heads)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine])
-    learner = Learner(cfg, model, meta["N"], engine=ops.ENGINES[engine])
-    return z, meta, ocfg, model, traj, sampler, learner
-
-
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", ["tiny_mixed", "tiny_mixed_kl", "tiny_wide_mixed"])
 def test_mixed_rollout_matches_reference_golden(name, engine):
     """the sampler against the reference's own trajectories (same weights, tape and recovered per-member noise)"""
-    from tests.golden_utils import state_from
-
-    E._need(engine)
-    z, meta, ocfg, model, traj, sampler, _ = _build_fixture(name, engine)
-    dcols = _discrete_cols(ocfg.action_heads)
-    sampler.reset()
-    for it in range(meta["iters"]):
-        model.load_state_dict(state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/"), strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(DEV).contiguous()
-        sampler.rollout()
-        got = {k: v.cpu() for k, v in traj.items()}
-        ref = {k: torch.from_numpy(z[f"it{it}/traj/{k}"]) for k in ["obs", "actions", "action_logits", "log_prob_actions",
-                                                                    "values", "rewards", "dones", "time_outs"]}
-        for k in ["obs", "dones", "time_outs"]:
-            assert torch.equal(got[k].view(ref[k].shape), ref[k]), k
-        assert torch.equal(got["actions"][:, :, dcols], ref["actions"][:, :, dcols])          # Discrete indices
-        np.testing.assert_allclose(got["actions"].numpy(), ref["actions"].numpy(), rtol=2e-5, atol=E.TOL)
-        np.testing.assert_allclose(got["rewards"].numpy(), ref["rewards"].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["action_logits"].numpy(), ref["action_logits"].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), ref["values"][:, :-1].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), ref["log_prob_actions"].numpy(), atol=E.TOL)
+    case = load_mixed_case(name)
+    replay_sampler(case, build_case(case, engine), exact=("obs", "dones", "time_outs", "rewards", "actions"), states=False,
+                   discrete_cols=discrete_cols(case[2].action_heads))
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", ["tiny_mixed", "tiny_mixed_kl", "tiny_wide_mixed"])
 def test_mixed_learner_matches_reference_golden(name, engine):
     """Learner.train on the reference's trajectories: loss terms (1e-5) and post-Adam weights (2e-5)"""
-    from tests.golden_utils import state_from, traj_from
-
-    ops = _ops()
-    E._need(engine)
-    z, meta, ocfg, model, traj, _, learner = _build_fixture(name, engine)
-    for it in range(meta["iters"]):
-        E.upload_traj(traj, traj_from(z, it, ocfg))
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        log = learner.minibatch_log().numpy()
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=E.TOL, rtol=1e-5, err_msg=key)
-        got = model.state_dict()
-        for k, v in state_from(z, f"it{it}/state/").items():
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * E.TOL
-            np.testing.assert_allclose(got[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = load_mixed_case(name)
+    replay_learner(case, build_case(case, engine), prep=False)
 
 
 # ----------------------------------------------------------------------------------------------- host envs
@@ -529,7 +360,7 @@ def test_tuple_with_box_host_env_trains_and_enjoys(tmp_path):
     """Tuple(Discrete(4), Box(4)) CPU env through run_rl: the env receives (numpy integer, float32 ndarray[4]) per step,
     and the deterministic policy enjoy() loads from the checkpoint has learned both members (a random policy scores
     about -5 per 16-step episode, a perfect one 16)"""
-    _ops()
+    ops_for()
     MixedIdentityEnv.received.clear()
     cfg = _train("MixedIdentity-v0", lambda i: MixedIdentityEnv(), tmp_path, 60000)
     assert set(MixedIdentityEnv.received) == {(np.int32, np.dtype(np.float32), (4,))}
@@ -537,7 +368,7 @@ def test_tuple_with_box_host_env_trains_and_enjoys(tmp_path):
 
 
 def test_tuple_multi_agent_host_env_receives_member_batches(tmp_path):
-    _ops()
+    ops_for()
     MultiAgentMixedEnv.received.clear()
     _train("MixedIdentityMA-v0", lambda i: MultiAgentMixedEnv(), tmp_path, 2000)
     assert ("multi", np.dtype(np.int32), (2, 4)) in MultiAgentMixedEnv.received      # (step() checks the layout)
@@ -545,7 +376,7 @@ def test_tuple_multi_agent_host_env_receives_member_batches(tmp_path):
 
 def test_tuple_of_discrete_host_env_trains(tmp_path):
     """Tuple(Discrete(4), Discrete(3)) CPU env (rejected by the host adapter before): trains, and member 0 is learned"""
-    _ops()
+    ops_for()
     MixedIdentityEnv.received.clear()
     cfg = _train("TupleDiscrete-v0", lambda i: MixedIdentityEnv(discrete_only=True), tmp_path, 40000)
     assert MixedIdentityEnv.received and all(np.issubdtype(r[0], np.integer) for r in MixedIdentityEnv.received)

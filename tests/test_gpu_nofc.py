@@ -10,24 +10,15 @@ import torch
 import torch.nn.functional as F
 
 import tests.resnet_oracle as R
-import tests.test_gpu_engine as E
+from tests import dict_obs_oracle as DO
+from tests.device_harness import (ENGINES, TOL, MiniCartPole, build, build_case, check_finite, graphed_learner_matches_eager,
+                                  make_cfg, mixed_closed_loop_vs_oracle, need, replay_learner, replay_sampler, runner)
 from tests.golden_utils import load_case, state_from, traj_from
-from tests.test_gpu_host_env import MiniCartPole
 
 pytestmark = pytest.mark.gpu
 R.install()
 
 CASES = ["tiny_linear", "tiny_linear_box", "tiny_conv_nofc", "tiny_conv_nofc_gru", "tiny_resnet_nofc"]
-
-
-def _learner(ocfg, N, st0, tape, engine, **over):
-    from sample_factory_b200 import ops
-    from sample_factory_b200.learner import Learner
-
-    dev = torch.device("cuda", 0)
-    _, model, traj, _, sampler, _ = E.build(ocfg, N, st0, tape, dev, engine=engine)
-    cfg = E.make_cfg(ocfg, **over)
-    return model, traj, sampler, Learner(cfg, model, N, engine=ops.ENGINES[engine])
 
 
 def _upload(traj, src):
@@ -37,120 +28,76 @@ def _upload(traj, src):
         traj[k].copy_(v.view(traj[k].shape))
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", CASES)
 def test_sampler_matches_reference_golden(name, engine):
     """Discrete actions bit-exact, logits / values / log-probs (and Box actions) at 1e-5"""
-    E.test_rollout_matches_reference_golden(name, engine)
+    case = load_case(name)
+    replay_sampler(case, build_case(case, engine))
 
 
 def _learner_vs_golden(name, engine, graph=False, share_weights=True):
-    from sample_factory_b200 import ops
-
-    E._need(engine)
     z, meta, ocfg = load_case(name)
-    ocfg = dataclasses.replace(ocfg, actor_critic_share_weights=share_weights)
-    shuffle = "it0/mb_indices" in z.files
-    model, traj, _, learner = _learner(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]), engine,
-                                       shuffle_minibatches=shuffle, learner_cuda_graph=graph)
-    assert learner.use_graph == graph and learner.shuffle == shuffle
-    assert learner.heads_plan.P == 0 and not learner.heads_plan.separate
-    for it in range(meta["iters"]):
-        assert learner.train_step == int(z[f"it{it}/train_step_before"])
-        _upload(traj, traj_from(z, it, ocfg))
-        if shuffle:
-            learner.set_minibatch_permutation(z[f"it{it}/mb_indices"])
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        p = f"it{it}/prep/"
-        assert torch.equal(learner.valids_flat.view(-1).cpu(), torch.from_numpy(z[p + "valids"]))
-        np.testing.assert_allclose(traj["values"][:, -1].cpu().numpy(), z[p + "bootstrap_values"], atol=E.TOL)
-        np.testing.assert_allclose(learner.advantages.view(-1).cpu().numpy(), z[p + "advantages"], atol=E.TOL)
-        np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), z[p + "returns"], atol=E.TOL)
-        log = learner.minibatch_log().numpy()
-        assert log.shape[0] == len(z[f"it{it}/loss/policy_loss"])
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=E.TOL, rtol=1e-5, err_msg=key)
-        got = model.state_dict()
-        for k, v in R.post_state(z, it).items():
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * E.TOL
-            np.testing.assert_allclose(got[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = z, meta, dataclasses.replace(ocfg, actor_critic_share_weights=share_weights)
+    rig = build_case(case, engine, learner_cuda_graph=graph)
+    assert rig.learner.use_graph == graph
+    assert rig.learner.heads_plan.P == 0 and not rig.learner.heads_plan.separate
+    replay_learner(case, rig, upload=_upload, state_of=R.post_state)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", CASES)
 def test_learner_matches_reference_golden(name, engine):
     """returns, advantages, losses at 1e-5, post-Adam weights at 2e-5, normaliser statistics"""
     _learner_vs_golden(name, engine)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", ["tiny_linear_box", "tiny_conv_nofc_gru"])
 def test_graphed_learner_matches_reference_golden(name, engine):
     """the same with train() as one CUDA graph (the one-epoch fixtures; tiny_linear_box's second iteration replays it)"""
     _learner_vs_golden(name, engine, graph=True)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", ["tiny_linear", "tiny_conv_nofc", "tiny_resnet_nofc"])
 def test_graphed_learner_matches_eager(name, engine):
     """graph replay bit-identical to launch-by-launch training, four calls (capture, then replays)"""
-    E._need(engine)
     z, meta, ocfg = load_case(name)
     ocfg = dataclasses.replace(ocfg, num_epochs=1)
     st0, tape = state_from(z, "init/"), torch.from_numpy(z["tape"])
-    modelA, trajA, _, learnerA = _learner(ocfg, meta["N"], st0, tape, engine)
-    modelB, trajB, _, learnerB = _learner(ocfg, meta["N"], st0, tape, engine, learner_cuda_graph=True)
-    assert learnerB.use_graph and not learnerA.use_graph
-    for it in range(4):
-        _upload(trajA, traj_from(z, it % meta["iters"], ocfg))
-        _upload(trajB, traj_from(z, it % meta["iters"], ocfg))
-        learnerA.train(trajA)
-        learnerB.train(trajB)
-        torch.cuda.synchronize()
-        assert torch.equal(modelA.flat, modelB.flat), it
-        assert torch.equal(learnerA.minibatch_log(), learnerB.minibatch_log())
-    assert learnerB.graph_replay_launches > 0
+    a = build(ocfg, meta["N"], st0, tape, engine)
+    b = build(ocfg, meta["N"], st0, tape, engine, learner_cuda_graph=True)
+
+    def feed(it):
+        for rig in (a, b):
+            _upload(rig.traj, traj_from(z, it % meta["iters"], ocfg))
+    graphed_learner_matches_eager(a, b, feed)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_dict_identity_matches_reference_golden(engine):
     """identity key encoders, no core / decoder: the heads read the packed normalised row (sampler; learner eager and as
     one CUDA graph, whose second iteration replays it)"""
-    import tests.test_gpu_dict_obs as D
+    need(engine)
+    case = DO.load_dict_case("tiny_dict_identity")
+    replay_sampler(case, build_case(case, engine), exact=("obs", "dones", "rewards", "actions"))
+    for graph in (False, True):
+        rig = build_case(case, engine, learner_cuda_graph=graph)
+        assert rig.learner.use_graph == graph
+        replay_learner(case, rig, traj_of=DO.traj_from)
 
-    E._need(engine)
-    D.test_sampler_matches_reference_golden("tiny_dict_identity", engine)
-    D._learner_vs_golden("tiny_dict_identity", engine, graph=False)
-    D._learner_vs_golden("tiny_dict_identity", engine, graph=True)
 
-
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_separate_identity_towers_match_reference_golden(engine):
     """ActorCriticSeparateWeights with identity towers has the parameters of the shared identity model: the tiny_linear
     fixture holds for it too (sampler and learner), with a state row of two placeholders"""
-    E._need(engine)
-    dev = torch.device("cuda", 0)
     z, meta, ocfg = load_case("tiny_linear")
-    ocfg = dataclasses.replace(ocfg, actor_critic_share_weights=False)
-    cfg, model, traj, _, sampler, _ = E.build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]), dev,
-                                              engine=engine)
-    assert model.spec.rnn_state_size == 2 and not sampler.heads_plan.separate
-    sampler.reset()
-    for it in range(meta["iters"]):
-        st = state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/")
-        model.load_state_dict(st, strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(dev).contiguous()
-        sampler.rollout()
-        ref = lambda k: z[f"it{it}/traj/{k}"]     # noqa: E731
-        assert np.array_equal(traj["actions"].cpu().numpy().reshape(ref("actions").shape), ref("actions"))
-        for k in ["action_logits", "log_prob_actions"]:
-            np.testing.assert_allclose(traj[k].cpu().numpy(), ref(k), atol=E.TOL, err_msg=k)
-        np.testing.assert_allclose(traj["values"][:, :-1].cpu().numpy(), ref("values")[:, :-1], atol=E.TOL)
+    case = z, meta, dataclasses.replace(ocfg, actor_critic_share_weights=False)
+    rig = build_case(case, engine)
+    assert rig.model.spec.rnn_state_size == 2 and not rig.sampler.heads_plan.separate
+    replay_sampler(case, rig, exact=("actions",), states=False)
     _learner_vs_golden("tiny_linear", engine, share_weights=False)
-
 
 
 # ----------------------------------------------------------------------------------------------- heads on conv features
@@ -172,7 +119,7 @@ FEATURE_CASES = {
 _RESNET_STAGE0 = "ResNet stage-0 conv gradients at 32 rows of [4,84,84]: up to 6e-4 relative off float64, cause open"
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("case,conv_params", [("atari_narrow", True), ("atari_wide", True), ("resnet_narrow", False),
                                               pytest.param("resnet_narrow", True, marks=pytest.mark.xfail(
                                                   reason=_RESNET_STAGE0, strict=False))])
@@ -186,7 +133,7 @@ def test_heads_on_conv_features_match_torch_autograd(case, conv_params, engine):
     from sample_factory_b200.policy import forward_policy
     from oracle import appo_oracle as O
 
-    E._need(engine)
+    need(engine)
     c = FEATURE_CASES[case]
     dev = torch.device("cuda", 0)
     ops.bind_device(dev)
@@ -202,7 +149,7 @@ def test_heads_on_conv_features_match_torch_autograd(case, conv_params, engine):
     ocfg = O.OracleCfg(obs_dim=D, num_actions=A, rollout=1, recurrence=1, batch_size=B, num_batches_per_epoch=1,
                        encoder_mlp_layers=[], nonlinearity=c["act"], obs_shape=shape,
                        encoder_conv_architecture=c["arch"], encoder_conv_mlp_layers=[])
-    learner = Learner(E.make_cfg(ocfg), model, B, engine=ops.ENGINES[engine])
+    learner = Learner(make_cfg(ocfg), model, B, engine=ops.ENGINES[engine])
     assert learner.heads_plan.P == 0 and learner.heads_plan.wide == c["wide"]
     gen = torch.Generator().manual_seed(7)
     x = torch.randn(B, D, generator=gen).clamp_(-5, 5)
@@ -287,7 +234,7 @@ def _closed_loop_cfg(case):
                              encoder_conv_mlp_layers=[], adam_eps=1e-5, max_grad_norm=0.5, **common), (4, 84, 84)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("case", ["tuple_linear", "wide_linear", "atari6_nofc", "atari18_nofc"])
 def test_closed_loop_vs_oracle(case, engine):
     """sampler + learner for two iterations against the CPU oracle on the same tape, noise and initial weights: a Tuple
@@ -296,7 +243,7 @@ def test_closed_loop_vs_oracle(case, engine):
     from sample_factory_b200 import ops
     from oracle import appo_oracle as O
 
-    E._need(engine)
+    need(engine)
     dev = torch.device("cuda", 0)
     N, T, ocfg, image = _closed_loop_cfg(case)
     st0 = O.init_state(ocfg, seed=3)
@@ -305,7 +252,7 @@ def test_closed_loop_vs_oracle(case, engine):
         tape = torch.randint(0, 256, (2 * T + 1, N, ocfg.obs_dim), dtype=torch.uint8, generator=gen)
     else:
         tape = torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=gen) * 1.2 - 0.2
-    cfg, model, traj, env, sampler, learner = E.build(ocfg, N, st0, tape, dev, engine=engine)
+    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, engine)
     assert model.spec.wide_heads == (case in ("wide_linear", "atari18_nofc"))
     olearner = O.OracleLearner(ocfg, st0)
     oenv = O.TapeVecEnv(tape, ocfg.num_actions)
@@ -326,34 +273,31 @@ def test_closed_loop_vs_oracle(case, engine):
         # differences allowed below: relative 1e-4 on top of the 1e-5
         rtol = 1e-4 if (image and it > 0) else 1e-7
         for k in ["action_logits", "log_prob_actions"]:
-            np.testing.assert_allclose(got[k].numpy(), otraj[k].numpy(), atol=E.TOL, rtol=rtol, err_msg=k)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), otraj["values"][:, :-1].numpy(), atol=E.TOL, rtol=rtol)
+            np.testing.assert_allclose(got[k].numpy(), otraj[k].numpy(), atol=TOL, rtol=rtol, err_msg=k)
+        np.testing.assert_allclose(got["values"][:, :-1].numpy(), otraj["values"][:, :-1].numpy(), atol=TOL, rtol=rtol)
         n0 = len(olearner.log)
         buff = olearner.train(otraj)
         learner.train(traj)
-        np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), buff["returns"].numpy(), atol=E.TOL)
+        np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), buff["returns"].numpy(), atol=TOL)
         log = learner.minibatch_log().numpy()
         for j, d in enumerate(olearner.log[n0:]):
             for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss"]:
-                assert abs(log[j, ops.LS[key]] - d[key]) < E.TOL, (it, j, key, log[j, ops.LS[key]], d[key])
+                assert abs(log[j, ops.LS[key]] - d[key]) < TOL, (it, j, key, log[j, ops.LS[key]], d[key])
         sd = model.state_dict()
         # post-Adam weights: 2e-5 as for the fixtures; conv weights under 3xTF32 at 5e-5 (an element whose gradient is of
         # the order of adam_eps moves by lr * g / (|g| + eps), which turns the engine's 1e-7-level gradient differences
         # into up to 4.0e-5 on 2 of 8192 conv_head.0 weights after four steps with 18 actions)
-        wtol = 5 * E.TOL if (image and engine != "simt") else 2 * E.TOL
+        wtol = 5 * TOL if (image and engine != "simt") else 2 * TOL
         for k in O.param_names(ocfg):
             np.testing.assert_allclose(sd[k].cpu().numpy(), olearner.st[k].numpy(), atol=wtol, err_msg=k)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
-def test_mixed_tuple_linear_closed_loop_vs_oracle(engine, monkeypatch):
+@pytest.mark.parametrize("engine", ENGINES)
+def test_mixed_tuple_linear_closed_loop_vs_oracle(engine):
     """Tuple(Discrete(3), Box(2), Discrete(4)) on the normalised observation (no MLP layer): the mixed-Tuple closed loop
     of test_gpu_mixed_tuple.py with encoder_mlp_layers=[]"""
-    import tests.test_gpu_mixed_tuple as M
-
-    monkeypatch.setitem(M.CASES, "mixed_linear", dict(heads=M.CASES["mixed"]["heads"],
-                                                      kw=dict(M.CASES["mixed"]["kw"], encoder_mlp_layers=[])))
-    M.test_mixed_closed_loop_vs_oracle("mixed_linear", engine)
+    mixed_closed_loop_vs_oracle([("discrete", 3), ("box", 2), ("discrete", 4)],
+                                dict(exploration_loss_coeff=0.01, encoder_mlp_layers=[]), engine, partials=False)
 
 # ----------------------------------------------------------------------------------------------- full size
 # learner (8192 rows: im2col scratch of the three convs, their outputs and gradients, the features and their gradient,
@@ -367,14 +311,12 @@ def test_config4_stack_without_fc_layer_1024_envs():
     minibatches of 8192) with --encoder_conv_mlp_layers empty: three iterations through the public Runner, the heads on
     the 3136 conv features"""
     from sample_factory_b200.envs import TapeVecEnv
-    from tests.test_gpu_configs import _check_finite, _runner
-
     dev = torch.device("cuda", 0)
     N, T = 1024, 32
     torch.cuda.reset_peak_memory_stats()
     tape = torch.randint(0, 256, (T + 1, N, 4 * 84 * 84), dtype=torch.uint8,
                          generator=torch.Generator().manual_seed(1)).to(dev)
-    r = _runner("synthetic_atari_nofc", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
+    r = runner("synthetic_atari_nofc", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
                 ["--use_rnn=False", "--async_rl=False", f"--rollout={T}", "--recurrence=1", "--batch_size=8192",
                  "--num_batches_per_epoch=4", "--num_epochs=4", "--encoder_conv_architecture=convnet_atari",
                  "--encoder_conv_mlp_layers", "--nonlinearity=relu", "--obs_scale=255.0",
@@ -383,7 +325,7 @@ def test_config4_stack_without_fc_layer_1024_envs():
     assert sp.fc_encoder_layers == [] and sp.tail_input_size == 3136 and not sp.wide_heads
     key = "encoder.encoders.obs.enc.conv_head.0.weight"
     before = r.model.params[key].clone()
-    _check_finite(r, 3, 3 * N * T)
+    check_finite(r, 3, 3 * N * T)
     assert not torch.equal(before, r.model.params[key])
     peak = torch.cuda.max_memory_allocated()
     print(f"convnet_atari without FC, 1024 envs x 32, batch 8192: peak allocated {peak / 2 ** 30:.2f} GiB")

@@ -9,31 +9,13 @@ import torch
 import torch.nn.functional as F
 
 import tests.resnet_oracle as R
-import tests.test_gpu_engine as E
 from oracle import appo_oracle as O
+from tests.device_harness import (ENGINES, build, build_case, check_finite, dev, g, graphed_learner_matches_eager, ops_for,
+                                  replay_learner, replay_sampler, runner, upload_traj)
 from tests.golden_utils import load_case, state_from, traj_from
 
 pytestmark = pytest.mark.gpu
 R.install()
-
-
-@pytest.fixture(scope="module")
-def dev():
-    from sample_factory_b200 import ops
-
-    d = torch.device("cuda", 0)
-    ops.bind_device(d)
-    return d
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    return ops
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 def _act_cpu(name, x):
@@ -55,7 +37,7 @@ def _nchw(rows, B, C, H, W):
 def test_im2col_pad_act_matches_unfold(dev, act, nchw, B, C, H, W, stride):
     """col = im2col(act(x)) with padding 1 == F.unfold(act(x), 3, padding=1), bit for bit (act evaluated by torch on the
     device: the same expm1f / fmaxf the kernel applies)"""
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(B, C, H, W, generator=g(1)) * 2
     xa = _act_cpu(act, x.to(dev)).cpu()
     ref = F.unfold(xa, 3, padding=1, stride=stride).transpose(1, 2).reshape(-1, C * 9)
@@ -90,7 +72,7 @@ def _pool_device(ops, x, dev):
 @pytest.mark.parametrize("B,C,H,W", [(2, 16, 22, 22), (3, 32, 11, 11), (2, 5, 6, 9), (1, 3, 1, 1)])
 def test_maxpool_forward_matches_torch(dev, B, C, H, W):
     """values and selected positions bit for bit, with many ties (3 distinct values) and -inf regions"""
-    ops = _ops()
+    ops = ops_for()
     x = torch.randint(0, 3, (B, C, H, W), generator=g(2)).float()
     x[0, 0, : min(H, 3), : min(W, 3)] = float("-inf")      # a window of -inf only: the first in-bounds element is chosen
     if B > 1:
@@ -102,7 +84,7 @@ def test_maxpool_forward_matches_torch(dev, B, C, H, W):
 
 
 def test_maxpool_forward_nan_propagates(dev):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randn(2, 4, 9, 9, generator=g(4))
     x[0, 1, 4, 4] = float("nan")
     x[1, 2, 0, 0] = float("nan")
@@ -115,7 +97,7 @@ def test_maxpool_forward_nan_propagates(dev):
 
 @pytest.mark.parametrize("B,C,H,W", [(2, 16, 22, 22), (3, 32, 11, 11), (2, 7, 5, 8)])
 def test_maxpool_backward_matches_autograd(dev, B, C, H, W):
-    ops = _ops()
+    ops = ops_for()
     x = torch.randint(0, 4, (B, C, H, W), generator=g(5)).float()
     x[0] = torch.randn(C, H, W, generator=g(6))
     x.requires_grad_(True)
@@ -139,7 +121,7 @@ def _act_grad_cpu(name, z):
 @pytest.mark.parametrize("from_input,residual", [(True, True), (True, False), (False, False)])
 def test_col2im_pad_act_backward(dev, act, from_input, residual):
     """dx = col2im(dcol) * act'(x) (+ dres) against F.fold and autograd's act'"""
-    ops = _ops()
+    ops = ops_for()
     B, C, H, W = 3, 16, 11, 9
     dcol = torch.randn(B * H * W, C * 9, generator=g(8))
     z = torch.randn(B, C, H, W, generator=g(9))
@@ -159,9 +141,7 @@ def test_col2im_pad_act_backward(dev, act, from_input, residual):
 @pytest.mark.parametrize("M,N,K", [(1000, 16, 144), (300, 32, 288), (4099, 32, 288), (77, 16, 27)])
 def test_linear_residual_forward(dev, engine, M, N, K):
     """y = x W^T + b + r in both GEMM engines (K = 27: the 3-channel first conv, which the wgmma engine hands to SIMT)"""
-    ops = _ops()
-    if engine != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
+    ops = ops_for(engine)
     x = torch.randn(M, K, generator=g(11))
     Wt = torch.randn(N, K, generator=g(12)) / K ** 0.5
     b = torch.randn(N, generator=g(13))
@@ -180,9 +160,7 @@ def test_resnet_head_forward_backward(dev, B, shape, act, engine_name):
     """ResnetHead vs the ResnetEncoder's arithmetic (oracle.encoder_forward's structure) under CPU autograd: features and
     every conv weight / bias gradient, at the tolerances of the plain conv head's test (scaled by the magnitude of the
     reference values, which grow along the residual stream)"""
-    ops = _ops()
-    if engine_name != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
+    ops = ops_for(engine_name)
     from sample_factory_b200.conv_encoder import ResnetHead
     from sample_factory_b200.model import ModelSpec, PolicyModel
 
@@ -225,9 +203,10 @@ def test_resnet_head_forward_backward(dev, B, shape, act, engine_name):
 
 
 # ----------------------------------------------------------------------------------------------- reference fixture
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_rollout_matches_reference_golden_resnet(engine):
-    E.test_rollout_matches_reference_golden("tiny_resnet", engine)
+    case = load_case("tiny_resnet")
+    replay_sampler(case, build_case(case, engine))
 
 
 # One loss term exceeds the shared check's budget under 3xTF32 and stays at that tolerance, marked as an expected failure
@@ -243,53 +222,34 @@ _VALUE_LOSS_3XTF32 = "3xTF32 value_loss of minibatch 2 is 1.83e-5 off (allowed 1
                                                                                                   strict=False))])
 def test_learner_matches_reference_golden_resnet(engine):
     """returns, advantages, loss terms and normaliser statistics (the shared check) ..."""
-    E.test_learner_matches_reference_golden("tiny_resnet", engine)
+    case = load_case("tiny_resnet")
+    replay_learner(case, build_case(case, engine), rewards=True)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_learner_weights_match_reference_golden_resnet(engine):
     """... and the post-Adam weights, which the fixture stores as float16 differences from the initial weights (<= 2e-7
     of rounding), at the shared check's 2e-5"""
-    E._need(engine)
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = load_case("tiny_resnet")
-    _, model, traj, _, _, learner = E.build(ocfg, meta["N"], state_from(z, "init/"), torch.from_numpy(z["tape"]), dev,
-                                            engine=engine)
-    E.upload_traj(traj, traj_from(z, 0, ocfg))
-    learner.train(traj)
-    torch.cuda.synchronize()
-    ref, got = R.post_state(z, 0), model.state_dict()
-    for k in O.param_names(ocfg):
-        np.testing.assert_allclose(got[k].cpu().numpy(), ref[k].numpy(), atol=2 * E.TOL, rtol=1e-6, err_msg=k)
+    case = load_case("tiny_resnet")
+    names = O.param_names(case[2])
+    replay_learner(case, build_case(case, engine), prep=False, losses=False,
+                   state_of=lambda z, it: {k: v for k, v in R.post_state(z, it).items() if k in names})
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_graphed_learner_matches_eager_resnet(engine):
     """the resnet learner replayed as one CUDA graph is bit-identical to the launch-by-launch learner"""
-    from sample_factory_b200 import ops
-    from sample_factory_b200.learner import Learner
-
-    E._need(engine)
-    dev = torch.device("cuda", 0)
     z, meta, ocfg = load_case("tiny_resnet")
     tape = torch.from_numpy(z["tape"])
     st0 = state_from(z, "init/")
     ocfg = dataclasses.replace(ocfg, num_epochs=1)     # (the learner's graph covers one epoch per train() call)
-    _, modelA, trajA, _, _, learnerA = E.build(ocfg, meta["N"], st0, tape, dev, engine=engine)
-    cfgB, modelB, trajB, _, _, _ = E.build(ocfg, meta["N"], st0, tape, dev, engine=engine)
-    cfgB.learner_cuda_graph = True
-    learnerB = Learner(cfgB, modelB, meta["N"], engine=ops.ENGINES[engine])
-    assert learnerB.use_graph and not learnerA.use_graph
-    for it in range(4):      # (the first call captures the graph, later calls replay it)
-        E.upload_traj(trajA, traj_from(z, it % meta["iters"], ocfg))
-        E.upload_traj(trajB, traj_from(z, it % meta["iters"], ocfg))
-        learnerA.train(trajA)
-        learnerB.train(trajB)
-        torch.cuda.synchronize()
-        assert torch.equal(modelA.flat, modelB.flat), it
-        assert torch.equal(modelA.exp_avg_sq, modelB.exp_avg_sq)
-        assert torch.equal(learnerA.minibatch_log(), learnerB.minibatch_log())
-    assert learnerB.graph_replay_launches > 0
+    a = build(ocfg, meta["N"], st0, tape, engine)
+    b = build(ocfg, meta["N"], st0, tape, engine, learner_cuda_graph=True)
+
+    def feed(it):      # (the first call captures the graph, later calls replay it)
+        for r in (a, b):
+            upload_traj(r.traj, traj_from(z, it % meta["iters"], ocfg))
+    graphed_learner_matches_eager(a, b, feed, exp_avg_sq=True)
 
 
 # ----------------------------------------------------------------------------------------------- full size
@@ -302,13 +262,11 @@ def test_resnet_atari_1024_envs():
     """uint8 [4,84,84] frames, resnet_impala + FC 512, ReLU, 1024 envs, rollout 16, batch 4096, learner as a CUDA graph:
     two iterations through the public Runner"""
     from sample_factory_b200.envs import TapeVecEnv
-    from tests.test_gpu_configs import _check_finite, _runner
-
     dev = torch.device("cuda", 0)
     N, T = 1024, 16
     torch.cuda.reset_peak_memory_stats()
     tape = torch.randint(0, 256, (T + 1, N, 4 * 84 * 84), dtype=torch.uint8, generator=g(1)).to(dev)
-    r = _runner("synthetic_atari_resnet", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
+    r = runner("synthetic_atari_resnet", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 6, obs_shape=(4, 84, 84)),
                 ["--use_rnn=False", "--async_rl=False", f"--rollout={T}", "--recurrence=1", "--batch_size=4096",
                  "--num_batches_per_epoch=4", "--num_epochs=1", "--encoder_conv_architecture=resnet_impala",
                  "--encoder_conv_mlp_layers", "512", "--nonlinearity=relu", "--obs_scale=255.0",
@@ -317,7 +275,7 @@ def test_resnet_atari_1024_envs():
     assert sp.is_resnet and sp.conv_out_size == 32 * 11 * 11 and r.learner.use_graph
     key = "encoder.encoders.obs.conv_head.0.weight"
     before = r.model.params[key].clone()
-    _check_finite(r, 2, 2 * N * T)
+    check_finite(r, 2, 2 * N * T)
     assert not torch.equal(before, r.model.params[key])
     peak = torch.cuda.max_memory_allocated()
     print(f"resnet_impala 1024 envs x 16, batch 4096: peak allocated {peak / 2 ** 30:.2f} GiB")

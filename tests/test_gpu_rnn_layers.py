@@ -9,48 +9,10 @@ import torch
 
 from oracle import appo_oracle as O
 from tests import rnn_layers_oracle as RO
-from tests.golden_utils import state_from, traj_from
-from tests.test_gpu_engine import make_cfg
+from tests.device_harness import (DEV, ENGINES, TOL, build, build_case, check_finite, graphed_learner_matches_eager,
+                                  make_cfg, model_spec, ops_for, replay_learner, replay_sampler, runner)
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-ENGINES = ["simt", "3xtf32"]
-
-
-def _ops(engine="simt"):
-    from sample_factory_b200 import ops
-
-    ops.bind_device(torch.device("cuda", 0))
-    if engine != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return ops
-
-
-def _spec(ocfg, **kw):
-    from sample_factory_b200.model import ModelSpec
-
-    return ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), list(ocfg.decoder_mlp_layers),
-                     ocfg.nonlinearity, ocfg.normalize_input, ocfg.normalize_returns, ocfg.obs_subtract_mean,
-                     ocfg.obs_scale, ocfg.use_rnn, ocfg.rnn_type, ocfg.rnn_size, rnn_num_layers=ocfg.rnn_num_layers, **kw)
-
-
-def _build(ocfg, N, state, tape, engine, graph=False, **over):
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-
-    ops = _ops(engine)
-    dev = torch.device("cuda", 0)
-    cfg = make_cfg(ocfg, rnn_num_layers=ocfg.rnn_num_layers, **over)
-    model = PolicyModel(_spec(ocfg), dev)
-    model.load_state_dict(state, strict=False)
-    traj = alloc_for_spec(model.spec, N, ocfg.rollout, dev)
-    env = TapeVecEnv(tape.to(dev).contiguous(), ocfg.num_actions)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine], use_cuda_graph=graph)
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
-    return cfg, model, traj, sampler, learner
 
 
 # ------------------------------------------------------------------------------------------------ RnnCore vs torch
@@ -66,7 +28,7 @@ def _core(rnn, rnn_type, L, H, D, engine):
     from sample_factory_b200.model import ModelSpec, PolicyModel
     from sample_factory_b200.rnn_core import RnnCore
 
-    ops = _ops(engine)
+    ops = ops_for(engine)
     spec = ModelSpec(D, 3, [D], [], "elu", False, False, use_rnn=True, rnn_type=rnn_type, rnn_size=H, rnn_num_layers=L)
     model = PolicyModel(spec, torch.device("cuda", 0))
     model.load_state_dict({f"core.core.{k}": v.detach().clone() for k, v in rnn.state_dict().items()}, strict=False)
@@ -156,7 +118,7 @@ def test_misaligned_layer_slices_take_the_simt_gemm():
     wgmma engine those GEMMs run as gemm_simt_kernel (the step test above checks their results), an aligned H runs none"""
     from torch.profiler import ProfilerActivity, profile
 
-    _ops("3xtf32")
+    ops_for("3xtf32")
     counts = {}
     for H in (30, 32):
         rnn = torch.nn.GRU(24, H, 2)
@@ -186,66 +148,22 @@ GOLDEN = ["tiny_gru2", "tiny_lstm3"]
 def test_sampler_matches_reference_golden(name, engine):
     """the sampler on the reference's weights, obs tape and Exp(1) noise: actions bit-exact, the recorded states and the
     policy outputs at 1e-5, and the state recorded after a done step zero in every layer"""
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = RO.load_stacked_case(name)
-    tape = torch.from_numpy(z["tape"])
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), tape, engine)
-    assert model.spec.rnn_state_size == O.rnn_state_size(ocfg) == traj["rnn_states"].shape[2]
-    sampler.reset()
-    T = ocfg.rollout
-    for it in range(meta["iters"]):
-        st = state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/")
-        model.load_state_dict(st, strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(dev).contiguous()
-        sampler.rollout()
-        got = {k: v.cpu() for k, v in traj.items()}
-        ref = {k: torch.from_numpy(z[f"it{it}/traj/{k}"]) for k in
-               ["obs", "actions", "action_logits", "log_prob_actions", "values", "rewards", "dones", "rnn_states"]}
-        for k in ["obs", "rewards", "dones"]:
-            assert torch.equal(got[k].view(ref[k].shape), ref[k]), k
-        assert torch.equal(got["actions"].view(ref["actions"].shape), ref["actions"]), "action indices must be bit-exact"
-        np.testing.assert_allclose(got["rnn_states"].numpy(), ref["rnn_states"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["action_logits"].numpy(), ref["action_logits"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), ref["values"][:, :-1].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), ref["log_prob_actions"].numpy(), atol=TOL)
+    case = RO.load_stacked_case(name)
+    rig = build_case(case, engine)
+    ocfg, T = case[2], case[2].rollout
+    assert rig.model.spec.rnn_state_size == O.rnn_state_size(ocfg) == rig.traj["rnn_states"].shape[2]
+
+    def state_zero_after_done(got, it):
         after_done = got["rnn_states"][:, 1:T + 1][got["dones"].view(-1, T).bool()]
         assert after_done.shape[0] > 0 and torch.all(after_done == 0)
+    replay_sampler(case, rig, exact=("obs", "rewards", "dones", "actions"), check_iteration=state_zero_after_done)
 
 
 def _learner_vs_golden(name, engine, graph):
-    from sample_factory_b200 import ops
-
-    z, meta, ocfg = RO.load_stacked_case(name)
-    tape = torch.from_numpy(z["tape"])
-    over = dict(learner_cuda_graph=graph)
-    shuffle = any(k.endswith("/mb_indices") for k in z.files)
-    if shuffle:
-        over["shuffle_minibatches"] = True
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), tape, engine, **over)
-    assert learner.use_graph == graph and learner.shuffle == shuffle
-    for it in range(meta["iters"]):
-        assert learner.train_step == int(z[f"it{it}/train_step_before"])
-        for k, v in traj_from(z, it, ocfg).items():
-            traj[k].copy_(v.view(traj[k].shape))
-        if shuffle:
-            learner.set_minibatch_permutation(z[f"it{it}/mb_indices"])
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        p = f"it{it}/prep/"
-        assert torch.equal(learner.valids_flat.view(-1).cpu(), torch.from_numpy(z[p + "valids"]))
-        np.testing.assert_allclose(traj["values"][:, -1].cpu().numpy(), z[p + "bootstrap_values"], atol=TOL)
-        np.testing.assert_allclose(learner.advantages.view(-1).cpu().numpy(), z[p + "advantages"], atol=TOL)
-        np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), z[p + "returns"], atol=TOL)
-        log = learner.minibatch_log().numpy()
-        assert log.shape[0] == len(z[f"it{it}/loss/policy_loss"])
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=TOL, rtol=1e-5, err_msg=key)
-        got_state = model.state_dict()
-        for k, v in state_from(z, f"it{it}/state/").items():
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * TOL
-            np.testing.assert_allclose(got_state[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = RO.load_stacked_case(name)
+    rig = build_case(case, engine, learner_cuda_graph=graph)
+    assert rig.learner.use_graph == graph
+    replay_learner(case, rig)
 
 
 @pytest.mark.parametrize("engine", ENGINES)
@@ -264,34 +182,29 @@ def test_graphed_learner_matches_reference_golden(engine):
 
 def test_graphed_sampler_and_learner_match_eager():
     """two-layer GRU: the CUDA-graph sampler and learner produce exactly the eager trajectories and weights"""
-    ops = _ops()
-    eng = "3xtf32" if ops.tc_available() else "simt"
+    eng = "3xtf32" if ops_for().tc_available() else "simt"
     N, T = 64, 8
     ocfg = RO.StackedCfg(obs_dim=20, num_actions=5, encoder_mlp_layers=[64], rollout=T, recurrence=T, batch_size=N * T // 2,
                        num_batches_per_epoch=2, use_rnn=True, rnn_type="gru", rnn_size=64, rnn_num_layers=2)
     st0 = O.init_state(ocfg, seed=4)
     tape = torch.randn(3 * T + 1, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(5))
-    _, modelA, trajA, samplerA, learnerA = _build(ocfg, N, st0, tape, eng)
-    _, modelB, trajB, samplerB, learnerB = _build(ocfg, N, st0, tape, eng, graph=True, learner_cuda_graph=True)
-    assert learnerB.use_graph and not learnerA.use_graph
-    for smp in (samplerA, samplerB):
+    a = build(ocfg, N, st0, tape, eng)
+    b = build(ocfg, N, st0, tape, eng, graph=True, learner_cuda_graph=True)
+    for smp in (a.sampler, b.sampler):
         smp.reset()
         smp.rollout()
-    for smp in (samplerA, samplerB):     # (graph capture ran the first rollout eagerly: re-align both)
+    for smp in (a.sampler, b.sampler):     # (graph capture ran the first rollout eagerly: re-align both)
         smp.reset()
         smp.step_counter.zero_()
-    for it in range(3):
-        for smp, lrn in ((samplerA, learnerA), (samplerB, learnerB)):
-            smp.set_policy_version(lrn.train_step)
-            smp.rollout()
+
+    def feed(it):
+        for r in (a, b):
+            r.sampler.set_policy_version(r.learner.train_step)
+            r.sampler.rollout()
         torch.cuda.synchronize()
-        for k in trajA:
-            assert torch.equal(trajA[k], trajB[k]), (it, k)
-        learnerA.train(trajA)
-        learnerB.train(trajB)
-        torch.cuda.synchronize()
-        assert torch.equal(modelA.flat, modelB.flat), it
-        assert torch.equal(learnerA.minibatch_log(), learnerB.minibatch_log()), it
+        for k in a.traj:
+            assert torch.equal(a.traj[k], b.traj[k]), (it, k)
+    graphed_learner_matches_eager(a, b, feed, iters=3)
 
 
 # ------------------------------------------------------------------------------------------------ enjoy / full size
@@ -306,7 +219,7 @@ def test_enjoy_two_layer_checkpoint_matches_oracle(tmp_path):
     from sample_factory_b200.envs import TapeVecEnv, register_env
     from sample_factory_b200.model import PolicyModel
 
-    ops = _ops()
+    ops = ops_for()
     dev = torch.device("cuda", 0)
     N, T = 48, 8
     ocfg = RO.StackedCfg(obs_dim=12, num_actions=5, encoder_mlp_layers=[32], rollout=T, recurrence=T, use_rnn=True,
@@ -315,13 +228,13 @@ def test_enjoy_two_layer_checkpoint_matches_oracle(tmp_path):
     tape = torch.randn(40, N, ocfg.obs_dim, generator=torch.Generator().manual_seed(4)) * 2
     register_env("rnn2_enjoy", lambda full_env_name, cfg, env_config, render_mode=None: TapeVecEnv(tape.to(dev).contiguous(), 5))
     cfg = make_cfg(ocfg, env="rnn2_enjoy", train_dir=str(tmp_path), experiment="api", cuda_graph=False, seed=0,
-                   gemm_engine="simt", rnn_num_layers=2)
+                   gemm_engine="simt")
     cfg.cli_args = {}
     os.makedirs(os.path.join(str(tmp_path), "api"), exist_ok=True)
     saved = {k: v for k, v in vars(cfg).items() if isinstance(v, (int, float, str, bool, list, type(None)))}
     with open(os.path.join(str(tmp_path), "api", "config.json"), "w") as f:
         json.dump(saved, f)
-    model = PolicyModel(_spec(ocfg), dev)
+    model = PolicyModel(model_spec(ocfg), DEV)
     model.load_state_dict(st, strict=False)
     save_checkpoint(cfg, model, SimpleNamespace(policy_id=0, train_step=5, env_steps=100, opt_step=5, curr_lr=1e-4))
     max_ep = 60
@@ -356,7 +269,7 @@ def test_run_rl_trains_three_gru_layers(tmp_path):
     from sample_factory_b200.envs import TapeVecEnv, register_env
     from sample_factory_b200.train import run_rl
 
-    _ops()
+    ops_for()
     dev = torch.device("cuda", 0)
     tape = torch.randn(33, 256, 16, generator=torch.Generator().manual_seed(6)).to(dev)
     register_env("rnn3_run_rl", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 4))
@@ -383,8 +296,6 @@ def test_cfg5_two_lstm_layers_4096_envs_per_gpu():
     measured by this test on an H100 80GB HBM3); the large items: the trajectories with 2048-wide states (0.6 GB), the
     flat [E, 2048] state copy (0.5 GB), per layer the BPTT buffers the backward reads (gates / state_in / state_out /
     core_out, 0.6 GB), the gate and gradient buffers all layers share (1.1 GB)."""
-    from tests.test_gpu_configs import _check_finite, _runner
-
     from sample_factory_b200.envs import TapeVecEnv
 
     dev = torch.device("cuda", 0)
@@ -393,7 +304,7 @@ def test_cfg5_two_lstm_layers_4096_envs_per_gpu():
     torch.cuda.reset_peak_memory_stats()
     base = torch.cuda.memory_allocated()
     tape = torch.randn(2 * T + 1, N, 256, generator=torch.Generator().manual_seed(2)).to(dev)
-    r = _runner("synthetic_isaac_l2", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
+    r = runner("synthetic_isaac_l2", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
                 ["--use_rnn=True", "--rnn_type=lstm", "--rnn_size=512", "--rnn_num_layers=2", "--async_rl=False",
                  f"--rollout={T}", f"--recurrence={T}", "--batch_size=32768", "--num_batches_per_epoch=2",
                  "--num_epochs=2", "--encoder_mlp_layers", "512", "256", "128", "--value_bootstrap=True",
@@ -404,7 +315,7 @@ def test_cfg5_two_lstm_layers_4096_envs_per_gpu():
     assert "core.core.weight_ih_l1" in r.model.params and r.model.params["core.core.weight_ih_l1"].shape == (2048, 512)
     lr0 = r.learner.curr_lr
     w1 = r.model.params["core.core.weight_hh_l1"].clone()
-    st = _check_finite(r, 3, 3 * N * T)
+    st = check_finite(r, 3, 3 * N * T)
     assert st["num_valid"] == 32768
     assert r.learner.curr_lr != lr0
     assert not torch.equal(w1, r.model.params["core.core.weight_hh_l1"])      # the upper layer trains

@@ -1,5 +1,5 @@
 """The fp16 form of the persistent rollout kernel stores h1 by TMA from shared-memory staging boxes.  Whole rollouts are
-compared against the per-step launches with the rule of test_gpu_engine._compare_rollout_runs (bit-identical but for
+compared against the per-step launches with the rule of device_harness.compare_rollout_runs (bit-identical but for
 logits / values / log-probs, 2e-6) at the bench shape (4096 envs, 512-512, T = 32: clusters of two) and at 4000 envs
 (the last 64-row block has 32 rows, so the TMA stores clip), for every activation.
 
@@ -12,8 +12,7 @@ import pytest
 import torch
 
 from oracle import appo_oracle as O
-from tests.test_gpu_engine import _compare_rollout_runs
-from tests.test_gpu_rollout_pipeline import _pair, _state
+from tests.device_harness import compare_rollout_runs, rollout_pair, rollout_state
 
 pytestmark = pytest.mark.gpu
 
@@ -23,7 +22,7 @@ def _check(N, nonlinearity, T=32, hidden=512, rollouts=2):
 
     ocfg = O.OracleCfg(obs_dim=64, num_actions=8, encoder_mlp_layers=[hidden, hidden], rollout=T, recurrence=1,
                        batch_size=N * T // 2, num_batches_per_epoch=2, nonlinearity=nonlinearity)
-    model, _, (ss, ts, es), (sp, tp, ep) = _pair(ocfg, N, seed=11 + N + T)
+    model, _, (ss, ts, es), (sp, tp, ep) = rollout_pair(ocfg, N, seed=11 + N + T)
     ss.reset()
     sp.reset()
     for it in range(rollouts):
@@ -35,7 +34,7 @@ def _check(N, nonlinearity, T=32, hidden=512, rollouts=2):
         sp.rollout()
         assert ops.rollout_last_form() == 1
         torch.cuda.synchronize()
-        _compare_rollout_runs(_state(ss, ts, es), _state(sp, tp, ep), f"{nonlinearity} N={N} rollout {it}")
+        compare_rollout_runs(rollout_state(ss, ts, es), rollout_state(sp, tp, ep), f"{nonlinearity} N={N} rollout {it}")
 
     bound = float(model.bound_h[0])
     shift = max(-100, min(100, 15 - math.frexp(bound)[1]))    # f16_shift_for_bound: bound * 2^shift in [2^14, 2^15)

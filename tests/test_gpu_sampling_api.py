@@ -7,14 +7,12 @@ import pytest
 import torch
 
 from oracle import appo_oracle as O
+from tests.device_harness import TOL, make_cfg
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
 
 
 def _cfg(ocfg, env_name, tmp_path, **over):
-    from tests.test_gpu_engine import make_cfg
-
     cfg = make_cfg(ocfg, env=env_name, train_dir=str(tmp_path), experiment="api", cuda_graph=False, seed=0,
                    gemm_engine="simt", **over)
     return cfg

@@ -11,49 +11,10 @@ import torch
 
 from oracle import appo_oracle as O
 from tests import separate_rnn_oracle as SO
-from tests.golden_utils import state_from, traj_from
-from tests.test_gpu_engine import make_cfg
+from tests.device_harness import (ENGINES, MiniCartPole, build, build_case, check_finite, ops_for, replay_learner,
+                                  replay_sampler, runner)
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-ENGINES = ["simt", "3xtf32"]
-
-
-def _ops(engine="simt"):
-    from sample_factory_b200 import ops
-
-    ops.bind_device(torch.device("cuda", 0))
-    if engine != "simt" and not ops.tc_available():
-        pytest.skip("wgmma engine not available")
-    return ops
-
-
-def _spec(ocfg):
-    from sample_factory_b200.model import ModelSpec
-
-    return ModelSpec(ocfg.obs_dim, ocfg.num_actions, list(ocfg.encoder_mlp_layers), list(ocfg.decoder_mlp_layers),
-                     ocfg.nonlinearity, ocfg.normalize_input, ocfg.normalize_returns, ocfg.obs_subtract_mean,
-                     ocfg.obs_scale, ocfg.use_rnn, ocfg.rnn_type, ocfg.rnn_size, continuous=ocfg.continuous,
-                     share_weights=False, rnn_num_layers=ocfg.rnn_num_layers)
-
-
-def _build(ocfg, N, state, tape, engine, graph=False, **over):
-    from sample_factory_b200.envs import TapeVecEnv
-    from sample_factory_b200.learner import Learner
-    from sample_factory_b200.model import PolicyModel
-    from sample_factory_b200.sampler import DeviceSampler
-    from sample_factory_b200.trajectory import alloc_for_spec
-
-    ops = _ops(engine)
-    dev = torch.device("cuda", 0)
-    cfg = make_cfg(ocfg, rnn_num_layers=ocfg.rnn_num_layers, **over)
-    model = PolicyModel(_spec(ocfg), dev)
-    model.load_state_dict(state, strict=False)
-    traj = alloc_for_spec(model.spec, N, ocfg.rollout, dev)
-    env = TapeVecEnv(tape.to(dev).contiguous(), ocfg.num_actions, continuous=ocfg.continuous)
-    sampler = DeviceSampler(cfg, env, model, traj, engine=ops.ENGINES[engine], use_cuda_graph=graph)
-    learner = Learner(cfg, model, N, engine=ops.ENGINES[engine])
-    return cfg, model, traj, sampler, learner
 
 
 # ------------------------------------------------------------------------------------------------ vs the reference
@@ -66,74 +27,24 @@ def test_sampler_matches_reference_golden(name, engine):
     """the sampler on the reference's weights, obs tape and noise: Discrete actions bit-exact (Box actions, floats of the
     means, and their rewards at 1e-5), the [actor | critic] state rows, logits, values and log-probs at 1e-5, and both
     halves of the state recorded after a done step zero"""
-    dev = torch.device("cuda", 0)
-    z, meta, ocfg = SO.load_separate_rnn_case(name)
-    tape = torch.from_numpy(z["tape"])
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), tape, engine)
-    assert model.spec.rnn_state_size == O.rnn_state_size(ocfg) == traj["rnn_states"].shape[2]
-    sampler.reset()
-    T = ocfg.rollout
-    for it in range(meta["iters"]):
-        st = state_from(z, "init/") if it == 0 else state_from(z, f"it{it - 1}/state/")
-        model.load_state_dict(st, strict=False)
-        sampler.set_policy_version(int(z[f"it{it}/train_step_before"]))
-        sampler.noise = torch.from_numpy(z[f"it{it}/noise"]).to(dev).contiguous()
-        sampler.rollout()
-        got = {k: v.cpu() for k, v in traj.items()}
-        ref = {k: torch.from_numpy(z[f"it{it}/traj/{k}"]) for k in
-               ["obs", "actions", "action_logits", "log_prob_actions", "values", "rewards", "dones", "rnn_states"]}
-        for k in ["obs", "dones"]:
-            assert torch.equal(got[k].view(ref[k].shape), ref[k]), k
-        if ocfg.continuous:
-            for k in ["actions", "rewards"]:
-                np.testing.assert_allclose(got[k].view(ref[k].shape).numpy(), ref[k].numpy(), atol=TOL, err_msg=k)
-        else:
-            assert torch.equal(got["rewards"].view(ref["rewards"].shape), ref["rewards"])
-            assert torch.equal(got["actions"].view(ref["actions"].shape), ref["actions"]), "action indices must be bit-exact"
-        np.testing.assert_allclose(got["rnn_states"].numpy(), ref["rnn_states"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["action_logits"].numpy(), ref["action_logits"].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), ref["values"][:, :-1].numpy(), atol=TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), ref["log_prob_actions"].numpy(), atol=TOL)
+    case = SO.load_separate_rnn_case(name)
+    rig = build_case(case, engine)
+    ocfg, T = case[2], case[2].rollout
+    assert rig.model.spec.rnn_state_size == O.rnn_state_size(ocfg) == rig.traj["rnn_states"].shape[2]
+    S = rig.model.spec.rnn_tower_state_size
+
+    def check_states(got, it):
         after_done = got["rnn_states"][:, 1:T + 1][got["dones"].view(-1, T).bool()]
         assert after_done.shape[0] > 0 and torch.all(after_done == 0)
-        S = model.spec.rnn_tower_state_size
         assert got["rnn_states"][..., :S].abs().max() > 0 and got["rnn_states"][..., S:].abs().max() > 0
+    replay_sampler(case, rig, exact=("obs", "dones", "rewards", "actions"), check_iteration=check_states)
 
 
 def _learner_vs_golden(name, engine, graph):
-    from sample_factory_b200 import ops
-
-    z, meta, ocfg = SO.load_separate_rnn_case(name)
-    tape = torch.from_numpy(z["tape"])
-    over = dict(learner_cuda_graph=graph)
-    shuffle = any(k.endswith("/mb_indices") for k in z.files)
-    if shuffle:
-        over["shuffle_minibatches"] = True
-    cfg, model, traj, sampler, learner = _build(ocfg, meta["N"], state_from(z, "init/"), tape, engine, **over)
-    assert learner.use_graph == graph and learner.shuffle == shuffle
-    for it in range(meta["iters"]):
-        assert learner.train_step == int(z[f"it{it}/train_step_before"])
-        for k, v in traj_from(z, it, ocfg).items():
-            traj[k].copy_(v.view(traj[k].shape))
-        if shuffle:
-            learner.set_minibatch_permutation(z[f"it{it}/mb_indices"])
-        learner.train(traj)
-        torch.cuda.synchronize()
-        assert learner.train_step == int(z[f"it{it}/train_step_after"])
-        p = f"it{it}/prep/"
-        assert torch.equal(learner.valids_flat.view(-1).cpu(), torch.from_numpy(z[p + "valids"]))
-        np.testing.assert_allclose(traj["values"][:, -1].cpu().numpy(), z[p + "bootstrap_values"], atol=TOL)
-        if not ocfg.with_vtrace:
-            np.testing.assert_allclose(learner.advantages.view(-1).cpu().numpy(), z[p + "advantages"], atol=TOL)
-            np.testing.assert_allclose(learner.returns.view(-1).cpu().numpy(), z[p + "returns"], atol=TOL)
-        log = learner.minibatch_log().numpy()
-        assert log.shape[0] == len(z[f"it{it}/loss/policy_loss"])
-        for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss", "adv_mean", "adv_std"]:
-            np.testing.assert_allclose(log[:, ops.LS[key]], z[f"it{it}/loss/{key}"], atol=TOL, rtol=1e-5, err_msg=key)
-        got_state = model.state_dict()
-        for k, v in state_from(z, f"it{it}/state/").items():
-            tol = (1e-6 if k.startswith("returns_normalizer") else 1e-8) if v.dtype == torch.float64 else 2 * TOL
-            np.testing.assert_allclose(got_state[k].cpu().numpy().reshape(v.shape), v.numpy(), atol=tol, rtol=1e-6, err_msg=k)
+    case = SO.load_separate_rnn_case(name)
+    rig = build_case(case, engine, learner_cuda_graph=graph)
+    assert rig.learner.use_graph == graph
+    replay_learner(case, rig)
 
 
 @pytest.mark.parametrize("engine", ENGINES)
@@ -194,7 +105,7 @@ def test_two_tower_bptt_matches_torch_autograd(rnn_type, dec, engine):
     """512 rows, R = 16, H = 128, two layers: the learner's minibatch forward (values, logits) and its explicit backward
     (heads over the concatenated tail -> per tower decoder -> BPTT -> W_ih / encoder) against nn.GRU / nn.LSTM towers
     with autograd, for given d(logits) / d(values) -- every parameter gradient of both towers and of the heads"""
-    ops = _ops(engine)
+    ops = ops_for(engine)
     dev = torch.device("cuda", 0)
     n, R, H, L, D, A = 32, 16, 128, 2, 40, 6
     B = n * R
@@ -214,8 +125,8 @@ def test_two_tower_bptt_matches_torch_autograd(rnn_type, dec, engine):
         for i, lin in enumerate(m.dec):
             sd[f"{tw}decoder.mlp.{2 * i}.weight"], sd[f"{tw}decoder.mlp.{2 * i}.bias"] = lin.weight, lin.bias
     sd[O.CRITIC_W], sd[O.CRITIC_B], sd[O.ACTION_W], sd[O.ACTION_B] = critic.weight, critic.bias, action.weight, action.bias
-    cfg, model, traj, sampler, learner = _build(ocfg, 2 * n, {k: v.detach().clone() for k, v in sd.items()},
-                                                torch.zeros(2, 2 * n, D), engine)     # (minibatches of n chunks)
+    cfg, model, traj, _, sampler, learner = build(ocfg, 2 * n, {k: v.detach().clone() for k, v in sd.items()},
+                                                  torch.zeros(2, 2 * n, D), engine)     # (minibatches of n chunks)
     Sw = model.spec.rnn_tower_state_size
     x = torch.randn(B, D, generator=gen)
     states = torch.rand(B, 2 * Sw, generator=gen) - 0.5
@@ -260,8 +171,6 @@ def test_cfg5_separate_weights_4096_envs_per_gpu():
     """config 5's stack with --actor_critic_share_weights=False through Runner: Box(256) obs, per tower MLP [512,256,128]
     -> LSTM-512, 4096 envs, rollout = recurrence = 16, 2 x 32768 minibatches, 2 epochs, three iterations: finite losses,
     both towers train, the state rows [actor | critic] reset at dones, and the peak allocated memory bounded"""
-    from tests.test_gpu_configs import _check_finite, _runner
-
     from sample_factory_b200.envs import TapeVecEnv
 
     dev = torch.device("cuda", 0)
@@ -270,7 +179,7 @@ def test_cfg5_separate_weights_4096_envs_per_gpu():
     torch.cuda.reset_peak_memory_stats()
     base = torch.cuda.memory_allocated()
     tape = torch.randn(2 * T + 1, N, 256, generator=torch.Generator().manual_seed(2)).to(dev)
-    r = _runner("synthetic_isaac_sep", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
+    r = runner("synthetic_isaac_sep", lambda name, cfg, env_config, render_mode=None: TapeVecEnv(tape, 8),
                 ["--use_rnn=True", "--rnn_type=lstm", "--rnn_size=512", "--actor_critic_share_weights=False",
                  "--async_rl=False", f"--rollout={T}", f"--recurrence={T}", "--batch_size=32768",
                  "--num_batches_per_epoch=2", "--num_epochs=2", "--encoder_mlp_layers", "512", "256", "128",
@@ -279,7 +188,7 @@ def test_cfg5_separate_weights_4096_envs_per_gpu():
     assert not r.model.spec.share_weights and r.model.spec.rnn_state_size == 2048
     assert r.traj["rnn_states"].shape == (N, T + 1, 2048)
     w = {tw: r.model.params[f"{tw}core.core.weight_hh_l0"].clone() for tw in SO.TOWERS}
-    st = _check_finite(r, 3, 3 * N * T)
+    st = check_finite(r, 3, 3 * N * T)
     assert st["num_valid"] == 32768
     for tw in SO.TOWERS:
         assert not torch.equal(w[tw], r.model.params[f"{tw}core.core.weight_hh_l0"]), tw
@@ -295,8 +204,6 @@ def test_cfg5_separate_weights_4096_envs_per_gpu():
 def test_host_env_run_rl_and_enjoy_with_default_gru(tmp_path):
     """a gymnasium-API CPU env (the CartPole re-implementation) through run_rl with --actor_critic_share_weights=False and
     otherwise default model flags (GRU-512 core per tower); enjoy() then loads the checkpoint it wrote"""
-    from tests.test_gpu_host_env import MiniCartPole
-
     from sample_factory_b200.cfg import parse_full_cfg, parse_sf_args
     from sample_factory_b200.checkpoint import checkpoint_dir, get_checkpoints
     from sample_factory_b200.enjoy import enjoy
@@ -304,7 +211,7 @@ def test_host_env_run_rl_and_enjoy_with_default_gru(tmp_path):
     from sample_factory_b200.host_env import BatchedHostEnv
     from sample_factory_b200.train import run_rl
 
-    _ops()
+    ops_for()
     dev = torch.device("cuda", 0)
     register_env("MiniCartPoleSep-v0", lambda name, cfg, env_config, render_mode=None: BatchedHostEnv(
         lambda i: MiniCartPole(max_steps=50), 32, dev, seed=cfg.seed))

@@ -6,67 +6,27 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-import tests.test_gpu_engine as E
 from oracle import appo_oracle as O
+from tests.device_harness import (DEV, ENGINES, TOL, build, build_case, g, graphed_learner_matches_eager,
+                                  graphed_sampler_matches_eager, masked_rows, need, ops_for, replay_learner, replay_sampler,
+                                  sampled_feed, wide_tail)
+from tests.golden_utils import load_case
 
 pytestmark = pytest.mark.gpu
-DEV = torch.device("cuda", 0)
-
-
-def _ops():
-    from sample_factory_b200 import ops
-
-    ops.bind_device(DEV)
-    return ops
-
-
-def g(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def _tail(ops, h, Wv, bv, logits, A, noise=None, mask=None, deterministic=False, **kw):
-    """run sfb200_heads_tail_wide on rows already holding the logits; returns (values, actions, log_prob, pv)"""
-    M = h.shape[0]
-    values = torch.full((M,), float("nan"), device=DEV)
-    width = kw.get("act_dim", 0) if kw.get("continuous") else (len(kw["head_sizes"]) if kw.get("head_sizes") else 1)
-    actions = torch.full((M, width), float("nan"), device=DEV)
-    lp = torch.full((M,), float("nan"), device=DEV)
-    pv_out = torch.full((M,), float("nan"), device=DEV)
-    pv = torch.full((1,), 7.0, device=DEV)
-    env = torch.empty((M, width), dtype=torch.float32 if kw.get("continuous") else torch.int32, device=DEV)
-    if mask is not None or deterministic:
-        ops.set_sampling_mode(mask, deterministic)
-    try:
-        ops.heads_tail_wide(h, Wv, bv, logits, logits.stride(0), A, values, 1, noise=noise, actions_f32=actions,
-                            actions_stride=width, env_actions=env, log_prob=lp, log_prob_stride=1,
-                            policy_version_scalar=pv, policy_version_out=pv_out, pv_stride=1, philox_seed=5, **kw)
-    finally:
-        ops.set_sampling_mode(None, False)
-    torch.cuda.synchronize()
-    assert torch.all(pv_out == 7.0)
-    return values.cpu(), actions.cpu(), lp.cpu(), env.cpu()
-
-
-def _masked_rows(M, A, seed):
-    mask = torch.rand(M, A, generator=g(seed)) > 0.6
-    mask[0] = False                  # a row that allows nothing: uniform fallback
-    mask[1] = False
-    mask[1, A - 1] = True            # only the last action
-    return mask
 
 
 @pytest.mark.parametrize("A", [32, 33, 45, 96, 362, 1024])
 @pytest.mark.parametrize("mode", ["plain", "mask", "deterministic"])
 def test_categorical_tail_matches_torch(A, mode):
-    ops = _ops()
+    ops = ops_for()
     M, H = 300, 96
     h = torch.randn(M, H, generator=g(A))
     Wv, bv = torch.randn(1, H, generator=g(1)) * 0.1, torch.randn(1, generator=g(2))
     logits = torch.randn(M, A, generator=g(3)) * 2
     q = torch.empty(M, A).exponential_(generator=g(4))
-    mask = _masked_rows(M, A, 5) if mode == "mask" else None
+    mask = masked_rows(M, A, 5) if mode == "mask" else None
     ld = logits.clone().to(DEV)
-    v, act, lp, env = _tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, noise=q.to(DEV),
+    v, act, lp, env = wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, noise=q.to(DEV),
                             mask=None if mask is None else mask.to(DEV), deterministic=mode == "deterministic")
     assert torch.equal(ld.cpu(), logits)      # the stored logits stay the raw logits
     np.testing.assert_allclose(v.numpy(), (h.double() @ Wv.double().view(-1) + bv.double()).numpy(), atol=1e-5)
@@ -86,14 +46,14 @@ def test_categorical_tail_matches_torch(A, mode):
 
 @pytest.mark.parametrize("segs", [[24, 5, 16], [300, 62], [8, 16, 8, 992]])
 def test_tuple_tail_matches_torch(segs):
-    ops = _ops()
+    ops = ops_for()
     A = sum(segs)
     M, H = 200, 64
     h = torch.randn(M, H, generator=g(1))
     Wv, bv = torch.randn(1, H, generator=g(2)) * 0.1, torch.randn(1, generator=g(3))
     logits = torch.randn(M, A, generator=g(4)) * 2
     q = torch.empty(M, A).exponential_(generator=g(5))
-    v, act, lp, env = _tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), logits.clone().to(DEV), A, noise=q.to(DEV),
+    v, act, lp, env = wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), logits.clone().to(DEV), A, noise=q.to(DEV),
                             head_sizes=segs)
     start, ref_lp = 0, torch.zeros(M)
     for k, n in enumerate(segs):
@@ -108,7 +68,7 @@ def test_tuple_tail_matches_torch(segs):
                                               (1024, False)])
 @pytest.mark.parametrize("deterministic", [False, True])
 def test_gaussian_tail_matches_torch(act_dim, adaptive, deterministic):
-    ops = _ops()
+    ops = ops_for()
     M, H = 128, 64
     h = torch.randn(M, H, generator=g(1))
     Wv, bv = torch.randn(1, H, generator=g(2)) * 0.1, torch.randn(1, generator=g(3))
@@ -118,7 +78,7 @@ def test_gaussian_tail_matches_torch(act_dim, adaptive, deterministic):
     eps = torch.randn(M, act_dim, generator=g(6))
     params = raw.clone().to(DEV)
     A = 2 * act_dim if adaptive else act_dim
-    v, act, lp, env = _tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, noise=eps.to(DEV),
+    v, act, lp, env = wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, noise=eps.to(DEV),
                             deterministic=deterministic, continuous=True, act_dim=act_dim, adaptive_stddev=adaptive,
                             learned_log_std=None if adaptive else learned.to(DEV), tanh_scale=ts)
     means = raw[:, :act_dim] if adaptive else torch.tanh(raw[:, :act_dim] / ts) * ts
@@ -139,13 +99,13 @@ def test_gaussian_tail_matches_torch(act_dim, adaptive, deterministic):
 @pytest.mark.parametrize("masked", [False, True])
 def test_wide_tail_matches_narrow_heads(A, masked):
     """Up to 31 logits the wide tail puts every logit on the lane the narrow tail uses: same action indices bit for bit"""
-    ops = _ops()
+    ops = ops_for()
     M, H = 512, 64
     h = torch.randn(M, H, generator=g(A)).to(DEV)
     Wv, bv = (torch.randn(1, H, generator=g(1)) * 0.2).to(DEV), torch.randn(1, generator=g(2)).to(DEV)
     Wa, ba = (torch.randn(A, H, generator=g(3)) * 0.3).to(DEV), torch.randn(A, generator=g(4)).to(DEV)
     q = torch.empty(M, A).exponential_(generator=g(5)).to(DEV)
-    mask = _masked_rows(M, A, 6).to(DEV) if masked else None
+    mask = masked_rows(M, A, 6).to(DEV) if masked else None
     vals, logits = torch.empty(M, device=DEV), torch.empty(M, A, device=DEV)
     acts, lp = torch.empty(M, device=DEV), torch.empty(M, device=DEV)
     if mask is not None:
@@ -153,7 +113,7 @@ def test_wide_tail_matches_narrow_heads(A, masked):
     ops.heads_forward(h, Wv, bv, Wa, ba, vals, 1, logits, A, noise=q, actions_f32=acts, actions_stride=1, log_prob=lp,
                       log_prob_stride=1)
     ops.set_sampling_mode(None, False)
-    v2, a2, lp2, _ = _tail(ops, h, Wv, bv, logits.clone(), A, noise=q, mask=mask)
+    v2, a2, lp2, _ = wide_tail(ops, h, Wv, bv, logits.clone(), A, noise=q, mask=mask)
     assert torch.equal(a2.view(-1), acts.cpu())
     np.testing.assert_allclose(v2.numpy(), vals.cpu().numpy(), atol=1e-6)
     np.testing.assert_allclose(lp2.numpy(), lp.cpu().numpy(), atol=1e-6)
@@ -161,7 +121,7 @@ def test_wide_tail_matches_narrow_heads(A, masked):
 
 def test_philox_sampling_distribution_a362():
     """Philox draws: action frequencies follow the (masked) softmax, and no masked action is ever drawn"""
-    ops = _ops()
+    ops = ops_for()
     A, M, H = 362, 20000, 32
     row = torch.randn(A, generator=g(1)) * 1.5
     mask_row = torch.rand(A, generator=g(2)) > 0.3
@@ -214,7 +174,7 @@ def _torch_ppo(lp, lp_old, ent, kl, values, v_old, targets, adv, valids, c_ent, 
 @pytest.mark.parametrize("A", [33, 96, 362, 1024])
 @pytest.mark.parametrize("expl", ["entropy", "symmetric_kl"])
 def test_categorical_loss_and_ratio_match_autograd(A, expl):
-    ops = _ops()
+    ops = ops_for()
     B = 600
     adv, valids, v_old, targets, values = _loss_inputs(B, A)
     logits = torch.randn(B, A, generator=g(1)) * 1.5
@@ -257,7 +217,7 @@ def test_categorical_loss_and_ratio_match_autograd(A, expl):
 @pytest.mark.parametrize("segs", [[24, 5, 16], [300, 62], [8, 16, 8, 992]])
 @pytest.mark.parametrize("expl", ["entropy", "symmetric_kl"])
 def test_tuple_loss_and_ratio_match_autograd(segs, expl):
-    ops = _ops()
+    ops = ops_for()
     A, B = sum(segs), 400
     adv, valids, v_old, targets, values = _loss_inputs(B, A)
     logits = torch.randn(B, A, generator=g(1)) * 1.5
@@ -302,7 +262,7 @@ def test_tuple_loss_and_ratio_match_autograd(segs, expl):
 @pytest.mark.parametrize("act_dim", [17, 40, 512])
 @pytest.mark.parametrize("adaptive", [True, False])
 def test_gaussian_loss_and_ratio_match_autograd(act_dim, adaptive):
-    ops = _ops()
+    ops = ops_for()
     B = 300
     adv, valids, v_old, targets, values = _loss_inputs(B, act_dim)
     ts = 0.0 if adaptive else 1.5
@@ -351,14 +311,14 @@ def test_gaussian_loss_and_ratio_match_autograd(act_dim, adaptive):
 
 
 # ----------------------------------------------------------------------------------------------- heads backward
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("tail", ["elu", "tanh", "gru", "separate"])
 @pytest.mark.parametrize("A", [45, 362])
 def test_wide_heads_backward_matches_autograd(engine, tail, A):
     """linear_backward (dWa, dz) + sfb200_heads_wide_backward vs autograd through critic_linear / distribution_linear and
     the tail's activation (a GRU tail feeds the heads its raw output: act' = 1, no bias gradient)"""
-    E._need(engine)
-    ops = _ops()
+    need(engine)
+    ops = ops_for()
     B, H = 700, 128
     sep = tail == "separate"
     act = {"elu": "elu", "tanh": "tanh", "gru": "none", "separate": "elu"}[tail]
@@ -406,16 +366,18 @@ def test_wide_heads_backward_matches_autograd(engine, tail, A):
 WIDE_CASES = ["tiny_wide_mask", "tiny_wide_tuple", "tiny_wide_gauss", "tiny_wide_gauss_learned"]
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", WIDE_CASES)
 def test_wide_rollout_matches_reference_golden(name, engine):
-    E.test_rollout_matches_reference_golden(name, engine)
+    case = load_case(name)
+    replay_sampler(case, build_case(case, engine))
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 @pytest.mark.parametrize("name", WIDE_CASES)
 def test_wide_learner_matches_reference_golden(name, engine):
-    E.test_learner_matches_reference_golden(name, engine)
+    case = load_case(name)
+    replay_learner(case, build_case(case, engine), rewards=True)
 
 
 def _wide_ocfg(N, T, **kw):
@@ -428,58 +390,32 @@ def _wide_ocfg(N, T, **kw):
 def test_wide_graphed_learner_and_sampler_match_eager():
     """Discrete(362) with masks: the learner replayed as one CUDA graph and the graphed sampler give the same bits as the
     launch-by-launch versions"""
-    ops = _ops()
-    from sample_factory_b200.learner import Learner
-
     N, T = 128, 8
     ocfg = _wide_ocfg(N, T)
     st0 = O.init_state(ocfg, seed=2)
     tape = torch.randn(6 * T + 1, N, ocfg.obs_dim, generator=g(3))
-    eng = "3xtf32" if ops.tc_available() else "simt"
-    cfgA, modelA, trajA, envA, samplerA, learnerA = E.build(ocfg, N, st0, tape, DEV, engine=eng)
-    cfgB, modelB, trajB, envB, samplerB, _ = E.build(ocfg, N, st0, tape, DEV, engine=eng, graph=True)
-    assert modelA.spec.wide_heads and samplerB.use_cuda_graph and samplerA.heads_plan.P == 0
-    cfgB.learner_cuda_graph = True
-    learnerB = Learner(cfgB, modelB, N, engine=ops.ENGINES[eng])
-    assert learnerB.use_graph
+    eng = "3xtf32" if ops_for().tc_available() else "simt"
+    a = build(ocfg, N, st0, tape, eng)
+    b = build(ocfg, N, st0, tape, eng, graph=True, learner_cuda_graph=True)
+    assert a.model.spec.wide_heads and b.sampler.use_cuda_graph and a.sampler.heads_plan.P == 0
     # graphed sampler: its first rollout runs eagerly and captures, so compare a second rollout from the same state
-    for smp in (samplerA, samplerB):
-        smp.reset()
-        smp.rollout()
-    for smp in (samplerA, samplerB):
-        smp.reset()
-        smp.step_counter.zero_()
-        smp.rollout()
-    torch.cuda.synchronize()
-    for k in trajA:
-        assert torch.equal(trajA[k], trajB[k]), f"graphed sampler differs from eager for {k}"
-    for it in range(4):
-        samplerA.set_policy_version(learnerA.train_step)
-        samplerA.rollout()
-        for k in trajA:
-            trajB[k].copy_(trajA[k])
-        learnerA.train(trajA)
-        learnerB.train(trajB)
-        torch.cuda.synchronize()
-        assert torch.equal(modelA.flat, modelB.flat), it
-        assert torch.equal(modelA.exp_avg_sq, modelB.exp_avg_sq)
-        assert torch.equal(learnerA.minibatch_log(), learnerB.minibatch_log())
-    assert learnerB.graph_replay_launches > 0
+    graphed_sampler_matches_eager(a, b)
+    graphed_learner_matches_eager(a, b, sampled_feed(a, b), exp_avg_sq=True)
 
 
-@pytest.mark.parametrize("engine", E.ENGINES)
+@pytest.mark.parametrize("engine", ENGINES)
 def test_closed_loop_vs_oracle_discrete362_masked(engine):
     """1024 tape envs, Discrete(362) with action masks, MLP 512-512: sampler + learner for 2 iterations against the oracle
     on the same tape, noise and initial weights"""
     from sample_factory_b200 import ops
 
-    E._need(engine)
+    need(engine)
     N, T = 1024, 8
     ocfg = _wide_ocfg(N, T, batch_size=N * T // 4, num_batches_per_epoch=4, encoder_mlp_layers=[512, 512])
     st0 = O.init_state(ocfg, seed=3)
     gen = g(11)
     tape = torch.randn(2 * T + 1, N, ocfg.obs_dim, generator=gen) * 1.2 - 0.2
-    cfg, model, traj, env, sampler, learner = E.build(ocfg, N, st0, tape, DEV, engine=engine)
+    cfg, model, traj, env, sampler, learner = build(ocfg, N, st0, tape, engine)
     olearner = O.OracleLearner(ocfg, st0)
     oenv = O.TapeVecEnv(tape, ocfg.num_actions, with_action_mask=True)
     olast = oenv.reset()
@@ -496,16 +432,16 @@ def test_closed_loop_vs_oracle_discrete362_masked(engine):
         assert mism == 0.0, f"action mismatch fraction {mism}"
         for k in ["obs", "rewards", "dones", "time_outs", "policy_id", "policy_version"]:
             assert torch.equal(got[k], otraj[k]), k
-        np.testing.assert_allclose(got["action_logits"].numpy(), otraj["action_logits"].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["values"][:, :-1].numpy(), otraj["values"][:, :-1].numpy(), atol=E.TOL)
-        np.testing.assert_allclose(got["log_prob_actions"].numpy(), otraj["log_prob_actions"].numpy(), atol=E.TOL)
+        np.testing.assert_allclose(got["action_logits"].numpy(), otraj["action_logits"].numpy(), atol=TOL)
+        np.testing.assert_allclose(got["values"][:, :-1].numpy(), otraj["values"][:, :-1].numpy(), atol=TOL)
+        np.testing.assert_allclose(got["log_prob_actions"].numpy(), otraj["log_prob_actions"].numpy(), atol=TOL)
         n0 = len(olearner.log)
         olearner.train(otraj)
         learner.train(traj)
         log = learner.minibatch_log().numpy()
         for j, d in enumerate(olearner.log[n0:]):
             for key in ["policy_loss", "value_loss", "exploration_loss", "kl_loss"]:
-                assert abs(log[j, ops.LS[key]] - d[key]) < E.TOL, (it, j, key, log[j, ops.LS[key]], d[key])
+                assert abs(log[j, ops.LS[key]] - d[key]) < TOL, (it, j, key, log[j, ops.LS[key]], d[key])
         sd = model.state_dict()
         for k in O.param_names(ocfg):
-            np.testing.assert_allclose(sd[k].cpu().numpy(), olearner.st[k].numpy(), atol=2 * E.TOL, err_msg=k)
+            np.testing.assert_allclose(sd[k].cpu().numpy(), olearner.st[k].numpy(), atol=2 * TOL, err_msg=k)

@@ -12,6 +12,7 @@ from sample_factory_b200.cfg import default_cfg
 from sample_factory_b200.learner import Learner
 from sample_factory_b200.model import ModelSpec
 from tests import mixed_oracle as MO
+from tests.golden_utils import load_mixed_case
 
 
 def _spec(heads, **kw):
@@ -117,17 +118,6 @@ def test_restatement_matches_torch_distributions():
 
 # ----------------------------------------------------------------------------------------------- reference fixtures
 MIXED_CASES = ["tiny_mixed", "tiny_mixed_kl", "tiny_wide_mixed"]
-
-
-def load_mixed_case(name):
-    """a fixture of tests/golden/make_golden_mixed.py -> (npz, meta, MixedCfg)"""
-    import dataclasses
-
-    from tests.golden_utils import load_case
-
-    z, meta, cfg = load_case(name)
-    MO.install()
-    return z, meta, MO.MixedCfg(**dataclasses.asdict(cfg), action_heads=[tuple(h) for h in meta["action_heads"]])
 
 
 @pytest.mark.parametrize("name", MIXED_CASES)
