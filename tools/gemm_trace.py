@@ -21,12 +21,13 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+from tools.feature_bench import card  # noqa: E402
 
 M, H, OBS, A = 32768, 512, 64, 8
 
@@ -133,10 +134,10 @@ def main():
          lambda: ops.linear_backward(dz, x0, W1, ops.ACT["none"], dW1, None, None, eng, ws)),
     ]
     trace = torch.zeros(4096 * ops.GEMM_TRACE_WORDS, dtype=torch.int64, device=dev)
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    result = {"gpu": gpu, "lib": args.lib or "in-tree", "reps": args.reps, "gemms": {}}
-    print(f"{gpu}; library: {result['lib']}; means over {args.reps} launches, us")
+    hw = card()
+    result = {**hw, "lib": args.lib or "in-tree", "reps": args.reps, "gemms": {}}
+    print(f"{hw['gpu']} ({hw['power_limit_w']} W, {hw['max_sm_clock_mhz']} MHz); library: {result['lib']}; means over "
+          f"{args.reps} launches, us")
     try:
         for name, fn in gemms:
             fn()

@@ -14,12 +14,13 @@ import argparse
 import json
 import os
 import re
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+from tools.feature_bench import card  # noqa: E402
 
 import torch  # noqa: E402
 
@@ -87,10 +88,9 @@ def main():
         d["launches_per_iter"] += 1.0 / args.iters
     total = sum(d["us_per_iter"] for d in per.values())
     rows = sorted(per.items(), key=lambda kv: -kv[1]["us_per_iter"])
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    hw = card()
     result = {
-        "gpu": gpu,
+        **hw,
         "workload": bench.WORKLOAD,
         "iters": args.iters,
         "gpu_us_per_iter": total,
@@ -100,7 +100,8 @@ def main():
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "learner_profile.json"), "w") as f:
         json.dump(result, f, indent=1)
-    print(f"{gpu}: {total / 1e3:.3f} ms of kernel time per iteration")
+    print(f"{hw['gpu']} ({hw['power_limit_w']} W, {hw['max_sm_clock_mhz']} MHz): {total / 1e3:.3f} ms of kernel time per "
+          "iteration")
     for k, d in rows[:20]:
         print(f"  {d['us_per_iter']:9.1f} us  {d['launches_per_iter']:6.1f} x  {k}")
 

@@ -25,12 +25,13 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+from tools.feature_bench import card  # noqa: E402
 
 import torch  # noqa: E402
 
@@ -134,18 +135,18 @@ def main():
         lib().call("sfb200_rollout_set_trace", None)
     form = {1: "fp16 split", 0: "tf32 split"}.get(ops.rollout_last_form(), "?")
     per = {name: round(s / count, 2) for (name, _, _), s in zip(PHASES, sums)}
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    hw = card()
     sub = {name: round(v / n, 2) for (name, _, _), v, n in zip(SUBPHASES, sub_sums, sub_counts) if n}
     total = sum(per.values())
     waves = cta_summary(ctas, total)
-    result = {"gpu": gpu, "workload": bench.WORKLOAD, "form": form, "rollouts": args.iters, "steps_per_rollout": T,
+    result = {**hw, "workload": bench.WORKLOAD, "form": form, "rollouts": args.iters, "steps_per_rollout": T,
               "us_per_step": per, "us_per_step_total": round(total, 2), "us_per_step_sub": sub,
               "occupancy": {"clusters_needed": needed, "clusters_resident": resident}, "ctas": waves}
     os.makedirs(args.out, exist_ok=True)
     with open(os.path.join(args.out, "rollout_trace.json"), "w") as f:
         json.dump(result, f, indent=1)
-    print(f"{gpu}: persistent rollout kernel, {form} form, us per step (mean of steps 1..{T - 1}, {args.iters} rollouts)")
+    print(f"{hw['gpu']} ({hw['power_limit_w']} W, {hw['max_sm_clock_mhz']} MHz): persistent rollout kernel, {form} form, "
+          f"us per step (mean of steps 1..{T - 1}, {args.iters} rollouts)")
     for name, v in per.items():
         print(f"  {name:16s} {v:8.2f}")
     print(f"  {'step':16s} {total:8.2f}")
