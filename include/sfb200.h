@@ -753,6 +753,26 @@ int sfb200_clip_lamb_step(float* p, float* g, float* m, float* v, int64_t n, con
                           double beta1, double beta2, double eps, double weight_decay, double min_trust,
                           double max_grad_norm, const double* lr_scale_num, const double* lr_scale_den,
                           float* grad_norm_out, void* workspace, void* stream);
+/* Graph-replayable LAMB, to sfb200_clip_lamb_step what sfb200_clip_adam_step_dev is to sfb200_clip_adam_step: the
+ * optimizer steps already taken (int64[1]) and the learning rate (double[1]) are read from device memory.  The kernel
+ * forms the bias corrections (float)(1/(1 - beta1^t)) and (float)(1/sqrt(1 - beta2^t)) with the host path's double
+ * expression; the update itself is the same code. */
+int sfb200_clip_lamb_step_dev(float* p, float* g, float* m, float* v, int64_t n, const int64_t* seg_offsets,
+                              const int64_t* seg_numel, int num_tensors, int64_t max_numel, const int64_t* steps_done_dev,
+                              const double* lr_dev, double beta1, double beta2, double eps, double weight_decay,
+                              double min_trust, double max_grad_norm, const double* lr_scale_num,
+                              const double* lr_scale_den, float* grad_norm_out, void* workspace, void* stream);
+
+/* The learner's learning-rate rule between two minibatches, on the device (one thread), for a learner replayed as CUDA
+ * graphs.  Updates lr_dev (double[1]) in place with float64 operations that are each rounded (nothing contracted), so
+ * the result is bit-identical to the host's Python arithmetic (learner.py KlAdaptiveScheduler / LinearDecayScheduler):
+ *   rule 0, KL-adaptive per minibatch: kl = kl_dev[0] (the minibatch's kl_old_mean, all-reduced under data parallelism)
+ *       if kl > 2 thr: lr = max(lr / 1.5, min_lr);  then if kl < 0.5 thr: lr = min(lr * 1.5, max_lr)
+ *   rule 1, linear decay: step = ++step_dev[0] (the schedule's own counter, not the optimizer's);
+ *       lr = step >= num_updates ? 0 : lr0 + (0 - lr0) * (step / num_updates)
+ * Arguments a rule does not use are ignored (may be NULL / 0). */
+int sfb200_lr_schedule_step(int rule, double* lr_dev, const double* kl_dev, double kl_threshold, double min_lr,
+                            double max_lr, int64_t* step_dev, int64_t num_updates, double lr0, void* stream);
 
 /* ---------------------------------------------------------------- data parallel (NVLink peer memory) ----
  * New functionality (the reference has no collective, SURVEY 2a / 8e): G ranks x N envs == one process with G*N envs.

@@ -44,12 +44,14 @@ __global__ void __launch_bounds__(256) lamb_stage1_kernel(const float* __restric
                                                           float* __restrict__ m, float* __restrict__ v,
                                                           const int64_t* __restrict__ seg_off,
                                                           const int64_t* __restrict__ seg_n, float b1, float omb1, float b2,
-                                                          float omb2, float inv_bc1, float inv_bc2_sqrt, float eps, float wd,
+                                                          float omb2, float inv_bc1, float inv_bc2_sqrt,
+                                                          const int64_t* __restrict__ steps_done_dev, double beta1,
+                                                          double beta2, float eps, float wd,
                                                           float max_norm, const double* __restrict__ gpart, int n_gpart,
                                                           float* __restrict__ grad_norm_out, double* __restrict__ part,
                                                           int chunks_max) {
     __shared__ double sm[2][8];
-    __shared__ float s_coef;
+    __shared__ float s_coef, s_inv_bc1, s_inv_bc2_sqrt;
     if (threadIdx.x < 32) {
         double t = 0.0;
         for (int k = threadIdx.x; k < n_gpart; k += 32) t += gpart[k];
@@ -58,10 +60,22 @@ __global__ void __launch_bounds__(256) lamb_stage1_kernel(const float* __restric
             const float total = (float)sqrt(t);
             s_coef = max_norm > 0.f ? fminf(__fdiv_rn(max_norm, total + 1e-6f), 1.0f) : 1.f;
             if (grad_norm_out && blockIdx.x == 0 && blockIdx.y == 0) grad_norm_out[0] = total;
+            if (steps_done_dev) {
+                // the step count lives on the device (a CUDA-graph-replayed learner): the host expression of
+                // sfb200_clip_lamb_step, in double and in the same order
+                const double step = (double)(steps_done_dev[0] + 1);
+                const double bc1 = __dsub_rn(1.0, pow(beta1, step)), bc2 = __dsub_rn(1.0, pow(beta2, step));
+                inv_bc1 = (float)__ddiv_rn(1.0, bc1);
+                inv_bc2_sqrt = (float)__ddiv_rn(1.0, __dsqrt_rn(bc2));
+            }
+            s_inv_bc1 = inv_bc1;
+            s_inv_bc2_sqrt = inv_bc2_sqrt;
         }
     }
     __syncthreads();
     const float coef = s_coef;
+    inv_bc1 = s_inv_bc1;
+    inv_bc2_sqrt = s_inv_bc2_sqrt;
     const int t_idx = blockIdx.y;
     const int64_t off = seg_off[t_idx], n = seg_n[t_idx];
     const int64_t c0 = (int64_t)blockIdx.x * kLambChunk;
@@ -118,18 +132,47 @@ __global__ void __launch_bounds__(256) lamb_stage3_kernel(float* __restrict__ p,
                                                           const int64_t* __restrict__ seg_off,
                                                           const int64_t* __restrict__ seg_n,
                                                           const float* __restrict__ trust, double lr,
+                                                          const double* __restrict__ lr_dev,
                                                           const double* __restrict__ lr_num,
                                                           const double* __restrict__ lr_den) {
     const int t_idx = blockIdx.y;
     const int64_t off = seg_off[t_idx], n = seg_n[t_idx];
-    double lr_eff = lr;
-    if (lr_num && lr_den) lr_eff = lr * lr_num[0] / lr_den[0];          // learner.py:788-794
+    double lr_eff = lr_dev ? lr_dev[0] : lr;
+    if (lr_num && lr_den) lr_eff = lr_eff * lr_num[0] / lr_den[0];      // learner.py:788-794
     const float step = (float)lr_eff * trust[t_idx];
     const int64_t c0 = (int64_t)blockIdx.x * kLambChunk;
     for (int64_t i = c0 + threadIdx.x; i < n && i < c0 + kLambChunk; i += 256) {
         const int64_t j = off + i;
         p[j] = p[j] - step * u[j];                                      // p.add_(adam_step, alpha=-lr * trust_ratio)
     }
+}
+
+// Learning-rate rules between minibatches (learner.py KlAdaptiveScheduler / LinearDecayScheduler) for a learner replayed
+// as CUDA graphs.  One thread; every operation is an explicitly rounded double operation so nothing is contracted and
+// the result is bit-identical to the host's Python float arithmetic.  Python's max(a, b) / min(a, b) return `a` unless
+// `b` is strictly larger / smaller: the selects below keep that order.
+__global__ void lr_schedule_kernel(int rule, double* __restrict__ lr_dev, const double* __restrict__ kl_dev,
+                                   double thr, double min_lr, double max_lr, int64_t* __restrict__ step_dev,
+                                   int64_t num_updates, double lr0) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    double lr = lr_dev[0];
+    if (rule == 0) {
+        const double kl = kl_dev[0];
+        if (kl > __dmul_rn(2.0, thr)) {
+            const double t = __ddiv_rn(lr, 1.5);
+            lr = min_lr > t ? min_lr : t;
+        }
+        if (kl < __dmul_rn(0.5, thr)) {
+            const double t = __dmul_rn(lr, 1.5);
+            lr = max_lr < t ? max_lr : t;
+        }
+    } else {
+        const int64_t step = step_dev[0] + 1;
+        step_dev[0] = step;
+        lr = step >= num_updates ? 0.0
+                                 : __dadd_rn(lr0, __dmul_rn(__dsub_rn(0.0, lr0), __ddiv_rn((double)step, (double)num_updates)));
+    }
+    lr_dev[0] = lr;
 }
 
 }  // namespace sfb
@@ -194,13 +237,13 @@ int64_t sfb200_lamb_workspace_bytes(int num_tensors, int64_t max_numel) {
     return (int64_t)kNormBlocks * 8 + (int64_t)num_tensors * chunks * 2 * 8 + (int64_t)num_tensors * 4 + 64;
 }
 
-int sfb200_clip_lamb_step(float* p, float* g, float* m, float* v, int64_t n, const int64_t* seg_offsets,
-                          const int64_t* seg_numel, int num_tensors, int64_t max_numel, int64_t step, double lr,
-                          double beta1, double beta2, double eps, double weight_decay, double min_trust,
-                          double max_grad_norm, const double* lr_scale_num, const double* lr_scale_den,
-                          float* grad_norm_out, void* workspace, void* stream) {
+static int clip_lamb_impl(float* p, float* g, float* m, float* v, int64_t n, const int64_t* seg_offsets,
+                          const int64_t* seg_numel, int num_tensors, int64_t max_numel, int64_t step,
+                          const int64_t* step_dev, double lr, const double* lr_dev, double beta1, double beta2, double eps,
+                          double weight_decay, double min_trust, double max_grad_norm, const double* lr_scale_num,
+                          const double* lr_scale_den, float* grad_norm_out, void* workspace, void* stream) {
     SFB_CHECK_ARG(p && g && m && v && seg_offsets && seg_numel && workspace && n > 0 && num_tensors > 0 && max_numel > 0 &&
-                      step >= 1, "clip_lamb_step: bad arguments");
+                      (step >= 1 || step_dev), "clip_lamb_step: bad arguments");
     SFB_CHECK_ARG((lr_scale_num == nullptr) == (lr_scale_den == nullptr), "clip_lamb_step: lr_scale num/den mismatch");
     SFB_CHECK_ARG(min_trust >= 0.0 && min_trust <= 1.0, "clip_lamb_step: min_trust must be in [0, 1]");
     cudaStream_t st = (cudaStream_t)stream;
@@ -212,17 +255,53 @@ int sfb200_clip_lamb_step(float* p, float* g, float* m, float* v, int64_t n, con
     if (nb > kNormBlocks) nb = kNormBlocks;
     sumsq_kernel<<<(unsigned)nb, 256, 0, st>>>(g, n, gpart);     // global grad norm over the whole flat buffer (padding is 0)
     SFB_LAUNCH_OK();
-    const double bc1 = 1.0 - pow(beta1, (double)step);
-    const double bc2 = 1.0 - pow(beta2, (double)step);
+    float inv_bc1 = 0.f, inv_bc2_sqrt = 0.f;     // (formed in the kernel from *step_dev when the step lives on the device)
+    if (!step_dev) {
+        const double bc1 = 1.0 - pow(beta1, (double)step);
+        const double bc2 = 1.0 - pow(beta2, (double)step);
+        inv_bc1 = (float)(1.0 / bc1);
+        inv_bc2_sqrt = (float)(1.0 / sqrt(bc2));
+    }
     dim3 grid((unsigned)chunks, (unsigned)num_tensors);
     lamb_stage1_kernel<<<grid, 256, 0, st>>>(p, g, m, v, seg_offsets, seg_numel, (float)beta1, (float)(1.0 - beta1), (float)beta2,
-                                             (float)(1.0 - beta2), (float)(1.0 / bc1), (float)(1.0 / sqrt(bc2)), (float)eps,
+                                             (float)(1.0 - beta2), inv_bc1, inv_bc2_sqrt, step_dev, beta1, beta2, (float)eps,
                                              (float)weight_decay, (float)max_grad_norm, gpart, (int)nb, grad_norm_out, part,
                                              chunks);
     SFB_LAUNCH_OK();
     lamb_stage2_kernel<<<(unsigned)num_tensors, 32, 0, st>>>(part, seg_numel, chunks, (float)min_trust, trust);
     SFB_LAUNCH_OK();
-    lamb_stage3_kernel<<<grid, 256, 0, st>>>(p, g, seg_offsets, seg_numel, trust, lr, lr_scale_num, lr_scale_den);
+    lamb_stage3_kernel<<<grid, 256, 0, st>>>(p, g, seg_offsets, seg_numel, trust, lr, lr_dev, lr_scale_num, lr_scale_den);
+    SFB_LAUNCH_OK();
+    return 0;
+}
+
+int sfb200_clip_lamb_step(float* p, float* g, float* m, float* v, int64_t n, const int64_t* seg_offsets,
+                          const int64_t* seg_numel, int num_tensors, int64_t max_numel, int64_t step, double lr,
+                          double beta1, double beta2, double eps, double weight_decay, double min_trust,
+                          double max_grad_norm, const double* lr_scale_num, const double* lr_scale_den,
+                          float* grad_norm_out, void* workspace, void* stream) {
+    return clip_lamb_impl(p, g, m, v, n, seg_offsets, seg_numel, num_tensors, max_numel, step, nullptr, lr, nullptr, beta1,
+                          beta2, eps, weight_decay, min_trust, max_grad_norm, lr_scale_num, lr_scale_den, grad_norm_out,
+                          workspace, stream);
+}
+
+int sfb200_clip_lamb_step_dev(float* p, float* g, float* m, float* v, int64_t n, const int64_t* seg_offsets,
+                              const int64_t* seg_numel, int num_tensors, int64_t max_numel, const int64_t* steps_done_dev,
+                              const double* lr_dev, double beta1, double beta2, double eps, double weight_decay,
+                              double min_trust, double max_grad_norm, const double* lr_scale_num,
+                              const double* lr_scale_den, float* grad_norm_out, void* workspace, void* stream) {
+    SFB_CHECK_ARG(steps_done_dev && lr_dev, "clip_lamb_step_dev: the device step counter and learning rate are required");
+    return clip_lamb_impl(p, g, m, v, n, seg_offsets, seg_numel, num_tensors, max_numel, 0, steps_done_dev, 0.0, lr_dev,
+                          beta1, beta2, eps, weight_decay, min_trust, max_grad_norm, lr_scale_num, lr_scale_den,
+                          grad_norm_out, workspace, stream);
+}
+
+int sfb200_lr_schedule_step(int rule, double* lr_dev, const double* kl_dev, double kl_threshold, double min_lr,
+                            double max_lr, int64_t* step_dev, int64_t num_updates, double lr0, void* stream) {
+    SFB_CHECK_ARG(lr_dev && (rule == 0 || rule == 1) && (rule != 0 || kl_dev) && (rule != 1 || step_dev),
+                  "lr_schedule_step: bad arguments");
+    lr_schedule_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(rule, lr_dev, kl_dev, kl_threshold, min_lr, max_lr, step_dev,
+                                                          num_updates, lr0);
     SFB_LAUNCH_OK();
     return 0;
 }

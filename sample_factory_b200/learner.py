@@ -113,7 +113,8 @@ class Learner:
         self.policy_id = cfg.policy_id
         self.train_step = 0  # number of SGD steps == policy version (learner.py:142, :388-392)
         self.env_steps = 0
-        self.curr_lr = cfg.learning_rate
+        self._curr_lr = cfg.learning_rate        # (see the curr_lr property: lr_dev holds it while train() replays graphs)
+        self._lr_on_device = False
         self.lr_scheduler = get_lr_scheduler(cfg)
         self.last_stats: Dict[str, float] = {}
 
@@ -276,30 +277,32 @@ class Learner:
             self.perm_dev = torch.arange(E, dtype=torch.int32, device=dev)
             self._perm_queue: List[np.ndarray] = []      # explicit permutations for the next epochs (tests); else np.random
             self._sh: Dict[str, Tensor] = {}
-        # CUDA-graph replay of the whole train() (cfg.learner_cuda_graph): possible when nothing in it depends on host
-        # state -- constant lr schedule, one epoch (no early-stopping read-back), Adam.  The step counters and the
-        # learning rate then live in device memory (read by the *_dev entry points).  Data parallel: opt-in with
-        # SFB200_DP_GRAPH=1 -- the NCCL all-reduces are then captured with the kernels; off by default until the multi-rank capture is covered
-        # by the equivalence test (tests/dp_worker.py, see DESIGN section 7).
+        # CUDA-graph replay of train() (cfg.learner_cuda_graph): one graph per epoch and trajectory set.  The step
+        # counters, the learning rate and the per-minibatch learning-rate rules live in device memory (the *_dev entry
+        # points, sfb200_lr_schedule_step); what stays on the host is the one sync per epoch the eager path also takes
+        # (early stopping, kl_adaptive_epoch), between two replays.
         # Data parallel: every exchange is a libsfb200 kernel over NVLink peer memory (csrc/comm.cu) -- the gradient lives in
         # the comm buffer the peers read, so train() is kernels only and is captured like the single-GPU learner.
-        # SFB200_DP_COMM=nccl keeps the exchanges on torch.distributed (then the graph needs SFB200_DP_GRAPH=1).
+        # SFB200_DP_COMM=nccl keeps the exchanges on torch.distributed: its graph is opt-in with SFB200_DP_GRAPH=1 (the
+        # NCCL all-reduces are then captured with the kernels) and limited to constant lr, one epoch and Adam, the case
+        # the multi-rank equivalence test covers (tests/dp_worker.py, see DESIGN section 7).
         self.comm: Optional[PeerComm] = None
         if self.world_size > 1 and model.flat.is_cuda and peer_comm_wanted():
             self.comm = PeerComm(dev, model.flat.numel(), self.pg)
             model.rebind_grad(self.comm.grad)
             self.grad_reduced = torch.zeros_like(model.flat)
             self._ls_keep, self._ls_max, self._ls_min, self._ls_avg = _ls_masks()
-        dp_graph = self.comm is not None or os.environ.get("SFB200_DP_GRAPH", "0") == "1"
-        self.use_graph = (bool(getattr(cfg, "learner_cuda_graph", False)) and cfg.lr_schedule == "constant" and
-                          cfg.num_epochs == 1 and cfg.optimizer == "adam" and (self.world_size == 1 or dp_graph))
-        self.counters_dev = torch.zeros(2, dtype=torch.int64, device=dev)     # [optimizer steps taken, train_step]
+        nccl_graph = (os.environ.get("SFB200_DP_GRAPH", "0") == "1" and cfg.lr_schedule == "constant" and
+                      cfg.num_epochs == 1 and cfg.optimizer == "adam")
+        self.use_graph = (bool(getattr(cfg, "learner_cuda_graph", False)) and
+                          (self.world_size == 1 or self.comm is not None or nccl_graph))
+        # [optimizer steps taken, train_step, linear-decay schedule step]
+        self.counters_dev = torch.zeros(3, dtype=torch.int64, device=dev)
         self.lr_dev = torch.full((1,), float(cfg.learning_rate), dtype=torch.float64, device=dev)
-        self._graph: Optional[torch.cuda.CUDAGraph] = None
-        self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
-        self._graph_batch_ptrs = None
-        self._graph_calls = 0
-        self._graph_launches = 0
+        self._graph: Optional[torch.cuda.CUDAGraph] = None            # the last graph replayed
+        self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}          # (trajectory set, epoch) -> its graph
+        self._epoch_launches: Dict[int, int] = {}                     # epoch -> launches of its body (eager warm-up)
+        self._replayed_launches = 0
 
     # ------------------------------------------------------------------------------------------------------------
     def _allreduce(self, t: Tensor) -> None:
@@ -556,7 +559,8 @@ class Learner:
                 dev_ctr = self.use_graph
                 ops.dp_grad_allreduce_clip_adam(
                     self.comm.comm, grad, m.flat, m.exp_avg, m.exp_avg_sq, self.opt_step,
-                    self.counters_dev[0:1] if dev_ctr else None, self.curr_lr, self.lr_dev if dev_ctr else None,
+                    self.counters_dev[0:1] if dev_ctr else None, 0.0 if dev_ctr else self.curr_lr,
+                    self.lr_dev if dev_ctr else None,
                     cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps, cfg.max_grad_norm, self.num_valid_dev,
                     self.exp_size_total_dev(), self.grad_norm_log[log_idx: log_idx + 1], self.comm.workspace)
                 if dev_ctr:
@@ -568,7 +572,13 @@ class Learner:
             ops.dp_grad_allreduce(self.comm.comm, grad, self.comm.workspace)
         elif self.world_size > 1:
             dist.all_reduce(m.grad, op=dist.ReduceOp.SUM, group=self.pg)
-        if cfg.optimizer == "lamb":
+        if cfg.optimizer == "lamb" and self.use_graph:
+            ops.clip_lamb_step_dev(m.flat, grad, m.exp_avg, m.exp_avg_sq, self.lamb_off, self.lamb_numel, self.lamb_max,
+                                   self.counters_dev[0:1], self.lr_dev, cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps, 1e-4,
+                                   0.01, cfg.max_grad_norm, self.num_valid_dev, self.exp_size_total_dev(),
+                                   self.grad_norm_log[log_idx : log_idx + 1], self.lamb_ws)
+            ops.advance_counters(self.counters_dev[0:1], self.counters_dev[1:2])
+        elif cfg.optimizer == "lamb":
             ops.clip_lamb_step(m.flat, grad, m.exp_avg, m.exp_avg_sq, self.lamb_off, self.lamb_numel, self.lamb_max,
                                self.opt_step, self.curr_lr, cfg.adam_beta1, cfg.adam_beta2, cfg.adam_eps, 1e-4, 0.01,
                                cfg.max_grad_norm, self.num_valid_dev, self.exp_size_total_dev(),
@@ -772,6 +782,8 @@ class Learner:
         cfg = self.cfg
         if self.use_graph:
             return self._train_graphed(batch)
+        if self._lr_on_device:      # graphs ran before (use_graph was switched off since): continue from the device's lr
+            self._curr_lr, self._lr_on_device = float(self.lr_dev.item()), False
         launches0 = ops.launch_count()
         if self.shuffle:
             self._upload_permutation()
@@ -804,17 +816,10 @@ class Learner:
             if reduced_upto < log_idx:     # data parallel: global loss statistics before any host decision / report
                 self._allreduce_loss_rows(self.loss_stats_log[reduced_upto: log_idx])
                 reduced_upto = log_idx
-            need_host = cfg.num_epochs > 1 or self.lr_scheduler.invoke_after_each_epoch()
-            if need_host:
-                rows = self.loss_stats_log[first:log_idx].cpu()        # one sync per epoch (reference: per minibatch)
-                if self.lr_scheduler.invoke_after_each_epoch():
-                    recent_kls.extend(rows[:, ops.LS["kl_old_mean"]].tolist())
-                    self.curr_lr = self.lr_scheduler.update(self.curr_lr, recent_kls)
-                actor = rows[:, ops.LS["policy_loss"]] + rows[:, ops.LS["exploration_loss"]] + rows[:, ops.LS["kl_loss"]]
-                new_loss = float(actor.mean())                          # :827
-                if abs(prev_epoch_actor_loss - new_loss) < 1e-6:        # :829-837 early stopping
+            if self._needs_epoch_sync():
+                prev_epoch_actor_loss = self._end_of_epoch(first, log_idx, recent_kls, prev_epoch_actor_loss)
+                if prev_epoch_actor_loss is None:
                     break
-                prev_epoch_actor_loss = new_loss
         if self.shuffle:
             self._perm_queue = []          # (permutations set for epochs an early stop skipped do not leak into the next call)
         self.num_minibatches_done = log_idx
@@ -854,57 +859,130 @@ class Learner:
         self.curr_lr = other.curr_lr
         self.train_step += self.cfg.max_policy_lag + 1
 
-    def _train_body(self, batch: Dict[str, Tensor]) -> None:
-        """one epoch of minibatch steps with no host dependence (the graph-capturable form of train())"""
-        self._prepare_batch(batch)
-        for b in range(self.cfg.num_batches_per_epoch):
-            self._minibatch_step(batch, b, b)
-        self._allreduce_loss_rows(self.loss_stats_log[: self.cfg.num_batches_per_epoch])
+    @property
+    def curr_lr(self) -> float:
+        """The learning rate.  While train() replays CUDA graphs it lives in lr_dev, where the device-side rules advance
+        it: reading it then is a host sync, and setting it writes lr_dev (checkpoint resume, PBT)."""
+        return float(self.lr_dev.item()) if self._lr_on_device else self._curr_lr
+
+    @curr_lr.setter
+    def curr_lr(self, lr: float) -> None:
+        if self.use_graph:
+            self.lr_dev.fill_(float(lr))
+            self._lr_on_device = True
+        else:
+            self._curr_lr, self._lr_on_device = lr, False
+
+    def _needs_epoch_sync(self) -> bool:
+        """the host reads an epoch's loss rows (early stopping, kl_adaptive_epoch) unless nothing could use them"""
+        return self.cfg.num_epochs > 1 or self.lr_scheduler.invoke_after_each_epoch()
+
+    def _end_of_epoch(self, first: int, last: int, recent_kls: List[float], prev_loss: float) -> Optional[float]:
+        """The host decisions after the epoch whose loss rows are [first, last), with one sync (the reference syncs per
+        minibatch): the per-epoch learning-rate rule, then early stopping (:827-837).  -> the epoch's actor loss, or
+        None to stop."""
+        rows = self.loss_stats_log[first:last].cpu()
+        if self.lr_scheduler.invoke_after_each_epoch():
+            recent_kls.extend(rows[:, ops.LS["kl_old_mean"]].tolist())
+            self.curr_lr = self.lr_scheduler.update(self.curr_lr, recent_kls)
+        actor = rows[:, ops.LS["policy_loss"]] + rows[:, ops.LS["exploration_loss"]] + rows[:, ops.LS["kl_loss"]]
+        new_loss = float(actor.mean())
+        return None if abs(prev_loss - new_loss) < 1e-6 else new_loss
+
+    def _epoch_body(self, batch: Dict[str, Tensor], epoch: int) -> None:
+        """Epoch `epoch` of train() with no host dependence (the graph-capturable form).  Epoch 0 prepares the batch; a
+        later epoch over shuffled minibatches gathers them in its new order first.  The per-minibatch learning-rate rules
+        run on the device after every optimizer step, on the all-reduced loss row like the eager path."""
+        cfg, sched = self.cfg, self.lr_scheduler
+        nmb = cfg.num_batches_per_epoch
+        if epoch == 0:
+            self._prepare_batch(batch)
+        elif self.shuffle:
+            self._bind_minibatch_arrays(batch)
+            if not cfg.with_vtrace:
+                self._minibatch_adv_partials()
+        kl_per_minibatch = isinstance(sched, KlAdaptiveScheduler) and sched.invoke_after_each_minibatch()
+        first = epoch * nmb
+        for b in range(nmb):
+            i = first + b
+            self._minibatch_step(batch, b, i)
+            if kl_per_minibatch:
+                self._allreduce_loss_rows(self.loss_stats_log[i: i + 1])
+                ops.lr_schedule_kl_adaptive(self.lr_dev, self.loss_stats_log[i, ops.LS["kl_old_mean"]], sched.thr,
+                                            sched.min_lr, sched.max_lr)
+            elif isinstance(sched, LinearDecayScheduler):
+                ops.lr_schedule_linear_decay(self.lr_dev, self.counters_dev[2:3], sched.num_updates, sched.lr0)
+        if not kl_per_minibatch:
+            self._allreduce_loss_rows(self.loss_stats_log[first: first + nmb])
+
+    def _run_epoch(self, batch: Dict[str, Tensor], ptrs: tuple, epoch: int) -> int:
+        """Epoch `epoch` of a graphed train(): eagerly the first time any trajectory set reaches it (kernel attributes,
+        allocator warm-up), then captured once per trajectory set and replayed.  -> the launches replayed."""
+        if epoch not in self._epoch_launches:
+            n0 = ops.launch_count()
+            self._epoch_body(batch, epoch)
+            self._epoch_launches[epoch] = ops.launch_count() - n0
+            return 0
+        graph = self._graphs.get((ptrs, epoch))
+        captured = graph is None
+        if captured:
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            # (multi-rank with NCCL exchanges: the watchdog thread polls events while this thread captures)
+            mode = "thread_local" if (self.world_size > 1 and self.comm is None) else "global"
+            with torch.cuda.graph(graph, capture_error_mode=mode):
+                self._epoch_body(batch, epoch)
+            self._graphs[(ptrs, epoch)] = graph
+        self._graph = graph
+        graph.replay()
+        return 0 if captured else self._epoch_launches[epoch]     # (a capture pass counted its launches itself)
 
     def _train_graphed(self, batch: Dict[str, Tensor]) -> Dict[str, float]:
-        """train() as ONE graph launch: the first call runs eagerly (kernel attributes, allocator warm-up), the second
-        captures, later calls replay.  Host mirrors of the counters advance alongside the device ones."""
-        cfg = self.cfg
+        """train() as one graph launch per epoch, with the eager path's host sync between two epochs only where it has a
+        decision to take.  Host mirrors of the counters advance by the minibatches that ran."""
+        cfg, sched = self.cfg, self.lr_scheduler
         nmb = cfg.num_batches_per_epoch
         # one captured graph per trajectory set (the runner may train on several row ranges of the rollout buffers, or on an
         # accumulation buffer: cfg/arguments.py:147-178 allows datasets that are a fraction / a multiple of one rollout)
         ptrs = tuple(v.data_ptr() for v in batch.values())
-        # the device counters / lr follow the host values whenever these were changed from outside (checkpoint resume)
-        self.counters_dev.copy_(torch.tensor([self.opt_step, self.train_step], dtype=torch.int64), non_blocking=True)
-        self.lr_dev.fill_(float(self.curr_lr))
+        # the device counters follow the host values whenever these were changed from outside (checkpoint resume)
+        decay_step = sched.step if isinstance(sched, LinearDecayScheduler) else 0
+        self.counters_dev.copy_(torch.tensor([self.opt_step, self.train_step, decay_step], dtype=torch.int64),
+                                non_blocking=True)
+        if not self._lr_on_device:
+            self.lr_dev.fill_(float(self._curr_lr))
+            self._lr_on_device = True
         opt0, train0 = self.opt_step, self.train_step
+        recent_kls: List[float] = []
+        prev_epoch_actor_loss = 1e9
+        done = replayed = launches = 0
+        for epoch in range(cfg.num_epochs):
+            if self.shuffle:
+                self._upload_permutation()       # (H2D copy enqueued in front of the graph; the gathers are captured)
+            replayed += self._run_epoch(batch, ptrs, epoch)
+            launches += self._epoch_launches[epoch]
+            done += nmb
+            if self._needs_epoch_sync():
+                prev_epoch_actor_loss = self._end_of_epoch(done - nmb, done, recent_kls, prev_epoch_actor_loss)
+                if prev_epoch_actor_loss is None:
+                    break
         if self.shuffle:
-            self._upload_permutation()           # (H2D copy enqueued in front of the graph; the gathers are captured)
-        if self._graph_calls == 0:
-            n0 = ops.launch_count()
-            self._train_body(batch)
-            self._graph_launches = ops.launch_count() - n0
-        else:
-            graph = self._graphs.get(ptrs)
-            if graph is None:
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                # (multi-rank with NCCL exchanges: the watchdog thread polls events while this thread captures)
-                mode = "thread_local" if (self.world_size > 1 and self.comm is None) else "global"
-                with torch.cuda.graph(graph, capture_error_mode=mode):
-                    self._train_body(batch)
-                self._graphs[ptrs] = graph
-            self._graph = graph
-            self._graph_batch_ptrs = ptrs
-            graph.replay()
-        self._graph_calls += 1
+            self._perm_queue = []
         # _minibatch_step advanced the host mirrors during eager / capture passes only: set them explicitly
-        self.opt_step, self.train_step = opt0 + nmb, train0 + nmb
-        self.num_minibatches_done = nmb
-        self._snapshot_policy_lag(batch, nmb)
-        self.kernel_launches = self._graph_launches
+        self.opt_step, self.train_step = opt0 + done, train0 + done
+        if isinstance(sched, LinearDecayScheduler):
+            sched.step += done
+        self.num_minibatches_done = done
+        self._snapshot_policy_lag(batch, done)
+        self.kernel_launches = launches
+        self._replayed_launches = replayed
         self.env_steps += self.E * self.world_size * (cfg.env_frameskip if cfg.summaries_use_frameskip else 1)
         return dict(env_steps=self.env_steps, train_step=self.train_step)
 
     @property
     def graph_replay_launches(self) -> int:
         """kernel launches of the last train() that happened through graph replay (not seen by the launch counter)"""
-        return self._graph_launches if (self.use_graph and self._graph is not None and self._graph_calls > 2) else 0
+        return self._replayed_launches if self.use_graph else 0
 
     def _snapshot_policy_lag(self, batch: Dict[str, Tensor], n: int) -> None:
         """Keep the last minibatch's policy versions: the caller may overwrite the trajectory set (async join) before

@@ -1077,8 +1077,39 @@ def clip_adam_step_dev(p: Tensor, g: Tensor, m: Tensor, v: Tensor, steps_done_de
                _p(lr_scale_den, F64), _p(grad_norm_out, F32), workspace.data_ptr(), _stream())
 
 
+def clip_lamb_step_dev(p: Tensor, g: Tensor, m: Tensor, v: Tensor, seg_offsets: Tensor, seg_numel: Tensor, max_numel: int,
+                       steps_done_dev: Tensor, lr_dev: Tensor, beta1: float, beta2: float, eps: float, weight_decay: float,
+                       min_trust: float, max_grad_norm: float, lr_scale_num: Optional[Tensor],
+                       lr_scale_den: Optional[Tensor], grad_norm_out: Optional[Tensor], workspace: Tensor) -> None:
+    """clip_lamb_step with the step counter (int64[1], steps already taken) and the learning rate (float64[1]) in device
+    memory -- every argument is then static, so the launch can be replayed from a CUDA graph"""
+    for t in (p, g, m, v):
+        assert t.is_contiguous() and t.dim() == 1
+    T = seg_offsets.numel()
+    assert seg_numel.numel() == T and workspace.numel() * workspace.element_size() >= lamb_workspace_bytes(T, max_numel)
+    lib().call("sfb200_clip_lamb_step_dev", _p(p, F32), _p(g, F32), _p(m, F32), _p(v, F32), p.numel(), _p(seg_offsets, I64),
+               _p(seg_numel, I64), T, max_numel, _p(steps_done_dev, I64), _p(lr_dev, F64), beta1, beta2, eps, weight_decay,
+               min_trust, max_grad_norm, _p(lr_scale_num, F64), _p(lr_scale_den, F64), _p(grad_norm_out, F32),
+               workspace.data_ptr(), _stream())
+
+
 def advance_counters(a: Optional[Tensor], b: Optional[Tensor]) -> None:
     lib().call("sfb200_advance_counters", _p(a, I64), _p(b, I64), _stream())
+
+
+LR_RULE_KL_ADAPTIVE, LR_RULE_LINEAR_DECAY = 0, 1
+
+
+def lr_schedule_kl_adaptive(lr_dev: Tensor, kl_dev: Tensor, threshold: float, min_lr: float, max_lr: float) -> None:
+    """KlAdaptiveScheduler.update on one minibatch's KL (a float64 element of its loss row), applied to lr_dev in place"""
+    lib().call("sfb200_lr_schedule_step", LR_RULE_KL_ADAPTIVE, _p(lr_dev, F64), _p(kl_dev, F64), threshold, min_lr, max_lr,
+               None, 0, 0.0, _stream())
+
+
+def lr_schedule_linear_decay(lr_dev: Tensor, step_dev: Tensor, num_updates: int, lr0: float) -> None:
+    """LinearDecayScheduler.update: advances the schedule's device step counter (int64[1]) and writes lr_dev"""
+    lib().call("sfb200_lr_schedule_step", LR_RULE_LINEAR_DECAY, _p(lr_dev, F64), None, 0.0, 0.0, 0.0, _p(step_dev, I64),
+               num_updates, lr0, _stream())
 
 
 # ------------------------------------------------------------------------------------------------ recurrent core
