@@ -11,6 +11,10 @@ RO.load_stacked_case, SO.load_separate_rnn_case or DO.load_dict_case -- and then
 The keyword options of the replays name where a feature's check differs from the default one."""
 import math
 import os
+import re
+import subprocess
+import time
+import warnings
 from collections import namedtuple
 
 import numpy as np
@@ -44,6 +48,47 @@ def ops_for(engine="simt"):
 
 def g(seed):
     return torch.Generator().manual_seed(seed)
+
+
+TEMPLATED = r"\w+_kernel<[^<>]*>"           # the templated sfb kernels
+ANY_KERNEL = r"\w+_kernel(?:<[^<>]*>)?"      # every sfb kernel, templated or not
+
+
+def launched(fn, names=TEMPLATED, expected=None):
+    """the sfb kernels fn launches whose name (without the namespace) matches `names`.  The profiler keeps only device
+    records whose time stamps fall inside its capture window, so the window is padded on both sides.  Even so a record
+    can go missing (seen after a module had run many profiles with heavy device work between them).  fn is idempotent
+    and launches at least one kernel, so the profile is taken again when it holds no sfb kernel at all or, given the
+    `expected` set, only a strict subset of it.  A lost record only ever removes a name: a call that launches a kernel
+    outside `expected` shows it in every profile, and one that really launches fewer kernels shows the same strict
+    subset every time, so neither can pass check_launched."""
+    from torch.profiler import ProfilerActivity, profile
+
+    for attempt in range(3):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            time.sleep(0.02)
+            fn()
+            torch.cuda.synchronize()
+            time.sleep(0.02)
+        evs = [e.name for e in prof.events()]
+        mangled = [n for n in evs if n.startswith("_Z")]
+        if mangled:
+            evs += subprocess.run(["c++filt"], input="\n".join(mangled), capture_output=True, text=True,
+                                  check=True).stdout.splitlines()
+        got = {m.group(1) for n in evs for m in [re.search(rf"sfb::({names})", n)] if m}
+        if not any("sfb::" in n for n in evs):
+            warnings.warn(f"profile {attempt} recorded no sfb kernel ({len(evs)} events): taken again")
+        elif expected is not None and got < set(expected):
+            warnings.warn(f"profile {attempt} recorded only {sorted(got)} of {sorted(expected)}: taken again")
+        else:
+            break
+    return got
+
+
+def check_launched(fn, kernels, names=TEMPLATED):
+    got = launched(fn, names, expected=kernels)
+    assert got == set(kernels), f"launched {sorted(got)}, expected {sorted(kernels)}"
 
 
 @pytest.fixture(scope="module")

@@ -19,8 +19,6 @@ import math
 import os
 import re
 import subprocess
-import time
-import warnings
 
 import numpy as np
 import pytest
@@ -28,7 +26,7 @@ import torch
 
 from oracle import appo_oracle as O
 from tests import mixed_oracle as MO
-from tests.device_harness import DEV, g, masked_rows, ops_for, wide_tail
+from tests.device_harness import DEV, check_launched, g, masked_rows, ops_for, wide_tail
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BUILD = os.path.join(ROOT, "sample_factory_b200", "csrc", "build")
@@ -201,36 +199,6 @@ def test_every_instantiation_has_a_case():
 
 
 # ----------------------------------------------------------------------------------------------- helpers
-def _launched(fn):
-    """the templated sfb kernels fn launches.  The profiler keeps only device records whose time stamps fall inside its
-    capture window, so the window is padded on both sides.  fn is idempotent and launches at least one kernel: a
-    profile that holds no sfb kernel at all lost its device records and is taken again.  (A lost record can only fail
-    the exact comparison in _check_launched, never make a wrong instantiation pass.)"""
-    from torch.profiler import ProfilerActivity, profile
-
-    for attempt in range(3):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-            time.sleep(0.02)
-            fn()
-            torch.cuda.synchronize()
-            time.sleep(0.02)
-        names = [e.name for e in prof.events()]
-        mangled = [n for n in names if n.startswith("_Z")]
-        if mangled:
-            names += subprocess.run(["c++filt"], input="\n".join(mangled), capture_output=True, text=True,
-                                    check=True).stdout.splitlines()
-        if any("sfb::" in n for n in names):
-            break
-        warnings.warn(f"profile {attempt} recorded no sfb kernel ({len(names)} events): taken again")
-    return {m.group(1) for n in names for m in [re.search(r"sfb::(\w+_kernel<[^<>]*>)", n)] if m}
-
-
-def _check_launched(fn, kernels):
-    got = _launched(fn)
-    assert got == set(kernels), f"launched {sorted(got)}, expected {sorted(kernels)}"
-
-
 def _heads_of(space, layout):
     if space == "discrete":
         return [("discrete", layout)]
@@ -388,7 +356,7 @@ def _run_loss(space, layout, expl, valid, kernels):
                                        1.0, dl, dv, stats, ws)
             ops.action_ratio_mixed(dd["params"], kinds, sizes, dd["actions"], dd["lp_old"], ratio)
 
-    _check_launched(run, kernels)
+    check_launched(run, kernels)
     s = {k: stats[i].item() for k, i in ops.LS.items() if i < ops.LS_SIZE}
     out = dict(dl=dl.cpu(), dls=None if dls is None else dls.cpu(), dv=dv.cpu(), ratio=ratio.cpu())
     return d, s, out
@@ -513,7 +481,7 @@ def test_heads_tail_wide(space, layout, mode, kernels):
         kw = dict(noise=eps.to(DEV), deterministic=det, continuous=True, act_dim=ad, adaptive_stddev=adaptive,
                   learned_log_std=None if adaptive else learned.to(DEV), tanh_scale=0.0 if adaptive else TS)
         res = []
-        _check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, **kw)), kernels)
+        check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), params, A, **kw)), kernels)
         v, act, lp, env = res[0]
         means = raw[:, :ad] if adaptive else torch.tanh(raw[:, :ad] / TS) * TS
         log_std = raw[:, ad:] if adaptive else learned.expand(M, ad)
@@ -539,7 +507,7 @@ def test_heads_tail_wide(space, layout, mode, kernels):
         if space == "tuple":
             kw["head_sizes"] = segs
         res = []
-        _check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, **kw)), kernels)
+        check_launched(lambda: res.append(wide_tail(ops, h.to(DEV), Wv.to(DEV), bv.to(DEV), ld, A, **kw)), kernels)
         v, act, lp, env = res[0]
         assert torch.equal(ld.cpu(), logits)
         qq = torch.ones_like(q) if det else q
@@ -596,7 +564,7 @@ def test_heads_tail_wide_mixed(layout, kernels, deterministic):
     if deterministic:
         ops.set_sampling_mode(None, True)
     try:
-        _check_launched(run, kernels)
+        check_launched(run, kernels)
     finally:
         ops.set_sampling_mode(None, False)
     assert torch.equal(pd.cpu(), params)
@@ -649,7 +617,7 @@ def test_heads_forward(rows, H, ldh, A, mode, kernels):
     mask_dev = mask.to(DEV)              # (the sampling mode keeps a pointer to it)
     ops.set_sampling_mode(mask_dev if mode == "mask" else None, mode == "deterministic")
     try:
-        _check_launched(run, kernels)
+        check_launched(run, kernels)
     finally:
         ops.set_sampling_mode(None, False)
     hh = h.double()
@@ -693,7 +661,7 @@ def test_heads_backward(rows, H, A, act, kernels):
     ws = torch.empty(ops.heads_backward_workspace_bytes(H, A) // 4 + 4, device=DEV)
     args = (h.to(DEV), Wv.to(DEV).view(-1), Wa.to(DEV), dlogits.to(DEV), dvalues.to(DEV), ops.ACT[act], dz, dWv, dbv,
             dWa, dba, dbp, ws)
-    _check_launched(lambda: ops.heads_backward(*args), kernels)
+    check_launched(lambda: ops.heads_backward(*args), kernels)
     tol = dict(atol=1e-5, rtol=1e-4)          # test_gpu_kernels.test_heads_backward
     np.testing.assert_allclose(dz.cpu().numpy(), dz_ref.numpy(), **tol)
     np.testing.assert_allclose(dWa.cpu().numpy(), (dlogits.double().t() @ h.double()).numpy(), **tol)

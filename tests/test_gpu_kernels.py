@@ -10,7 +10,7 @@ import torch
 
 from oracle import appo_oracle as O
 
-from tests.device_harness import TOL, dev, g, ops_for  # noqa: F401  (dev: fixture)
+from tests.device_harness import TOL, dev, g, launched, ops_for  # noqa: F401  (dev: fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -747,11 +747,15 @@ def test_rnn_cell_forward_backward(dev, rnn_type, M, H, IN):
 @pytest.mark.parametrize("engine_name", ["simt", "3xtf32"])
 @pytest.mark.parametrize("rnn_type", ["gru", "lstm"])
 @pytest.mark.parametrize("random_dones", [True, False])
-@pytest.mark.parametrize("T,N,D", [(5, 1, 1), (5, 64, 10), (27, 1, 42), (27, 64, 10), (37, 64, 42)])
+@pytest.mark.parametrize("T,N,D", [(5, 1, 1), (5, 64, 10), (27, 1, 42), (27, 64, 10), (37, 64, 42), (5, 64, 32),
+                                   (27, 64, 64)])
 def test_bptt_matches_loopy_torch_rnn(dev, T, N, D, random_dones, rnn_type, engine_name):
     """The reference's own recurrent-core check (tests/algo/test_rnn.py:10-75: T in {5,27,37}, N in {1,64}, D in {1,10,42},
     dones every 7th step or random) against the device BPTT: a step-by-step torch nn.GRU / nn.LSTM loop that zeroes the
-    state after a done is the ground truth for the forward outputs AND, through autograd, for every gradient."""
+    state after a done is the ground truth for the forward outputs AND, through autograd, for every gradient.
+    At the reference's sizes the forward gate GEMMs run the SIMT kernels under either engine (their k, D, is below 8 or
+    not a multiple of 4, so the wgmma engine does not take W_ih or W_hh); D = 32 and 64 are added so that under "3xtf32"
+    the gate GEMMs run gemm_wgmma_kernel, which the profile of the forward pass asserts."""
     ops = ops_for()
     from sample_factory_b200.model import ModelSpec, PolicyModel
     from sample_factory_b200.rnn_core import RnnCore
@@ -794,7 +798,15 @@ def test_bptt_matches_loopy_torch_rnn(dev, T, N, D, random_dones, rnn_type, engi
     core = RnnCore(model, engine)
     b = core.alloc_bptt(B, T)
     valids = torch.ones(B, dtype=torch.bool, device=dev)
-    got = core.forward_bptt(x.detach().to(dev), states.to(dev), dones.to(dev), valids, b)
+    xd, sd, dd = x.detach().to(dev), states.to(dev), dones.to(dev)
+    res = []
+    kernels = launched(lambda: res.append(core.forward_bptt(xd, sd, dd, valids, b)))
+    got = res[-1]
+    wgmma = sorted(k for k in kernels if k.startswith("gemm_wgmma_kernel<"))
+    if engine_name == "3xtf32" and D % 4 == 0 and D >= 8:
+        assert wgmma, f"the gate GEMMs did not run on the wgmma engine: {sorted(kernels)}"
+    else:
+        assert not wgmma and "gemm_simt_kernel<true, true>" in kernels, sorted(kernels)
     np.testing.assert_allclose(got.cpu().numpy(), loopy.detach().numpy(), atol=4e-6)      # the reference test's tolerance
 
     model.grad.zero_()
